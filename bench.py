@@ -1,8 +1,8 @@
 #!/usr/bin/env python3
-"""bench.py -- headline benchmark of the B200-native Qwen3-TTS decode engine.
+"""bench.py -- headline benchmark of the H100-native Qwen3-TTS decode engine.
 
 Metric (BASELINE.json): xRealTime (RTF = audio seconds / wall seconds) and p50 TTFA, Qwen3-TTS-12Hz-1.7B streaming,
-chunk_size=8, on 1/2/4/8 B200 (independent replicas, no collective on this path).
+chunk_size=8, on 1/2/4/8 H100 (independent replicas, no collective on this path).
 
 A "step" is one streaming voice-clone request of SURVEY.md section 8(d) config 3: an ICL prompt of P=232 positions
 (a 30-word reference transcript + a 17-word text + 174 reference codec frames = 13.9 s of reference audio, assembled
@@ -27,6 +27,8 @@ Weights are random-init at the real 1.7B geometry, inputs synthetic (no checkpoi
   cpu_baseline / --impl reference: the CPU oracle (torch eager fp32, dynamic KV) on a bounded sample, host threads
   --sweep      chunk (BASELINE config 5: chunk_size in {1,2,4,8,16}) / prompt (TTFA over P in {10,40,96,232} split
                into prefill, first chunk, first window) ; --size 0.6B = config 2
+  --dump-outputs DIR  after the timed steps, the PCM of the last timed step (codes when --no-codec) as DIR/*.npy;
+               weights, prompt and sampling noise are seeded, so two builds can be compared output for output
 """
 from __future__ import annotations
 
@@ -73,16 +75,18 @@ def parse():
     ap.add_argument("--sweep", default="none", choices=["none", "chunk", "prompt", "all"])
     ap.add_argument("--num-ctas", type=int, default=0)
     ap.add_argument("--cpu-frames", type=int, default=64)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step returned as DIR/<name>.npy (float32 PCM / float64 codes)")
     return ap.parse_args()
 
 
 # ----------------------------------------------------------------------------------------------------------------
-# clocks sampler (B200_PROFILING.md recipe)
+# clocks sampler: SM clock, power limit and throttle reasons during the timed window (read-only nvidia-smi queries)
 # ----------------------------------------------------------------------------------------------------------------
 class Clocks:
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
-         "clocks_event_reasons.sw_power_cap")
+         "clocks_event_reasons.sw_power_cap,power.limit")
 
     def __init__(self, index: int):
         self.rows, self.proc, self.index = [], None, index
@@ -111,8 +115,9 @@ class Clocks:
                 for name, v in zip(("hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"), r[4:8]):
                     if v.lower().startswith("active"):
                         reasons.add(name)
+        pl = [float(r[8]) for r in self.rows if len(r) >= 9 and r[8].replace(".", "").isdigit()]
         return {"sm_mhz": statistics.median(sm) if sm else None, "sm_max_mhz": max(mx) if mx else None,
-                "reasons": sorted(reasons), "samples": len(sm)}
+                "power_limit_w": max(pl) if pl else None, "reasons": sorted(reasons), "samples": len(sm)}
 
 
 # ----------------------------------------------------------------------------------------------------------------
@@ -181,15 +186,13 @@ def run_reference(args):
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
         return
-    vals = []
-    for i in range(args.warmup + args.steps):
-        rtf, dt, nth, desc = cpu_oracle_run(args, args.cpu_frames)
-        if i >= args.warmup:
-            vals.append((rtf, dt))
-        if i == 0 and args.warmup > 0 and dt > 60:  # keep the whole run within minutes
-            args.warmup = 0
-            vals.append((rtf, dt))
+    for _ in range(args.warmup):
+        if cpu_oracle_run(args, args.cpu_frames)[1] > 60:  # one slow warm-up run is enough
             break
+    vals = []
+    for _ in range(args.steps):
+        rtf, dt, nth, desc = cpu_oracle_run(args, args.cpu_frames)
+        vals.append((rtf, dt))
     v = statistics.mean(x[0] for x in vals)
     ms = statistics.mean(x[1] for x in vals) * 1000
     print(json.dumps({
@@ -212,7 +215,7 @@ def workload_config(args, P=None, **extra):
                      f"({args.ref_frames} reference frames), {args.frames} frames, chunk_size={args.chunk}, "
                      f"T=0.9 top_k=50 top_p=1.0 penalty=1.05, min_new_tokens=max_new_tokens (fixed work)",
          "batch_per_gpu": 1, "parallelism": f"replicas x{args.gpus} (no collective)",
-         "l2_policy": "per-step weight stream (3.2 GB tape) exceeds the 126 MB L2; no explicit flush needed",
+         "l2_policy": "per-step weight stream (3.2 GB tape) exceeds the 50 MB L2; no explicit flush needed",
          "codec_policy": "reference window policy (model.py:1052-1135), sample-identical; Phase 1 of a request with an ICL "
                          "reference runs on a copy of that reference's warmed decoder stream (cached per voice like the voice "
                          "prompt; the e2e leg clears both caches every step, so it pays the reference decode each time)"}
@@ -221,7 +224,7 @@ def workload_config(args, P=None, **extra):
 
 
 # ----------------------------------------------------------------------------------------------------------------
-# B200 arm
+# engine arm
 # ----------------------------------------------------------------------------------------------------------------
 def craft_request(model, P_target: int, ref_frames: int):
     """(text, ref_text, ref_audio, prepared tuple) whose ICL prompt (non_streaming_mode=True: text first, then the
@@ -272,8 +275,9 @@ def run_b200(args):
     kw = dict(max_new_tokens=args.frames, min_new_tokens=args.frames, chunk_size=args.chunk)
     chunk_ms, ttfa_ms = [], []
 
-    def step_resident(timed: bool, chunk=None, prompt=None):
-        """prompt resident in HBM; codes -> PCM per chunk on device.  Returns frames."""
+    def step_resident(timed: bool, chunk=None, prompt=None, keep=None):
+        """prompt resident in HBM; codes -> PCM per chunk on device.  Returns frames; `keep` (a list) collects a copy
+        of every chunk the caller receives."""
         torch.manual_seed(rank * 1000 + len(ttfa_ms))
         e0 = torch.cuda.Event(enable_timing=True)
         e0.record()
@@ -288,6 +292,8 @@ def run_b200(args):
             if first is None:
                 first = torch.cuda.Event(enable_timing=True)
                 first.record()
+            if keep is not None:
+                keep.append(pcm.clone())
             n += t["chunk_steps"]
             if timed and "kernel_ms" in t:
                 chunk_ms.append(t["kernel_ms"])
@@ -329,11 +335,14 @@ def run_b200(args):
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     ev0.record()
     frames = 0
-    for _ in range(args.steps):
-        frames += step_resident(True)
+    last_out = [] if args.dump_outputs else None
+    for i in range(args.steps):
+        frames += step_resident(True, keep=last_out if i == args.steps - 1 else None)
     ev1.record()
     barrier()
     ms = ev0.elapsed_time(ev1)
+    if last_out and rank == 0:
+        dump_outputs(args.dump_outputs, {"codes" if args.no_codec else "pcm": torch.cat([x.reshape(-1) for x in last_out])})
     launches = eng.launch_count + model.codec_launches() - l0
     clk = clocks.stop() if rank == 0 else None
     # ---- extra leg: the same request with the STATEFUL streaming codec (SURVEY 8(f) item 2; not the headline: its
@@ -394,8 +403,8 @@ def run_b200(args):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
-    peak_kind = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6650 GB/s (B200_PROFILING.md)"
+    peak = float(peaks.get("hbm_gbs", 3350.0))
+    peak_kind = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "H100 SXM data sheet, 3350 GB/s"
     t_bytes, p_bytes = eng.tape_bytes()
     esz = 2
     Lt, nKV = tcfg.num_hidden_layers, tcfg.num_key_value_heads
@@ -412,18 +421,6 @@ def run_b200(args):
     b_alg = w_alg + kv_bytes
     b_stream = t_bytes + kv_bytes + p_bytes
     k_ms = statistics.mean(chunk_ms) if chunk_ms else None
-    traffic, traffic_file = None, None
-    for f in ("r2_decode_kernel_ncu.csv", "r1c_decode_kernel_ncu.csv"):
-        if os.path.exists(os.path.join(ROOT, "profiles", f)):
-            traffic_file = f
-            break
-    try:  # DRAM bytes of one launch from the committed ncu capture of this kernel (profiles/)
-        for line in open(os.path.join(ROOT, "profiles", traffic_file)):
-            f = line.strip().split(",")
-            if len(f) == 4 and f[0] == "0" and f[1] in ("dram__bytes_read.sum", "dram__bytes_write.sum"):
-                traffic = (traffic or 0.0) + float(f[3]) * {"Gbyte": 1e9, "Mbyte": 1e6, "Kbyte": 1e3, "byte": 1.0}[f[2]]
-    except Exception:
-        traffic = None
     talker = None
     try:
         ppos = int(pbar)
@@ -447,15 +444,14 @@ def run_b200(args):
     if k_ms:
         ach = b_alg * args.chunk / (k_ms / 1000) / 1e9
         roof = {"bound": "hbm", "kernel": "fq3_decode_kernel<bf16> (one launch = one %d-frame chunk)" % args.chunk,
-                "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak, "traffic": traffic,
-                "traffic_source": ("ncu --set full capture of one 8-frame launch, profiles/" + traffic_file) if traffic_file else None,
+                "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
                 "peak_source": peak_kind, "alg_bytes_per_frame": b_alg, "launch_ms": k_ms,
                 "streamed_bytes_per_frame": b_stream, "streamed_frac": b_stream * args.chunk / (k_ms / 1000) / 1e9 / peak,
                 "ms_per_frame": k_ms / args.chunk, "talker_step": talker}
     out = {
         "metric": METRIC, "value": value, "unit": "x realtime", "n_gpus": world, "steps": args.steps,
         "warmup": args.warmup, "ms_per_step": ms / args.steps, "higher_is_better": True, "scaling": "weak",
-        "vs_baseline": None, "dtype": "bf16", "data": "synthetic",
+        "vs_baseline": None, "dtype": "bf16", "data": "synthetic", "gpu": torch.cuda.get_device_name(dev),
         "config": workload_config(args, P=P, ttfa_ms_p50=statistics.median(ttfa_ms) if ttfa_ms else None,
                                   ttfa_ms_e2e_p50=statistics.median(e_ttfa) if e_ttfa else None,
                                   ttfa_ms_e2e_cached_voice_p50=statistics.median(e_ttfa_cached) if e_ttfa_cached else None,
@@ -513,6 +509,15 @@ def run_b200(args):
     print(json.dumps(out))
     if world > 1:
         dist.destroy_process_group()
+
+
+def dump_outputs(d: str, arrays):
+    """arrays: name -> tensor; floating outputs as float32, integer outputs (codes) as float64 (exact)"""
+    import numpy as np
+    os.makedirs(d, exist_ok=True)
+    for name, t in arrays.items():
+        t = t.detach().cpu()
+        np.save(os.path.join(d, name + ".npy"), t.double().numpy() if not t.is_floating_point() else t.float().numpy())
 
 
 def run_config4(args, model, cfg, dev, rank, barrier):

@@ -1,8 +1,8 @@
 #!/usr/bin/env python3
-"""OpenAI-compatible TTS server over the B200 engine with CONTINUOUS BATCHING.
+"""OpenAI-compatible TTS server over the H100 engine with CONTINUOUS BATCHING.
 
 Same endpoint and wire format as the reference's example server (POST /v1/audio/speech, response_format wav | pcm,
-streaming WAV with an unknown-length header; /root/reference/examples/openai_server.py:91-118,215-263), but requests are
+streaming WAV with an unknown-length header; the reference's examples/openai_server.py:91-118,215-263), but requests are
 not serialised behind a lock (:71,181): up to --max-batch requests share every pass over the model weights and new
 requests join between chunks (faster_qwen3_tts/serving.py).
 
@@ -26,7 +26,7 @@ def build_app(model, batcher, voices, default_voice):
     from pydantic import BaseModel
     from faster_qwen3_tts.serving import to_pcm16, voice_clone_request, wav_header
 
-    app = FastAPI(title="faster-qwen3-tts (B200 engine) OpenAI-compatible API")
+    app = FastAPI(title="faster-qwen3-tts (H100 engine) OpenAI-compatible API")
 
     class SpeechRequest(BaseModel):
         model: str = "tts-1"

@@ -1,5 +1,5 @@
 // fq3_codec.cu -- K4: the waveform decoder stack of the codec (conv_in -> 4 x [SnakeBeta, causal ConvTranspose,
-// 3 residual units] -> SnakeBeta -> conv_out -> clamp) as hand-written sm_100a kernels behind the C ABI.
+// 3 residual units] -> SnakeBeta -> conv_out -> clamp) as hand-written sm_90a kernels behind the C ABI.
 // Replaces the cuDNN/cuBLAS launches issued by the reference's `speech_tokenizer.decode` call sites
 // (faster_qwen3_tts/model.py:924,1093,1122) for the FLOP-dominant part of the decoder (94% of its FLOPs).
 //
@@ -27,7 +27,7 @@
 #include "fq3_gemm.cuh"
 #include "fq3_gemm_tc.cuh"
 
-extern int g_fq3_gemm_backend;  // 0 = tcgen05/TMA kernel when the shape allows, 1 = force the mma.sync kernel
+extern int g_fq3_gemm_backend;  // 0 = wgmma/TMA kernel when the shape allows, 1 = force the mma.sync kernel
 
 namespace {
 
@@ -557,7 +557,7 @@ static int launch_conv(fq3_codec* c, const Layer& L, const __nv_bfloat16* X, con
   if (g_fq3_gemm_backend != 1) {
     const int r = fq3tc::launch_tc(a, stream, g_fq3_gemm_backend);
     if (r == 0) return 0;
-    if (r < 0) return cfail(FQ3_ERR_CUDA, "tcgen05 conv launch failed: ", cudaGetErrorString(cudaGetLastError()));
+    if (r < 0) return cfail(FQ3_ERR_CUDA, "wgmma conv launch failed: ", cudaGetErrorString(cudaGetLastError()));
   }
   dim3 grid(((T + BM - 1) / BM) * batch, (L.N + BN - 1) / BN);
   FQ3_LAUNCH((conv_gemm_kernel), grid, CTHREADS, CONV_SMEM, stream, a);
@@ -783,7 +783,7 @@ static int fe_gemm(fq3_codec* c, const __nv_bfloat16* X, const __nv_bfloat16* W,
   if (g_fq3_gemm_backend != 1) {
     const int r = fq3tc::launch_tc(a, stream, g_fq3_gemm_backend);
     if (r == 0) return 0;
-    if (r < 0) return cfail(FQ3_ERR_CUDA, "tcgen05 GEMM launch failed: ", cudaGetErrorString(cudaGetLastError()));
+    if (r < 0) return cfail(FQ3_ERR_CUDA, "wgmma GEMM launch failed: ", cudaGetErrorString(cudaGetLastError()));
   }
   dim3 grid((rows + BM - 1) / BM, (N + BN - 1) / BN);
   FQ3_LAUNCH((conv_gemm_kernel), grid, CTHREADS, CONV_SMEM, stream, a);

@@ -1,4 +1,4 @@
-// fq3_decode.cuh -- the persistent decode kernel (sm_100a).
+// fq3_decode.cuh -- the persistent decode kernel (sm_90a).
 //
 // One cooperative launch runs a whole chunk of codec frames on device: per frame the 15-pass code predictor
 // (reference: faster_qwen3_tts/predictor_graph.py:115-167), the 16-row embedding sum (generate.py:163-171), the

@@ -1,4 +1,4 @@
-// fq3_decode_batch.cuh -- batched persistent decode kernel (sm_100a): up to 32 request slots share ONE pass over the
+// fq3_decode_batch.cuh -- batched persistent decode kernel (sm_90a): up to 32 request slots share ONE pass over the
 // weight tape per step (BASELINE config 4: concurrent requests per GPU; the reference's batch handling is the
 // left-padded prompt batch of faster_qwen3_tts/model.py:774-787 with per-row pad counts, talker_graph.py:177-187).
 //

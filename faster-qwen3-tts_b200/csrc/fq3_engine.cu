@@ -1,5 +1,5 @@
 // fq3_engine.cu -- C ABI implementation (see include/fq3_engine.h): engine lifecycle, weight-tape packing,
-// launches of the persistent decode kernel (fq3_decode.cuh).  sm_100a only.
+// launches of the persistent decode kernel (fq3_decode.cuh).  sm_90a only.
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdarg.h>
@@ -160,30 +160,33 @@ __global__ void pack_kernel(const PackGrp* __restrict__ pg, int npg, const void*
 __global__ void pack_mma_kernel(const PackGrp* __restrict__ pg, int npg, const void* const* __restrict__ rowsrc,
                                 uint8_t* __restrict__ tape) {
   for (int b = blockIdx.x; b < npg; b += gridDim.x) {
-    const PackGrp g = pg[b];
-    const int n_mt = g.rows & 0xff, kind = g.rows >> 8, G = g.m;
-    const long long total = (long long)g.ntiles * n_mt * G * 128;
-    uint4* dst = reinterpret_cast<uint4*>(tape + g.tape_off);
-    for (long long q = threadIdx.x; q < total; q += blockDim.x) {
-      const int lane = (int)(q & 31), st = (int)((q >> 5) & 3);
-      long long rem = q >> 7;
-      const int qq = (int)(rem % G);
+    // header fields read one by one and 32-bit index arithmetic (a group holds ntiles * G <= K / 64 k-groups of at most
+    // 2 m-tiles, far below 2^31 elements): with a struct copy and 64-bit division, ptxas for sm_90a took G from a
+    // uniform register it never wrote, and the tape came out wrong
+    const int n_mt = pg[b].rows & 0xff, kind = pg[b].rows >> 8, G = pg[b].m, ntiles = pg[b].ntiles, K = pg[b].K;
+    const uint32_t rowsrc_idx = pg[b].rowsrc_idx;
+    const int total = ntiles * n_mt * G * 128;
+    uint4* dst = reinterpret_cast<uint4*>(tape + pg[b].tape_off);
+    for (int q = threadIdx.x; q < total; q += blockDim.x) {
+      const int lane = q & 31, st = (q >> 5) & 3;
+      int rem = q >> 7;
+      const int qq = rem % G;
       rem /= G;
-      const int mt = (int)(rem % n_mt);
-      const int tl = (int)(rem / n_mt);
+      const int mt = rem % n_mt;
+      const int tl = rem / n_mt;
       const int gq = lane >> 2, t = lane & 3;
       const int kk = 64 * (tl * G + qq) + 16 * t + 4 * st;
       const uint8_t *ra, *rb;
       int kb = kk;
       if (kind == 0) {
-        ra = reinterpret_cast<const uint8_t*>(rowsrc[g.rowsrc_idx + mt * 16 + gq]);
-        rb = reinterpret_cast<const uint8_t*>(rowsrc[g.rowsrc_idx + mt * 16 + gq + 8]);
+        ra = reinterpret_cast<const uint8_t*>(rowsrc[rowsrc_idx + mt * 16 + gq]);
+        rb = reinterpret_cast<const uint8_t*>(rowsrc[rowsrc_idx + mt * 16 + gq + 8]);
       } else if (kind == 1) {
-        ra = rb = reinterpret_cast<const uint8_t*>(rowsrc[g.rowsrc_idx + gq]);
-        kb = g.K / 2 + kk;
+        ra = rb = reinterpret_cast<const uint8_t*>(rowsrc[rowsrc_idx + gq]);
+        kb = K / 2 + kk;
       } else {
-        ra = reinterpret_cast<const uint8_t*>(rowsrc[g.rowsrc_idx + 2 * (mt * 8 + gq)]);
-        rb = reinterpret_cast<const uint8_t*>(rowsrc[g.rowsrc_idx + 2 * (mt * 8 + gq) + 1]);
+        ra = reinterpret_cast<const uint8_t*>(rowsrc[rowsrc_idx + 2 * (mt * 8 + gq)]);
+        rb = reinterpret_cast<const uint8_t*>(rowsrc[rowsrc_idx + 2 * (mt * 8 + gq) + 1]);
       }
       const uint2 a = *reinterpret_cast<const uint2*>(ra + (size_t)kk * 2);
       const uint2 c = *reinterpret_cast<const uint2*>(rb + (size_t)kb * 2);
@@ -269,7 +272,7 @@ extern "C" int fq3_engine_create(const fq3_config* cfg, fq3_engine** out) {
   CK(cudaSetDevice(cfg->device));
   cudaDeviceProp prop;
   CK(cudaGetDeviceProperties(&prop, cfg->device));
-  if (prop.major < 10) return fail(FQ3_ERR_INVALID, "sm_100a required (device is sm_%d%d)", prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0) return fail(FQ3_ERR_INVALID, "sm_90a required (device is sm_%d%d)", prop.major, prop.minor);
   int coop = 0;
   CK(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, cfg->device));
   if (!coop) return fail(FQ3_ERR_INVALID, "device lacks cooperative launch");
@@ -365,7 +368,9 @@ extern "C" int fq3_engine_create(const fq3_config* cfg, fq3_engine** out) {
   k.has_mtp = cfg->has_mtp_projection; k.ncb = cfg->num_code_groups - 1; k.eos = cfg->codec_eos_token_id;
   k.max_seq_len = cfg->max_seq_len;
   k.dbg = e->dbg; k.dbg_stride_layer = e->dbg_stride;
-  k.pred_pin_layers = 2;
+  // no predictor layer is streamed with L2 evict_last: one 1.7B predictor layer is 31 MB, and on a 50 MB L2 pinning one or
+  // two of them measured 5 % / 8 % slower per frame than pinning none (H100 80GB HBM3, 400 W limit; FQ3_PRED_PIN overrides)
+  k.pred_pin_layers = 0;
   if (const char* v = getenv("FQ3_PRED_PIN")) k.pred_pin_layers = std::max(atoi(v), 0);   // tuning knob
   {
     // split-key talker attention (bf16 engines): S CTAs per q-head; a slice must fit the 4 ring tiles it may hold
@@ -373,7 +378,7 @@ extern "C" int fq3_engine_create(const fq3_config* cfg, fq3_engine** out) {
     if (Sx < 2 || (cfg->max_seq_len + Sx - 1) / Sx > 4 * KVT_KEYS) Sx = 0;
     if (const char* v = getenv("FQ3_ATTN_SPLIT")) Sx = std::min(Sx, std::max(atoi(v), 0)) < 2 ? 0 : std::min(Sx, atoi(v));
     k.attn_split = Sx;
-    k.attn_split_min = 192;   // measured on B200 (1.7B geometry): split wins from ~250 cached keys up (0.93 vs 1.01 ms/step at 300)
+    k.attn_split_min = 192;   // cached keys from which the split path runs (FQ3_ATTN_SPLIT_MIN overrides it)
     if (const char* v = getenv("FQ3_ATTN_SPLIT_MIN")) k.attn_split_min = std::max(atoi(v), 0);
     k.PART = e->PART;
     k.attn_cnt = e->bar + 1024;
@@ -735,7 +740,7 @@ extern "C" int fq3_engine_load_weights(fq3_engine* e, const fq3_tensor* tensors,
   CK(cudaMemcpyAsync(d_rowsrc, rowsrc.data(), rowsrc.size() * sizeof(void*), cudaMemcpyHostToDevice, stream));
   CK(cudaMemcpyAsync(d_pack, pack.data(), pack.size() * sizeof(PackGrp), cudaMemcpyHostToDevice, stream));
   {
-    const int grid = (int)std::min<size_t>(pack.size(), 148 * 16);
+    const int grid = (int)std::min<size_t>(pack.size(), 132 * 16);
     if (e->bf16) pack_mma_kernel<<<grid, 256, 0, stream>>>(d_pack, (int)pack.size(), (const void* const*)d_rowsrc, e->tape);
     else pack_kernel<false><<<grid, 256, 0, stream>>>(d_pack, (int)pack.size(), (const void* const*)d_rowsrc, e->tape);
     e->launches++;
@@ -1097,6 +1102,6 @@ extern "C" int fq3_num_ctas(fq3_engine* e) { return e ? e->ncta : 0; }
 extern "C" int64_t fq3_launch_count(fq3_engine* e) { return e ? e->launches : 0; }
 extern "C" const char* fq3_last_error(void) { return g_err; }
 extern "C" int fq3_max_batch(fq3_engine* e) { return e ? e->max_batch : 0; }
-extern "C" const char* fq3_version(void) { return "fq3-b200 0.2.0 (sm_100a)"; }
+extern "C" const char* fq3_version(void) { return "fq3-h100 0.2.0 (sm_90a)"; }
 
 #include "fq3_prefill.cuh"

@@ -17,7 +17,7 @@ namespace fq3gemm {
 
 // ---- programmatic dependent launch (PDL): the K3 / K4 chains are hundreds of short dependent kernels; with
 // programmatic stream serialization kernel N+1 is scheduled as soon as every CTA of kernel N has started, runs its
-// prologue (barrier init, TMEM allocation, tensor-map prefetch, parameter staging) and blocks in griddepcontrol.wait
+// prologue (barrier init, tensor-map prefetch) and blocks in griddepcontrol.wait
 // until kernel N has completed and flushed its memory -- launch latency and prologue leave the critical path, memory
 // semantics are those of ordinary stream order.  Every kernel launched through launch_pdl() calls pdl_wait() before
 // its first access to memory another kernel may have written.  FQ3_NO_PDL=1 launches them plainly (A/B).

@@ -1,11 +1,12 @@
-// fq3_gemm_tc.cuh -- the implicit-GEMM causal conv / linear kernel on 5th-generation tensor cores (sm_100a):
-//   * operands staged by TMA (cp.async.bulk.tensor.2d, SASS UTMALDG) into 128B/64B-swizzled shared-memory tiles;
+// fq3_gemm_tc.cuh -- the implicit-GEMM causal conv / linear kernel on Hopper tensor cores (sm_90a):
+//   * operands staged by TMA (cp.async.bulk.tensor.2d/3d, SASS UTMALDG) into 128B/64B-swizzled shared-memory tiles;
 //     the causal left padding and the M/N tails are TMA out-of-bounds zero fill (negative row coordinates),
-//   * tcgen05.mma (SASS UTCHMMA) issued by one thread, 128 x 96 fp32 accumulator in TMEM,
-//   * warp-specialised: warp 0 = TMA producer, warp 1 = MMA issuer (+ TMEM alloc), warps 2-5 = epilogue
-//     (tcgen05.ld -> bias / residual / SnakeBeta / SwiGLU -> 16-byte bf16 stores),
-//   * 3-stage (BK=64) / 4-stage (BK=32) full/empty mbarrier ring sized so 2-4 CTAs co-reside per SM; tcgen05.commit
-//     releases stages and publishes the accumulator.
+//   * warp-specialised: warps 0-3 form one consumer warpgroup that issues wgmma.mma_async m64n96k16 (SASS HGMMA,
+//     both operands read from shared memory through matrix descriptors, 128 x 96 fp32 accumulator in registers) and
+//     then runs the epilogue; warp 4 is the TMA producer,
+//   * 3-stage (BK=64) / 4-stage (BK=32) full/empty mbarrier ring sized so 2-3 CTAs co-reside per SM,
+//   * epilogue: the accumulator is staged through shared memory so that each consumer thread owns one output row
+//     (bias / residual / SnakeBeta / SwiGLU -> 16-byte bf16 stores).
 // Same arguments and epilogue semantics as the mma.sync kernel in fq3_gemm.cuh (which remains as the fallback for
 // Cin % 32 != 0 and as an A/B reference: fq3_set_gemm_backend()).
 #pragma once
@@ -21,20 +22,29 @@
 
 namespace fq3tc {
 
-constexpr int TBM = 128, TBN = 96, TTHREADS = 192;
-constexpr int TMEM_COLS = 128;
+constexpr int TBM = 128, TBN = 96, TTHREADS = 160;   // warps 0-3: consumer warpgroup, warp 4: TMA producer
+constexpr int SC_LD = TBN + 1;                        // fp32 staging row stride (odd: row-per-thread reads hit 32 banks)
+constexpr int SC_BYTES = TBM * SC_LD * 4;
 
-// DEEP = 1: grids that do not fill the machine (<= one CTA per SM) get a deep ring (latency-bound main loop);
-// DEEP = 0: large grids get small rings so 2-4 CTAs co-reside per SM and overlap each other's prologue / epilogue.
-template <int BK, int DEEP>
+// KIND 0: one tile per CTA with a small ring, so 2-3 CTAs co-reside per SM and overlap each other's prologue / epilogue;
+// KIND 1: one tile per CTA with a deep ring, for grids that do not fill the machine (latency-bound main loop);
+// KIND 2: persistent tile loop (A/B only), with a staging buffer of its own so the ring keeps filling during the epilogue.
+template <int BK, int KIND>
 struct Cfg {
   static constexpr int A_BYTES = TBM * BK * 2;
   static constexpr int B_BYTES = TBN * BK * 2;
   static constexpr int STAGE = A_BYTES + B_BYTES;
-  static constexpr int STAGES = DEEP ? (BK == 64 ? 7 : 12) : (BK == 64 ? 3 : 4);
-  static constexpr int SMEM = STAGES * STAGE + 1024 /*align slack*/ + 256 /*barriers*/ + 4 * TBN * 4 /*epilogue params*/;
+  static constexpr int STAGES = KIND == 1 ? (BK == 64 ? 7 : 12) : KIND == 2 ? (BK == 64 ? 6 : 10) : (BK == 64 ? 3 : 4);
+  static constexpr int RING = STAGES * STAGE;
+  static constexpr int EP_OFF = RING + 256 /*barriers*/;
+  static constexpr int SC_OFF = KIND == 2 ? EP_OFF + 4 * TBN * 4 : 0;  // one tile per CTA: staging reuses the drained ring
+  static constexpr int SMEM = 1024 /*align slack*/ + EP_OFF + 4 * TBN * 4 /*epilogue params*/ + (KIND == 2 ? SC_BYTES : 0);
   static constexpr uint32_t SBO = (8 * BK * 2) >> 4;          // 8-row group stride, 16-byte units
-  static constexpr uint64_t LAYOUT = BK == 64 ? 2ull : 4ull;  // SWIZZLE_128B : SWIZZLE_64B
+  static constexpr uint64_t LAYOUT = BK == 64 ? 1ull : 2ull;  // wgmma descriptor: SWIZZLE_128B : SWIZZLE_64B
+  static constexpr uint32_t A_HALF = (64 * BK * 2) >> 4;      // rows 64..127 of the A tile, 16-byte units
+  static_assert(KIND == 2 || RING >= SC_BYTES, "accumulator staging must fit in the ring");
+  static_assert(2 * STAGES * 8 <= 256, "barriers exceed their slot");
+  static_assert(SMEM <= 232448, "exceeds the 227 KB per-CTA shared-memory limit");
 };
 
 __device__ __forceinline__ uint32_t su32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -43,6 +53,9 @@ __device__ __forceinline__ void mb_init(uint64_t* b, uint32_t n) {
 }
 __device__ __forceinline__ void mb_expect(uint64_t* b, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(su32(b)), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mb_arrive(uint64_t* b) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(su32(b)) : "memory");
 }
 // bounded wait: a descriptor / protocol bug traps instead of hanging the GPU
 __device__ __forceinline__ void mb_wait(uint64_t* b, uint32_t parity) {
@@ -64,33 +77,34 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* tm, in
   asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
                ::"r"(su32(dst)), "l"(tm), "r"(su32(bar)), "r"(c0), "r"(c1), "r"(c2) : "memory");
 }
+// wgmma matrix descriptor of a K-major swizzled tile (tiles are 1024-byte aligned: base offset 0)
 __device__ __forceinline__ uint64_t smem_desc(const void* p, uint32_t sbo, uint64_t layout) {
   uint64_t d = 0;
   d |= (uint64_t)((su32(p) >> 4) & 0x3fff);   // start address
   d |= (uint64_t)1 << 16;                     // leading byte offset (unused for swizzled K-major) = 1
   d |= (uint64_t)(sbo & 0x3fff) << 32;        // stride byte offset
-  d |= (uint64_t)1 << 46;                     // descriptor version (Blackwell)
-  d |= layout << 61;
+  d |= layout << 62;
   return d;
 }
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t acc) {
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// d[64 x 96] (+)= A[64 x 16] * B[96 x 16]^T, bf16 operands K-major in shared memory, fp32 accumulator
+__device__ __forceinline__ void wgmma_m64n96(float (&d)[48], uint64_t da, uint64_t db, uint32_t acc) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(acc) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(su32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %50, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n96k16.f32.bf16.bf16 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,"
+      "%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47}, %48, %49, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+        "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),
+        "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+        "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
+      : "l"(da), "l"(db), "r"(acc)
+      : "memory");
 }
 
 // epilogue of one accumulator row (r: 96 fp32 columns of output row m of sequence bidx, columns n0..n0+95);
@@ -163,163 +177,34 @@ if (m < a.T) {
 }
 }
 
-template <int BK, int DEEP>
-static __global__ void __launch_bounds__(TTHREADS, DEEP ? 1 : 2)
+// Tiles are numbered M fastest (tile = nt * tiles_mb + bidx * tiles_m + m-tile), so the CTAs running concurrently
+// share one weight tile (L2 / TMA locality).  KIND 0/1 launch one CTA per tile; KIND 2 launches one CTA per SM that
+// walks a strided list of tiles, with the ring running ahead into the next tile while the epilogue of this one runs.
+template <int BK, int KIND>
+static __global__ void __launch_bounds__(TTHREADS, KIND == 0 ? 2 : 1)
     conv_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW,
-                        const __grid_constant__ fq3gemm::ConvArgs a) {
-  using C = Cfg<BK, DEEP>;
+                        const __grid_constant__ fq3gemm::ConvArgs a, const int tiles_m, const int tiles_mb, const int ntiles) {
+  using C = Cfg<BK, KIND>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* tiles = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint64_t* full = reinterpret_cast<uint64_t*>(tiles + C::STAGES * C::STAGE);
+  uint64_t* full = reinterpret_cast<uint64_t*>(tiles + C::RING);
   uint64_t* empty = full + C::STAGES;
-  uint64_t* accum = empty + C::STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(accum + 1);
-  float* ep = reinterpret_cast<float*>(tiles + C::STAGES * C::STAGE + 256);  // [4][TBN]: bias, exp(alpha), 1/(exp(beta)+eps), scale
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int tiles_m = (a.T + TBM - 1) / TBM;
-  const int bidx = blockIdx.x / tiles_m;   // sequence of the batch (own causal padding: TMA zero-fills rows < 0 of ITS time axis)
-  const int m0 = (blockIdx.x - bidx * tiles_m) * TBM, n0 = blockIdx.y * TBN;
-  const int kc = a.Cin / BK, nks = a.taps * kc;
-
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < C::STAGES; ++i) { mb_init(&full[i], 1); mb_init(&empty[i], 1); }
-    mb_init(accum, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmX) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmW) : "memory");
-  }
-  if (warp == 1) {  // TMEM allocation (one full warp), address published through shared memory
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(su32(tmem_slot)), "n"(TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem = *tmem_slot;
-  fq3gemm::pdl_launch();   // the next kernel of the chain may start its own prologue ...
-  fq3gemm::pdl_wait();     // ... and this one touches activations only after its predecessor has completed
-
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    if (lane == 0) {
-      for (int ks = 0; ks < nks; ++ks) {
-        const int s = ks % C::STAGES;
-        mb_wait(&empty[s], ((ks / C::STAGES) & 1) ^ 1);
-        const int tap = ks / kc, c0 = (ks - tap * kc) * BK;
-        const int shift = (a.taps - 1 - tap) * a.dil;
-        uint8_t* A = tiles + s * C::STAGE;
-        uint8_t* B = A + C::A_BYTES;
-        mb_expect(&full[s], C::STAGE);
-        tma_load_3d(A, &tmX, c0, m0 - shift + a.x_row0, bidx, &full[s]);    // rows < 0 or >= T of this sequence are zero-filled by TMA
-        tma_load_2d(B, &tmW, tap * a.Cin + c0, n0, &full[s]);
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      constexpr uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(TBN >> 3) << 17) | ((uint32_t)(TBM >> 4) << 24);
-      for (int ks = 0; ks < nks; ++ks) {
-        const int s = ks % C::STAGES;
-        mb_wait(&full[s], (ks / C::STAGES) & 1);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint8_t* A = tiles + s * C::STAGE;
-        const uint64_t da = smem_desc(A, C::SBO, C::LAYOUT), db = smem_desc(A + C::A_BYTES, C::SBO, C::LAYOUT);
-#pragma unroll
-        for (int k = 0; k < BK / 16; ++k)  // advance 16 elements = 32 bytes = 2 x 16-byte units along K
-          umma_bf16(tmem, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, (ks | k) ? 1u : 0u);
-        umma_commit(&empty[s]);   // stage reusable once these MMAs have read it
-      }
-      umma_commit(accum);         // accumulator complete
-    }
-  } else {
-    // ===================== epilogue (warps 2..5) =====================
-    // per-column parameters of this tile go to shared memory while the main loop runs (no modulo / dependent global
-    // loads on the critical path after the accumulator is ready)
-    for (int i = threadIdx.x - 64; i < TBN; i += 128) {
-      const int n = n0 + i;
-      const bool ok = n < a.N && a.mode != 1;
-      ep[i] = (ok && a.bias) ? a.bias[n % a.bias_mod] : 0.f;
-      ep[TBN + i] = (ok && a.Yact) ? a.ea[n % a.act_mod] : 0.f;
-      ep[2 * TBN + i] = (ok && a.Yact) ? a.ib[n % a.act_mod] : 0.f;
-      ep[3 * TBN + i] = (ok && a.scale) ? a.scale[n % a.scale_mod] : 1.f;
-    }
-    asm volatile("bar.sync 1, 128;" ::: "memory");
-    mb_wait(accum, 0);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const int q = warp & 3;                 // TMEM lane quarter this warp may access
-    const int m = m0 + q * 32 + lane;
-    uint32_t r[3][32];
-#pragma unroll
-    for (int j = 0; j < 3; ++j) tmem_ld32(tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(j * 32), r[j]);
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-    tc_epilogue_row(a, ep, r, m, bidx, n0);
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  }
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "n"(TMEM_COLS) : "memory");
-  }
-}
-
-
-// ------------------------------------------------------------------------------------------------------------
-// Persistent variant (A/B only -- measured 3-15 % SLOWER than the one-tile-per-CTA kernel on the codec shapes: with one
-// CTA per SM a single TMA thread and a single MMA thread issue every k-step of ~50 ns, whereas 2-4 co-resident one-tile
-// CTAs give the SM several independent issue chains and overlap each other's prologue / epilogue anyway):
-// one CTA per SM walks a strided list of output tiles; the fp32 accumulator is DOUBLE-BUFFERED in
-// TMEM (2 x 128 columns), so the epilogue of tile i (tcgen05.ld -> bias / residual / SnakeBeta -> stores) runs while
-// the TMA / MMA warps are already in the main loop of tile i+1; barriers, TMEM and the descriptor prefetch are paid
-// once per CTA instead of once per tile, and the smem ring never drains between tiles.  Tile order: M fastest, so the
-// CTAs running concurrently share one weight tile (L2 / TMA locality).
-// ------------------------------------------------------------------------------------------------------------
-template <int BK>
-struct PCfg {
-  static constexpr int A_BYTES = TBM * BK * 2;
-  static constexpr int B_BYTES = TBN * BK * 2;
-  static constexpr int STAGE = A_BYTES + B_BYTES;
-  static constexpr int STAGES = BK == 64 ? 6 : 10;
-  static constexpr int SMEM = STAGES * STAGE + 1024 /*align slack*/ + 512 /*barriers*/ + 4 * TBN * 4 /*epilogue params*/;
-  static constexpr uint32_t SBO = (8 * BK * 2) >> 4;
-  static constexpr uint64_t LAYOUT = BK == 64 ? 2ull : 4ull;
-};
-constexpr int PTMEM_COLS = 256;
-
-template <int BK>
-static __global__ void __launch_bounds__(TTHREADS, 1)
-    conv_gemm_tcp_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW,
-                         const __grid_constant__ fq3gemm::ConvArgs a, const int tiles_m, const int tiles_mb, const int ntiles) {
-  using C = PCfg<BK>;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* tiles = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint64_t* full = reinterpret_cast<uint64_t*>(tiles + C::STAGES * C::STAGE);
-  uint64_t* empty = full + C::STAGES;
-  uint64_t* accf = empty + C::STAGES;   // [2] accumulator buffer complete (MMA -> epilogue)
-  uint64_t* acce = accf + 2;            // [2] accumulator buffer drained (epilogue -> MMA)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acce + 2);
-  float* ep = reinterpret_cast<float*>(tiles + C::STAGES * C::STAGE + 512);
+  float* ep = reinterpret_cast<float*>(tiles + C::EP_OFF);  // [4][TBN]: bias, exp(alpha), 1/(exp(beta)+eps), scale
+  float* sc = reinterpret_cast<float*>(tiles + C::SC_OFF);  // [TBM][SC_LD] fp32 accumulator tile
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int kc = a.Cin / BK, nks = a.taps * kc;
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < C::STAGES; ++i) { mb_init(&full[i], 1); mb_init(&empty[i], 1); }
-    for (int i = 0; i < 2; ++i) { mb_init(&accf[i], 1); mb_init(&acce[i], 4); }
+    for (int i = 0; i < C::STAGES; ++i) { mb_init(&full[i], 1); mb_init(&empty[i], 128); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmX) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmW) : "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(su32(tmem_slot)), "n"(PTMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem = *tmem_slot;
   fq3gemm::pdl_launch();   // the next kernel of the chain may start its own prologue ...
   fq3gemm::pdl_wait();     // ... and this one touches activations only after its predecessor has completed
 
-  if (warp == 0) {
+  if (warp == 4) {
     // ===================== TMA producer =====================
     if (lane == 0) {
       uint32_t it = 0;
@@ -333,70 +218,72 @@ static __global__ void __launch_bounds__(TTHREADS, 1)
           const int shift = (a.taps - 1 - tap) * a.dil;
           uint8_t* A = tiles + s * C::STAGE;
           mb_expect(&full[s], C::STAGE);
-          tma_load_3d(A, &tmX, c0, m0 - shift + a.x_row0, bidx, &full[s]);
+          tma_load_3d(A, &tmX, c0, m0 - shift + a.x_row0, bidx, &full[s]);   // rows < 0 or >= T of this sequence are zero-filled by TMA
           tma_load_2d(A + C::A_BYTES, &tmW, tap * a.Cin + c0, n0, &full[s]);
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      constexpr uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(TBN >> 3) << 17) | ((uint32_t)(TBM >> 4) << 24);
-      uint32_t it = 0, j = 0;
-      for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++j) {
-        const uint32_t b = j & 1u;
-        mb_wait(&acce[b], ((j >> 1) & 1u) ^ 1u);     // the epilogue has drained this accumulator buffer
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t tacc = tmem + b * 128u;
-        for (int ks = 0; ks < nks; ++ks, ++it) {
-          const int s = (int)(it % C::STAGES);
-          mb_wait(&full[s], (it / C::STAGES) & 1u);
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint8_t* A = tiles + s * C::STAGE;
-          const uint64_t da = smem_desc(A, C::SBO, C::LAYOUT), db = smem_desc(A + C::A_BYTES, C::SBO, C::LAYOUT);
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k)
-            umma_bf16(tacc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, (ks | k) ? 1u : 0u);
-          umma_commit(&empty[s]);
-        }
-        umma_commit(&accf[b]);
-      }
-    }
-  } else {
-    // ===================== epilogue (warps 2..5) =====================
-    const int q = warp & 3;
-    uint32_t j = 0;
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++j) {
-      const int nt = tile / tiles_mb, mb = tile - nt * tiles_mb;
-      const int bidx = mb / tiles_m, m0 = (mb - bidx * tiles_m) * TBM, n0 = nt * TBN;
-      asm volatile("bar.sync 1, 128;" ::: "memory");   // everyone is done with the previous tile's parameters
-      for (int i = threadIdx.x - 64; i < TBN; i += 128) {
-        const int n = n0 + i;
-        const bool ok = n < a.N && a.mode != 1;
-        ep[i] = (ok && a.bias) ? a.bias[n % a.bias_mod] : 0.f;
-        ep[TBN + i] = (ok && a.Yact) ? a.ea[n % a.act_mod] : 0.f;
-        ep[2 * TBN + i] = (ok && a.Yact) ? a.ib[n % a.act_mod] : 0.f;
-        ep[3 * TBN + i] = (ok && a.scale) ? a.scale[n % a.scale_mod] : 1.f;
-      }
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      const uint32_t b = j & 1u;
-      mb_wait(&accf[b], (j >> 1) & 1u);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      uint32_t r[3][32];
-#pragma unroll
-      for (int jj = 0; jj < 3; ++jj) tmem_ld32(tmem + b * 128u + ((uint32_t)(q * 32) << 16) + (uint32_t)(jj * 32), r[jj]);
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(su32(&acce[b])) : "memory");
-      tc_epilogue_row(a, ep, r, m0 + q * 32 + lane, bidx, n0);
-    }
+    return;
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "n"(PTMEM_COLS) : "memory");
+
+  // ===================== consumer warpgroup: wgmma main loop + epilogue =====================
+  const int t = threadIdx.x;   // 0..127
+  uint32_t it = 0;
+  for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    const int nt = tile / tiles_mb, mb = tile - nt * tiles_mb;
+    const int bidx = mb / tiles_m, m0 = (mb - bidx * tiles_m) * TBM, n0 = nt * TBN;
+    // per-column parameters of this tile go to shared memory while the first stages are in flight
+    for (int i = t; i < TBN; i += 128) {
+      const int n = n0 + i;
+      const bool ok = n < a.N && a.mode != 1;
+      ep[i] = (ok && a.bias) ? a.bias[n % a.bias_mod] : 0.f;
+      ep[TBN + i] = (ok && a.Yact) ? a.ea[n % a.act_mod] : 0.f;
+      ep[2 * TBN + i] = (ok && a.Yact) ? a.ib[n % a.act_mod] : 0.f;
+      ep[3 * TBN + i] = (ok && a.scale) ? a.scale[n % a.scale_mod] : 1.f;
+    }
+    float acc[2][48];   // rows 0-63 / 64-127 of the tile
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int i = 0; i < 48; ++i) acc[h][i] = 0.f;
+    for (int ks = 0; ks < nks; ++ks, ++it) {
+      const int s = (int)(it % C::STAGES);
+      mb_wait(&full[s], (it / C::STAGES) & 1u);
+      const uint8_t* A = tiles + s * C::STAGE;
+      const uint64_t da = smem_desc(A, C::SBO, C::LAYOUT), db = smem_desc(A + C::A_BYTES, C::SBO, C::LAYOUT);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < BK / 16; ++k) {  // advance 16 elements = 32 bytes = 2 x 16-byte units along K
+        wgmma_m64n96(acc[0], da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (ks | k) ? 1u : 0u);
+        wgmma_m64n96(acc[1], da + (uint64_t)(C::A_HALF + 2 * k), db + (uint64_t)(2 * k), (ks | k) ? 1u : 0u);
+      }
+      wgmma_commit();
+      wgmma_wait<1>();                                            // the previous stage's MMAs have read their operands
+      if (ks > 0) mb_arrive(&empty[(it - 1) % C::STAGES]);
+    }
+    wgmma_wait<0>();
+    if (nks > 0) mb_arrive(&empty[(it - 1) % C::STAGES]);
+    asm volatile("bar.sync 1, 128;" ::: "memory");   // all MMAs of the warpgroup are done before the staging buffer is written
+    {
+      // accumulator fragment: register 4j + 2h + c holds row 16 * warp + lane / 4 + 8h, column 8j + 2 (lane % 4) + c
+      const int r0 = warp * 16 + (lane >> 2), c0 = 2 * (lane & 3);
+#pragma unroll
+      for (int hm = 0; hm < 2; ++hm)
+#pragma unroll
+        for (int j = 0; j < 12; ++j)
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int c = 0; c < 2; ++c) sc[(hm * 64 + r0 + 8 * h) * SC_LD + 8 * j + c0 + c] = acc[hm][4 * j + 2 * h + c];
+    }
+    asm volatile("bar.sync 1, 128;" ::: "memory");
+    uint32_t r[3][32];
+#pragma unroll
+    for (int j = 0; j < 3; ++j)
+#pragma unroll
+      for (int i = 0; i < 32; ++i) r[j][i] = __float_as_uint(sc[t * SC_LD + j * 32 + i]);
+    tc_epilogue_row(a, ep, r, m0 + t, bidx, n0);
+    asm volatile("bar.sync 1, 128;" ::: "memory");   // staging buffer and parameters are free for the next tile
   }
 }
 
@@ -478,19 +365,26 @@ static bool cached_map(CUtensorMap* tm, const void* base, uint64_t batch /*0: 2-
   return true;
 }
 
+template <int BK, int KIND>
+static bool set_smem_attr() {
+  return cudaFuncSetAttribute(conv_gemm_tc_kernel<BK, KIND>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<BK, KIND>::SMEM) == cudaSuccess;
+}
+template <int BK, int KIND>
+static void launch_kind(int grid, const CUtensorMap& tmX, const CUtensorMap& tmW, const fq3gemm::ConvArgs& a, int tiles_m,
+                        int tiles_mb, int ntiles, cudaStream_t stream) {
+  FQ3_LAUNCH((conv_gemm_tc_kernel<BK, KIND>), grid, TTHREADS, (Cfg<BK, KIND>::SMEM), stream, tmX, tmW, a, tiles_m, tiles_mb, ntiles);
+}
+
 // returns 0 on success, 1 if this shape must use the mma.sync fallback, <0 on CUDA error
-// variant: 0 = one tile per CTA, 2-4 CTAs co-resident per SM (default: measured faster, profiles/r2c_codec_gemm_variants.jsonl),
-//          2 = persistent kernel (double-buffered TMEM accumulator) whenever a CTA would get more than one tile
+// variant: 0 = one tile per CTA, 2-3 CTAs co-resident per SM (default),
+//          2 = persistent kernel whenever a CTA would get more than one tile
 static int launch_tc(const fq3gemm::ConvArgs& a, cudaStream_t stream, int variant = 0) {
   static bool attr_done = false;
-  static int num_sms = 148;
+  static int num_sms = 132;
   if (!attr_done) {
-    if (cudaFuncSetAttribute(conv_gemm_tc_kernel<64, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<64, 0>::SMEM) != cudaSuccess) return -1;
-    if (cudaFuncSetAttribute(conv_gemm_tc_kernel<32, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<32, 0>::SMEM) != cudaSuccess) return -1;
-    if (cudaFuncSetAttribute(conv_gemm_tc_kernel<64, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<64, 1>::SMEM) != cudaSuccess) return -1;
-    if (cudaFuncSetAttribute(conv_gemm_tc_kernel<32, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<32, 1>::SMEM) != cudaSuccess) return -1;
-    if (cudaFuncSetAttribute(conv_gemm_tcp_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, PCfg<64>::SMEM) != cudaSuccess) return -1;
-    if (cudaFuncSetAttribute(conv_gemm_tcp_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, PCfg<32>::SMEM) != cudaSuccess) return -1;
+    if (!set_smem_attr<64, 0>() || !set_smem_attr<32, 0>() || !set_smem_attr<64, 1>() || !set_smem_attr<32, 1>() ||
+        !set_smem_attr<64, 2>() || !set_smem_attr<32, 2>())
+      return -1;
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev);
@@ -500,25 +394,23 @@ static int launch_tc(const fq3gemm::ConvArgs& a, cudaStream_t stream, int varian
   if (!BK || (a.N & 7) || (((uintptr_t)a.X | (uintptr_t)a.W) & 15)) return 1;
   if ((a.Yraw && ((uintptr_t)a.Yraw & 15)) || (a.Yact && ((uintptr_t)a.Yact & 15)) || (a.R && ((uintptr_t)a.R & 15))) return 1;
   if (a.mode == 1 ? (a.N % 32 != 0) : (a.N % 8 != 0)) return 1;
-  CUtensorMap tmX, tmW;
   const int nb = a.batch > 1 ? a.batch : 1;
+  const long long tiles_m = (a.T + TBM - 1) / TBM, tiles_mb = tiles_m * nb;
+  const long long ntiles = tiles_mb * ((a.N + TBN - 1) / TBN);
+  if (ntiles >= (1ll << 30)) return 1;
+  CUtensorMap tmX, tmW;
   if (!cached_map(&tmX, a.X, (uint64_t)nb, (uint64_t)(a.x_rows > 0 ? a.x_rows : a.T), (uint64_t)a.Cin, TBM, BK)) return 1;
   if (!cached_map(&tmW, a.W, 0, (uint64_t)a.N, (uint64_t)a.taps * a.Cin, TBN, BK)) return 1;
-  dim3 grid(((a.T + TBM - 1) / TBM) * nb, (a.N + TBN - 1) / TBN);
-  const long long ntiles = (long long)grid.x * grid.y;
-  if (variant == 2 && ntiles > num_sms && ntiles < (1ll << 30)) {
-    const int tiles_m = (a.T + TBM - 1) / TBM;
-    if (BK == 64) FQ3_LAUNCH((conv_gemm_tcp_kernel<64>), num_sms, TTHREADS, PCfg<64>::SMEM, stream, tmX, tmW, a, tiles_m, tiles_m * nb, (int)ntiles);
-    else FQ3_LAUNCH((conv_gemm_tcp_kernel<32>), num_sms, TTHREADS, PCfg<32>::SMEM, stream, tmX, tmW, a, tiles_m, tiles_m * nb, (int)ntiles);
-    return cudaGetLastError() == cudaSuccess ? 0 : -1;
-  }
-  const bool deep = (long long)grid.x * grid.y <= (long long)num_sms * 3 / 2;
-  if (BK == 64) {
-    if (deep) FQ3_LAUNCH((conv_gemm_tc_kernel<64, 1>), grid, TTHREADS, (Cfg<64, 1>::SMEM), stream, tmX, tmW, a);
-    else FQ3_LAUNCH((conv_gemm_tc_kernel<64, 0>), grid, TTHREADS, (Cfg<64, 0>::SMEM), stream, tmX, tmW, a);
+  const int tm = (int)tiles_m, tmb = (int)tiles_mb, nt = (int)ntiles;
+  if (variant == 2 && ntiles > num_sms) {
+    if (BK == 64) launch_kind<64, 2>(num_sms, tmX, tmW, a, tm, tmb, nt, stream);
+    else launch_kind<32, 2>(num_sms, tmX, tmW, a, tm, tmb, nt, stream);
+  } else if (ntiles <= (long long)num_sms * 3 / 2) {
+    if (BK == 64) launch_kind<64, 1>(nt, tmX, tmW, a, tm, tmb, nt, stream);
+    else launch_kind<32, 1>(nt, tmX, tmW, a, tm, tmb, nt, stream);
   } else {
-    if (deep) FQ3_LAUNCH((conv_gemm_tc_kernel<32, 1>), grid, TTHREADS, (Cfg<32, 1>::SMEM), stream, tmX, tmW, a);
-    else FQ3_LAUNCH((conv_gemm_tc_kernel<32, 0>), grid, TTHREADS, (Cfg<32, 0>::SMEM), stream, tmX, tmW, a);
+    if (BK == 64) launch_kind<64, 0>(nt, tmX, tmW, a, tm, tmb, nt, stream);
+    else launch_kind<32, 0>(nt, tmX, tmW, a, tm, tmb, nt, stream);
   }
   return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }

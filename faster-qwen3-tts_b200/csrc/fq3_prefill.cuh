@@ -376,7 +376,7 @@ static int pf_gemm(fq3_engine* e, const __nv_bfloat16* X, const __nv_bfloat16* W
   if (g_fq3_gemm_backend != 1) {
     const int r = fq3tc::launch_tc(a, stream, g_fq3_gemm_backend);
     if (r == 0) return 0;
-    if (r < 0) return fail(FQ3_ERR_CUDA, "tcgen05 GEMM launch failed: %s", cudaGetErrorString(cudaGetLastError()));
+    if (r < 0) return fail(FQ3_ERR_CUDA, "wgmma GEMM launch failed: %s", cudaGetErrorString(cudaGetLastError()));
   }
   dim3 grid((T + fq3gemm::BM - 1) / fq3gemm::BM, (N + fq3gemm::BN - 1) / fq3gemm::BN);
   fq3gemm::conv_gemm_kernel<<<grid, fq3gemm::CTHREADS, fq3gemm::CONV_SMEM, stream>>>(a);

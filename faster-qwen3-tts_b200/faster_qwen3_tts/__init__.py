@@ -1,4 +1,4 @@
-"""B200-native drop-in for andimarafioti/faster-qwen3-tts (hot path only; see DESIGN.md)."""
+"""H100-native drop-in for andimarafioti/faster-qwen3-tts (hot path only; see DESIGN.md)."""
 __version__ = "0.3.2+b200.1"
 
 __all__ = ["FasterQwen3TTS", "__version__"]

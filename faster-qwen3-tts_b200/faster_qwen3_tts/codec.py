@@ -13,7 +13,7 @@ Total upsample 1920.  "parity unpinned" (analogue geometry, synthetic weights).
 
 The torch module below is the weight container and the library (cuDNN / cuBLAS) functional baseline
 (``backend="torch"``).  ``backend="engine"`` -- the default on CUDA -- runs the WHOLE decode, codes in / PCM out, in
-the hand-written sm_100a kernels behind the C ABI (``fq3_codec_decode_codes``, csrc/fq3_codec.cu): no library kernel
+the hand-written sm_90a kernels behind the C ABI (``fq3_codec_decode_codes``, csrc/fq3_codec.cu): no library kernel
 is launched (DESIGN.md, kernel K4).
 """
 from __future__ import annotations
@@ -213,7 +213,7 @@ class SpeechTokenizer:
     """The decode side of the upstream speech tokenizer, as the reference consumes it
     (``decode({"audio_codes": [B,T,16]}) -> ([wav], sample_rate)``).
 
-    backend="engine": codes -> PCM entirely in the hand-written sm_100a kernels of csrc/fq3_codec.cu through the C
+    backend="engine": codes -> PCM entirely in the hand-written sm_90a kernels of csrc/fq3_codec.cu through the C
     ABI: front end (code-embedding mean, 8-layer sliding-window pre-transformer, 2 x (ConvTranspose k=2 + ConvNeXt))
     and waveform stack (conv_in, 4 upsampling blocks, conv_out) -- ``fq3_codec_decode_codes``.
     ``native_front=False`` (or FQ3_CODEC_TORCH_FRONT=1) keeps the round-1 split for A/B runs: front end as torch ops

@@ -1,8 +1,8 @@
-"""ctypes binding of the B200-native decode engine (include/fq3_engine.h).
+"""ctypes binding of the H100-native decode engine (include/fq3_engine.h).
 
 Python stays a thin host: every tensor crossing this boundary is a torch CUDA tensor whose ``data_ptr()`` is
 handed to the C ABI; all arithmetic of the decode loop happens inside ``libfq3_engine.so`` (hand-written
-sm_100a CUDA, csrc/).  There is NO fallback: if the shared library is missing or no CUDA device is present the
+sm_90a CUDA, csrc/).  There is NO fallback: if the shared library is missing or no CUDA device is present the
 constructors raise.
 """
 from __future__ import annotations
@@ -72,13 +72,13 @@ EXPORTS = [
 
 
 def build_extension(verbose: bool = False) -> str:
-    """Compile csrc/*.cu into libfq3_engine.so for sm_100a (cross-compiles without a GPU)."""
+    """Compile csrc/*.cu into libfq3_engine.so for sm_90a (cross-compiles without a GPU)."""
     srcs = sorted(os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith(".cu"))
     deps = srcs + [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith(".cuh")] + \
         [os.path.join(INCLUDE, f) for f in os.listdir(INCLUDE)]
     if os.path.exists(LIB_PATH) and all(os.path.getmtime(LIB_PATH) >= os.path.getmtime(d) for d in deps):
         return LIB_PATH
-    cmd = ["nvcc", "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-shared",
+    cmd = ["nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-shared",
            "-Xcompiler", "-fPIC", "-I", INCLUDE, "-o", LIB_PATH] + srcs
     if verbose:
         print(" ".join(cmd))
@@ -96,7 +96,7 @@ def load_library() -> C.CDLL:
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(
             f"{LIB_PATH} is missing. Build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc -gencode arch=compute_100a,code=sm_100a). There is no CPU / PyTorch fallback for the decode path.")
+            "(nvcc -gencode arch=compute_90a,code=sm_90a). There is no CPU / PyTorch fallback for the decode path.")
     lib = C.CDLL(LIB_PATH)
     lib.fq3_last_error.restype = C.c_char_p
     lib.fq3_version.restype = C.c_char_p
@@ -160,10 +160,9 @@ def load_library() -> C.CDLL:
 
 
 def set_gemm_backend(name: str):
-    """Dense layers of K3 (prefill) and K4 (codec): 'tcgen05' (default: one 128x96 tile per CTA, 2-4 CTAs per SM),
-    'tcgen05_persistent' (tile loop with a double-buffered TMEM accumulator; measured slower on these shapes) or 'mma'
-    (mma.sync kernel) -- the last two for A/B runs."""
-    load_library().fq3_set_gemm_backend({"tcgen05": 0, "mma": 1, "tcgen05_persistent": 2}[name])
+    """Dense layers of K3 (prefill) and K4 (codec): 'wgmma' (default: one 128x96 tile per CTA, 2-3 CTAs per SM),
+    'wgmma_persistent' (one CTA per SM walking a list of tiles) or 'mma' (mma.sync kernel) -- the last two for A/B runs."""
+    load_library().fq3_set_gemm_backend({"wgmma": 0, "mma": 1, "wgmma_persistent": 2}[name])
 
 
 class EngineError(RuntimeError):
@@ -198,7 +197,7 @@ class Engine:
                  num_code_groups: int = 16, codec_eos_token_id: int = 2150, has_mtp_projection: bool = True,
                  num_ctas: int = 0, rope_positions: Optional[int] = None, max_batch: int = 1):
         if not torch.cuda.is_available():
-            raise RuntimeError("fq3 engine needs a CUDA device (sm_100a); no CPU fallback exists")
+            raise RuntimeError("fq3 engine needs a CUDA device (sm_90a); no CPU fallback exists")
         self.lib = load_library()
         dev = torch.device(device)
         self.device = torch.device("cuda", dev.index if dev.index is not None else torch.cuda.current_device())

@@ -1,11 +1,11 @@
-"""FasterQwen3TTS -- the reference's public wrapper (faster_qwen3_tts/model.py:21-1505) over the B200 engine.
+"""FasterQwen3TTS -- the reference's public wrapper (faster_qwen3_tts/model.py:21-1505) over the H100 engine.
 
 Kept verbatim from the reference: constructor signature, ``from_pretrained`` / ``warmup`` / ``_warmup`` /
 ``generate`` / ``generate_voice_clone[_streaming]`` / ``generate_custom_voice[_streaming]`` /
 ``generate_voice_design[_streaming]`` names, positional order, keyword defaults, return shapes, error types, the
 ``speech_tokenizer`` / ``sample_rate`` surface, and the streaming codec-window policy (model.py:1052-1135).
 
-Replaced: the two graph objects are thin handles on one fq3 engine (persistent sm_100a kernel); per-chunk work
+Replaced: the two graph objects are thin handles on one fq3 engine (persistent sm_90a kernel); per-chunk work
 is one kernel launch + one codec decode.
 
 Prompt assembly (model.py:278-805) is restated here and in ``prompt.py`` (embedding layout pinned against the
@@ -256,7 +256,7 @@ class FasterQwen3TTS:
         if backend not in ("torch", "ggml", "qwentts"):
             raise ValueError(f"Unsupported backend {backend!r}. Expected 'torch', 'ggml', or 'qwentts'.")
         if backend in ("ggml", "qwentts"):
-            raise NotImplementedError("the qwentts.cpp / GGML adapter is out of scope of the B200 engine "
+            raise NotImplementedError("the qwentts.cpp / GGML adapter is out of scope of the H100 engine "
                                       "(SURVEY.md section 2 row 9); use backend='torch'")
         if isinstance(dtype, str):
             dtype = getattr(torch, dtype)

@@ -1,5 +1,5 @@
 """TalkerGraph -- same public surface as the reference class (faster_qwen3_tts/talker_graph.py:21-214) but backed
-by the persistent sm_100a decode kernel instead of StaticCache + torch.cuda.CUDAGraph.
+by the persistent sm_90a decode kernel instead of StaticCache + torch.cuda.CUDAGraph.
 
 There is nothing to capture: ``capture()`` only validates that the engine is ready, no mask table is built (the
 causal / left-pad mask is implicit in ``position`` and ``n_left_pad`` inside the kernel) and no StaticCache exists

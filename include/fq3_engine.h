@@ -1,5 +1,5 @@
 /*
- * fq3_engine.h -- C ABI of the B200-native Qwen3-TTS decode engine.
+ * fq3_engine.h -- C ABI of the H100-native Qwen3-TTS decode engine.
  *
  * Drop-in boundary for the hot path of andimarafioti/faster-qwen3-tts.  The reference has no FFI on its torch
  * path (the seam is a Python duck type); the nearest precedent is the qwentts.cpp C ABI it reaches through
@@ -209,7 +209,7 @@ int fq3_codec_decode(fq3_codec* c, const void* x_dev, int32_t T4, float* pcm_out
 int fq3_codec_decode_batch(fq3_codec* c, const void* x_dev, int32_t batch, int32_t T4, float* pcm_out_dev, void* stream);
 /* The decoder's front end -- everything of speech_tokenizer.decode before conv_in: 16-codebook embedding mean,
  * sliding-window pre-transformer (RMSNorm, RoPE, layer scale, SwiGLU), 2 x (ConvTranspose k=s + ConvNeXt) -- as
- * hand-written kernels + the same tcgen05 GEMM.  geom = {Q, codebook_size, hidden, intermediate, n_heads, n_layers,
+ * hand-written kernels + the same wgmma GEMM.  geom = {Q, codebook_size, hidden, intermediate, n_heads, n_layers,
  * sliding_window, n_up, ratio_0 ..}; fgeom = {rms_norm_eps, rope_theta}.  Tensor names / layouts: csrc/fq3_codec.cu. */
 int fq3_codec_load_frontend(fq3_codec* c, const int32_t* geom, int32_t n_geom, const float* fgeom, int32_t n_fgeom,
                             const fq3_tensor* tensors, int32_t n, void* stream);
@@ -241,8 +241,8 @@ int64_t fq3_codec_launch_count(fq3_codec* c);
 void fq3_codec_destroy(fq3_codec* c);
 const char* fq3_codec_last_error(void);
 
-/* dense-layer kernel selection for K3/K4: 0 = tcgen05 + TMA implicit GEMM, one tile per CTA, when the shape allows
- * (default); 1 = always the mma.sync kernel; 2 = persistent tcgen05 kernel with a double-buffered TMEM accumulator
+/* dense-layer kernel selection for K3/K4: 0 = wgmma + TMA implicit GEMM, one tile per CTA, when the shape allows
+ * (default); 1 = always the mma.sync kernel; 2 = persistent wgmma kernel that walks a list of tiles per CTA
  * (1, 2: A/B references). */
 int fq3_set_gemm_backend(int32_t backend);
 

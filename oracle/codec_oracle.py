@@ -5,7 +5,7 @@ matches the reference on fixed seeds within 1e-3 max-abs PCM"): a purely functio
 nn.Module, no product import) that consumes a plain ``{name: tensor}`` weight dict.
 
 What it restates: the decoder behind ``speech_tokenizer.decode`` that the reference calls at
-/root/reference/faster_qwen3_tts/model.py:924,1093,1122.  The real Qwen3-TTS 12 Hz tokenizer decoder ships inside the
+the reference's faster_qwen3_tts/model.py:924,1093,1122.  The real Qwen3-TTS 12 Hz tokenizer decoder ships inside the
 un-vendored ``qwen-tts`` package (pyproject.toml:27); the closest readable source in this image is the Qwen3-Omni
 ``Code2Wav`` of transformers 5.5 (``transformers/models/qwen3_omni_moe/modeling_qwen3_omni_moe.py``):
   code-offset embedding + mean over the 16 quantisers                                   :3766-3772

@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
 """Generate tests/golden/*.npz by EXECUTING THE REFERENCE'S OWN CODE in this container.
 
-TEST INFRASTRUCTURE.  Needs /root/reference (read-only); never runs on the GPU box -- the fixtures it writes
+TEST INFRASTRUCTURE.  Needs a checkout of the reference (FQ3_REFERENCE_DIR, read-only); never runs on a GPU -- the fixtures it writes
 are committed and are what the tests read.
 
 What is executed from the reference (loaded by file path, unmodified):
@@ -10,7 +10,7 @@ What is executed from the reference (loaded by file path, unmodified):
   * faster_qwen3_tts/streaming.py  fast_generate_streaming (chunk scheduler)
 
 The two graph objects and the talker those schedulers drive are duck-typed doubles (the contract of
-/root/reference/tests/test_sampling.py:26-93) whose arithmetic is the CPU oracle, so the recorded codes pin the
+the reference's tests/test_sampling.py:26-93) whose arithmetic is the CPU oracle, so the recorded codes pin the
 oracle's restatement of the *control flow* (EOS, min_new_tokens, suppress range, penalty history, trailing-text
 indexing, max_seq_len stop, chunking).  torch.multinomial inside the reference's sampling module is replaced
 by the inverse-CDF noise contract (its Philox stream is not reproducible); the probabilities it was handed are
@@ -42,7 +42,7 @@ sys.path.insert(0, ROOT)
 
 from oracle import qwen3_tts_oracle as O  # noqa: E402
 
-REF = "/root/reference/faster_qwen3_tts"
+REF = os.path.join(os.environ.get("FQ3_REFERENCE_DIR", "reference"), "faster_qwen3_tts")
 
 
 def load_reference():

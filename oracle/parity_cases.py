@@ -1,6 +1,6 @@
 """Deterministic decode-step talker double + case list for the parity (dynamic-cache) streaming path  --  TEST
 INFRASTRUCTURE.  Shared by oracle/make_golden.py (which drives the REFERENCE's own ``parity_generate_streaming``,
-/root/reference/faster_qwen3_tts/streaming.py:192-359, with it) and tests/test_parity_stream_cpu.py (which drives the
+the reference's faster_qwen3_tts/streaming.py:192-359, with it) and tests/test_parity_stream_cpu.py (which drives the
 product's restatement with the same double and compares against the recorded fixture).
 
 The double implements the upstream ``talker.forward`` contract that path relies on: a prefill call

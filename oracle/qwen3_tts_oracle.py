@@ -6,11 +6,11 @@ Only ``tests/``, ``__graft_entry__.smoke()`` and ``bench.py``'s ``cpu_baseline``
 
 What it restates (plain torch on CPU, fp32 or bf16, dims taken from a config dict):
 
-* the reference's per-frame orchestration      -- /root/reference/faster_qwen3_tts/generate.py:46-50,124-134,149-199
-                                                   /root/reference/faster_qwen3_tts/streaming.py:106-188
-* the predictor's 15-step loop                  -- /root/reference/faster_qwen3_tts/predictor_graph.py:115-167
-* the talker single-token step + KV/mask state  -- /root/reference/faster_qwen3_tts/talker_graph.py:97-107,153-214
-* sampling                                      -- /root/reference/faster_qwen3_tts/sampling.py:10-66
+* the reference's per-frame orchestration      -- faster_qwen3_tts/generate.py:46-50,124-134,149-199
+                                                   faster_qwen3_tts/streaming.py:106-188
+* the predictor's 15-step loop                  -- faster_qwen3_tts/predictor_graph.py:115-167
+* the talker single-token step + KV/mask state  -- faster_qwen3_tts/talker_graph.py:97-107,153-214
+* sampling                                      -- faster_qwen3_tts/sampling.py:10-66
 
 The layer arithmetic itself lives in the un-vendored ``qwen-tts>=0.1.1`` / ``transformers>=4.57,<5``
 packages (pyproject.toml:27-28 of the reference), which are absent from this image.  It is restated here
@@ -234,7 +234,7 @@ def run_stack(
 
 
 # --------------------------------------------------------------------------------------
-# sampling  (follows /root/reference/faster_qwen3_tts/sampling.py:10-66 line by line)
+# sampling  (follows the reference's faster_qwen3_tts/sampling.py:10-66 line by line)
 # --------------------------------------------------------------------------------------
 
 

@@ -11,7 +11,7 @@ for p in (ROOT, PKG):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100; select with -m gpu)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -23,7 +23,7 @@ def pytest_collection_modifyitems(config, items):
         have = False
     if have:
         return
-    skip = pytest.mark.skip(reason="needs a CUDA device (sm_100a)")
+    skip = pytest.mark.skip(reason="needs a CUDA device (sm_90a)")
     for it in items:
         if "gpu" in it.keywords:
             it.add_marker(skip)

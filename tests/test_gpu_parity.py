@@ -1,4 +1,4 @@
-"""GPU parity: the sm_100a engine (through the C ABI) against the CPU oracle on the same seeded inputs.
+"""GPU parity: the sm_90a engine (through the C ABI) against the CPU oracle on the same seeded inputs.
 
 Bars (north_star): codec-token indices bit-exact (fp32, greedy and noise-contract sampling); bf16 within a
 stated logit tolerance plus the reference's structural invariants (tests/test_e2e_parity.py:40-101)."""

@@ -31,13 +31,19 @@ class _FakeReq:
 
 
 class _FakeSched:
-    """max_batch slots; every step emits min(n, remaining) 'frames' whose values identify (request, frame)."""
+    """max_batch slots; every step emits min(n, remaining) 'frames' whose values identify (request, frame).
+    It reports no runnable work until its slots are full or every request was submitted, so the worker keeps
+    admitting until then: whether three clients overlap no longer depends on how fast their threads start."""
 
     def __init__(self, max_batch):
         self.max_batch, self.active, self.peak, self.batch_sizes = max_batch, {}, 0, []
+        self.all_submitted = threading.Event()
+        self._started = False
 
     def __len__(self):
-        return len(self.active)
+        if not self._started:
+            self._started = len(self.active) >= self.max_batch or self.all_submitted.is_set()
+        return len(self.active) if self._started else 0
 
     def has_capacity(self):
         return len(self.active) < self.max_batch
@@ -88,6 +94,7 @@ def test_continuous_batcher_join_leave_and_isolation():
         threads.append(th)
         time.sleep(0.002 * (i % 3))   # staggered arrivals: some join while others are mid-stream
     bad = b.submit(lambda: (None, 0, 0, 0, None), max_new_tokens=5)
+    sched.all_submitted.set()
     with pytest.raises(ValueError):
         list(bad)
     for th in threads:

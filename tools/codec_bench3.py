@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
 """Codec decode (codes -> PCM through fq3_codec_decode_codes) timed with CUDA events for the GEMM variants:
-one-tile-per-CTA tcgen05 (default), persistent tcgen05, mma.sync; reports ms, TFLOP/s of the dense layers and
-the max PCM difference between variants.  python tools/codec_bench3.py [--variants tcgen05,tcgen05_persistent,mma]"""
+one-tile-per-CTA wgmma (default), persistent wgmma, mma.sync; reports ms, TFLOP/s of the dense layers and
+the max PCM difference between variants.  python tools/codec_bench3.py [--variants wgmma,wgmma_persistent,mma]"""
 import argparse
 import json
 import os
@@ -15,7 +15,7 @@ from faster_qwen3_tts.codec import build_codec  # noqa: E402
 from faster_qwen3_tts.engine import set_gemm_backend  # noqa: E402
 
 ap = argparse.ArgumentParser()
-ap.add_argument("--variants", default="tcgen05,tcgen05_persistent")
+ap.add_argument("--variants", default="wgmma,wgmma_persistent")
 ap.add_argument("--cases", default="1x33,1x182,32x33,8x33")
 a = ap.parse_args()
 st = build_codec(dtype=torch.bfloat16, device="cuda", seed=1)
@@ -43,4 +43,4 @@ for case in a.cases.split(","):
         ref.setdefault(key, out.clone())
         print(json.dumps({"case": case, "variant": v, "ms": round(ms, 4), "tflops": round(flops / ms / 1e9, 1),
                           "gflop": round(flops / 1e9, 1), "max_abs_diff_vs_first_variant": d}), flush=True)
-set_gemm_backend("tcgen05")
+set_gemm_backend("wgmma")

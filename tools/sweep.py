@@ -1,5 +1,5 @@
 import os, sys, json, torch
-ROOT = "/root/repo" if os.path.isdir("/root/repo/tools") else os.getcwd()
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path[:0] = [ROOT, os.path.join(ROOT, "faster-qwen3-tts_b200")]
 from faster_qwen3_tts.model import FasterQwen3TTS
 from faster_qwen3_tts.engine import SamplingParams
