@@ -5,8 +5,8 @@
 //
 // One kernel does every dense layer: a causal conv1d as an implicit GEMM over channels-last bf16 activations
 //     Y[t, n] = bias[n] + sum_{tap, ci} W[n, tap, ci] * X[t - (taps-1-tap)*dil, ci]        (X[<0] = 0)
-//   * M = time, N = output channels, K = taps x Cin; 128 x 96 x 32 tiles, 8 warps (2 x 4), bf16 mma.sync
-//     m16n8k16 with fp32 accumulation, ldmatrix from XOR-swizzled shared memory, 4-stage cp.async pipeline.
+//   * M = time, N = output channels, K = taps x Cin; fq3gemm::gemm (fq3_gemm.cu): 128 x 96 tiles, wgmma with fp32
+//     accumulation, TMA-staged operands.
 //   * A causal ConvTranspose1d(k = 2r, stride r) is the same kernel with 2 taps and N' = r*Cout "phase" channels;
 //     the [T, r*Cout] result IS the [T*r, Cout] upsampled sequence (pixel shuffle is a reinterpretation).
 //   * Epilogue fuses bias, residual add, and the NEXT layer's SnakeBeta (x + sin^2(a x) / (b + eps)), writing the raw
@@ -25,9 +25,6 @@
 
 #include "../../include/fq3_engine.h"
 #include "fq3_gemm.cuh"
-#include "fq3_gemm_tc.cuh"
-
-extern int g_fq3_gemm_backend;  // 0 = wgmma/TMA kernel when the shape allows, 1 = force the mma.sync kernel
 
 namespace {
 
@@ -78,24 +75,6 @@ __global__ void conv_out_kernel(const __nv_bfloat16* __restrict__ X, const float
     }
   }
   out[t] = fminf(1.f, fmaxf(-1.f, s));
-}
-
-// first SnakeBeta applied to the bf16 input of the stack is folded into conv_in's epilogue; the stack input itself
-// (output of the upsampling front end) arrives channels-first from torch -> transpose + cast here
-__global__ void to_channels_last_kernel(const __nv_bfloat16* __restrict__ X, int C, int T, __nv_bfloat16* __restrict__ Y) {
-  __shared__ __nv_bfloat16 tile[32][33];
-  X += (size_t)blockIdx.z * C * T;      // blockIdx.z = sequence of the batch
-  Y += (size_t)blockIdx.z * C * T;
-  const int c0 = blockIdx.y * 32, t0 = blockIdx.x * 32;
-  for (int i = threadIdx.y; i < 32; i += blockDim.y) {
-    const int c = c0 + i, t = t0 + threadIdx.x;
-    tile[i][threadIdx.x] = (c < C && t < T) ? X[(size_t)c * T + t] : __float2bfloat16(0.f);
-  }
-  __syncthreads();
-  for (int i = threadIdx.y; i < 32; i += blockDim.y) {
-    const int t = t0 + i, c = c0 + threadIdx.x;
-    if (t < T && c < C) Y[(size_t)t * C + c] = tile[threadIdx.x][i];
-  }
 }
 
 
@@ -388,9 +367,7 @@ extern "C" int fq3_codec_create(const int32_t* geom, int32_t n_geom, fq3_codec**
   c->dev = geom[0]; c->hidden = geom[1]; c->decoder_dim = geom[2]; c->n_blocks = geom[3];
   if (c->n_blocks < 1 || c->n_blocks > 8 || n_geom < 4 + c->n_blocks) { delete c; return cfail(FQ3_ERR_INVALID, "bad codec geometry"); }
   for (int i = 0; i < c->n_blocks; ++i) c->rates[i] = geom[4 + i];
-  if (c->hidden % BK || c->decoder_dim % (BK << c->n_blocks)) { delete c; return cfail(FQ3_ERR_INVALID, "codec channels must be multiples of 32 at every level"); }
-  CodecDevGuard dev_guard(c->dev);
-  CCK(cudaFuncSetAttribute(conv_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, CONV_SMEM));
+  if (c->hidden % 32 || c->decoder_dim % (32 << c->n_blocks)) { delete c; return cfail(FQ3_ERR_INVALID, "codec channels must be multiples of 32 at every level"); }
   *out = c;
   return 0;
 }
@@ -554,14 +531,7 @@ static int launch_conv(fq3_codec* c, const Layer& L, const __nv_bfloat16* X, con
   a.x_row0 = x_row0; a.x_rows = x_rows;
   a.batch = batch;
   c->launches++;
-  if (g_fq3_gemm_backend != 1) {
-    const int r = fq3tc::launch_tc(a, stream, g_fq3_gemm_backend);
-    if (r == 0) return 0;
-    if (r < 0) return cfail(FQ3_ERR_CUDA, "wgmma conv launch failed: ", cudaGetErrorString(cudaGetLastError()));
-  }
-  dim3 grid(((T + BM - 1) / BM) * batch, (L.N + BN - 1) / BN);
-  FQ3_LAUNCH((conv_gemm_kernel), grid, CTHREADS, CONV_SMEM, stream, a);
-  CCK(cudaGetLastError());
+  if (const char* err = gemm(a, stream)) return cfail(FQ3_ERR_CUDA, "codec conv GEMM: ", err);
   return 0;
 }
 
@@ -619,24 +589,6 @@ static int stack_run(fq3_codec* c, const __nv_bfloat16* xcl, int batch, int T4, 
   c->launches++;
   CCK(cudaGetLastError());
   return 0;
-}
-
-// x_dev: [batch][hidden][T4] bf16 channels-first (output of a torch front end), pcm_out_dev float32 [batch][T4 * prod(rates)]:
-// `batch` independent windows of equal length share every launch (each with its own causal left padding)
-extern "C" int fq3_codec_decode_batch(fq3_codec* c, const void* x_dev, int32_t batch, int32_t T4, float* pcm_out_dev,
-                                      void* stream_) {
-  if (!c || !x_dev || !pcm_out_dev || T4 <= 0 || batch <= 0) return cfail(FQ3_ERR_INVALID, "null argument");
-  if (c->layers.empty()) return cfail(FQ3_ERR_STATE, "codec weights not loaded");
-  CodecDevGuard dev_guard(c->dev);
-  cudaStream_t stream = (cudaStream_t)stream_;
-  int rc;
-  if ((rc = stack_reserve(c, batch, T4))) return rc;
-  {
-    dim3 g((T4 + 31) / 32, (c->hidden + 31) / 32, batch), b(32, 8);
-    to_channels_last_kernel<<<g, b, 0, stream>>>((const __nv_bfloat16*)x_dev, c->hidden, T4, c->buf[0]);
-    c->launches++;
-  }
-  return stack_run(c, c->buf[0], batch, T4, pcm_out_dev, stream);
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -780,14 +732,7 @@ static int fe_gemm(fq3_codec* c, const __nv_bfloat16* X, const __nv_bfloat16* W,
   a.X = X; a.W = W; a.bias = bias; a.R = R; a.Yraw = Y; a.T = rows; a.Cin = K; a.N = N; a.taps = 1; a.dil = 1;
   a.bias_mod = bias_mod; a.act_mod = 1; a.mode = mode; a.scale = scale; a.scale_mod = N; a.batch = 1;
   c->launches++;
-  if (g_fq3_gemm_backend != 1) {
-    const int r = fq3tc::launch_tc(a, stream, g_fq3_gemm_backend);
-    if (r == 0) return 0;
-    if (r < 0) return cfail(FQ3_ERR_CUDA, "wgmma GEMM launch failed: ", cudaGetErrorString(cudaGetLastError()));
-  }
-  dim3 grid((rows + BM - 1) / BM, (N + BN - 1) / BN);
-  FQ3_LAUNCH((conv_gemm_kernel), grid, CTHREADS, CONV_SMEM, stream, a);
-  CCK(cudaGetLastError());
+  if (const char* err = gemm(a, stream)) return cfail(FQ3_ERR_CUDA, "codec front-end GEMM: ", err);
   return 0;
 }
 
@@ -1115,10 +1060,6 @@ extern "C" int fq3_codec_stream_decode(fq3_codec* c, fq3_codec_stream* const* st
   CCK(cudaGetLastError());
   for (int b = 0; b < batch; ++b) streams[b]->frames += T;
   return 0;
-}
-
-extern "C" int fq3_codec_decode(fq3_codec* c, const void* x_dev, int32_t T4, float* pcm_out_dev, void* stream_) {
-  return fq3_codec_decode_batch(c, x_dev, 1, T4, pcm_out_dev, stream_);
 }
 
 extern "C" double fq3_codec_flops(fq3_codec* c, int32_t T4) { return c ? c->flops_per_frame * T4 : 0.0; }

@@ -112,12 +112,6 @@ struct fq3_engine {
   bool pf_ready = false;
 };
 
-int g_fq3_gemm_backend = 0;  // shared with fq3_codec.cu
-extern "C" int fq3_set_gemm_backend(int32_t backend) {
-  g_fq3_gemm_backend = backend == 2 ? 2 : (backend ? 1 : 0);
-  return 0;
-}
-
 static size_t smem_bytes() { return sizeof(Smem); }
 
 // ------------------------------------------------------------------------------------------------------------

@@ -6,10 +6,9 @@
 // [layer][kv_head][slot][128] cache.  Per layer: RMSNorm rows -> QKV GEMM -> q/k-norm + RoPE + KV append ->
 // causal GQA attention (eager semantics: bf16 scores, fp32 softmax rounded to bf16, bf16 P.V) -> o_proj GEMM with
 // fused residual -> RMSNorm rows -> gate/up GEMM with fused SwiGLU (interleaved columns) -> down GEMM with fused
-// residual.  GEMMs are the shared implicit-GEMM tensor-core kernel (fq3_gemm.cuh, taps = 1).
+// residual.  GEMMs are the shared implicit-GEMM tensor-core kernel (fq3gemm::gemm, taps = 1).
 #pragma once
 #include "fq3_gemm.cuh"
-#include "fq3_gemm_tc.cuh"
 
 namespace pf {
 
@@ -94,74 +93,6 @@ __global__ void rope_kv_kernel(__nv_bfloat16* __restrict__ QKV, int P, int nH, i
 #pragma unroll
     for (int i = 0; i < 4; ++i) dst[lane + 32 * i] = __float2bfloat16_rn(v[i]);
   }
-}
-
-// causal GQA attention over the cache; block = (8 queries) x (1 head), warp w owns query i0 + w.
-// dynamic smem: scores [8][Ppad] fp32 + q [8][128] fp32
-__global__ void __launch_bounds__(256) attn_prefill_kernel(const __nv_bfloat16* __restrict__ QKV, int P, int nH, int nKV,
-                                                          const __nv_bfloat16* __restrict__ kc,
-                                                          const __nv_bfloat16* __restrict__ vc, int S, int n_left_pad,
-                                                          __nv_bfloat16* __restrict__ OUT) {
-  extern __shared__ float sm[];
-  fq3gemm::pdl_launch();
-  fq3gemm::pdl_wait();
-  const int Ppad = (P + 31) & ~31;
-  float* sc = sm;                 // [8][Ppad]
-  float* qs = sm + 8 * Ppad;      // [8][128]
-  const int h = blockIdx.y, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int i = blockIdx.x * 8 + warp;
-  const int g = h / (nH / nKV);
-  const int ld = (nH + 2 * nKV) * 128;
-  const bool active = i < P;
-  if (active)
-#pragma unroll
-    for (int e = 0; e < 4; ++e) qs[warp * 128 + lane + 32 * e] = __bfloat162float(QKV[(size_t)i * ld + h * 128 + lane + 32 * e]);
-  __syncwarp();
-  if (!active) return;
-  const __nv_bfloat16* kb = kc + (size_t)g * S * 128;
-  const __nv_bfloat16* vb = vc + (size_t)g * S * 128;
-  const float scale = 0.08838834764831845f;
-  float* my = sc + warp * Ppad;
-  const float* q = qs + warp * 128;
-  // scores: lane handles keys j = n_left_pad + lane, +32, ...
-  float mx = -INFINITY;
-  for (int j = n_left_pad + lane; j <= i; j += 32) {
-    const uint4* kr = reinterpret_cast<const uint4*>(kb + (size_t)j * 128);
-    float d = 0.f;
-#pragma unroll
-    for (int c = 0; c < 16; ++c) {
-      const uint4 w = __ldg(kr + c);
-      const float4 qa = *reinterpret_cast<const float4*>(q + c * 8), qb = *reinterpret_cast<const float4*>(q + c * 8 + 4);
-      d = fmaf(qa.x, __uint_as_float(w.x << 16), d); d = fmaf(qa.y, __uint_as_float(w.x & 0xffff0000u), d);
-      d = fmaf(qa.z, __uint_as_float(w.y << 16), d); d = fmaf(qa.w, __uint_as_float(w.y & 0xffff0000u), d);
-      d = fmaf(qb.x, __uint_as_float(w.z << 16), d); d = fmaf(qb.y, __uint_as_float(w.z & 0xffff0000u), d);
-      d = fmaf(qb.z, __uint_as_float(w.w << 16), d); d = fmaf(qb.w, __uint_as_float(w.w & 0xffff0000u), d);
-    }
-    const float s = rb(rb(d) * scale);
-    my[j] = s;
-    mx = fmaxf(mx, s);
-  }
-#pragma unroll
-  for (int o = 16; o; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-  float sum = 0.f;
-  for (int j = n_left_pad + lane; j <= i; j += 32) {
-    const float e = expf(my[j] - mx);
-    my[j] = e;
-    sum += e;
-  }
-#pragma unroll
-  for (int o = 16; o; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-  __syncwarp();
-  // P.V: lane owns dims [4*lane, 4*lane+4)
-  float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
-  for (int j = n_left_pad; j <= i; ++j) {
-    const float p = rb(my[j] / sum);
-    const uint2 w = __ldg(reinterpret_cast<const uint2*>(vb + (size_t)j * 128) + lane);
-    a0 = fmaf(p, __uint_as_float(w.x << 16), a0); a1 = fmaf(p, __uint_as_float(w.x & 0xffff0000u), a1);
-    a2 = fmaf(p, __uint_as_float(w.y << 16), a2); a3 = fmaf(p, __uint_as_float(w.y & 0xffff0000u), a3);
-  }
-  __nv_bfloat16* o = OUT + (size_t)i * nH * 128 + h * 128 + 4 * lane;
-  o[0] = __float2bfloat16_rn(a0); o[1] = __float2bfloat16_rn(a1); o[2] = __float2bfloat16_rn(a2); o[3] = __float2bfloat16_rn(a3);
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -361,11 +292,6 @@ __global__ void __launch_bounds__(128) attn_prefill_mma_kernel(const __nv_bfloat
 
 }  // namespace pf
 
-static const bool g_fq3_scalar_prefill_attention = [] {
-  const char* v = getenv("FQ3_PREFILL_SCALAR_ATTN");
-  return v && atoi(v) != 0;
-}();
-
 static int pf_gemm(fq3_engine* e, const __nv_bfloat16* X, const __nv_bfloat16* W, const __nv_bfloat16* R,
                    __nv_bfloat16* Y, int T, int K, int N, int mode, cudaStream_t stream) {
   fq3gemm::ConvArgs a;
@@ -373,14 +299,7 @@ static int pf_gemm(fq3_engine* e, const __nv_bfloat16* X, const __nv_bfloat16* W
   a.X = X; a.W = W; a.R = R; a.Yraw = Y; a.T = T; a.Cin = K; a.N = N; a.taps = 1; a.dil = 1;
   a.bias_mod = 1; a.act_mod = 1; a.mode = mode;
   e->launches++;
-  if (g_fq3_gemm_backend != 1) {
-    const int r = fq3tc::launch_tc(a, stream, g_fq3_gemm_backend);
-    if (r == 0) return 0;
-    if (r < 0) return fail(FQ3_ERR_CUDA, "wgmma GEMM launch failed: %s", cudaGetErrorString(cudaGetLastError()));
-  }
-  dim3 grid((T + fq3gemm::BM - 1) / fq3gemm::BM, (N + fq3gemm::BN - 1) / fq3gemm::BN);
-  fq3gemm::conv_gemm_kernel<<<grid, fq3gemm::CTHREADS, fq3gemm::CONV_SMEM, stream>>>(a);
-  CK(cudaGetLastError());
+  if (const char* err = fq3gemm::gemm(a, stream)) return fail(FQ3_ERR_CUDA, "prefill GEMM: %s", err);
   return 0;
 }
 
@@ -398,13 +317,19 @@ extern "C" int fq3_engine_set_prefill_weights(fq3_engine* e, const fq3_tensor* t
     for (int i = 0; i < n; ++i)
       if (!strcmp(tensors[i].name, w.nm)) {
         if (tensors[i].numel != w.numel) return fail(FQ3_ERR_INVALID, "prefill tensor '%s': bad numel", w.nm);
+        if ((uintptr_t)tensors[i].dev_ptr & 15) return fail(FQ3_ERR_INVALID, "prefill tensor '%s' is not 16-byte aligned", w.nm);
         *w.dst = tensors[i].dev_ptr;
       }
     if (!*w.dst) return fail(FQ3_ERR_INVALID, "missing prefill tensor '%s'", w.nm);
   }
   if (H > 2048 || H % 32 || I % 32) return fail(FQ3_ERR_INVALID, "prefill geometry unsupported");
+  const int nH = T.num_attention_heads, nKV = T.num_key_value_heads;
+  if (nH != nKV && nH != 2 * nKV)
+    return fail(FQ3_ERR_INVALID, "prefill: talker GQA ratio num_attention_heads / num_key_value_heads = %d / %d is "
+                "unsupported (the prefill attention takes ratios 1 and 2)", nH, nKV);
+  if (T.vocab_size % 8)
+    return fail(FQ3_ERR_INVALID, "prefill: talker vocab_size %d is not a multiple of 8 (N of the head GEMM)", T.vocab_size);
   DevGuard dev_guard(e->dev);
-  CK(cudaFuncSetAttribute(fq3gemm::conv_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, fq3gemm::CONV_SMEM));
   const size_t S = e->cfg.max_seq_len;
   const size_t wide = std::max<size_t>(qd + 2 * kd, (size_t)I);
   if (!e->pf_buf[0]) {
@@ -414,10 +339,6 @@ extern "C" int fq3_engine_set_prefill_weights(fq3_engine* e, const fq3_tensor* t
     CK(cudaMalloc(&e->pf_buf[3], S * wide * 2));   // qkv / act
     CK(cudaMalloc(&e->pf_buf[4], S * qd * 2));     // attention out
   }
-  // per FUNCTION, not per engine: size it for the largest cache any engine may have (SEQMAX), so a second engine
-  // with a shorter max_seq_len cannot lower the limit under the first one
-  CK(cudaFuncSetAttribute(pf::attn_prefill_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                          (int)((8 * (size_t)fq3::SEQMAX + 8 * 128) * sizeof(float))));
   e->pf_ready = true;
   return 0;
 }
@@ -430,6 +351,7 @@ extern "C" int fq3_prefill(fq3_engine* e, int32_t slot, const void* embeds_dev, 
     if ((rcs = check_slot(e, slot))) return rcs;
   }
   if (!e->pf_ready) return fail(FQ3_ERR_STATE, "fq3_engine_set_prefill_weights has not been called");
+  if ((uintptr_t)logits_out_dev & 15) return fail(FQ3_ERR_INVALID, "logits_out_dev must be 16-byte aligned");
   if (P <= 0) return fail(FQ3_ERR_INVALID, "empty prompt");
   if (P > e->cfg.max_seq_len)
     return fail(FQ3_ERR_TOO_LONG, "Input is too long: prefill has %d tokens but max_seq_len=%d. Use shorter text or shorter reference audio.", P, e->cfg.max_seq_len);
@@ -446,8 +368,6 @@ extern "C" int fq3_prefill(fq3_engine* e, int32_t slot, const void* embeds_dev, 
   bf* att = (bf*)e->pf_buf[4];
   CK(cudaMemcpyAsync(x, embeds_dev, (size_t)P * H * 2, cudaMemcpyDeviceToDevice, stream));
   const KParams& k = e->kp;
-  const int Ppad = (P + 31) & ~31;
-  const size_t attn_smem = (size_t)(8 * Ppad + 8 * 128) * sizeof(float);
   int rc;
   for (int l = 0; l < L; ++l) {
     FQ3_LAUNCH((pf::rmsnorm_rows_kernel), P, 256, 0, stream, x, (const bf*)k.t.ln_in + (size_t)l * H, H, T.rms_norm_eps, hn);
@@ -464,13 +384,10 @@ extern "C" int fq3_prefill(fq3_engine* e, int32_t slot, const void* embeds_dev, 
     {
       const bf* kl = (const bf*)slot_tk(e, slot) + (size_t)l * nKV * S * 128;
       const bf* vl = (const bf*)slot_tv(e, slot) + (size_t)l * nKV * S * 128;
-      const int rep = nH / nKV;
-      if (!g_fq3_scalar_prefill_attention && rep == 2)
+      if (nH == 2 * nKV)   // fq3_engine_set_prefill_weights admits GQA ratios 1 and 2 only
         FQ3_LAUNCH((pf::attn_prefill_mma_kernel<2>), dim3((P + 31) / 32, nKV), 128, 0, stream, wide, P, nH, nKV, kl, vl, S, n_left_pad, att);
-      else if (!g_fq3_scalar_prefill_attention && rep == 1)
+      else
         FQ3_LAUNCH((pf::attn_prefill_mma_kernel<1>), dim3((P + 31) / 32, nKV), 128, 0, stream, wide, P, nH, nKV, kl, vl, S, n_left_pad, att);
-      else   // other GQA ratios (and FQ3_PREFILL_SCALAR_ATTN=1 for A/B runs): the scalar-FMA kernel of round 1
-        FQ3_LAUNCH((pf::attn_prefill_kernel), dim3((P + 7) / 8, nH), 256, attn_smem, stream, wide, P, nH, nKV, kl, vl, S, n_left_pad, att);
     }
     e->launches++;
     if ((rc = pf_gemm(e, att, (const bf*)e->pf_o + (size_t)l * H * qd, x, x1, P, qd, H, 0, stream))) return rc;

@@ -216,26 +216,19 @@ class SpeechTokenizer:
     backend="engine": codes -> PCM entirely in the hand-written sm_90a kernels of csrc/fq3_codec.cu through the C
     ABI: front end (code-embedding mean, 8-layer sliding-window pre-transformer, 2 x (ConvTranspose k=2 + ConvNeXt))
     and waveform stack (conv_in, 4 upsampling blocks, conv_out) -- ``fq3_codec_decode_codes``.
-    ``native_front=False`` (or FQ3_CODEC_TORCH_FRONT=1) keeps the round-1 split for A/B runs: front end as torch ops
-    (CUDA-graphed per window length), stack in the engine.  backend="torch": the plain library implementation."""
+    backend="torch": the plain library implementation."""
 
-    def __init__(self, decoder: Code2Wav, backend: str = "torch", graph_front: bool = True, native_front: bool = None):
-        import os
+    def __init__(self, decoder: Code2Wav, backend: str = "torch"):
         self.decoder = decoder
         self.sample_rate = decoder.config.sample_rate
         self.launches = 0
         self.backend = backend
-        self.graph_front = graph_front
         self._h = None
-        self._graphs = {}
-        self._seen = {}
         self._stream_pool = []      # released stream handles: a request re-uses one (async reset) instead of cudaMalloc / cudaFree
         self._ref_templates = {}    # content hash of a voice reference's codes -> stream warmed with them (bounded)
-        self.native_front = (os.environ.get("FQ3_CODEC_TORCH_FRONT", "0") != "1") if native_front is None else native_front
         if backend == "engine":
             self._init_engine()
-            if self.native_front:
-                self._init_frontend()
+            self._init_frontend()
 
     # ---- engine plumbing -------------------------------------------------------------------------------
     def _init_engine(self):
@@ -330,62 +323,11 @@ class SpeechTokenizer:
         except Exception:
             pass
 
-    def _front(self, codes: torch.Tensor) -> torch.Tensor:
-        """codes [1,Q,T] -> hidden after the upsampling front end, [1, H, 4T] (model dtype)."""
-        d = self.decoder
-        c = d.config
-        B, Q, T = codes.shape
-        off = (torch.arange(Q, device=codes.device) * c.codebook_size).view(1, Q, 1)
-        x = d.code_embedding(codes + off).mean(1)
-        hd = c.hidden_size // c.num_attention_heads
-        inv = 1.0 / (c.rope_theta ** (torch.arange(0, hd, 2, dtype=torch.float32, device=x.device) / hd))
-        fr = torch.arange(T, dtype=torch.float32, device=x.device)[:, None] * inv[None]
-        emb = torch.cat((fr, fr), dim=-1)
-        cos, sin = emb.cos().to(x.dtype)[None, None], emb.sin().to(x.dtype)[None, None]
-        i = torch.arange(T, device=x.device)
-        allowed = (i[None, :] <= i[:, None]) & (i[None, :] > i[:, None] - c.sliding_window)
-        for l in d.layers:
-            x = l(x, cos, sin, allowed)
-        x = d.norm(x).transpose(1, 2)
-        for up, nx in d.upsample:
-            x = nx(up(x))
-        return x
-
-    def _front_graphed(self, codes: torch.Tensor) -> torch.Tensor:
-        T = (codes.shape[0], codes.shape[-1])
-        g = self._graphs.get(T)
-        if g is None:
-            # capture only shapes that come back (the fixed-size Phase-2 window of a stream): one-off lengths -- the
-            # non-streaming total length, the growing Phase-1 re-decodes -- run eager instead of paying warm-up + capture
-            # and pinning an activation pool each
-            self._seen[T] = self._seen.get(T, 0) + 1
-            if self._seen[T] < 2:
-                if len(self._seen) > 4096:
-                    self._seen.clear()
-                return self._front(codes)
-            static_in = codes.clone()
-            s = torch.cuda.Stream(device=codes.device)
-            s.wait_stream(torch.cuda.current_stream(codes.device))
-            with torch.cuda.stream(s):
-                for _ in range(2):
-                    self._front(static_in)
-            torch.cuda.current_stream(codes.device).wait_stream(s)
-            graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graph):
-                static_out = self._front(static_in)
-            g = self._graphs[T] = (graph, static_in, static_out)
-            if len(self._graphs) > 16:     # bound the cache (every entry pins its activation pool)
-                self._graphs.pop(next(iter(self._graphs)))
-        graph, static_in, static_out = g
-        static_in.copy_(codes)
-        graph.replay()
-        return static_out
-
     @torch.inference_mode()
     def decode(self, payload) -> Tuple[List[torch.Tensor], int]:
         codes = payload["audio_codes"]  # [B, T, Q]
         dev = next(self.decoder.parameters()).device
-        if self.backend == "engine" and self.native_front:
+        if self.backend == "engine":
             import ctypes as C
             codes = codes.to(device=dev, dtype=torch.long).contiguous()
             B, T, Q = codes.shape
@@ -399,37 +341,21 @@ class SpeechTokenizer:
                 raise RuntimeError(self._lib.fq3_codec_last_error().decode())
             self.launches = int(self._lib.fq3_codec_launch_count(self._h))
             return [pcm[b] for b in range(B)], self.sample_rate
-        codes = codes.to(dev).transpose(1, 2).contiguous()
-        if self.backend != "engine":
-            wav = self.decoder(codes)
-            self.launches += 1
-            return [w.reshape(-1).float() for w in wav], self.sample_rate
-        import ctypes as C
-        # all rows of the payload have the same length: the front end and the waveform stack take them as ONE batch
-        # (every launch covers all windows; each window keeps its own causal left padding)
-        B = codes.shape[0]
-        x = (self._front_graphed(codes) if self.graph_front else self._front(codes)).to(torch.bfloat16).contiguous()
-        T4 = x.shape[2]
-        pcm = torch.empty(B, T4 * (self.decoder.config.total_upsample // 4), dtype=torch.float32, device=dev)
-        with torch.cuda.device(dev):
-            rc = self._lib.fq3_codec_decode_batch(self._h, C.c_void_p(x.data_ptr()), B, T4, C.c_void_p(pcm.data_ptr()),
-                                                  C.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
-        if rc:
-            raise RuntimeError(self._lib.fq3_codec_last_error().decode())
-        self.launches = int(self._lib.fq3_codec_launch_count(self._h))
-        return [pcm[b] for b in range(B)], self.sample_rate
+        wav = self.decoder(codes.to(dev).transpose(1, 2).contiguous())
+        self.launches += 1
+        return [w.reshape(-1).float() for w in wav], self.sample_rate
 
     # ---- stateful streaming (fq3_codec_stream_*) -----------------------------------------------------------
     @property
     def supports_streams(self) -> bool:
-        """decoder streams exist only on the engine codec with the native front end"""
-        return self.backend == "engine" and self.native_front and self._h is not None
+        """decoder streams exist only on the engine codec"""
+        return self.backend == "engine" and self._h is not None
 
     def open_stream(self) -> "CodecStream":
         """A decoder stream that keeps every causal layer's history on the device: ``push(codes[n,16])`` returns the
         1920*n samples of exactly those frames, at the cost of n frames (no window re-decode)."""
         if not self.supports_streams:
-            raise RuntimeError("stateful streaming needs the engine backend with the native front end")
+            raise RuntimeError("stateful streaming needs the engine backend")
         return CodecStream(self)
 
     def clear_reference_cache(self) -> None:

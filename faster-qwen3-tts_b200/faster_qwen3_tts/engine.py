@@ -62,8 +62,8 @@ EXPORTS = [
     "fq3_set_generation_state", "fq3_talker_step", "fq3_predictor_run", "fq3_sample_logits", "fq3_begin_request",
     "fq3_decode_chunk", "fq3_get_past_hidden", "fq3_debug_enable", "fq3_debug_read", "fq3_tape_bytes",
     "fq3_num_ctas", "fq3_launch_count", "fq3_last_error", "fq3_version", "fq3_barrier_test",
-    "fq3_engine_set_prefill_weights", "fq3_prefill", "fq3_set_gemm_backend", "fq3_max_batch", "fq3_debug_gemv",
-    "fq3_codec_create", "fq3_codec_load_weights", "fq3_codec_decode", "fq3_codec_decode_batch", "fq3_codec_flops",
+    "fq3_engine_set_prefill_weights", "fq3_prefill", "fq3_max_batch", "fq3_debug_gemv",
+    "fq3_codec_create", "fq3_codec_load_weights", "fq3_codec_flops",
     "fq3_codec_load_frontend", "fq3_codec_decode_codes", "fq3_codec_frontend_flops",
     "fq3_codec_stream_create", "fq3_codec_stream_reset", "fq3_codec_stream_destroy", "fq3_codec_stream_frames",
     "fq3_codec_stream_decode", "fq3_codec_stream_copy", "fq3_codec_launch_count",
@@ -126,7 +126,6 @@ def load_library() -> C.CDLL:
     lib.fq3_tape_bytes.argtypes = [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
     lib.fq3_num_ctas.argtypes = [C.c_void_p]
     lib.fq3_barrier_test.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]
-    lib.fq3_set_gemm_backend.argtypes = [C.c_int32]
     lib.fq3_engine_set_prefill_weights.argtypes = [C.c_void_p, C.POINTER(Tensor), C.c_int32]
     lib.fq3_prefill.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
                                 C.c_void_p]
@@ -134,8 +133,6 @@ def load_library() -> C.CDLL:
     lib.fq3_codec_destroy.argtypes = [C.c_void_p]
     lib.fq3_codec_destroy.restype = None
     lib.fq3_codec_load_weights.argtypes = [C.c_void_p, C.POINTER(Tensor), C.c_int32, C.c_void_p]
-    lib.fq3_codec_decode.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
-    lib.fq3_codec_decode_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
     lib.fq3_codec_load_frontend.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.POINTER(C.c_float), C.c_int32,
                                             C.POINTER(Tensor), C.c_int32, C.c_void_p]
     lib.fq3_codec_decode_codes.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
@@ -157,12 +154,6 @@ def load_library() -> C.CDLL:
     lib.fq3_codec_last_error.restype = C.c_char_p
     _lib = lib
     return lib
-
-
-def set_gemm_backend(name: str):
-    """Dense layers of K3 (prefill) and K4 (codec): 'wgmma' (default: one 128x96 tile per CTA, 2-3 CTAs per SM),
-    'wgmma_persistent' (one CTA per SM walking a list of tiles) or 'mma' (mma.sync kernel) -- the last two for A/B runs."""
-    load_library().fq3_set_gemm_backend({"wgmma": 0, "mma": 1, "wgmma_persistent": 2}[name])
 
 
 class EngineError(RuntimeError):

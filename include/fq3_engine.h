@@ -151,11 +151,12 @@ int fq3_sample_logits(fq3_engine* e, const void* logits_dev, int32_t V, const fq
                       int32_t suppress_eos, int64_t* token_out_dev, void* stream);
 
 /* ---- K3: hand-written prefill (bf16 engines) ------------------------------------------------------------------ */
-/* Borrow row-major weights for the prompt GEMMs (caller keeps them alive): t.qkv [L,(nH+2nKV)*128,H] (q,k,v rows
- * concatenated), t.o [L,H,nH*128], t.gu [L,2I,H] (gate/up rows interleaved), t.down [L,H,I], t.head [V,H]. */
+/* Borrow row-major weights for the prompt GEMMs (caller keeps them alive, 16-byte aligned): t.qkv [L,(nH+2nKV)*128,H]
+ * (q,k,v rows concatenated), t.o [L,H,nH*128], t.gu [L,2I,H] (gate/up rows interleaved), t.down [L,H,I], t.head [V,H].
+ * Requires H <= 2048, H % 32 == 0, I % 32 == 0, V % 8 == 0 and nH / nKV in {1, 2}. */
 int fq3_engine_set_prefill_weights(fq3_engine* e, const fq3_tensor* tensors, int32_t n);
 /* talker.forward prefill (generate.py:107-118) + TalkerGraph.prefill_kv (talker_graph.py:153-170) in one call:
- * embeds_dev [P,H] -> KV cache slots [0,P) of request slot `slot`, logits_out_dev [V] (codec_head on the last
+ * embeds_dev [P,H] -> KV cache slots [0,P) of request slot `slot`, logits_out_dev [V] (16-byte aligned; codec_head on the last
  * position), hidden_out_dev [H] (post-norm hidden of the last position = past_hidden).  Positions are
  * cache index - n_left_pad (clamped at 0); keys below n_left_pad are masked. */
 int fq3_prefill(fq3_engine* e, int32_t slot, const void* embeds_dev, int32_t P, int32_t n_left_pad,
@@ -196,17 +197,12 @@ int fq3_num_ctas(fq3_engine* e);
 /* number of kernels launched by this engine since creation (bench.py "gpu_launches") */
 int64_t fq3_launch_count(fq3_engine* e);
 
-/* ---- K4: codec waveform decoder stack (replaces the cuDNN path under speech_tokenizer.decode, model.py:924,1093,1122)
- * geom = {device, hidden_size, decoder_dim, n_blocks, rate_0..rate_{n-1}}.  Tensor names / layouts: csrc/fq3_codec.cu.
- * fq3_codec_decode: x_dev bf16 [hidden][T4] (channels-first output of the front end) -> pcm float32 [T4*prod(rates)],
- * clamped to [-1,1]. */
+/* ---- K4: codec decoder (replaces the cuDNN path under speech_tokenizer.decode, model.py:924,1093,1122)
+ * geom = {device, hidden_size, decoder_dim, n_blocks, rate_0..rate_{n-1}}; hidden_size and decoder_dim >> n_blocks must
+ * be multiples of 32.  fq3_codec_load_weights: the waveform stack.  Tensor names / layouts: csrc/fq3_codec.cu. */
 typedef struct fq3_codec fq3_codec;
 int fq3_codec_create(const int32_t* geom, int32_t n_geom, fq3_codec** out);
 int fq3_codec_load_weights(fq3_codec* c, const fq3_tensor* tensors, int32_t n, void* stream);
-int fq3_codec_decode(fq3_codec* c, const void* x_dev, int32_t T4, float* pcm_out_dev, void* stream);
-/* `batch` windows of equal length in one set of launches (concurrent requests, BASELINE config 4): x_dev bf16
- * [batch][hidden][T4], pcm float32 [batch][T4*prod(rates)]; every window has its own causal left padding. */
-int fq3_codec_decode_batch(fq3_codec* c, const void* x_dev, int32_t batch, int32_t T4, float* pcm_out_dev, void* stream);
 /* The decoder's front end -- everything of speech_tokenizer.decode before conv_in: 16-codebook embedding mean,
  * sliding-window pre-transformer (RMSNorm, RoPE, layer scale, SwiGLU), 2 x (ConvTranspose k=s + ConvNeXt) -- as
  * hand-written kernels + the same wgmma GEMM.  geom = {Q, codebook_size, hidden, intermediate, n_heads, n_layers,
@@ -214,8 +210,9 @@ int fq3_codec_decode_batch(fq3_codec* c, const void* x_dev, int32_t batch, int32
 int fq3_codec_load_frontend(fq3_codec* c, const int32_t* geom, int32_t n_geom, const float* fgeom, int32_t n_fgeom,
                             const fq3_tensor* tensors, int32_t n, void* stream);
 /* speech_tokenizer.decode({"audio_codes": [batch,T,16]}) (model.py:924,1093,1122; SURVEY 8(b) fq3_codec_decode):
- * codes_dev int64 [batch][T][Q] -> pcm float32 [batch][T * total_upsample] clamped to [-1,1].  No library kernel is
- * launched.  Requires fq3_codec_load_weights + fq3_codec_load_frontend. */
+ * codes_dev int64 [batch][T][Q] -> pcm float32 [batch][T * total_upsample] clamped to [-1,1].  `batch` windows of equal
+ * length share every launch; each has its own causal left padding.  No library kernel is launched.  Requires
+ * fq3_codec_load_weights + fq3_codec_load_frontend. */
 int fq3_codec_decode_codes(fq3_codec* c, const int64_t* codes_dev, int32_t batch, int32_t T, float* pcm_out_dev,
                            void* stream);
 /* Stateful streaming decode (SURVEY 8(f) item 2; replaces the reference's Phase-1 re-decode of everything so far and
@@ -240,11 +237,6 @@ double fq3_codec_frontend_flops(fq3_codec* c, int32_t T);
 int64_t fq3_codec_launch_count(fq3_codec* c);
 void fq3_codec_destroy(fq3_codec* c);
 const char* fq3_codec_last_error(void);
-
-/* dense-layer kernel selection for K3/K4: 0 = wgmma + TMA implicit GEMM, one tile per CTA, when the shape allows
- * (default); 1 = always the mma.sync kernel; 2 = persistent wgmma kernel that walks a list of tiles per CTA
- * (1, 2: A/B references). */
-int fq3_set_gemm_backend(int32_t backend);
 
 const char* fq3_last_error(void);
 const char* fq3_version(void);

@@ -2,6 +2,7 @@
 
 Bars (north_star): codec-token indices bit-exact (fp32, greedy and noise-contract sampling); bf16 within a
 stated logit tolerance plus the reference's structural invariants (tests/test_e2e_parity.py:40-101)."""
+import dataclasses
 import os
 
 import numpy as np
@@ -303,6 +304,20 @@ def test_native_prefill_vs_oracle_bf16(tiny16):
     p.pg.do_sample = True
     print("native vs module prefill rows equal:", int((a == b).all(dim=1).sum()), "of", a.shape[0])
     assert a.shape == b.shape
+
+
+@pytest.mark.parametrize("talker_change, reason", [
+    ({"num_key_value_heads": 1}, "GQA ratio"),
+    ({"vocab_size": 1282}, r"vocab_size 1282 is not a multiple of 8|rows 1282 / K \d+ not tileable")])
+def test_native_prefill_refuses_unsupported_talker_geometry(talker_change, reason):
+    """K3 takes GQA ratios 1 and 2 and a talker vocabulary that is a multiple of 8 (the head GEMM's N): building a bf16
+    engine whose talker has a GQA ratio of 4, or a vocabulary = 2 (mod 8), fails while its weights load.  The bf16 decode
+    tape already refuses such a vocabulary (its head rows come in units of 8); fq3_engine_set_prefill_weights refuses it
+    again for callers that set the prefill weights first."""
+    cfg = O.cfg_tiny()
+    cfg = dataclasses.replace(cfg, talker=dataclasses.replace(cfg.talker, **talker_change))
+    with pytest.raises(RuntimeError, match=reason):
+        Pair(cfg, seed=0, dtype=torch.bfloat16, max_seq_len=128)
 
 
 def test_public_api_end_to_end_tiny():

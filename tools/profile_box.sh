@@ -19,6 +19,6 @@ ncu --set full --clock-control none -k regex:fq3_decode_batch_kernel -s 2 -c 1 -
     python tools/batch_bench.py --batches 32 --frames 16 > "$OUT/ncu_batch_$R.log" 2>&1
 ncu -i /tmp/prof_batch_$R.ncu-rep --page raw --csv > "$OUT/prof_batch_${R}_raw.csv" 2>/dev/null
 ncu --set full --clock-control none -k regex:conv_gemm_tc_kernel -s 200 -c 24 -f -o /tmp/prof_gemm_$R \
-    python tools/codec_bench3.py --variants wgmma --cases 1x33 > "$OUT/ncu_gemm_$R.log" 2>&1
+    python tools/codec_bench3.py --cases 1x33 > "$OUT/ncu_gemm_$R.log" 2>&1
 ncu -i /tmp/prof_gemm_$R.ncu-rep --page raw --csv > "$OUT/prof_gemm_${R}_raw.csv" 2>/dev/null
 du -sh "$OUT"; ls -la "$OUT" | grep -E "prof_|launches_" | awk '{print $5, $9}'
