@@ -41,7 +41,11 @@ constexpr int MAXGRP = 512;          // row groups per CTA
 constexpr int MAXSEG = 256;          // GEMV segments
 constexpr int SEQMAX = 4096;
 
-enum Mode { MODE_FUSED = 0, MODE_TALKER_STEP = 1, MODE_PRED_RUN = 2, MODE_BARRIER_TEST = 3, MODE_GEMV_TEST = 4 };
+enum Mode { MODE_FUSED = 0, MODE_TALKER_STEP = 1, MODE_PRED_RUN = 2, MODE_GEMV_TEST = 3 };
+
+// split-key talker attention runs from this many cached keys on (below, one CTA per q-head is faster); run_layers and
+// Producer::stack_layers must take the same decision, so both read this one constant
+constexpr int ATTN_SPLIT_MIN = 192;
 
 struct Grp {           // one row group of one segment, as seen by one CTA (<= 32 rows, full K)
   uint32_t off16;      // tape offset / 16
@@ -84,7 +88,7 @@ struct KParams {
   const void* t_embed;
   const void* p_embeds;
   const void* mtp_b;
-  const void* mtp_tab;   // [ncb][Vp][Hp] = mtp(embeds[i][code]) precomputed at load time (nullptr: project on the fly)
+  const void* mtp_tab;   // [ncb][Vp][Hp] = mtp(embeds[i][code]) precomputed at load time (has_mtp only)
   int has_mtp, ncb, eos;
   int* state;          // [0] token [1] step [2] gen_step [3] finished [4] emitted(last launch)
   float* past_hidden;  // [Ht] fp32 holding dtype-rounded values
@@ -104,12 +108,9 @@ struct KParams {
   float* dbg;
   int dbg_on;
   long long dbg_stride_layer;  // floats per layer record
-  int pred_pin_layers;         // predictor layers whose weights are streamed with L2 evict_last
   int attn_split;              // talker attention: CTAs per q-head (keys split across them, K/V slices TMA-staged); 0 = off
-  int attn_split_min;          // ... used only when at least this many keys are cached (below, one CTA per q-head is faster)
   float* PART;                 // [nH][attn_split][PART_STRIDE] partial attention results (acc[128], max, sum)
   unsigned* attn_cnt;          // [nH] arrival counters of the splits (cleared with the barrier words every launch)
-  int mma_tape;                // 1: bf16 tensor-core fragment layout, 0: fp32 row-chunk layout
   // ---- batched decode (fq3_decode_batch.cuh): B request slots share one pass over the weight tape
   int nslots;                  // columns of this launch (0: single-sequence kernel)
   const SlotParams* sl;        // [nslots] per-column request state (device)
@@ -242,19 +243,7 @@ struct Ctx {
 // ------------------------------------------------------------------------------------------------------------
 // grid barrier (consumer warps of all CTAs).  The producer warp never waits here.
 // ------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void grid_sync_v0(Ctx& c) {  // fence + relaxed atomic + fence (cooperative-groups style)
-  csync();
-  if (c.tid == 0) {
-    c.bar_target += (unsigned)c.P.ncta;
-    __threadfence();
-    atomicAdd(c.P.bar, 1u);
-    while (ld_acquire_u32(c.P.bar) < c.bar_target) {
-    }
-    __threadfence();
-  }
-  csync();
-}
-// default: bar.sync orders the CTA's writes before thread 0's release-reduction (cumulativity); pollers acquire.
+// bar.sync orders the CTA's writes before thread 0's release-reduction (cumulativity); pollers acquire.
 __device__ __forceinline__ void grid_sync(Ctx& c) {
   csync();
   if (c.tid == 0) {
@@ -278,69 +267,6 @@ __device__ __forceinline__ void grid_arrive(Ctx& c) {
 __device__ __forceinline__ void grid_wait(Ctx& c) {
   if (c.tid == 0) {
     while (ld_acquire_u32(c.P.bar) < c.bar_target) {
-    }
-  }
-  csync();
-}
-
-// experimental variants measured by tools/microbench.py (MODE_BARRIER_TEST)
-__device__ __forceinline__ void grid_sync_v1(Ctx& c) {  // release-reduction + acquire-poll, no separate fences
-  csync();
-  if (c.tid == 0) {
-    c.bar_target += (unsigned)c.P.ncta;
-    asm volatile("red.release.gpu.global.add.u32 [%0], %1;" ::"l"(c.P.bar), "r"(1u) : "memory");
-    while (ld_acquire_u32(c.P.bar) < c.bar_target) {
-    }
-  }
-  csync();
-}
-__device__ __forceinline__ void grid_sync_v2(Ctx& c) {  // two-level: 16 group counters (128 B apart) + top counter
-  csync();
-  if (c.tid == 0) {
-    const unsigned ng = 16;
-    const unsigned grp = blockIdx.x % ng;
-    const unsigned gsize = (c.P.ncta - grp + ng - 1) / ng;
-    c.bar_target += 1;  // epoch
-    unsigned* gc = c.P.bar + 32 * (1 + grp);
-    unsigned old;
-    asm volatile("atom.acq_rel.gpu.global.add.u32 %0, [%1], %2;" : "=r"(old) : "l"(gc), "r"(1u) : "memory");
-    if (old + 1 == gsize * c.bar_target)
-      asm volatile("red.release.gpu.global.add.u32 [%0], %1;" ::"l"(c.P.bar), "r"(1u) : "memory");
-    const unsigned want = ng < (unsigned)c.P.ncta ? ng : (unsigned)c.P.ncta;
-    while (ld_acquire_u32(c.P.bar) < want * c.bar_target) {
-    }
-  }
-  csync();
-}
-
-__device__ __forceinline__ unsigned ld_relaxed_u32(const unsigned* p) {
-  unsigned v;
-  asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-  return v;
-}
-__device__ __forceinline__ void grid_sync_v3(Ctx& c) {  // relaxed polling, a single acquire fence at the end
-  csync();
-  if (c.tid == 0) {
-    c.bar_target += (unsigned)c.P.ncta;
-    asm volatile("red.release.gpu.global.add.u32 [%0], %1;" ::"l"(c.P.bar), "r"(1u) : "memory");
-    while (ld_relaxed_u32(c.P.bar) < c.bar_target) {
-    }
-    asm volatile("fence.acq_rel.gpu;" ::: "memory");
-  }
-  csync();
-}
-__device__ __forceinline__ void grid_sync_v4(Ctx& c) {  // last arriver writes one flag per CTA (128 B apart)
-  csync();
-  if (c.tid == 0) {
-    c.bar_target += 1;  // epoch
-    unsigned old;
-    asm volatile("atom.acq_rel.gpu.global.add.u32 %0, [%1], %2;" : "=r"(old) : "l"(c.P.bar), "r"(1u) : "memory");
-    unsigned* flags = c.P.bar + 32;
-    if (old + 1 == (unsigned)c.P.ncta * c.bar_target) {
-      for (int i = 0; i < c.P.ncta; ++i)
-        asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(flags + 32 * i), "r"(c.bar_target) : "memory");
-    }
-    while (ld_acquire_u32(flags + 32 * blockIdx.x) < c.bar_target) {
     }
   }
   csync();
@@ -379,9 +305,6 @@ __device__ __forceinline__ void probe(Ctx& c, int& idx) {
 }
 
 __device__ __forceinline__ void probe_at(Ctx& c, int idx) {  // fixed slot (frame-level phases: slots 1024..)
-#ifdef FQ3_NO_FRAME_PROBES
-  return;
-#endif
   if ((c.P.dbg_on & 2) && blockIdx.x == 0 && c.tid == 0)
     reinterpret_cast<long long*>(c.P.dbg)[idx] = clock64();
 }
@@ -489,20 +412,30 @@ __device__ __forceinline__ KvSlice kv_slice(int nold, int S, int s) {
   return KvSlice{j0, j1 - j0, (j1 - j0 + KVT_KEYS - 1) / KVT_KEYS};
 }
 
+template <bool BF>
 struct Producer {
   const KParams& P;
   Smem& s;
-  uint32_t ctr;
-  bool stopped;
-  uint64_t pol_first, pol_last;  // L2 eviction policies: stream-once weights vs weights re-read 15x per frame
-  __device__ __forceinline__ void seg(int sg, bool keep = false) {
+  uint32_t ctr = 0;     // tiles issued
+  bool stopped = false;
+  uint64_t pol_first;   // L2 eviction policy of the weight stream (evict_first)
+  __device__ __forceinline__ explicit Producer(const KParams& p) : P(p), s(SMEM()) {
+    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol_first));
+  }
+  // tell the consumers' drain_producer() how many tiles were issued
+  __device__ __forceinline__ void finish() {
+    flag_st(&s.prod_issued, (int)ctr);
+    __threadfence_block();
+    flag_st(&s.prod_done, 1);
+  }
+  __device__ __forceinline__ void seg(int sg) {
     if (stopped) return;
     const uint32_t st = s.seg[sg];
     const int gbeg = (int)(st >> 8), gn = (int)(st & 255u);
     for (int gi = 0; gi < gn; ++gi) {
       const Grp g = s.grp[gbeg + gi];
       // fp32 tape: rows x m x 512-byte row chunks; bf16 tape: n_mt x G k-groups x 2048-byte fragment blocks
-      const uint32_t bytes = P.mma_tape ? (uint32_t)(g.rows & 0xff) * g.m * 2048u : (uint32_t)g.rows * g.m * 512u;
+      const uint32_t bytes = BF ? (uint32_t)(g.rows & 0xff) * g.m * 2048u : (uint32_t)g.rows * g.m * 512u;
       const uint8_t* src = P.tape + (size_t)g.off16 * 16;
       for (int tl = 0; tl < g.ntiles; ++tl) {
         const int stage = (int)(ctr % NS);
@@ -514,7 +447,7 @@ struct Producer {
           }
         }
         mbar_expect_tx(&s.full[stage], bytes);
-        bulk_g2s_hint(s.ring[stage], src + (size_t)tl * bytes, bytes, &s.full[stage], keep ? pol_last : pol_first);
+        bulk_g2s_hint(s.ring[stage], src + (size_t)tl * bytes, bytes, &s.full[stage], pol_first);
         ++ctr;
       }
     }
@@ -547,14 +480,12 @@ struct Producer {
     }
   }
   // kv_slot0 >= 0: talker step at cache slot kv_slot0 with split attention
-  __device__ __forceinline__ void stack_layers(const StackDev& S, int keep_layers = 0, int kv_slot0 = -1, int kv_start = 0) {
+  __device__ __forceinline__ void stack_layers(const StackDev& S, int kv_slot0 = -1, int kv_start = 0) {
     for (int l = 0; l < S.L; ++l)
       for (int q = 0; q < 4; ++q) {
-        seg(S.seg_base + 4 * l + q, l < keep_layers);
-#ifndef FQ3_NO_SPLIT
-        if (q == 0 && kv_slot0 >= 0 && P.attn_split > 0 && P.mma_tape && kv_slot0 - kv_start >= P.attn_split_min)
+        seg(S.seg_base + 4 * l + q);
+        if (BF && q == 0 && kv_slot0 >= 0 && P.attn_split > 0 && kv_slot0 - kv_start >= ATTN_SPLIT_MIN)
           kv_tiles(S, l, kv_slot0, kv_start);
-#endif
       }
   }
 };
@@ -1696,11 +1627,7 @@ __device__ void run_layers(Ctx& c, const StackDev& S, int nt, int slot0, int rpo
     } else {
       // ---- P2: attention.  bf16 talker steps: keys split over attn_split CTAs per q-head, K/V slices TMA-staged;
       //          otherwise one q-head per CTA reading the cache directly
-#ifdef FQ3_NO_SPLIT
-      const bool split = false;
-#else
-      const bool split = BF && is_talker && nt == 1 && P.attn_split > 0 && slot0 - kv_start >= P.attn_split_min;
-#endif
+      const bool split = BF && is_talker && nt == 1 && P.attn_split > 0 && slot0 - kv_start >= ATTN_SPLIT_MIN;
       if (split) attention_split<BF>(c, S, l, slot0, rpos0, kv_start);
       else
         for (int h = blockIdx.x; h < S.nH; h += gridDim.x) attention_head<BF>(c, S, l, h, nt, slot0, rpos0, kv_start);
@@ -1811,10 +1738,9 @@ __device__ void predictor_frame(Ctx& c, const float* u15, bool dbg) {
   for (int i = 0; i < P.ncb; ++i) {
     const int nt = (i == 0) ? 2 : 1;
     probe_at(c, 1024 + 8 * i + 0);
-    const bool tabled = i > 0 && P.has_mtp && P.mtp_tab != nullptr;
     if (i > 0) {
       const int prev = SMEM().codes[i];  // code sampled by pass i-1
-      if (tabled) {  // small_to_mtp_projection(codec_embedding[i-1](prev)) was tabulated when the weights were loaded
+      if (P.has_mtp) {  // small_to_mtp_projection(codec_embedding[i-1](prev)) was tabulated when the weights were loaded
         for (int k = c.tid; k < S.H; k += NCT)
           SMEM().xin[0][k] = ldw<BF>(P.mtp_tab, ((size_t)(i - 1) * S.V + prev) * S.H + k);
       } else {
@@ -1823,21 +1749,19 @@ __device__ void predictor_frame(Ctx& c, const float* u15, bool dbg) {
       }
       csync();
     }
-    bool x0_local;
-    if (P.has_mtp && !tabled) {
+    // pass 0 projects cat(past_hidden, cb0 embedding), which the table does not cover
+    const bool project = i == 0 && P.has_mtp;
+    if (project) {
       for (int t = 0; t < nt; ++t)
         for (int k = c.tid; k < Ht; k += NCT) xs_put<BF>(c, t * Ht + k, SMEM().xin[t][k]);
       csync();
       gemv_any<BF, false>(c, P.seg_mtp, nt, Ht, [&](int row, int) { return P.mtp_b ? ldw<BF>(P.mtp_b, row) : 0.f; },
                           [&](int row, int t, float v, float, float b) { P.X[(size_t)t * P.ldX + row] = rnd<BF>(v + b); });
       grid_sync(c);
-      x0_local = false;
-    } else {
-      x0_local = true;
     }
     const int slot0 = (i == 0) ? 0 : i + 1;
     probe_at(c, 1024 + 8 * i + 1);
-    run_layers<BF, false>(c, S, nt, slot0, slot0, 0, x0_local, dbg && i == 0);
+    run_layers<BF, false>(c, S, nt, slot0, slot0, 0, !project, dbg && i == 0);
     probe_at(c, 1024 + 8 * i + 2);
     head_logits<BF>(c, S.seg_head + i, S.H);
     probe_at(c, 1024 + 8 * i + 3);
@@ -1855,34 +1779,70 @@ __device__ void predictor_frame(Ctx& c, const float* u15, bool dbg) {
 // The producer warp's whole life, as one real function: its code generation (counters in registers, no spills) must
 // not depend on how much register pressure the consumer code around it creates -- a slow producer slows every phase.
 // ------------------------------------------------------------------------------------------------------------
+template <bool BF>
 __device__ __noinline__ void producer_main(const KParams& P) {
-  Smem& s = SMEM();
   const int lane = (int)(threadIdx.x & 31u);
-    if (lane == 0) {
-      Producer pr{P, s, 0u, false, 0ull, 0ull};
-      asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pr.pol_first));
-      asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pr.pol_last));
-      if (P.mode == MODE_BARRIER_TEST) {
-      } else if (P.mode == MODE_TALKER_STEP) {
-        pr.stack_layers(P.t, 0, P.position, P.n_left_pad);
-      } else {
-        const int iters = P.mode == MODE_FUSED ? P.n_frames : 1;
-        for (int f = 0; f < iters && !pr.stopped; ++f) {
-          for (int i = 0; i < P.ncb; ++i) {
-            if (P.has_mtp && (i == 0 || P.mtp_tab == nullptr)) pr.seg(P.seg_mtp, true);
-            pr.stack_layers(P.p, P.pred_pin_layers);
-            pr.seg(P.p.seg_head + i);
-          }
-          if (P.mode == MODE_FUSED) {
-            pr.stack_layers(P.t, 0, P.prefill_len + P.state[1] + f, P.n_left_pad);
-            pr.seg(P.t.seg_head);
-          }
+  if (lane == 0) {
+    Producer<BF> pr(P);
+    if (P.mode == MODE_TALKER_STEP) {
+      pr.stack_layers(P.t, P.position, P.n_left_pad);
+    } else {
+      const int iters = P.mode == MODE_FUSED ? P.n_frames : 1;
+      for (int f = 0; f < iters && !pr.stopped; ++f) {
+        for (int i = 0; i < P.ncb; ++i) {
+          if (P.has_mtp && i == 0) pr.seg(P.seg_mtp);
+          pr.stack_layers(P.p);
+          pr.seg(P.p.seg_head + i);
+        }
+        if (P.mode == MODE_FUSED) {
+          pr.stack_layers(P.t, P.prefill_len + P.state[1] + f, P.n_left_pad);
+          pr.seg(P.t.seg_head);
         }
       }
-      flag_st(&s.prod_issued, (int)pr.ctr);
-      __threadfence_block();
-      flag_st(&s.prod_done, 1);
     }
+    pr.finish();
+  }
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// CTA prologue and drain, shared by fq3_decode_kernel and fq3_decode_batch_kernel
+// ------------------------------------------------------------------------------------------------------------
+// this CTA's group / segment tables, the cb0 history bitmap (copied from `seen`, zeros when nullptr), the ring
+// mbarriers and the hand-shake words; the caller's __syncthreads() publishes them
+__device__ __forceinline__ void cta_prologue(const KParams& P, const uint32_t* seen) {
+  Smem& s = SMEM();
+  const int tid = threadIdx.x, cta = blockIdx.x;
+  const uint32_t g0 = __ldg(P.cta_grp_off + cta), g1 = __ldg(P.cta_grp_off + cta + 1);
+  for (uint32_t i = tid; i < g1 - g0; i += NTHREADS) s.grp[i] = P.grps[g0 + i];
+  for (int i = tid; i < P.nseg; i += NTHREADS) s.seg[i] = __ldg(P.segtab + (size_t)cta * P.nseg + i);
+  for (int i = tid; i < VMAX / 32; i += NTHREADS) s.seen[i] = seen ? seen[i] : 0u;
+  if (tid == 0) {
+    for (int i = 0; i < NS; ++i) {
+      mbar_init(&s.full[i], 1);
+      mbar_init(&s.empty[i], NCW);
+    }
+    s.stop_flag = 0;
+    s.prod_done = 0;
+    s.prod_issued = 0;
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+  }
+}
+
+// consumers at the end of a launch: stop the producer and wait for every bulk copy it has in flight
+__device__ __forceinline__ void drain_producer(Ctx& c) {
+  Smem& s = SMEM();
+  csync();
+  if (c.tid == 0) {
+    flag_st(&s.stop_flag, 1);
+    __threadfence_block();
+    while (!flag_ld(&s.prod_done)) {
+    }
+    __threadfence_block();
+    const uint32_t issued = (uint32_t)flag_ld(&s.prod_issued);
+    for (uint32_t t = c.tile_ctr; t < issued; ++t) mbar_wait(&s.full[t % NS], (t / NS) & 1u);
+  }
+  csync();
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -1890,46 +1850,20 @@ __device__ __noinline__ void producer_main(const KParams& P) {
 // ------------------------------------------------------------------------------------------------------------
 template <bool BF>
 __global__ void __launch_bounds__(NTHREADS, 1) fq3_decode_kernel(const __grid_constant__ KParams P) {
-  extern __shared__ __align__(128) uint8_t smem_raw[];
-  Smem& s = *reinterpret_cast<Smem*>(smem_raw);
+  Smem& s = SMEM();
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int cta = blockIdx.x;
 
-  // one-time setup: per-CTA group / segment tables, barriers
-  {
-    const uint32_t g0 = __ldg(P.cta_grp_off + cta), g1 = __ldg(P.cta_grp_off + cta + 1);
-    for (uint32_t i = tid; i < g1 - g0; i += NTHREADS) s.grp[i] = P.grps[g0 + i];
-    for (int i = tid; i < P.nseg; i += NTHREADS) s.seg[i] = __ldg(P.segtab + (size_t)cta * P.nseg + i);
-    for (int i = tid; i < VMAX / 32; i += NTHREADS) s.seen[i] = P.mode == MODE_FUSED ? P.seen[i] : 0u;
-    if (tid == 0) {
-      for (int i = 0; i < NS; ++i) {
-        mbar_init(&s.full[i], 1);
-        mbar_init(&s.empty[i], NCW);
-      }
-      s.stop_flag = 0;
-      s.prod_done = 0;
-      s.prod_issued = 0;
-      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    }
-  }
+  cta_prologue(P, P.mode == MODE_FUSED ? P.seen : nullptr);
   __syncthreads();
 
   if (warp == NCW) {
-    producer_main(P);
+    producer_main<BF>(P);
   } else {
     // ======================================= CONSUMERS ======================================
     Ctx c{P, tid, warp, lane, 0u, 0u};
     const int Ht = P.t.H;
-    if (P.mode == MODE_BARRIER_TEST) {
-      for (int i = 0; i < P.n_frames; ++i) {
-        if (P.position == 0) grid_sync_v0(c);
-        else if (P.position == 1) grid_sync_v1(c);
-        else if (P.position == 2) grid_sync_v2(c);
-        else if (P.position == 3) grid_sync_v3(c);
-        else grid_sync_v4(c);
-      }
-    } else if (P.mode == MODE_TALKER_STEP) {
+    if (P.mode == MODE_TALKER_STEP) {
       for (int k = tid; k < Ht; k += NCT) s.xin[0][k] = ldw<BF>(P.in_embeds, k);
       csync();
       run_layers<BF, true>(c, P.t, 1, P.position, P.position + P.rope_delta, P.n_left_pad, true, P.dbg_on != 0);
@@ -2004,18 +1938,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) fq3_decode_kernel(const __grid_co
         for (int i = tid; i < VMAX / 32; i += NCT) P.seen[i] = s.seen[i];
       }
     }
-    // ---- drain: stop the producer and wait for every bulk copy it has in flight
-    csync();
-    if (tid == 0) {
-      flag_st(&s.stop_flag, 1);
-      __threadfence_block();
-      while (!flag_ld(&s.prod_done)) {
-      }
-      __threadfence_block();
-      const uint32_t issued = (uint32_t)flag_ld(&s.prod_issued);
-      for (uint32_t t = c.tile_ctr; t < issued; ++t) mbar_wait(&s.full[t % NS], (t / NS) & 1u);
-    }
-    csync();
+    drain_producer(c);
   }
   __syncthreads();
 }

@@ -869,33 +869,28 @@ __device__ void stack_b(Ctx& c, const StackDev& S, const BView& v, int nt, uint3
 // producer warp of the batched kernel: the same tape walk as producer_main(), every segment replayed once per
 // column block (see gemv_b)
 // ------------------------------------------------------------------------------------------------------------
+template <bool BF>
 __device__ __noinline__ void producer_batch_main(const KParams& P) {
-  Smem& s = SMEM();
   const int lane = (int)(threadIdx.x & 31u);
   if (lane == 0) {
-    Producer pr{P, s, 0u, false, 0ull, 0ull};
-    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pr.pol_first));
-    asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pr.pol_last));
-    const bool bf = P.mma_tape != 0;
-    const int nb1 = col_blocks(bf, P.nslots), nb2 = col_blocks(bf, 2 * P.nslots);
-    auto rep = [&](int sg, int n, bool keep) {
-      for (int i = 0; i < n; ++i) pr.seg(sg, keep);
+    Producer<BF> pr(P);
+    const int nb1 = col_blocks(BF, P.nslots), nb2 = col_blocks(BF, 2 * P.nslots);
+    auto rep = [&](int sg, int n) {
+      for (int i = 0; i < n; ++i) pr.seg(sg);
     };
-    if (P.mode == MODE_GEMV_TEST) rep(P.gt_seg, col_blocks(bf, P.gt_ncols), false);
+    if (P.mode == MODE_GEMV_TEST) rep(P.gt_seg, col_blocks(BF, P.gt_ncols));
     for (int f = 0; P.mode != MODE_GEMV_TEST && f < P.n_frames && !pr.stopped; ++f) {
-      if (P.has_mtp) rep(P.seg_mtp, nb2, true);
+      if (P.has_mtp) rep(P.seg_mtp, nb2);
       for (int i = 0; i < P.ncb; ++i) {
         for (int l = 0; l < P.p.L; ++l)
-          for (int q = 0; q < 4; ++q) rep(P.p.seg_base + 4 * l + q, i == 0 ? nb2 : nb1, l < P.pred_pin_layers);
-        rep(P.p.seg_head + i, nb1, false);
+          for (int q = 0; q < 4; ++q) rep(P.p.seg_base + 4 * l + q, i == 0 ? nb2 : nb1);
+        rep(P.p.seg_head + i, nb1);
       }
       for (int l = 0; l < P.t.L; ++l)
-        for (int q = 0; q < 4; ++q) rep(P.t.seg_base + 4 * l + q, nb1, false);
-      rep(P.t.seg_head, nb1, false);
+        for (int q = 0; q < 4; ++q) rep(P.t.seg_base + 4 * l + q, nb1);
+      rep(P.t.seg_head, nb1);
     }
-    flag_st(&s.prod_issued, (int)pr.ctr);
-    __threadfence_block();
-    flag_st(&s.prod_done, 1);
+    pr.finish();
   }
 }
 
@@ -904,8 +899,7 @@ __device__ __noinline__ void producer_batch_main(const KParams& P) {
 // ------------------------------------------------------------------------------------------------------------
 template <bool BF>
 __global__ void __launch_bounds__(NTHREADS, 1) fq3_decode_batch_kernel(const __grid_constant__ KParams P) {
-  extern __shared__ __align__(128) uint8_t smem_raw[];
-  Smem& s = *reinterpret_cast<Smem*>(smem_raw);
+  Smem& s = SMEM();
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int cta = blockIdx.x;
   const int B = P.nslots;
@@ -915,35 +909,19 @@ __global__ void __launch_bounds__(NTHREADS, 1) fq3_decode_batch_kernel(const __g
   v.rank = cta / B;
   v.gsz = ((int)gridDim.x - v.b + B - 1) / B;
   const SlotParams& me = P.sl[v.b];
-  {
-    const uint32_t g0 = __ldg(P.cta_grp_off + cta), g1 = __ldg(P.cta_grp_off + cta + 1);
-    for (uint32_t i = tid; i < g1 - g0; i += NTHREADS) s.grp[i] = P.grps[g0 + i];
-    for (int i = tid; i < P.nseg; i += NTHREADS) s.seg[i] = __ldg(P.segtab + (size_t)cta * P.nseg + i);
-    for (int i = tid; i < VMAX / 32; i += NTHREADS) s.seen[i] = P.mode == MODE_GEMV_TEST ? 0u : me.seen[i];
-    if (tid < B && P.mode != MODE_GEMV_TEST) {
-      const int* st = P.sl[tid].state;
-      s.bst[BS_TOK][tid] = st[0];
-      s.bst[BS_STEP][tid] = st[1];
-      s.bst[BS_GEN][tid] = st[2];
-      s.bst[BS_FIN][tid] = 0;
-      s.bst[BS_EMIT][tid] = 0;
-    }
-    if (tid == 0) {
-      for (int i = 0; i < NS; ++i) {
-        mbar_init(&s.full[i], 1);
-        mbar_init(&s.empty[i], NCW);
-      }
-      s.stop_flag = 0;
-      s.prod_done = 0;
-      s.prod_issued = 0;
-      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    }
+  cta_prologue(P, P.mode == MODE_GEMV_TEST ? nullptr : me.seen);
+  if (tid < B && P.mode != MODE_GEMV_TEST) {
+    const int* st = P.sl[tid].state;
+    s.bst[BS_TOK][tid] = st[0];
+    s.bst[BS_STEP][tid] = st[1];
+    s.bst[BS_GEN][tid] = st[2];
+    s.bst[BS_FIN][tid] = 0;
+    s.bst[BS_EMIT][tid] = 0;
   }
   __syncthreads();
 
   if (warp == NCW) {
-    producer_batch_main(P);
+    producer_batch_main<BF>(P);
   } else {
     Ctx c{P, tid, warp, lane, 0u, 0u};
     const int Ht = P.t.H;
@@ -1119,18 +1097,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) fq3_decode_batch_kernel(const __g
       }
       for (int i = tid; i < VMAX / 32; i += NCT) me.seen[i] = s.seen[i];
     }
-    // ---- drain: stop the producer and wait for every bulk copy it has in flight
-    csync();
-    if (tid == 0) {
-      flag_st(&s.stop_flag, 1);
-      __threadfence_block();
-      while (!flag_ld(&s.prod_done)) {
-      }
-      __threadfence_block();
-      const uint32_t issued = (uint32_t)flag_ld(&s.prod_issued);
-      for (uint32_t t = c.tile_ctr; t < issued; ++t) mbar_wait(&s.full[t % NS], (t / NS) & 1u);
-    }
-    csync();
+    drain_producer(c);
   }
   __syncthreads();
 }

@@ -211,8 +211,7 @@ __global__ void __launch_bounds__(NCT, 1)
     sample_kernel(const __grid_constant__ KParams P, const void* logits, int V, Sampling sp, float u,
                   const long long* hist, int n_hist, int suppress_special, int eos, int suppress_eos,
                   long long* out) {
-  extern __shared__ __align__(128) uint8_t smem_raw[];
-  Smem& s = *reinterpret_cast<Smem*>(smem_raw);
+  Smem& s = SMEM();
   const int tid = threadIdx.x;
   for (int i = tid; i < VMAX / 32; i += NCT) s.seen[i] = 0u;
   __syncthreads();
@@ -362,18 +361,12 @@ extern "C" int fq3_engine_create(const fq3_config* cfg, fq3_engine** out) {
   k.has_mtp = cfg->has_mtp_projection; k.ncb = cfg->num_code_groups - 1; k.eos = cfg->codec_eos_token_id;
   k.max_seq_len = cfg->max_seq_len;
   k.dbg = e->dbg; k.dbg_stride_layer = e->dbg_stride;
-  // no predictor layer is streamed with L2 evict_last: one 1.7B predictor layer is 31 MB, and on a 50 MB L2 pinning one or
-  // two of them measured 5 % / 8 % slower per frame than pinning none (H100 80GB HBM3, 400 W limit; FQ3_PRED_PIN overrides)
-  k.pred_pin_layers = 0;
-  if (const char* v = getenv("FQ3_PRED_PIN")) k.pred_pin_layers = std::max(atoi(v), 0);   // tuning knob
   {
     // split-key talker attention (bf16 engines): S CTAs per q-head; a slice must fit the 4 ring tiles it may hold
     int Sx = e->bf16 ? std::min(e->ncta / std::max(T.num_attention_heads, 1), 16) : 0;
     if (Sx < 2 || (cfg->max_seq_len + Sx - 1) / Sx > 4 * KVT_KEYS) Sx = 0;
     if (const char* v = getenv("FQ3_ATTN_SPLIT")) Sx = std::min(Sx, std::max(atoi(v), 0)) < 2 ? 0 : std::min(Sx, atoi(v));
     k.attn_split = Sx;
-    k.attn_split_min = 192;   // cached keys from which the split path runs (FQ3_ATTN_SPLIT_MIN overrides it)
-    if (const char* v = getenv("FQ3_ATTN_SPLIT_MIN")) k.attn_split_min = std::max(atoi(v), 0);
     k.PART = e->PART;
     k.attn_cnt = e->bar + 1024;
   }
@@ -493,24 +486,23 @@ extern "C" int fq3_engine_load_weights(fq3_engine* e, const fq3_tensor* tensors,
     k.mtp_tab = nullptr;
     if (cfg.has_mtp_projection) {
       if ((rc = own("p.mtp_b", cfg.predictor.hidden_size, esz, &k.mtp_b))) return rc;
-      const char* off = getenv("FQ3_NO_MTP_TABLE");
+      // mtp_table_kernel stages 4 embedding rows in shared memory; Ht <= HMAX keeps them within the 48 KB default
+      static_assert(4 * HMAX * sizeof(float) <= 48 * 1024, "mtp_table_kernel staging exceeds 48 KB");
       const size_t sm = (size_t)4 * Ht * sizeof(float);
-      if (!(off && off[0] == '1') && sm <= 48 * 1024) {
-        const void* wm;
-        const int Hp = cfg.predictor.hidden_size;
-        if ((rc = need("p.mtp_w", (int64_t)Hp * Ht, &wm))) return rc;
-        const long long rows = (long long)k.ncb * cfg.predictor.vocab_size;
-        void* tab = nullptr;
-        auto it = e->tabs.find("p.mtp_table");
-        if (it != e->tabs.end() && it->second) cudaFree(it->second);
-        CK(cudaMalloc(&tab, (size_t)rows * Hp * esz));
-        e->tabs["p.mtp_table"] = tab;
-        const unsigned nb = (unsigned)((rows + 3) / 4);
-        if (e->bf16) mtp_table_kernel<true><<<nb, 256, sm, stream>>>(k.p_embeds, wm, k.mtp_b, tab, Ht, Hp, rows);
-        else mtp_table_kernel<false><<<nb, 256, sm, stream>>>(k.p_embeds, wm, k.mtp_b, tab, Ht, Hp, rows);
-        CK(cudaGetLastError());
-        k.mtp_tab = tab;
-      }
+      const void* wm;
+      const int Hp = cfg.predictor.hidden_size;
+      if ((rc = need("p.mtp_w", (int64_t)Hp * Ht, &wm))) return rc;
+      const long long rows = (long long)k.ncb * cfg.predictor.vocab_size;
+      void* tab = nullptr;
+      auto it = e->tabs.find("p.mtp_table");
+      if (it != e->tabs.end() && it->second) cudaFree(it->second);
+      CK(cudaMalloc(&tab, (size_t)rows * Hp * esz));
+      e->tabs["p.mtp_table"] = tab;
+      const unsigned nb = (unsigned)((rows + 3) / 4);
+      if (e->bf16) mtp_table_kernel<true><<<nb, 256, sm, stream>>>(k.p_embeds, wm, k.mtp_b, tab, Ht, Hp, rows);
+      else mtp_table_kernel<false><<<nb, 256, sm, stream>>>(k.p_embeds, wm, k.mtp_b, tab, Ht, Hp, rows);
+      CK(cudaGetLastError());
+      k.mtp_tab = tab;
     } else {
       k.mtp_b = nullptr;
     }
@@ -524,8 +516,7 @@ extern "C" int fq3_engine_load_weights(fq3_engine* e, const fq3_tensor* tensors,
     segs.push_back(SegHost{rows, K, 0});
     seg_rowsrc0.push_back((uint32_t)rowsrc.size());
   };
-  auto push_rows = [&](const void* base, int64_t row0, int rows, int K, int stride_rows = 1, int start = 0) {
-    (void)stride_rows; (void)start;
+  auto push_rows = [&](const void* base, int64_t row0, int rows, int K) {
     for (int r = 0; r < rows; ++r) rowsrc.push_back((const uint8_t*)base + (size_t)(row0 + r) * K * esz);
   };
   int seg_id = 0;
@@ -743,7 +734,6 @@ extern "C" int fq3_engine_load_weights(fq3_engine* e, const fq3_tensor* tensors,
   CK(cudaStreamSynchronize(stream));
   cudaFree(d_rowsrc);
   cudaFree(d_pack);
-  k.mma_tape = e->bf16 ? 1 : 0;
   k.tape = e->tape; k.grps = e->grps; k.segtab = e->segtab; k.cta_grp_off = e->cta_grp_off;
   // ---- byte accounting (algorithmic bytes)
   {
@@ -754,7 +744,7 @@ extern "C" int fq3_engine_load_weights(fq3_engine* e, const fq3_tensor* tensors,
     for (int i = 0; i < k.ncb; ++i) ph += segs[k.p.seg_head + i].bytes;
     if (k.seg_mtp >= 0) pm = segs[k.seg_mtp].bytes;
     e->talker_step_bytes = (int64_t)tl;
-    e->predictor_frame_bytes = (int64_t)(k.ncb * pl + (k.mtp_tab ? 1 : k.ncb) * pm + ph);
+    e->predictor_frame_bytes = (int64_t)(k.ncb * pl + pm + ph);
   }
   e->loaded = true;
   return 0;
@@ -938,8 +928,6 @@ static int launch_decode_batch(fq3_engine* e, const int32_t* slots, int n, int n
                                cudaStream_t stream) {
   if (!e->sl_dev) return fail(FQ3_ERR_STATE, "engine was created with max_batch = 1");
   if (n > e->ncta) return fail(FQ3_ERR_INVALID, "%d slots need at least as many CTAs (engine has %d)", n, e->ncta);
-  if (e->cfg.has_mtp_projection && !e->kp.mtp_tab)
-    return fail(FQ3_ERR_STATE, "batched decode needs the tabulated predictor input projection (unset FQ3_NO_MTP_TABLE)");
   for (int j = 0; j < n; ++j) {
     const int s = slots[j];
     const SlotHost& h = e->slots[s];
@@ -1058,16 +1046,6 @@ extern "C" int fq3_get_past_hidden(fq3_engine* e, int32_t slot, void* dst_dev, v
   e->launches++;
   CK(cudaGetLastError());
   return 0;
-}
-
-extern "C" int fq3_barrier_test(fq3_engine* e, int32_t n, int32_t kind, void* stream_) {
-  if (!e || !e->loaded) return fail(FQ3_ERR_STATE, "weights not loaded");
-  DevGuard dev_guard(e->dev);
-  KParams kp = e->kp;
-  kp.mode = MODE_BARRIER_TEST;
-  kp.n_frames = n;
-  kp.position = kind;
-  return launch_decode(e, kp, (cudaStream_t)stream_);
 }
 
 extern "C" int fq3_debug_enable(fq3_engine* e, int32_t on) {

@@ -61,8 +61,7 @@ EXPORTS = [
     "fq3_engine_create", "fq3_engine_load_weights", "fq3_engine_destroy", "fq3_import_kv", "fq3_export_kv",
     "fq3_set_generation_state", "fq3_talker_step", "fq3_predictor_run", "fq3_sample_logits", "fq3_begin_request",
     "fq3_decode_chunk", "fq3_get_past_hidden", "fq3_debug_enable", "fq3_debug_read", "fq3_tape_bytes",
-    "fq3_num_ctas", "fq3_launch_count", "fq3_last_error", "fq3_version", "fq3_barrier_test",
-    "fq3_engine_set_prefill_weights", "fq3_prefill", "fq3_max_batch", "fq3_debug_gemv",
+    "fq3_num_ctas", "fq3_launch_count", "fq3_last_error", "fq3_version", "fq3_engine_set_prefill_weights", "fq3_prefill", "fq3_max_batch", "fq3_debug_gemv",
     "fq3_codec_create", "fq3_codec_load_weights", "fq3_codec_flops",
     "fq3_codec_load_frontend", "fq3_codec_decode_codes", "fq3_codec_frontend_flops",
     "fq3_codec_stream_create", "fq3_codec_stream_reset", "fq3_codec_stream_destroy", "fq3_codec_stream_frames",
@@ -125,7 +124,6 @@ def load_library() -> C.CDLL:
     lib.fq3_debug_read.argtypes = [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p]
     lib.fq3_tape_bytes.argtypes = [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
     lib.fq3_num_ctas.argtypes = [C.c_void_p]
-    lib.fq3_barrier_test.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]
     lib.fq3_engine_set_prefill_weights.argtypes = [C.c_void_p, C.POINTER(Tensor), C.c_int32]
     lib.fq3_prefill.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
                                 C.c_void_p]
@@ -431,9 +429,6 @@ class Engine:
         buf = torch.empty(2 * n, dtype=torch.float32)
         _check(self.lib, self.lib.fq3_debug_read(self.h, 0, buf.numel(), buf.data_ptr()))
         return buf.view(torch.int64)
-
-    def barrier_test(self, n: int, kind: int):
-        _check(self.lib, self.lib.fq3_barrier_test(self.h, int(n), int(kind), self._stream()))
 
     def tape_bytes(self) -> Tuple[int, int]:
         a, b = C.c_int64(), C.c_int64()

@@ -189,8 +189,6 @@ int fq3_debug_gemv(fq3_engine* e, int32_t stack, int32_t layer, int32_t which, i
  * buffer; fq3_debug_read copies `count` floats starting at `offset` to host memory.  Layout in DESIGN.md. */
 int fq3_debug_enable(fq3_engine* e, int32_t on);
 int fq3_debug_read(fq3_engine* e, int64_t offset, int64_t count, float* host_dst);
-/* micro-benchmark: n grid barriers of flavour `kind` in one launch (tools/microbench.py) */
-int fq3_barrier_test(fq3_engine* e, int32_t n, int32_t kind, void* stream);
 /* bytes of packed weight tape streamed per talker step / per predictor frame (algorithmic bytes, for bench) */
 int fq3_tape_bytes(fq3_engine* e, int64_t* talker_step_bytes, int64_t* predictor_frame_bytes);
 int fq3_num_ctas(fq3_engine* e);

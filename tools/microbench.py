@@ -32,10 +32,6 @@ u = torch.rand(15, device="cuda")
 for ds in (False, True):
     ms = timeit(lambda: eng.predictor_run(pi, SamplingParams(do_sample=ds), u))
     print(json.dumps({"what": "predictor_run", "do_sample": ds, "ms": ms, "GBps": pb / ms / 1e6}))
-if hasattr(eng, "barrier_test"):
-    for kind in (0, 1, 2, 3, 4):
-        ms = timeit(lambda: eng.barrier_test(1000, kind), n=5)
-        print(json.dumps({"what": "barrier", "kind": kind, "us_per_barrier": ms}))
 
 # ---- phase timeline of CTA 0 (clock64 probes)
 names = ["norm_in", "gemv_qkv", "B1", "attn", "B2", "gemv_o(+load)", "B3", "norm+gemv_gu", "B4", "gemv_dn(+load)", "B5"]
