@@ -67,13 +67,26 @@ struct StackDev {
   int seg_base;        // segment id of layer 0 / QKV; layer l uses seg_base + 4*l + {0:QKV,1:O,2:GU,3:DN}
   int seg_head;        // first head segment
   const void *ln_in, *ln_post, *qnorm, *knorm, *ln_f;
-  void *kc, *vc;       // [L][nKV][S][128] model dtype
-  int S;
+  int S;               // cache slots per kv head: the request's caches are [L][nKV][S][128] model dtype
   const float *cos, *sin;  // [npos][128] fp32
   int npos;
 };
 
-struct SlotParams;  // fq3_decode_batch.cuh
+// one request: its caches, decode state and parameters.  The single-sequence kernel reads it from KParams::req, the
+// batched kernel one per column from KParams::sl.
+struct SlotParams {
+  void *kc, *vc;        // talker KV cache of this slot   [L][nKV][S][128]
+  void *pkc, *pvc;      // predictor KV cache of this slot [Lp][nKVp][32][128]
+  int* state;           // [0] token [1] step [2] gen_step [3] finished [4] emitted(last launch)
+  float* past_hidden;   // [HMAX] fp32 holding dtype-rounded values
+  uint32_t* seen;       // [VMAX/32] bitmap of cb0 history (sampling.py:22 unique())
+  const void* trailing;
+  const void* tts_pad;
+  const float* uniforms;
+  long long* codes_out; // [n_frames][16]
+  int prefill_len, rope_delta, n_left_pad, max_new, min_new, trailing_len;
+  Sampling sp_t, sp_p;
+};
 
 struct KParams {
   StackDev t, p;
@@ -82,24 +95,17 @@ struct KParams {
   const Grp* grps;
   const uint32_t* segtab;       // [cta][nseg] : (begin << 8) | n   (begin relative to this CTA's first group)
   const uint32_t* cta_grp_off;  // [ncta + 1]
-  float *X, *X1, *QKV, *ATT, *ACT, *LOGITS;
+  float *X, *X1, *QKV, *ACT, *LOGITS;
+  void* ATT;                    // model dtype: the talker attention output that feeds o_proj
   int ldX, ldQKV, ldATT, ldACT;
   unsigned* bar;
   const void* t_embed;
   const void* p_embeds;
   const void* mtp_b;
   const void* mtp_tab;   // [ncb][Vp][Hp] = mtp(embeds[i][code]) precomputed at load time (has_mtp only)
-  int has_mtp, ncb, eos;
-  int* state;          // [0] token [1] step [2] gen_step [3] finished [4] emitted(last launch)
-  float* past_hidden;  // [Ht] fp32 holding dtype-rounded values
-  uint32_t* seen;      // [VMAX/32] bitmap of cb0 history (sampling.py:22 unique())
-  int prefill_len, rope_delta, n_left_pad, max_new, min_new, trailing_len, max_seq_len;
-  const void* trailing;
-  const void* tts_pad;
-  const float* uniforms;
-  Sampling sp_t, sp_p;
+  int has_mtp, ncb, eos, max_seq_len;
+  SlotParams req;        // single-sequence kernel: the request of this launch
   int n_frames;
-  long long* codes_out;
   const void* in_embeds;
   void* hidden_out;
   int position;
@@ -310,14 +316,17 @@ __device__ __forceinline__ void probe_at(Ctx& c, int idx) {  // fixed slot (fram
 }
 
 // ------------------------------------------------------------------------------------------------------------
-// GEMV over one segment: rows of this CTA, streamed from the ring.  x: shared memory, NT vectors of stride xstride.
+// fp32 GEMV over one segment: rows of this CTA, streamed from the ring.  x: NT vectors of stride xstride, in shared
+// memory or (XG) in global memory, read through __ldcg; vectors t >= ncols read vector 0.  (bf16 runs gemv_mma.)
 // Epilogue epi(row0, v0[NT], v1[NT]) is called by lane 0 for each row pair (rows row0, row0+1).
 // ------------------------------------------------------------------------------------------------------------
-template <bool BF, int NT, class Epi>
-__device__ __forceinline__ void gemv_seg(Ctx& c, int seg, const float* x, int xstride, Epi epi) {
-  constexpr int EPL = BF ? 8 : 4;  // elements per lane per 16-byte load
+template <int NT, bool XG, class Epi>
+__device__ __forceinline__ void gemv_seg(Ctx& c, int seg, const float* x, int xstride, int ncols, Epi epi) {
   const uint32_t st = SMEM().seg[seg];
   const int gbeg = (int)(st >> 8), gn = (int)(st & 255u);
+  const float* xr[NT];
+#pragma unroll
+  for (int t = 0; t < NT; ++t) xr[t] = x + (size_t)(t < ncols ? t : 0) * xstride + c.lane * 4;
   for (int gi = 0; gi < gn; ++gi) {
     const Grp g = SMEM().grp[gbeg + gi];
     const int npairs = g.rows >> 1;
@@ -334,18 +343,12 @@ __device__ __forceinline__ void gemv_seg(Ctx& c, int seg, const float* x, int xs
       const uint8_t* tile = SMEM().ring[stage];
       for (int j = 0; j < m; ++j) {
         const int kb = tl * m + j;
-        float xv[NT][EPL];
+        float xv[NT][4];
 #pragma unroll
         for (int t = 0; t < NT; ++t) {
-          if constexpr (BF) {
-            const float4 a = *reinterpret_cast<const float4*>(x + t * xstride + kb * 256 + c.lane * 4);
-            const float4 b = *reinterpret_cast<const float4*>(x + t * xstride + kb * 256 + 128 + c.lane * 4);
-            xv[t][0] = a.x; xv[t][1] = a.y; xv[t][2] = a.z; xv[t][3] = a.w;
-            xv[t][4] = b.x; xv[t][5] = b.y; xv[t][6] = b.z; xv[t][7] = b.w;
-          } else {
-            const float4 a = *reinterpret_cast<const float4*>(x + t * xstride + kb * 128 + c.lane * 4);
-            xv[t][0] = a.x; xv[t][1] = a.y; xv[t][2] = a.z; xv[t][3] = a.w;
-          }
+          const float4* xp = reinterpret_cast<const float4*>(xr[t] + kb * 128);
+          const float4 a = XG ? __ldcg(xp) : *xp;
+          xv[t][0] = a.x; xv[t][1] = a.y; xv[t][2] = a.z; xv[t][3] = a.w;
         }
 #pragma unroll
         for (int sl = 0; sl < 2; ++sl) {
@@ -355,18 +358,11 @@ __device__ __forceinline__ void gemv_seg(Ctx& c, int seg, const float* x, int xs
             for (int h = 0; h < 2; ++h) {
               const int r = 2 * p + h;
               const uint4 w = *reinterpret_cast<const uint4*>(tile + ((size_t)(r * m + j) * 32 + c.lane) * 16);
-              float wf[EPL];
-              if constexpr (BF) {
-                wf[0] = bf_lo(w.x); wf[1] = bf_hi(w.x); wf[2] = bf_lo(w.y); wf[3] = bf_hi(w.y);
-                wf[4] = bf_lo(w.z); wf[5] = bf_hi(w.z); wf[6] = bf_lo(w.w); wf[7] = bf_hi(w.w);
-              } else {
-                wf[0] = __uint_as_float(w.x); wf[1] = __uint_as_float(w.y);
-                wf[2] = __uint_as_float(w.z); wf[3] = __uint_as_float(w.w);
-              }
+              const float wf[4] = {__uint_as_float(w.x), __uint_as_float(w.y), __uint_as_float(w.z), __uint_as_float(w.w)};
 #pragma unroll
               for (int t = 0; t < NT; ++t)
 #pragma unroll
-                for (int e = 0; e < EPL; ++e) acc[sl * 2 + h][t] = fmaf(wf[e], xv[t][e], acc[sl * 2 + h][t]);
+                for (int e = 0; e < 4; ++e) acc[sl * 2 + h][t] = fmaf(wf[e], xv[t][e], acc[sl * 2 + h][t]);
             }
           }
         }
@@ -461,8 +457,8 @@ struct Producer {
     const int h = b / Sx, sp = b - h * Sx, g = h / S.rep;
     const KvSlice sl = kv_slice(slot0 - kv_start, Sx, sp);
     const size_t row0 = (size_t)(layer * S.nKV + g) * S.S + kv_start + sl.j0;
-    const uint8_t* kb = reinterpret_cast<const uint8_t*>(S.kc) + row0 * 256;
-    const uint8_t* vb = reinterpret_cast<const uint8_t*>(S.vc) + row0 * 256;
+    const uint8_t* kb = reinterpret_cast<const uint8_t*>(P.req.kc) + row0 * 256;
+    const uint8_t* vb = reinterpret_cast<const uint8_t*>(P.req.vc) + row0 * 256;
     for (int tl = 0; tl < sl.ntile; ++tl) {
       const uint32_t bytes = (uint32_t)min(KVT_KEYS, sl.n - KVT_KEYS * tl) * 256u;
       const int stage = (int)(ctr % NS);
@@ -491,34 +487,21 @@ struct Producer {
 };
 
 // ------------------------------------------------------------------------------------------------------------
-// Attention for one q-head over the KV cache (transformers eager_attention_forward semantics, GQA by repeat_kv).
-// nt tokens (1, or 2 for the predictor prefill), cache slots slot0.., rotary positions rpos0...
-// Also applies q_norm/k_norm + RoPE to the new q/k and appends K,V to the cache (talker_graph StaticCache.update).
+// The new token's q-head h and the k and v rows of its kv group, out of its QKV row: warp 0 q, warp 1 k, warp 2 v; a
+// lane owns e, e+32, e+64, e+96.  q and k get q_norm / k_norm and RoPE at rotary position rpos; the three rows go to
+// qs / ks / vs.  append: this CTA also writes k and v to cache row `slot` (talker_graph StaticCache.update).  A split
+// attention (attention_split) reads cached rows through the async proxy (TMA), in this launch or a later one, so every
+// append is followed by a proxy fence.
 // ------------------------------------------------------------------------------------------------------------
 template <bool BF>
-__device__ void attention_head(Ctx& c, const StackDev& S, int layer, int h, int nt, int slot0, int rpos0,
-                               int kv_start) {
-  const KParams& P = c.P;
-  float* sc = SMEM().xs;                // scores: [nt][scw]
-  const int scw = (nt == 1) ? SEQMAX : 32;
-  float* qs = SMEM().xs + SEQMAX;       // [2][128]
-  float* ks = qs + 256;              // [2][128]
-  float* vs = ks + 256;              // [2][128]
-  float* opart = vs + 256;           // [8][128]
-  const int g = h / S.rep;
-  const size_t esz = BF ? 2 : 4;
-  const size_t head_stride = (size_t)S.S * 128;
-  uint8_t* kbase = reinterpret_cast<uint8_t*>(S.kc) + ((size_t)(layer * S.nKV + g) * head_stride) * esz;
-  uint8_t* vbase = reinterpret_cast<uint8_t*>(S.vc) + ((size_t)(layer * S.nKV + g) * head_stride) * esz;
-
-  // --- a. q/k norm + rope, v copy.  warp 3*t + {0:q,1:k,2:v}; lane owns e, e+32, e+64, e+96
-  if (c.warp < 3 * nt) {
-    const int t = c.warp / 3, what = c.warp % 3;
-    const float* src = P.QKV + (size_t)t * P.ldQKV + (what == 0 ? h * 128 : (what == 1 ? S.qd + g * 128 : S.qd + S.kd + g * 128));
+__device__ __forceinline__ void head_qkv(Ctx& c, const StackDev& S, int layer, int h, const float* qkv, int rpos,
+                                         float* qs, float* ks, float* vs, void* kc, void* vc, int slot, bool append) {
+  if (c.warp < 3) {
+    const int what = c.warp, g = h / S.rep;
+    const float* src = qkv + (what == 0 ? h * 128 : (what == 1 ? S.qd + g * 128 : S.qd + S.kd + g * 128));
     float v[4], nwv[4], cc[4], sv[4];
     {
-      int rp = rpos0 + t;
-      rp = rp < 0 ? 0 : (rp >= S.npos ? S.npos - 1 : rp);
+      const int rp = rpos < 0 ? 0 : (rpos >= S.npos ? S.npos - 1 : rpos);
       const float* cs = S.cos + (size_t)rp * 128;
       const float* sn = S.sin + (size_t)rp * 128;
       const void* nw = what == 0 ? S.qnorm : S.knorm;
@@ -547,150 +530,163 @@ __device__ void attention_head(Ctx& c, const StackDev& S, int layer, int h, int 
 #pragma unroll
       for (int i = 0; i < 4; ++i) v[i] = o[i];
     }
-    float* dst = (what == 0 ? qs : (what == 1 ? ks : vs)) + t * 128;
+    float* dst = what == 0 ? qs : (what == 1 ? ks : vs);
 #pragma unroll
     for (int i = 0; i < 4; ++i) dst[c.lane + 32 * i] = v[i];
-    if (what > 0 && (h % S.rep) == 0) {
-      uint8_t* cb = (what == 1 ? kbase : vbase) + (size_t)(slot0 + t) * 128 * esz;
+    if (what > 0 && append) {
+      uint8_t* cb = reinterpret_cast<uint8_t*>(what == 1 ? kc : vc) +
+                    ((size_t)(layer * S.nKV + g) * S.S + slot) * 128 * (BF ? 2 : 4);
 #pragma unroll
       for (int i = 0; i < 4; ++i) stw<BF>(cb, c.lane + 32 * i, v[i]);
+      asm volatile("fence.proxy.async.global;" ::: "memory");
     }
   }
   csync();
+}
 
+// ------------------------------------------------------------------------------------------------------------
+// Talker attention of one new token for one q-head over the KV cache (transformers eager_attention_forward semantics,
+// GQA by repeat_kv): cache slot slot0, rotary position rpos0, keys from kv_start on.  qkv: the token's QKV row; kc / vc:
+// the request's caches; the head's output goes to att[h*128 .. h*128+128) in model dtype.  Both kernels run it.
+// ------------------------------------------------------------------------------------------------------------
+template <bool BF>
+__device__ void attention_head(Ctx& c, const StackDev& S, int layer, int h, const float* __restrict__ qkv, void* kc, void* vc,
+                               void* att, int slot0, int rpos0, int kv_start) {
+  float* sc = SMEM().xs;            // scores [SEQMAX]
+  float* qs = SMEM().xs + SEQMAX;   // [128]
+  float* ks = qs + 128;             // [128]
+  float* vs = ks + 128;             // [128]
+  float* opart = vs + 128;          // [8][128]
+  const int g = h / S.rep;
+  const size_t esz = BF ? 2 : 4;
+  const uint8_t* kbase = reinterpret_cast<const uint8_t*>(kc) + ((size_t)(layer * S.nKV + g) * S.S * 128) * esz;
+  const uint8_t* vbase = reinterpret_cast<const uint8_t*>(vc) + ((size_t)(layer * S.nKV + g) * S.S * 128) * esz;
+  // --- a. q/k norm + rope, v copy; the first q-head of each kv group appends the new row
+  head_qkv<BF>(c, S, layer, h, qkv, rpos0, qs, ks, vs, kc, vc, slot0, (h % S.rep) == 0);
   const float scale = 0.08838834764831845f;  // 128^-0.5
-  for (int t = 0; t < nt; ++t) {
-    const int last = slot0 + t;          // newest key slot visible to token t
-    const int nk = last + 1 - kv_start;  // number of visible keys
-    const int nold = slot0 - kv_start;   // keys that live in the global cache
-    float* sct = sc + t * scw;
-    // --- b. scores
-    {
-      constexpr int LPK = BF ? 16 : 32;  // lanes per key (16 bytes per lane)
-      constexpr int KPW = 32 / LPK;      // keys per warp-instruction
-      constexpr int EPL = BF ? 8 : 4;
-      constexpr int U = 16;
-      const int sub = c.lane % LPK, kin = c.lane / LPK;
-      float q[EPL];
+  const int nk = slot0 + 1 - kv_start;       // visible keys
+  const int nold = slot0 - kv_start;         // keys that live in the global cache
+  // --- b. scores
+  {
+    constexpr int LPK = BF ? 16 : 32;  // lanes per key (16 bytes per lane)
+    constexpr int KPW = 32 / LPK;      // keys per warp-instruction
+    constexpr int EPL = BF ? 8 : 4;
+    constexpr int U = 16;
+    const int sub = c.lane % LPK, kin = c.lane / LPK;
+    float q[EPL];
 #pragma unroll
-      for (int e = 0; e < EPL; ++e) q[e] = qs[t * 128 + sub * EPL + e];
-      for (int base = 0; base < nold; base += NCW * KPW * U) {
-        uint4 kv[U];
+    for (int e = 0; e < EPL; ++e) q[e] = qs[sub * EPL + e];
+    for (int base = 0; base < nold; base += NCW * KPW * U) {
+      uint4 kv[U];
 #pragma unroll
-        for (int u = 0; u < U; ++u) {
-          const int jj = base + (u * NCW + c.warp) * KPW + kin;
-          if (jj < nold)
-            kv[u] = __ldcg(reinterpret_cast<const uint4*>(kbase + ((size_t)(kv_start + jj) * 128) * esz) + sub);
-          else
-            kv[u] = make_uint4(0, 0, 0, 0);
-        }
-#pragma unroll
-        for (int u = 0; u < U; ++u) {
-          const int jj = base + (u * NCW + c.warp) * KPW + kin;
-          float d = 0.f;
-          if constexpr (BF) {
-            d = fmaf(q[0], bf_lo(kv[u].x), d); d = fmaf(q[1], bf_hi(kv[u].x), d);
-            d = fmaf(q[2], bf_lo(kv[u].y), d); d = fmaf(q[3], bf_hi(kv[u].y), d);
-            d = fmaf(q[4], bf_lo(kv[u].z), d); d = fmaf(q[5], bf_hi(kv[u].z), d);
-            d = fmaf(q[6], bf_lo(kv[u].w), d); d = fmaf(q[7], bf_hi(kv[u].w), d);
-          } else {
-            d = fmaf(q[0], __uint_as_float(kv[u].x), d); d = fmaf(q[1], __uint_as_float(kv[u].y), d);
-            d = fmaf(q[2], __uint_as_float(kv[u].z), d); d = fmaf(q[3], __uint_as_float(kv[u].w), d);
-          }
-#pragma unroll
-          for (int o = LPK / 2; o; o >>= 1) d += __shfl_xor_sync(0xffffffffu, d, o);
-          if (sub == 0 && jj < nold) sct[jj] = rnd<BF>(rnd<BF>(d) * scale);
-        }
+      for (int u = 0; u < U; ++u) {
+        const int jj = base + (u * NCW + c.warp) * KPW + kin;
+        if (jj < nold)
+          kv[u] = __ldcg(reinterpret_cast<const uint4*>(kbase + ((size_t)(kv_start + jj) * 128) * esz) + sub);
+        else
+          kv[u] = make_uint4(0, 0, 0, 0);
       }
-      // new keys (held in shared memory): warp 0, one key per iteration
-      if (c.warp == 0) {
-        for (int j = 0; j <= t; ++j) {
-          float d = 0.f;
 #pragma unroll
-          for (int i = 0; i < 4; ++i) d = fmaf(qs[t * 128 + c.lane + 32 * i], ks[j * 128 + c.lane + 32 * i], d);
-#pragma unroll
-          for (int o = 16; o; o >>= 1) d += __shfl_xor_sync(0xffffffffu, d, o);
-          if (c.lane == 0) sct[nold + j] = rnd<BF>(rnd<BF>(d) * scale);
+      for (int u = 0; u < U; ++u) {
+        const int jj = base + (u * NCW + c.warp) * KPW + kin;
+        float d = 0.f;
+        if constexpr (BF) {
+          d = fmaf(q[0], bf_lo(kv[u].x), d); d = fmaf(q[1], bf_hi(kv[u].x), d);
+          d = fmaf(q[2], bf_lo(kv[u].y), d); d = fmaf(q[3], bf_hi(kv[u].y), d);
+          d = fmaf(q[4], bf_lo(kv[u].z), d); d = fmaf(q[5], bf_hi(kv[u].z), d);
+          d = fmaf(q[6], bf_lo(kv[u].w), d); d = fmaf(q[7], bf_hi(kv[u].w), d);
+        } else {
+          d = fmaf(q[0], __uint_as_float(kv[u].x), d); d = fmaf(q[1], __uint_as_float(kv[u].y), d);
+          d = fmaf(q[2], __uint_as_float(kv[u].z), d); d = fmaf(q[3], __uint_as_float(kv[u].w), d);
         }
+#pragma unroll
+        for (int o = LPK / 2; o; o >>= 1) d += __shfl_xor_sync(0xffffffffu, d, o);
+        if (sub == 0 && jj < nold) sc[jj] = rnd<BF>(rnd<BF>(d) * scale);
       }
     }
-    csync();
-    // --- c. softmax (fp32, then rounded to dtype like softmax(..., dtype=float32).to(q.dtype))
-    float mx = -INFINITY;
-    for (int j = c.tid; j < nk; j += NCT) mx = fmaxf(mx, sct[j]);
-    mx = block_max(c, mx);
-    float sm = 0.f;
-    for (int j = c.tid; j < nk; j += NCT) {
-      const float e = expf(sct[j] - mx);
-      sct[j] = e;
-      sm += e;
+    if (c.warp == 0) {  // the new key (shared memory)
+      float d = 0.f;
+#pragma unroll
+      for (int i = 0; i < 4; ++i) d = fmaf(qs[c.lane + 32 * i], ks[c.lane + 32 * i], d);
+#pragma unroll
+      for (int o = 16; o; o >>= 1) d += __shfl_xor_sync(0xffffffffu, d, o);
+      if (c.lane == 0) sc[nold] = rnd<BF>(rnd<BF>(d) * scale);
     }
-    sm = block_sum(c, sm);
-    for (int j = c.tid; j < nk; j += NCT) sct[j] = rnd<BF>(sct[j] / sm);
-    csync();
-    // --- d. P.V : 16-byte loads; bf16: 16 lanes per key (lane owns 8 dims), 2 keys per warp instruction
-    {
-      constexpr int LPK = BF ? 16 : 32;
-      constexpr int KPW = 32 / LPK;
-      constexpr int EPL = BF ? 8 : 4;
-      constexpr int U = 16;
-      const int sub = c.lane % LPK, kin = c.lane / LPK;
-      float acc[EPL];
-#pragma unroll
-      for (int e = 0; e < EPL; ++e) acc[e] = 0.f;
-      for (int base = 0; base < nold; base += NCW * KPW * U) {
-        uint4 vv[U];
-        float pv[U];
-#pragma unroll
-        for (int u = 0; u < U; ++u) {
-          const int jj = base + (u * NCW + c.warp) * KPW + kin;
-          if (jj < nold) {
-            vv[u] = __ldcg(reinterpret_cast<const uint4*>(vbase + ((size_t)(kv_start + jj) * 128) * esz) + sub);
-            pv[u] = sct[jj];
-          } else {
-            vv[u] = make_uint4(0, 0, 0, 0);
-            pv[u] = 0.f;
-          }
-        }
-#pragma unroll
-        for (int u = 0; u < U; ++u) {
-          if constexpr (BF) {
-            acc[0] = fmaf(pv[u], bf_lo(vv[u].x), acc[0]); acc[1] = fmaf(pv[u], bf_hi(vv[u].x), acc[1]);
-            acc[2] = fmaf(pv[u], bf_lo(vv[u].y), acc[2]); acc[3] = fmaf(pv[u], bf_hi(vv[u].y), acc[3]);
-            acc[4] = fmaf(pv[u], bf_lo(vv[u].z), acc[4]); acc[5] = fmaf(pv[u], bf_hi(vv[u].z), acc[5]);
-            acc[6] = fmaf(pv[u], bf_lo(vv[u].w), acc[6]); acc[7] = fmaf(pv[u], bf_hi(vv[u].w), acc[7]);
-          } else {
-            acc[0] = fmaf(pv[u], __uint_as_float(vv[u].x), acc[0]); acc[1] = fmaf(pv[u], __uint_as_float(vv[u].y), acc[1]);
-            acc[2] = fmaf(pv[u], __uint_as_float(vv[u].z), acc[2]); acc[3] = fmaf(pv[u], __uint_as_float(vv[u].w), acc[3]);
-          }
-        }
-      }
-      if constexpr (BF) {  // fold the two key halves of the warp: lanes sub and sub+16 own the same dims
-#pragma unroll
-        for (int e = 0; e < EPL; ++e) acc[e] += __shfl_xor_sync(0xffffffffu, acc[e], 16);
-      }
-      if (c.warp == 0 && kin == 0) {
-        for (int j = 0; j <= t; ++j) {
-          const float pj = sct[nold + j];
-#pragma unroll
-          for (int e = 0; e < EPL; ++e) acc[e] = fmaf(pj, vs[j * 128 + sub * EPL + e], acc[e]);
-        }
-      }
-      if (kin == 0) {
-        float* op = opart + c.warp * 128 + sub * EPL;
-#pragma unroll
-        for (int e = 0; e < EPL; ++e) op[e] = acc[e];
-      }
-    }
-    csync();
-    if (c.tid < 128) {
-      float o = 0.f;
-#pragma unroll
-      for (int w = 0; w < NCW; ++w) o += opart[w * 128 + c.tid];
-      P.ATT[(size_t)t * P.ldATT + h * 128 + c.tid] = rnd<BF>(o);
-    }
-    csync();
   }
+  csync();
+  // --- c. softmax (fp32, then rounded to dtype like softmax(..., dtype=float32).to(q.dtype))
+  float mx = -INFINITY;
+  for (int j = c.tid; j < nk; j += NCT) mx = fmaxf(mx, sc[j]);
+  mx = block_max(c, mx);
+  float sm = 0.f;
+  for (int j = c.tid; j < nk; j += NCT) {
+    const float e = expf(sc[j] - mx);
+    sc[j] = e;
+    sm += e;
+  }
+  sm = block_sum(c, sm);
+  for (int j = c.tid; j < nk; j += NCT) sc[j] = rnd<BF>(sc[j] / sm);
+  csync();
+  // --- d. P.V : 16-byte loads; bf16: 16 lanes per key (lane owns 8 dims), 2 keys per warp instruction
+  {
+    constexpr int LPK = BF ? 16 : 32;
+    constexpr int KPW = 32 / LPK;
+    constexpr int EPL = BF ? 8 : 4;
+    constexpr int U = 16;
+    const int sub = c.lane % LPK, kin = c.lane / LPK;
+    float acc[EPL];
+#pragma unroll
+    for (int e = 0; e < EPL; ++e) acc[e] = 0.f;
+    for (int base = 0; base < nold; base += NCW * KPW * U) {
+      uint4 vv[U];
+      float pv[U];
+#pragma unroll
+      for (int u = 0; u < U; ++u) {
+        const int jj = base + (u * NCW + c.warp) * KPW + kin;
+        if (jj < nold) {
+          vv[u] = __ldcg(reinterpret_cast<const uint4*>(vbase + ((size_t)(kv_start + jj) * 128) * esz) + sub);
+          pv[u] = sc[jj];
+        } else {
+          vv[u] = make_uint4(0, 0, 0, 0);
+          pv[u] = 0.f;
+        }
+      }
+#pragma unroll
+      for (int u = 0; u < U; ++u) {
+        if constexpr (BF) {
+          acc[0] = fmaf(pv[u], bf_lo(vv[u].x), acc[0]); acc[1] = fmaf(pv[u], bf_hi(vv[u].x), acc[1]);
+          acc[2] = fmaf(pv[u], bf_lo(vv[u].y), acc[2]); acc[3] = fmaf(pv[u], bf_hi(vv[u].y), acc[3]);
+          acc[4] = fmaf(pv[u], bf_lo(vv[u].z), acc[4]); acc[5] = fmaf(pv[u], bf_hi(vv[u].z), acc[5]);
+          acc[6] = fmaf(pv[u], bf_lo(vv[u].w), acc[6]); acc[7] = fmaf(pv[u], bf_hi(vv[u].w), acc[7]);
+        } else {
+          acc[0] = fmaf(pv[u], __uint_as_float(vv[u].x), acc[0]); acc[1] = fmaf(pv[u], __uint_as_float(vv[u].y), acc[1]);
+          acc[2] = fmaf(pv[u], __uint_as_float(vv[u].z), acc[2]); acc[3] = fmaf(pv[u], __uint_as_float(vv[u].w), acc[3]);
+        }
+      }
+    }
+    if constexpr (BF) {  // fold the two key halves of the warp: lanes sub and sub+16 own the same dims
+#pragma unroll
+      for (int e = 0; e < EPL; ++e) acc[e] += __shfl_xor_sync(0xffffffffu, acc[e], 16);
+    }
+    if (c.warp == 0 && kin == 0) {
+      const float pj = sc[nold];
+#pragma unroll
+      for (int e = 0; e < EPL; ++e) acc[e] = fmaf(pj, vs[sub * EPL + e], acc[e]);
+    }
+    if (kin == 0) {
+      float* op = opart + c.warp * 128 + sub * EPL;
+#pragma unroll
+      for (int e = 0; e < EPL; ++e) op[e] = acc[e];
+    }
+  }
+  csync();
+  if (c.tid < 128) {
+    float o = 0.f;
+#pragma unroll
+    for (int w = 0; w < NCW; ++w) o += opart[w * 128 + c.tid];
+    stw<BF>(att, (size_t)h * 128 + c.tid, o);
+  }
+  csync();
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -707,60 +703,14 @@ __device__ void attention_split(Ctx& c, const StackDev& S, int layer, int slot0,
   const KParams& P = c.P;
   const int Sx = P.attn_split, b = (int)blockIdx.x;
   if (b >= S.nH * Sx) return;  // spare CTAs
-  const int h = b / Sx, sp = b - h * Sx, g = h / S.rep;
+  const int h = b / Sx, sp = b - h * Sx;
   float* sc = SMEM().xs;           // scores / exponentials of this slice (+ the new key)
   float* qs = SMEM().xs + 512;     // [128]
   float* ks = qs + 128;            // [128]
   float* vs = ks + 128;            // [128]
   float* opart = vs + 128;         // [8][128]
-  const size_t esz = BF ? 2 : 4;
-  uint8_t* kbase = reinterpret_cast<uint8_t*>(S.kc) + ((size_t)(layer * S.nKV + g) * S.S * 128) * esz;
-  uint8_t* vbase = reinterpret_cast<uint8_t*>(S.vc) + ((size_t)(layer * S.nKV + g) * S.S * 128) * esz;
-  // --- a. q/k norm + rope, v copy: warp 0 q, warp 1 k, warp 2 v; lane owns e, e+32, e+64, e+96
-  if (c.warp < 3) {
-    const int what = c.warp;
-    const float* src = P.QKV + (what == 0 ? h * 128 : (what == 1 ? S.qd + g * 128 : S.qd + S.kd + g * 128));
-    float v[4], nwv[4], cc[4], sv[4];
-    int rp = rpos0;
-    rp = rp < 0 ? 0 : (rp >= S.npos ? S.npos - 1 : rp);
-    const float* cs = S.cos + (size_t)rp * 128;
-    const float* sn = S.sin + (size_t)rp * 128;
-    const void* nw = what == 0 ? S.qnorm : S.knorm;
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const int e = c.lane + 32 * i;
-      v[i] = __ldcg(src + e);
-      nwv[i] = what < 2 ? ldw<BF>(nw, (size_t)layer * 128 + e) : 0.f;
-      cc[i] = what < 2 ? __ldg(cs + e) : 0.f;
-      sv[i] = what < 2 ? __ldg(sn + e) : 0.f;
-    }
-    if (what < 2) {
-      float ss = v[0] * v[0] + v[1] * v[1] + v[2] * v[2] + v[3] * v[3];
-#pragma unroll
-      for (int o = 16; o; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
-      const float r = 1.0f / sqrtf(ss / 128.0f + S.eps);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) v[i] = rnd<BF>(nwv[i] * rnd<BF>(v[i] * r));
-      float o[4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const float rot = (i < 2) ? -v[i + 2] : v[i - 2];
-        o[i] = rnd<BF>(rnd<BF>(v[i] * rnd<BF>(cc[i])) + rnd<BF>(rot * rnd<BF>(sv[i])));
-      }
-#pragma unroll
-      for (int i = 0; i < 4; ++i) v[i] = o[i];
-    }
-    float* dst = what == 0 ? qs : (what == 1 ? ks : vs);
-#pragma unroll
-    for (int i = 0; i < 4; ++i) dst[c.lane + 32 * i] = v[i];
-    if (what > 0 && sp == 0 && (h % S.rep) == 0) {  // one CTA per kv group appends the new row to the cache
-      uint8_t* cb = (what == 1 ? kbase : vbase) + (size_t)slot0 * 128 * esz;
-#pragma unroll
-      for (int i = 0; i < 4; ++i) stw<BF>(cb, c.lane + 32 * i, v[i]);
-      asm volatile("fence.proxy.async.global;" ::: "memory");  // later steps read these rows through the async proxy (TMA)
-    }
-  }
-  csync();
+  // --- a. q/k norm + rope, v copy; one CTA per kv group appends the new row
+  head_qkv<BF>(c, S, layer, h, P.QKV, rpos0, qs, ks, vs, P.req.kc, P.req.vc, slot0, sp == 0 && (h % S.rep) == 0);
   const KvSlice sl = kv_slice(slot0 - kv_start, Sx, sp);
   const bool has_new = sp == Sx - 1;
   const int nloc = sl.n + (has_new ? 1 : 0);
@@ -879,7 +829,7 @@ __device__ void attention_split(Ctx& c, const StackDev& S, int layer, int slot0,
       L = fmaf(w, __ldcg(ph + (size_t)s2 * PART_STRIDE + 129), L);
       o = fmaf(w, __ldcg(ph + (size_t)s2 * PART_STRIDE + c.tid), o);
     }
-    P.ATT[h * 128 + c.tid] = rnd<BF>(o / L);
+    stw<BF>(P.ATT, (size_t)h * 128 + c.tid, o / L);
   }
   csync();
 }
@@ -1227,8 +1177,8 @@ __device__ __forceinline__ void gemv_any(Ctx& c, int seg, int nt, int K, Pre pre
         }
       }
     };
-    if (nt == 1) gemv_seg<false, 1>(c, seg, SMEM().xs, K, epi2);
-    else gemv_seg<false, 2>(c, seg, SMEM().xs, K, epi2);
+    if (nt == 1) gemv_seg<1, false>(c, seg, SMEM().xs, K, 1, epi2);
+    else gemv_seg<2, false>(c, seg, SMEM().xs, K, 2, epi2);
   }
 }
 
@@ -1245,10 +1195,10 @@ __device__ __forceinline__ float xs_get(Ctx& c, int idx) {
 }
 
 // ------------------------------------------------------------------------------------------------------------
-// Predictor-size attention (cache <= 32 slots, i.e. <= 17 keys): EVERY CTA computes all heads redundantly from the
-// QKV scratch and the tiny KV cache and writes the result straight into the staging vector that feeds o_proj.
-// This removes the attention exchange (ATT round trip) and one grid barrier per layer.  One warp per kv group;
-// a lane owns dims [4*lane, 4*lane+4) of every 128-vector; CTA 0 appends the new K/V to the cache.
+// Predictor-size attention (cache <= 32 slots, i.e. <= 17 keys) of one request, all heads: one warp per kv group; a
+// lane owns dims [4*lane, 4*lane+4) of every 128-vector.  The single-sequence kernel runs it redundantly in EVERY CTA
+// and writes the result straight into the staging vector that feeds o_proj (no attention exchange, one grid barrier
+// less per layer; CTA 0 appends the new K/V).  The batched kernel runs it in one CTA per request, which appends.
 // ------------------------------------------------------------------------------------------------------------
 // NT == 2 is the predictor prefill (slot0 == 0: no cached keys at all); NT == 1 the single-token passes.
 // Register budget is 168/thread (9 warps per SM), so K rows and V rows are fetched in two round trips.
@@ -1307,12 +1257,13 @@ struct SmallKV {  // cached K/V rows of this warp's kv group, fetched in the sha
   Raw k[16], v[16];
 };
 template <bool BF>
-__device__ __forceinline__ void small_kv_preload(Ctx& c, const StackDev& S, int layer, int slot0, SmallKV<BF>& pre) {
+__device__ __forceinline__ void small_kv_preload(Ctx& c, const StackDev& S, int layer, int slot0, const void* kc,
+                                                 const void* vc, SmallKV<BF>& pre) {
   using Raw = typename SmallKV<BF>::Raw;
   const size_t esz = BF ? 2 : 4;
   const int g = c.warp < S.nKV ? c.warp : 0;
-  const uint8_t* kb = reinterpret_cast<const uint8_t*>(S.kc) + ((size_t)(layer * S.nKV + g) * S.S * 128) * esz;
-  const uint8_t* vb = reinterpret_cast<const uint8_t*>(S.vc) + ((size_t)(layer * S.nKV + g) * S.S * 128) * esz;
+  const uint8_t* kb = reinterpret_cast<const uint8_t*>(kc) + ((size_t)(layer * S.nKV + g) * S.S * 128) * esz;
+  const uint8_t* vb = reinterpret_cast<const uint8_t*>(vc) + ((size_t)(layer * S.nKV + g) * S.S * 128) * esz;
 #pragma unroll
   for (int j = 0; j < 16; ++j) {
     if (j < slot0) {
@@ -1325,10 +1276,12 @@ __device__ __forceinline__ void small_kv_preload(Ctx& c, const StackDev& S, int 
   }
 }
 
-template <bool BF, int NT>
-__device__ void attention_small_all(Ctx& c, const StackDev& S, int layer, int slot0_, int rpos0,
-                                    const SmallKV<BF>* pre = nullptr) {
-  const KParams& P = c.P;
+//   qkv0: QKV row of token 0, token t lives qkv_tstride floats further; kc / vc: the request's predictor caches;
+//   append: this CTA writes the new K/V rows; pre: cached rows already in registers (or nullptr);
+//   out(t, i, v): stores element i of token t's attention output (model-dtype rounded)
+template <bool BF, int NT, class Out>
+__device__ void attention_small_all(Ctx& c, const StackDev& S, int layer, int slot0_, int rpos0, const float* __restrict__ qkv0,
+                                    size_t qkv_tstride, void* kc, void* vc, bool append, const SmallKV<BF>* pre, Out out) {
   constexpr int NOLD = NT == 2 ? 1 : 16;  // cached keys that can exist
   constexpr int MAXK = NT == 2 ? 2 : 17;
   const int slot0 = NT == 2 ? 0 : slot0_;
@@ -1345,8 +1298,8 @@ __device__ void attention_small_all(Ctx& c, const StackDev& S, int layer, int sl
     else r = make_float4(0, 0, 0, 0);
   };
   for (int g = c.warp; g < S.nKV; g += NCW) {
-    const uint8_t* kb = reinterpret_cast<const uint8_t*>(S.kc) + ((size_t)(layer * S.nKV + g) * S.S * 128) * esz;
-    const uint8_t* vb = reinterpret_cast<const uint8_t*>(S.vc) + ((size_t)(layer * S.nKV + g) * S.S * 128) * esz;
+    uint8_t* kb = reinterpret_cast<uint8_t*>(kc) + ((size_t)(layer * S.nKV + g) * S.S * 128) * esz;
+    uint8_t* vb = reinterpret_cast<uint8_t*>(vc) + ((size_t)(layer * S.nKV + g) * S.S * 128) * esz;
     // ---- round trip 1: cached K rows + everything about the new token(s)
     Raw kraw[NOLD];
 #pragma unroll
@@ -1372,12 +1325,12 @@ __device__ void attention_small_all(Ctx& c, const StackDev& S, int layer, int sl
       rp = rp < 0 ? 0 : (rp >= S.npos ? S.npos - 1 : rp);
       cs4[t] = __ldg(reinterpret_cast<const float4*>(S.cos + (size_t)rp * 128) + c.lane);
       sn4[t] = __ldg(reinterpret_cast<const float4*>(S.sin + (size_t)rp * 128) + c.lane);
-      const size_t tb = (size_t)t * P.ldQKV;
-      kr4[t] = __ldcg(reinterpret_cast<const float4*>(P.QKV + tb + S.qd + g * 128) + c.lane);
-      vr4[t] = __ldcg(reinterpret_cast<const float4*>(P.QKV + tb + S.qd + S.kd + g * 128) + c.lane);
+      const float* row = qkv0 + (size_t)t * qkv_tstride;
+      kr4[t] = __ldcg(reinterpret_cast<const float4*>(row + S.qd + g * 128) + c.lane);
+      vr4[t] = __ldcg(reinterpret_cast<const float4*>(row + S.qd + S.kd + g * 128) + c.lane);
 #pragma unroll
       for (int hh = 0; hh < 2; ++hh)
-        qr4[hh][t] = __ldcg(reinterpret_cast<const float4*>(P.QKV + tb + (g * S.rep + (hh < S.rep ? hh : 0)) * 128) + c.lane);
+        qr4[hh][t] = __ldcg(reinterpret_cast<const float4*>(row + (g * S.rep + (hh < S.rep ? hh : 0)) * 128) + c.lane);
     }
     auto norm_rope = [&](float* v, const float4& w4, const float4& c4, const float4& s4) {
       const float w[4] = {w4.x, w4.y, w4.z, w4.w}, cc[4] = {c4.x, c4.y, c4.z, c4.w}, sv[4] = {s4.x, s4.y, s4.z, s4.w};
@@ -1403,11 +1356,11 @@ __device__ void attention_small_all(Ctx& c, const StackDev& S, int layer, int sl
       knew[t][0] = kr4[t].x; knew[t][1] = kr4[t].y; knew[t][2] = kr4[t].z; knew[t][3] = kr4[t].w;
       vnew[t][0] = vr4[t].x; vnew[t][1] = vr4[t].y; vnew[t][2] = vr4[t].z; vnew[t][3] = vr4[t].w;
       norm_rope(knew[t], kn4, cs4[t], sn4[t]);
-      if (blockIdx.x == 0) {
+      if (append) {
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
-          stw<BF>(const_cast<uint8_t*>(kb) + (size_t)(slot0 + t) * 128 * esz, L4 + i, knew[t][i]);
-          stw<BF>(const_cast<uint8_t*>(vb) + (size_t)(slot0 + t) * 128 * esz, L4 + i, vnew[t][i]);
+          stw<BF>(kb + (size_t)(slot0 + t) * 128 * esz, L4 + i, knew[t][i]);
+          stw<BF>(vb + (size_t)(slot0 + t) * 128 * esz, L4 + i, vnew[t][i]);
         }
       }
     }
@@ -1530,8 +1483,7 @@ __device__ void attention_small_all(Ctx& c, const StackDev& S, int layer, int sl
 #pragma unroll
         for (int t = 0; t < NT; ++t)
 #pragma unroll
-          for (int i = 0; i < 4; ++i)
-            xs_put<BF>(c, t * S.qd + (g * S.rep + hh) * 128 + L4 + i, rnd<BF>(o4[hh][t][i]));
+          for (int i = 0; i < 4; ++i) out(t, (g * S.rep + hh) * 128 + L4 + i, rnd<BF>(o4[hh][t][i]));
   }
   csync();
 }
@@ -1590,6 +1542,8 @@ __device__ void run_layers(Ctx& c, const StackDev& S, int nt, int slot0, int rpo
   constexpr bool is_talker = TALKER;
   const KParams& P = c.P;
   const bool cta0 = blockIdx.x == 0;
+  void* kc = TALKER ? P.req.kc : P.req.pkc;  // the request's caches of this stack
+  void* vc = TALKER ? P.req.vc : P.req.pvc;
   int pi = 0;
   dbg = dbg && (P.dbg_on & 1);
   auto nopre = [](int, int) { return 0.f; };
@@ -1610,7 +1564,7 @@ __device__ void run_layers(Ctx& c, const StackDev& S, int nt, int slot0, int rpo
     const bool kv_pre = small_attn && nt == 1 && S.nKV <= NCW;
     SmallKV<BF> skv;
     grid_arrive(c);
-    if (kv_pre) small_kv_preload<BF>(c, S, l, slot0, skv);  // cached keys/values do not depend on this layer's QKV
+    if (kv_pre) small_kv_preload<BF>(c, S, l, slot0, kc, vc, skv);  // cached keys/values do not depend on this layer's QKV
     grid_wait(c);
     probe(c, pi);  // 3: after B1
     if (dbg && cta0) {
@@ -1620,17 +1574,19 @@ __device__ void run_layers(Ctx& c, const StackDev& S, int nt, int slot0, int rpo
     }
     if constexpr (!TALKER) {
       // ---- P2+P3 fused: redundant small attention straight into the staging vector (no exchange, no barrier)
-      if (nt == 1) attention_small_all<BF, 1>(c, S, l, slot0, rpos0, kv_pre ? &skv : nullptr);
-      else attention_small_all<BF, 2>(c, S, l, slot0, rpos0);
+      auto to_xs = [&](int t, int i, float v) { xs_put<BF>(c, t * S.qd + i, v); };
+      if (nt == 1) attention_small_all<BF, 1>(c, S, l, slot0, rpos0, P.QKV, P.ldQKV, kc, vc, cta0, kv_pre ? &skv : nullptr, to_xs);
+      else attention_small_all<BF, 2>(c, S, l, slot0, rpos0, P.QKV, P.ldQKV, kc, vc, cta0, nullptr, to_xs);
       probe(c, pi);  // 4
       probe(c, pi);  // 5
     } else {
-      // ---- P2: attention.  bf16 talker steps: keys split over attn_split CTAs per q-head, K/V slices TMA-staged;
-      //          otherwise one q-head per CTA reading the cache directly
+      // ---- P2: attention of the one talker token.  bf16 talker steps: keys split over attn_split CTAs per q-head, K/V
+      //          slices TMA-staged; otherwise one q-head per CTA reading the cache directly
       const bool split = BF && is_talker && nt == 1 && P.attn_split > 0 && slot0 - kv_start >= ATTN_SPLIT_MIN;
       if (split) attention_split<BF>(c, S, l, slot0, rpos0, kv_start);
       else
-        for (int h = blockIdx.x; h < S.nH; h += gridDim.x) attention_head<BF>(c, S, l, h, nt, slot0, rpos0, kv_start);
+        for (int h = blockIdx.x; h < S.nH; h += gridDim.x)
+          attention_head<BF>(c, S, l, h, P.QKV, kc, vc, P.ATT, slot0, rpos0, kv_start);
       if (!split && is_talker && (int)blockIdx.x >= S.nH && slot0 - kv_start > 64) {
         // idle CTAs pull the NEXT layer's keys/values into L2 (evict_last) so the attention CTAs see L2 latency
         const int ln = (l + 1) % S.L;
@@ -1646,7 +1602,7 @@ __device__ void run_layers(Ctx& c, const StackDev& S, int nt, int slot0, int rpo
           r /= lines_per_row;
           const int j = (int)(r % nk);
           const int g = (int)(r / nk);
-          const uint8_t* base = reinterpret_cast<const uint8_t*>(which ? S.vc : S.kc) +
+          const uint8_t* base = reinterpret_cast<const uint8_t*>(which ? vc : kc) +
                                 (((size_t)(ln * S.nKV + g) * S.S + kv_start + j) * 128) * esz + (size_t)ln_i * 128;
           asm volatile("prefetch.global.L2::evict_last [%0];" ::"l"(base));
         }
@@ -1655,8 +1611,12 @@ __device__ void run_layers(Ctx& c, const StackDev& S, int nt, int slot0, int rpo
       grid_sync(c);
       probe(c, pi);  // 5: after B2
       // ---- P3: o_proj + residual
-      for (int t = 0; t < nt; ++t)
-        for (int k = c.tid; k < S.qd; k += NCT) xs_put<BF>(c, t * S.qd + k, __ldcg(P.ATT + (size_t)t * P.ldATT + k));
+      // ATT (model dtype, written by other CTAs in this launch: L2-coherent loads, never __ldg) -> staging vector, as
+      // raw 16-byte vectors
+      {
+        const uint4* att = reinterpret_cast<const uint4*>(P.ATT);
+        for (int k = c.tid; k < S.qd * (BF ? 2 : 4) / 16; k += NCT) reinterpret_cast<uint4*>(SMEM().xs)[k] = __ldcg(att + k);
+      }
       csync();
     }
     if (dbg && cta0) {
@@ -1766,7 +1726,7 @@ __device__ void predictor_frame(Ctx& c, const float* u15, bool dbg) {
     head_logits<BF>(c, S.seg_head + i, S.H);
     probe_at(c, 1024 + 8 * i + 3);
     SampleArgs sa;
-    sa.logits = P.LOGITS; sa.V = S.V; sa.sp = P.sp_p; sa.u = u15 ? __ldg(u15 + i) : 0.f;
+    sa.logits = P.LOGITS; sa.V = S.V; sa.sp = P.req.sp_p; sa.u = u15 ? __ldg(u15 + i) : 0.f;
     sa.use_penalty = false; sa.sup0 = S.V; sa.suppress_eos = false; sa.eos = -1;
     const int tok = sample_block<BF>(c, sa);
     if (c.tid == 0) SMEM().codes[i + 1] = tok;
@@ -1785,7 +1745,7 @@ __device__ __noinline__ void producer_main(const KParams& P) {
   if (lane == 0) {
     Producer<BF> pr(P);
     if (P.mode == MODE_TALKER_STEP) {
-      pr.stack_layers(P.t, P.position, P.n_left_pad);
+      pr.stack_layers(P.t, P.position, P.req.n_left_pad);
     } else {
       const int iters = P.mode == MODE_FUSED ? P.n_frames : 1;
       for (int f = 0; f < iters && !pr.stopped; ++f) {
@@ -1795,7 +1755,7 @@ __device__ __noinline__ void producer_main(const KParams& P) {
           pr.seg(P.p.seg_head + i);
         }
         if (P.mode == MODE_FUSED) {
-          pr.stack_layers(P.t, P.prefill_len + P.state[1] + f, P.n_left_pad);
+          pr.stack_layers(P.t, P.req.prefill_len + P.req.state[1] + f, P.req.n_left_pad);
           pr.seg(P.t.seg_head);
         }
       }
@@ -1854,7 +1814,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) fq3_decode_kernel(const __grid_co
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int cta = blockIdx.x;
 
-  cta_prologue(P, P.mode == MODE_FUSED ? P.seen : nullptr);
+  cta_prologue(P, P.mode == MODE_FUSED ? P.req.seen : nullptr);
   __syncthreads();
 
   if (warp == NCW) {
@@ -1862,27 +1822,28 @@ __global__ void __launch_bounds__(NTHREADS, 1) fq3_decode_kernel(const __grid_co
   } else {
     // ======================================= CONSUMERS ======================================
     Ctx c{P, tid, warp, lane, 0u, 0u};
+    const SlotParams& rq = P.req;
     const int Ht = P.t.H;
     if (P.mode == MODE_TALKER_STEP) {
       for (int k = tid; k < Ht; k += NCT) s.xin[0][k] = ldw<BF>(P.in_embeds, k);
       csync();
-      run_layers<BF, true>(c, P.t, 1, P.position, P.position + P.rope_delta, P.n_left_pad, true, P.dbg_on != 0);
+      run_layers<BF, true>(c, P.t, 1, P.position, P.position + rq.rope_delta, rq.n_left_pad, true, P.dbg_on != 0);
       if (cta == 0)
         for (int k = tid; k < Ht; k += NCT) stw<BF>(P.hidden_out, k, xs_get<BF>(c, k));
     } else if (P.mode == MODE_PRED_RUN) {
       for (int k = tid; k < 2 * Ht; k += NCT) s.xin[k / Ht][k % Ht] = ldw<BF>(P.pred_input, k);
       csync();
-      predictor_frame<BF>(c, P.sp_p.do_sample ? P.pred_uniforms : nullptr, P.dbg_on != 0);
-      if (cta == 0 && tid < P.ncb) P.codes_out[tid] = (long long)s.codes[tid + 1];
+      predictor_frame<BF>(c, rq.sp_p.do_sample ? P.pred_uniforms : nullptr, P.dbg_on != 0);
+      if (cta == 0 && tid < P.ncb) rq.codes_out[tid] = (long long)s.codes[tid + 1];
     } else {
       // ---------------- fused frame loop: generate.py:149-199 / streaming.py:106-173 ----------------
-      int token = P.state[0], step = P.state[1], gen_step = P.state[2];
+      int token = rq.state[0], step = rq.state[1], gen_step = rq.state[2];
       int finished = 0, emitted = 0;
-      for (int k = tid; k < Ht; k += NCT) s.hid[k] = P.past_hidden[k];
+      for (int k = tid; k < Ht; k += NCT) s.hid[k] = rq.past_hidden[k];
       csync();
       while (true) {
         if (emitted >= P.n_frames) break;
-        if (step >= P.max_new) { finished = 1; break; }
+        if (step >= rq.max_new) { finished = 1; break; }
         if (token == P.eos) { finished = 2; break; }
         // predictor input: cat(past_hidden, codec_embedding(token))   generate.py:154-155
         for (int k = tid; k < Ht; k += NCT) {
@@ -1894,17 +1855,17 @@ __global__ void __launch_bounds__(NTHREADS, 1) fq3_decode_kernel(const __grid_co
           s.seen[token >> 5] |= 1u << (token & 31);
         }
         csync();
-        const float* urow = P.uniforms + (size_t)(step + 1) * 16;
+        const float* urow = rq.uniforms + (size_t)(step + 1) * 16;
         const int pslot = 2048 + 8 * (emitted & 63);
         probe_at(c, pslot + 0);
-        predictor_frame<BF>(c, P.sp_p.do_sample ? urow + 1 : nullptr, false);
+        predictor_frame<BF>(c, rq.sp_p.do_sample ? urow + 1 : nullptr, false);
         probe_at(c, pslot + 1);
-        if (cta == 0 && tid < 16) P.codes_out[(size_t)emitted * 16 + tid] = (long long)s.codes[tid];
+        if (cta == 0 && tid < 16) rq.codes_out[(size_t)emitted * 16 + tid] = (long long)s.codes[tid];
         emitted++;
         // next talker input: sum of 16 embedding rows + trailing text / tts_pad   generate.py:163-171
         {
-          const void* extra = gen_step < P.trailing_len ? P.trailing : P.tts_pad;
-          const size_t eoff = gen_step < P.trailing_len ? (size_t)gen_step * Ht : 0;
+          const void* extra = gen_step < rq.trailing_len ? rq.trailing : rq.tts_pad;
+          const size_t eoff = gen_step < rq.trailing_len ? (size_t)gen_step * Ht : 0;
           for (int k = tid; k < Ht; k += NCT) {
             float sm = ldw<BF>(P.t_embed, (size_t)token * Ht + k);
             for (int i = 0; i < P.ncb; ++i) sm += ldw<BF>(P.p_embeds, ((size_t)i * P.p.V + s.codes[i + 1]) * Ht + k);
@@ -1912,19 +1873,19 @@ __global__ void __launch_bounds__(NTHREADS, 1) fq3_decode_kernel(const __grid_co
           }
           csync();
         }
-        const int pos = P.prefill_len + step;
+        const int pos = rq.prefill_len + step;
         if (pos >= P.max_seq_len - 1) { finished = 3; step++; break; }   // generate.py:175-177 (frame already emitted)
         probe_at(c, pslot + 2);
-        run_layers<BF, true>(c, P.t, 1, pos, pos + P.rope_delta, P.n_left_pad, true, false);
+        run_layers<BF, true>(c, P.t, 1, pos, pos + rq.rope_delta, rq.n_left_pad, true, false);
         probe_at(c, pslot + 3);
         for (int k = tid; k < Ht; k += NCT) s.hid[k] = xs_get<BF>(c, k);   // past_hidden = post-norm hidden (generate.py:198)
         csync();
         head_logits<BF>(c, P.t.seg_head, Ht);
         probe_at(c, pslot + 4);
         SampleArgs sa;
-        sa.logits = P.LOGITS; sa.V = P.t.V; sa.sp = P.sp_t; sa.u = P.sp_t.do_sample ? __ldg(urow) : 0.f;
+        sa.logits = P.LOGITS; sa.V = P.t.V; sa.sp = rq.sp_t; sa.u = rq.sp_t.do_sample ? __ldg(urow) : 0.f;
         sa.use_penalty = true; sa.sup0 = P.t.V > 1024 ? P.t.V - 1024 : 0;
-        sa.suppress_eos = (step + 1) < P.min_new; sa.eos = P.eos;
+        sa.suppress_eos = (step + 1) < rq.min_new; sa.eos = P.eos;
         token = sample_block<BF>(c, sa);
         probe_at(c, pslot + 5);
         step++;
@@ -1932,10 +1893,10 @@ __global__ void __launch_bounds__(NTHREADS, 1) fq3_decode_kernel(const __grid_co
       }
       if (cta == 0) {
         if (tid == 0) {
-          P.state[0] = token; P.state[1] = step; P.state[2] = gen_step; P.state[3] = finished; P.state[4] = emitted;
+          rq.state[0] = token; rq.state[1] = step; rq.state[2] = gen_step; rq.state[3] = finished; rq.state[4] = emitted;
         }
-        for (int k = tid; k < Ht; k += NCT) P.past_hidden[k] = s.hid[k];
-        for (int i = tid; i < VMAX / 32; i += NCT) P.seen[i] = s.seen[i];
+        for (int k = tid; k < Ht; k += NCT) rq.past_hidden[k] = s.hid[k];
+        for (int i = tid; i < VMAX / 32; i += NCT) rq.seen[i] = s.seen[i];
       }
     }
     drain_producer(c);

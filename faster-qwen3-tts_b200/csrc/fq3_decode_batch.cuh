@@ -4,7 +4,8 @@
 //
 // Same tape, same producer warp / TMA ring, same grid barrier and the same per-element arithmetic (rounding points,
 // accumulation order inside a warp, cross-warp summation order) as the single-sequence kernel in fq3_decode.cuh: row b
-// of a batched launch produces bit-for-bit the codes a single-sequence launch produces for that request (tested).
+// of a batched launch produces bit-for-bit the codes a single-sequence launch produces for that request (tested).  The
+// attention functions and the fp32 GEMV are the single-sequence kernel's own, called with this slot's pointers.
 //
 // What changes with B > 1:
 //   * activations live in global memory (L2-resident) as [column][K] matrices, column = slot (predictor pass 0: column
@@ -24,20 +25,6 @@ namespace fq3 {
 
 constexpr int MAXB = 32;          // slots per launch
 constexpr int MAXCOL = 2 * MAXB;  // activation columns (predictor pass 0 carries 2 tokens per slot)
-
-struct SlotParams {
-  void *kc, *vc;        // talker KV cache of this slot   [L][nKV][S][128]
-  void *pkc, *pvc;      // predictor KV cache of this slot [Lp][nKVp][32][128]
-  int* state;           // [0] token [1] step [2] gen_step [3] finished [4] emitted(last launch)
-  float* past_hidden;   // [HMAX] fp32 holding dtype-rounded values
-  uint32_t* seen;       // [VMAX/32] cb0 history bitmap
-  const void* trailing;
-  const void* tts_pad;
-  const float* uniforms;
-  long long* codes_out; // [n_frames][16]
-  int prefill_len, rope_delta, n_left_pad, max_new, min_new, trailing_len;
-  Sampling sp_t, sp_p;
-};
 
 enum { BS_TOK = 0, BS_STEP = 1, BS_GEN = 2, BS_FIN = 3, BS_EMIT = 4 };
 
@@ -233,92 +220,25 @@ __device__ __noinline__ void gemv_mma_b(Ctx& c, int seg, int K, const __nv_bfloa
 }
 
 // ------------------------------------------------------------------------------------------------------------
-// fp32 (parity mode) GEMV over up to 8 activation columns: gemv_seg<false, NT> with x read from global memory.
+// fp32 (parity mode) GEMV over up to 8 activation columns of a global [col][ldx] matrix: gemv_seg with the EpiB
+// epilogue.
 // ------------------------------------------------------------------------------------------------------------
 __device__ __noinline__ void gemv_seg_b(Ctx& c, int seg, const float* __restrict__ xg, int ldx, int col0, int ncols,
                                         const EpiB e) {
   constexpr int NT = 8;
-  const uint32_t st = SMEM().seg[seg];
-  const int gbeg = (int)(st >> 8), gn = (int)(st & 255u);
-  const float* xr[NT];
+  gemv_seg<NT, true>(c, seg, xg + (size_t)col0 * ldx, ldx, ncols, [&](int row0, const float* v0, const float* v1) {
 #pragma unroll
-  for (int t = 0; t < NT; ++t) xr[t] = xg + (size_t)(col0 + (t < ncols ? t : 0)) * ldx + c.lane * 4;
-  for (int gi = 0; gi < gn; ++gi) {
-    const Grp g = SMEM().grp[gbeg + gi];
-    const int npairs = g.rows >> 1;
-    const int m = g.m;
-    float acc[4][NT];
-#pragma unroll
-    for (int a = 0; a < 4; ++a)
-#pragma unroll
-      for (int t = 0; t < NT; ++t) acc[a][t] = 0.f;
-    for (int tl = 0; tl < g.ntiles; ++tl) {
-      const int stage = (int)(c.tile_ctr % NS);
-      const uint32_t par = (c.tile_ctr / NS) & 1u;
-      mbar_wait(&SMEM().full[stage], par);
-      const uint8_t* tile = SMEM().ring[stage];
-      for (int j = 0; j < m; ++j) {
-        const int kb = tl * m + j;
-        float xv[NT][4];
-#pragma unroll
-        for (int t = 0; t < NT; ++t) {
-          const float4 a = __ldcg(reinterpret_cast<const float4*>(xr[t] + kb * 128));
-          xv[t][0] = a.x; xv[t][1] = a.y; xv[t][2] = a.z; xv[t][3] = a.w;
-        }
-#pragma unroll
-        for (int sl = 0; sl < 2; ++sl) {
-          const int p = c.warp + NCW * sl;
-          if (p < npairs) {
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              const int r = 2 * p + h;
-              const uint4 w = *reinterpret_cast<const uint4*>(tile + ((size_t)(r * m + j) * 32 + c.lane) * 16);
-              const float wf[4] = {__uint_as_float(w.x), __uint_as_float(w.y), __uint_as_float(w.z), __uint_as_float(w.w)};
-#pragma unroll
-              for (int t = 0; t < NT; ++t)
-#pragma unroll
-                for (int q = 0; q < 4; ++q) acc[sl * 2 + h][t] = fmaf(wf[q], xv[t][q], acc[sl * 2 + h][t]);
-            }
-          }
-        }
-      }
-      __syncwarp();
-      if (c.lane == 0) mbar_arrive(&SMEM().empty[stage]);
-      c.tile_ctr++;
-    }
-#pragma unroll
-    for (int sl = 0; sl < 2; ++sl) {
-      const int p = c.warp + NCW * sl;
-      if (p < npairs) {
-        float v0[NT], v1[NT];
-#pragma unroll
-        for (int t = 0; t < NT; ++t) {
-          float a = acc[sl * 2][t], b = acc[sl * 2 + 1][t];
-#pragma unroll
-          for (int o = 16; o; o >>= 1) {
-            a += __shfl_xor_sync(0xffffffffu, a, o);
-            b += __shfl_xor_sync(0xffffffffu, b, o);
-          }
-          v0[t] = a;
-          v1[t] = b;
-        }
-        if (c.lane == 0) {
-          const int row0 = g.row0 + 2 * p;
-#pragma unroll
-          for (int t = 0; t < NT; ++t) {
-            if (t < ncols) {
-              if (e.kind == EP_SWIGLU) {
-                epi_apply<false>(e, row0 >> 1, col0 + t, v0[t], v1[t], 0.f);
-              } else {
-                epi_apply<false>(e, row0, col0 + t, v0[t], 0.f, epi_pre<false>(e, row0, col0 + t));
-                epi_apply<false>(e, row0 + 1, col0 + t, v1[t], 0.f, epi_pre<false>(e, row0 + 1, col0 + t));
-              }
-            }
-          }
+    for (int t = 0; t < NT; ++t) {
+      if (t < ncols) {
+        if (e.kind == EP_SWIGLU) {
+          epi_apply<false>(e, row0 >> 1, col0 + t, v0[t], v1[t], 0.f);
+        } else {
+          epi_apply<false>(e, row0, col0 + t, v0[t], 0.f, epi_pre<false>(e, row0, col0 + t));
+          epi_apply<false>(e, row0 + 1, col0 + t, v1[t], 0.f, epi_pre<false>(e, row0 + 1, col0 + t));
         }
       }
     }
-  }
+  });
 }
 
 // column blocks per segment pass: the producer replays the segment once per block
@@ -377,398 +297,6 @@ __device__ __forceinline__ void norm_row_b(Ctx& c, Prov prov, const void* w, siz
 }
 
 // ------------------------------------------------------------------------------------------------------------
-// Talker attention for one (slot, q-head) item: attention_head() with one token, explicit pointers, model-dtype output.
-// ------------------------------------------------------------------------------------------------------------
-template <bool BF>
-__device__ void attn_item_b(Ctx& c, const StackDev& S, int layer, int h, const float* __restrict__ qkv, void* kc,
-                            void* vc, int slot0, int rpos0, int kv_start, void* att_out) {
-  float* sc = SMEM().xs;            // scores [SEQMAX]
-  float* qs = SMEM().xs + SEQMAX;   // [128]
-  float* ks = qs + 256;
-  float* vs = ks + 256;
-  float* opart = vs + 256;          // [8][128]
-  const int g = h / S.rep;
-  const size_t esz = BF ? 2 : 4;
-  const size_t head_stride = (size_t)S.S * 128;
-  uint8_t* kbase = reinterpret_cast<uint8_t*>(kc) + ((size_t)(layer * S.nKV + g) * head_stride) * esz;
-  uint8_t* vbase = reinterpret_cast<uint8_t*>(vc) + ((size_t)(layer * S.nKV + g) * head_stride) * esz;
-  if (c.warp < 3) {
-    const int what = c.warp;
-    const float* src = qkv + (what == 0 ? h * 128 : (what == 1 ? S.qd + g * 128 : S.qd + S.kd + g * 128));
-    float v[4], nwv[4], cc[4], sv[4];
-    {
-      int rp = rpos0;
-      rp = rp < 0 ? 0 : (rp >= S.npos ? S.npos - 1 : rp);
-      const float* cs = S.cos + (size_t)rp * 128;
-      const float* sn = S.sin + (size_t)rp * 128;
-      const void* nw = what == 0 ? S.qnorm : S.knorm;
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int e = c.lane + 32 * i;
-        v[i] = __ldcg(src + e);
-        nwv[i] = what < 2 ? ldw<BF>(nw, (size_t)layer * 128 + e) : 0.f;
-        cc[i] = what < 2 ? __ldg(cs + e) : 0.f;
-        sv[i] = what < 2 ? __ldg(sn + e) : 0.f;
-      }
-    }
-    if (what < 2) {
-      float ss = v[0] * v[0] + v[1] * v[1] + v[2] * v[2] + v[3] * v[3];
-#pragma unroll
-      for (int o = 16; o; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
-      const float r = 1.0f / sqrtf(ss / 128.0f + S.eps);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) v[i] = rnd<BF>(nwv[i] * rnd<BF>(v[i] * r));
-      float o[4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const float rot = (i < 2) ? -v[i + 2] : v[i - 2];
-        o[i] = rnd<BF>(rnd<BF>(v[i] * rnd<BF>(cc[i])) + rnd<BF>(rot * rnd<BF>(sv[i])));
-      }
-#pragma unroll
-      for (int i = 0; i < 4; ++i) v[i] = o[i];
-    }
-    float* dst = what == 0 ? qs : (what == 1 ? ks : vs);
-#pragma unroll
-    for (int i = 0; i < 4; ++i) dst[c.lane + 32 * i] = v[i];
-    if (what > 0 && (h % S.rep) == 0) {
-      uint8_t* cb = (what == 1 ? kbase : vbase) + (size_t)slot0 * 128 * esz;
-#pragma unroll
-      for (int i = 0; i < 4; ++i) stw<BF>(cb, c.lane + 32 * i, v[i]);
-      // a later single-sequence launch may read these rows through the async proxy (TMA-staged split attention)
-      asm volatile("fence.proxy.async.global;" ::: "memory");
-    }
-  }
-  csync();
-  const float scale = 0.08838834764831845f;  // 128^-0.5
-  const int nk = slot0 + 1 - kv_start;       // visible keys
-  const int nold = slot0 - kv_start;         // keys that live in the global cache
-  {
-    constexpr int LPK = BF ? 16 : 32;
-    constexpr int KPW = 32 / LPK;
-    constexpr int EPL = BF ? 8 : 4;
-    constexpr int U = 16;
-    const int sub = c.lane % LPK, kin = c.lane / LPK;
-    float q[EPL];
-#pragma unroll
-    for (int e = 0; e < EPL; ++e) q[e] = qs[sub * EPL + e];
-    for (int base = 0; base < nold; base += NCW * KPW * U) {
-      uint4 kv[U];
-#pragma unroll
-      for (int u = 0; u < U; ++u) {
-        const int jj = base + (u * NCW + c.warp) * KPW + kin;
-        if (jj < nold)
-          kv[u] = __ldcg(reinterpret_cast<const uint4*>(kbase + ((size_t)(kv_start + jj) * 128) * esz) + sub);
-        else
-          kv[u] = make_uint4(0, 0, 0, 0);
-      }
-#pragma unroll
-      for (int u = 0; u < U; ++u) {
-        const int jj = base + (u * NCW + c.warp) * KPW + kin;
-        float d = 0.f;
-        if constexpr (BF) {
-          d = fmaf(q[0], bf_lo(kv[u].x), d); d = fmaf(q[1], bf_hi(kv[u].x), d);
-          d = fmaf(q[2], bf_lo(kv[u].y), d); d = fmaf(q[3], bf_hi(kv[u].y), d);
-          d = fmaf(q[4], bf_lo(kv[u].z), d); d = fmaf(q[5], bf_hi(kv[u].z), d);
-          d = fmaf(q[6], bf_lo(kv[u].w), d); d = fmaf(q[7], bf_hi(kv[u].w), d);
-        } else {
-          d = fmaf(q[0], __uint_as_float(kv[u].x), d); d = fmaf(q[1], __uint_as_float(kv[u].y), d);
-          d = fmaf(q[2], __uint_as_float(kv[u].z), d); d = fmaf(q[3], __uint_as_float(kv[u].w), d);
-        }
-#pragma unroll
-        for (int o = LPK / 2; o; o >>= 1) d += __shfl_xor_sync(0xffffffffu, d, o);
-        if (sub == 0 && jj < nold) sc[jj] = rnd<BF>(rnd<BF>(d) * scale);
-      }
-    }
-    if (c.warp == 0) {  // the new key (shared memory)
-      float d = 0.f;
-#pragma unroll
-      for (int i = 0; i < 4; ++i) d = fmaf(qs[c.lane + 32 * i], ks[c.lane + 32 * i], d);
-#pragma unroll
-      for (int o = 16; o; o >>= 1) d += __shfl_xor_sync(0xffffffffu, d, o);
-      if (c.lane == 0) sc[nold] = rnd<BF>(rnd<BF>(d) * scale);
-    }
-  }
-  csync();
-  float mx = -INFINITY;
-  for (int j = c.tid; j < nk; j += NCT) mx = fmaxf(mx, sc[j]);
-  mx = block_max(c, mx);
-  float sm = 0.f;
-  for (int j = c.tid; j < nk; j += NCT) {
-    const float e = expf(sc[j] - mx);
-    sc[j] = e;
-    sm += e;
-  }
-  sm = block_sum(c, sm);
-  for (int j = c.tid; j < nk; j += NCT) sc[j] = rnd<BF>(sc[j] / sm);
-  csync();
-  {
-    constexpr int LPK = BF ? 16 : 32;
-    constexpr int KPW = 32 / LPK;
-    constexpr int EPL = BF ? 8 : 4;
-    constexpr int U = 16;
-    const int sub = c.lane % LPK, kin = c.lane / LPK;
-    float acc[EPL];
-#pragma unroll
-    for (int e = 0; e < EPL; ++e) acc[e] = 0.f;
-    for (int base = 0; base < nold; base += NCW * KPW * U) {
-      uint4 vv[U];
-      float pv[U];
-#pragma unroll
-      for (int u = 0; u < U; ++u) {
-        const int jj = base + (u * NCW + c.warp) * KPW + kin;
-        if (jj < nold) {
-          vv[u] = __ldcg(reinterpret_cast<const uint4*>(vbase + ((size_t)(kv_start + jj) * 128) * esz) + sub);
-          pv[u] = sc[jj];
-        } else {
-          vv[u] = make_uint4(0, 0, 0, 0);
-          pv[u] = 0.f;
-        }
-      }
-#pragma unroll
-      for (int u = 0; u < U; ++u) {
-        if constexpr (BF) {
-          acc[0] = fmaf(pv[u], bf_lo(vv[u].x), acc[0]); acc[1] = fmaf(pv[u], bf_hi(vv[u].x), acc[1]);
-          acc[2] = fmaf(pv[u], bf_lo(vv[u].y), acc[2]); acc[3] = fmaf(pv[u], bf_hi(vv[u].y), acc[3]);
-          acc[4] = fmaf(pv[u], bf_lo(vv[u].z), acc[4]); acc[5] = fmaf(pv[u], bf_hi(vv[u].z), acc[5]);
-          acc[6] = fmaf(pv[u], bf_lo(vv[u].w), acc[6]); acc[7] = fmaf(pv[u], bf_hi(vv[u].w), acc[7]);
-        } else {
-          acc[0] = fmaf(pv[u], __uint_as_float(vv[u].x), acc[0]); acc[1] = fmaf(pv[u], __uint_as_float(vv[u].y), acc[1]);
-          acc[2] = fmaf(pv[u], __uint_as_float(vv[u].z), acc[2]); acc[3] = fmaf(pv[u], __uint_as_float(vv[u].w), acc[3]);
-        }
-      }
-    }
-    if constexpr (BF) {
-#pragma unroll
-      for (int e = 0; e < EPL; ++e) acc[e] += __shfl_xor_sync(0xffffffffu, acc[e], 16);
-    }
-    if (c.warp == 0 && kin == 0) {
-      const float pj = sc[nold];
-#pragma unroll
-      for (int e = 0; e < EPL; ++e) acc[e] = fmaf(pj, vs[sub * EPL + e], acc[e]);
-    }
-    if (kin == 0) {
-      float* op = opart + c.warp * 128 + sub * EPL;
-#pragma unroll
-      for (int e = 0; e < EPL; ++e) op[e] = acc[e];
-    }
-  }
-  csync();
-  if (c.tid < 128) {
-    float o = 0.f;
-#pragma unroll
-    for (int w = 0; w < NCW; ++w) o += opart[w * 128 + c.tid];
-    stw<BF>(att_out, (size_t)h * 128 + c.tid, rnd<BF>(o));
-  }
-  csync();
-}
-
-// ------------------------------------------------------------------------------------------------------------
-// Predictor attention of ONE slot (<= 17 keys): attention_small_all() with explicit pointers, run by one CTA per
-// slot; one warp per kv group; K/V rows appended to the slot's cache; output rows in the model-dtype ATT matrix.
-//   qkv0 / att0: row of token 0; token t lives `tstride_*` elements further.
-// ------------------------------------------------------------------------------------------------------------
-template <bool BF, int NT>
-__device__ void attn_small_b(Ctx& c, const StackDev& S, int layer, int slot0_, int rpos0, const float* __restrict__ qkv0,
-                             size_t tstride_qkv, void* pkc, void* pvc, void* att0, size_t tstride_att) {
-  constexpr int NOLD = NT == 2 ? 1 : 16;
-  constexpr int MAXK = NT == 2 ? 2 : 17;
-  const int slot0 = NT == 2 ? 0 : slot0_;
-  const float scale = 0.08838834764831845f;
-  const size_t esz = BF ? 2 : 4;
-  const int L4 = 4 * c.lane;
-  using Raw = typename std::conditional<BF, uint2, float4>::type;
-  auto unpack = [](const Raw& r, float* o) {
-    if constexpr (BF) { o[0] = bf_lo(r.x); o[1] = bf_hi(r.x); o[2] = bf_lo(r.y); o[3] = bf_hi(r.y); }
-    else { o[0] = r.x; o[1] = r.y; o[2] = r.z; o[3] = r.w; }
-  };
-  auto zero_raw = [](Raw& r) {
-    if constexpr (BF) r = make_uint2(0, 0);
-    else r = make_float4(0, 0, 0, 0);
-  };
-  for (int g = c.warp; g < S.nKV; g += NCW) {
-    uint8_t* kb = reinterpret_cast<uint8_t*>(pkc) + ((size_t)(layer * S.nKV + g) * S.S * 128) * esz;
-    uint8_t* vb = reinterpret_cast<uint8_t*>(pvc) + ((size_t)(layer * S.nKV + g) * S.S * 128) * esz;
-    Raw kraw[NOLD];
-#pragma unroll
-    for (int j = 0; j < NOLD; ++j) {
-      if (j < slot0) kraw[j] = __ldcg(reinterpret_cast<const Raw*>(kb + (size_t)j * 128 * esz) + c.lane);
-      else zero_raw(kraw[j]);
-    }
-    float4 qn4, kn4, cs4[NT], sn4[NT], kr4[NT], vr4[NT], qr4[2][NT];
-    {
-      float qn[4], kn[4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        qn[i] = ldw<BF>(S.qnorm, (size_t)layer * 128 + L4 + i);
-        kn[i] = ldw<BF>(S.knorm, (size_t)layer * 128 + L4 + i);
-      }
-      qn4 = make_float4(qn[0], qn[1], qn[2], qn[3]);
-      kn4 = make_float4(kn[0], kn[1], kn[2], kn[3]);
-    }
-#pragma unroll
-    for (int t = 0; t < NT; ++t) {
-      int rp = rpos0 + t;
-      rp = rp < 0 ? 0 : (rp >= S.npos ? S.npos - 1 : rp);
-      cs4[t] = __ldg(reinterpret_cast<const float4*>(S.cos + (size_t)rp * 128) + c.lane);
-      sn4[t] = __ldg(reinterpret_cast<const float4*>(S.sin + (size_t)rp * 128) + c.lane);
-      const float* row = qkv0 + (size_t)t * tstride_qkv;
-      kr4[t] = __ldcg(reinterpret_cast<const float4*>(row + S.qd + g * 128) + c.lane);
-      vr4[t] = __ldcg(reinterpret_cast<const float4*>(row + S.qd + S.kd + g * 128) + c.lane);
-#pragma unroll
-      for (int hh = 0; hh < 2; ++hh)
-        qr4[hh][t] = __ldcg(reinterpret_cast<const float4*>(row + (g * S.rep + (hh < S.rep ? hh : 0)) * 128) + c.lane);
-    }
-    auto norm_rope = [&](float* v, const float4& w4, const float4& c4, const float4& s4) {
-      const float w[4] = {w4.x, w4.y, w4.z, w4.w}, cc[4] = {c4.x, c4.y, c4.z, c4.w}, sv[4] = {s4.x, s4.y, s4.z, s4.w};
-      float ss = v[0] * v[0] + v[1] * v[1] + v[2] * v[2] + v[3] * v[3];
-#pragma unroll
-      for (int o = 16; o; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
-      const float r = 1.0f / sqrtf(ss / 128.0f + S.eps);
-      float o4[4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) v[i] = rnd<BF>(w[i] * rnd<BF>(v[i] * r));
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const float other = __shfl_xor_sync(0xffffffffu, v[i], 16);
-        const float rot = c.lane < 16 ? -other : other;
-        o4[i] = rnd<BF>(rnd<BF>(v[i] * rnd<BF>(cc[i])) + rnd<BF>(rot * rnd<BF>(sv[i])));
-      }
-#pragma unroll
-      for (int i = 0; i < 4; ++i) v[i] = o4[i];
-    };
-    float knew[NT][4], vnew[NT][4];
-#pragma unroll
-    for (int t = 0; t < NT; ++t) {
-      knew[t][0] = kr4[t].x; knew[t][1] = kr4[t].y; knew[t][2] = kr4[t].z; knew[t][3] = kr4[t].w;
-      vnew[t][0] = vr4[t].x; vnew[t][1] = vr4[t].y; vnew[t][2] = vr4[t].z; vnew[t][3] = vr4[t].w;
-      norm_rope(knew[t], kn4, cs4[t], sn4[t]);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        stw<BF>(kb + (size_t)(slot0 + t) * 128 * esz, L4 + i, knew[t][i]);
-        stw<BF>(vb + (size_t)(slot0 + t) * 128 * esz, L4 + i, vnew[t][i]);
-      }
-    }
-    float q[2][NT][4];
-#pragma unroll
-    for (int hh = 0; hh < 2; ++hh)
-#pragma unroll
-      for (int t = 0; t < NT; ++t) {
-        q[hh][t][0] = qr4[hh][t].x; q[hh][t][1] = qr4[hh][t].y; q[hh][t][2] = qr4[hh][t].z; q[hh][t][3] = qr4[hh][t].w;
-        norm_rope(q[hh][t], qn4, cs4[t], sn4[t]);
-      }
-    float sc[2][NT][MAXK];
-#pragma unroll
-    for (int j = 0; j < MAXK; ++j) {
-      float kf[4] = {0.f, 0.f, 0.f, 0.f};
-      if (j < NOLD && j < slot0) unpack(kraw[j < NOLD ? j : 0], kf);
-#pragma unroll
-      for (int tn = 0; tn < NT; ++tn)
-        if (j == slot0 + tn) {
-#pragma unroll
-          for (int i = 0; i < 4; ++i) kf[i] = knew[tn][i];
-        }
-#pragma unroll
-      for (int hh = 0; hh < 2; ++hh)
-#pragma unroll
-        for (int t = 0; t < NT; ++t) {
-          float d = q[hh][t][0] * kf[0];
-          d = fmaf(q[hh][t][1], kf[1], d); d = fmaf(q[hh][t][2], kf[2], d); d = fmaf(q[hh][t][3], kf[3], d);
-          sc[hh][t][j] = d;
-        }
-    }
-    float dotk[2] = {0.f, 0.f};   // NT == 1: reduce-scatter of the 34 partial dot products (fq3_decode.cuh: rs_step)
-    if constexpr (NT == 1) {
-      float a[34];
-#pragma unroll
-      for (int hh = 0; hh < 2; ++hh)
-#pragma unroll
-        for (int j = 0; j < 17; ++j) a[hh * 17 + j] = sc[hh][0][j];
-      rs_step<34, 16>(a, c.lane);
-      rs_step<17, 8>(a, c.lane);
-      rs_step<9, 4>(a, c.lane);
-      rs_step<5, 2>(a, c.lane);
-      rs_step<3, 1>(a, c.lane);
-      rs34_gather(a, c.lane, dotk);
-    } else {
-#pragma unroll
-      for (int o = 16; o; o >>= 1)
-#pragma unroll
-        for (int hh = 0; hh < 2; ++hh)
-#pragma unroll
-          for (int t = 0; t < NT; ++t)
-#pragma unroll
-            for (int j = 0; j < MAXK; ++j) sc[hh][t][j] += __shfl_xor_sync(0xffffffffu, sc[hh][t][j], o);
-    }
-    Raw vraw[NOLD];
-#pragma unroll
-    for (int j = 0; j < NOLD; ++j) {
-      if (j < slot0) vraw[j] = __ldcg(reinterpret_cast<const Raw*>(vb + (size_t)j * 128 * esz) + c.lane);
-      else zero_raw(vraw[j]);
-    }
-#pragma unroll
-    for (int hh = 0; hh < 2; ++hh)
-#pragma unroll
-      for (int t = 0; t < NT; ++t) {
-        const int nk = slot0 + t + 1;
-        float mx = -INFINITY, mine = -INFINITY;
-        if constexpr (NT == 1) {
-          mine = (c.lane < nk) ? rnd<BF>(rnd<BF>(dotk[hh]) * scale) : -INFINITY;
-          mx = mine;
-#pragma unroll
-          for (int o = 16; o; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-        } else {
-#pragma unroll
-          for (int j = 0; j < MAXK; ++j) {
-            const float sj = j < nk ? rnd<BF>(rnd<BF>(sc[hh][t][j]) * scale) : -INFINITY;
-            mx = fmaxf(mx, sj);
-            if (j == c.lane) mine = sj;
-          }
-        }
-        const float e = (c.lane < nk) ? (BF ? __expf(mine - mx) : expf(mine - mx)) : 0.f;
-        float sm = e;
-#pragma unroll
-        for (int o = 16; o; o >>= 1) sm += __shfl_xor_sync(0xffffffffu, sm, o);
-        const float pmine = rnd<BF>(BF ? __fdividef(e, sm) : e / sm);
-#pragma unroll
-        for (int j = 0; j < MAXK; ++j) sc[hh][t][j] = __shfl_sync(0xffffffffu, pmine, j);
-      }
-    float o4[2][NT][4];
-#pragma unroll
-    for (int hh = 0; hh < 2; ++hh)
-#pragma unroll
-      for (int t = 0; t < NT; ++t)
-#pragma unroll
-        for (int i = 0; i < 4; ++i) o4[hh][t][i] = 0.f;
-#pragma unroll
-    for (int j = 0; j < MAXK; ++j) {
-      float vf[4] = {0.f, 0.f, 0.f, 0.f};
-      if (j < NOLD && j < slot0) unpack(vraw[j < NOLD ? j : 0], vf);
-#pragma unroll
-      for (int tn = 0; tn < NT; ++tn)
-        if (j == slot0 + tn) {
-#pragma unroll
-          for (int i = 0; i < 4; ++i) vf[i] = vnew[tn][i];
-        }
-#pragma unroll
-      for (int hh = 0; hh < 2; ++hh)
-#pragma unroll
-        for (int t = 0; t < NT; ++t)
-#pragma unroll
-          for (int i = 0; i < 4; ++i) o4[hh][t][i] = fmaf(sc[hh][t][j], vf[i], o4[hh][t][i]);
-    }
-#pragma unroll
-    for (int hh = 0; hh < 2; ++hh)
-      if (hh < S.rep)
-#pragma unroll
-        for (int t = 0; t < NT; ++t)
-#pragma unroll
-          for (int i = 0; i < 4; ++i)
-            stw<BF>(att0, (size_t)t * tstride_att + (g * S.rep + hh) * 128 + L4 + i, rnd<BF>(o4[hh][t][i]));
-  }
-  csync();
-}
-
-// ------------------------------------------------------------------------------------------------------------
 // per-CTA view of a batched launch
 // ------------------------------------------------------------------------------------------------------------
 struct BView {
@@ -814,15 +342,17 @@ __device__ void stack_b(Ctx& c, const StackDev& S, const BView& v, int nt, uint3
         const int b = SMEM().runl[idx / S.nH], h = idx % S.nH;
         const SlotParams& sp = P.sl[b];
         const int pos = sp.prefill_len + SMEM().bst[BS_STEP][b];
-        attn_item_b<BF>(c, S, l, h, P.QKVB + (size_t)b * P.ldQKV, sp.kc, sp.vc, pos, pos + sp.rope_delta, sp.n_left_pad,
-                        reinterpret_cast<uint8_t*>(P.ATTB) + (size_t)b * P.ldATT * (BF ? 2 : 4));
+        attention_head<BF>(c, S, l, h, P.QKVB + (size_t)b * P.ldQKV, sp.kc, sp.vc,
+                           reinterpret_cast<uint8_t*>(P.ATTB) + (size_t)b * P.ldATT * (BF ? 2 : 4), pos,
+                           pos + sp.rope_delta, sp.n_left_pad);
       }
     } else {
       if (mine && v.rank == 0) {
         const float* q0 = P.QKVB + (size_t)v.b * P.ldQKV;
         uint8_t* a0 = reinterpret_cast<uint8_t*>(P.ATTB) + (size_t)v.b * P.ldATT * (BF ? 2 : 4);
-        if (nt == 1) attn_small_b<BF, 1>(c, S, l, pass_slot0, pass_slot0, q0, 0, me.pkc, me.pvc, a0, 0);
-        else attn_small_b<BF, 2>(c, S, l, 0, 0, q0, (size_t)B * P.ldQKV, me.pkc, me.pvc, a0, (size_t)B * P.ldATT);
+        auto to_att = [&](int t, int i, float x) { stw<BF>(a0, (size_t)t * B * P.ldATT + i, x); };
+        if (nt == 1) attention_small_all<BF, 1>(c, S, l, pass_slot0, pass_slot0, q0, 0, me.pkc, me.pvc, true, nullptr, to_att);
+        else attention_small_all<BF, 2>(c, S, l, 0, 0, q0, (size_t)B * P.ldQKV, me.pkc, me.pvc, true, nullptr, to_att);
       }
     }
     grid_sync_p(c, PC_GEMV);

@@ -58,7 +58,7 @@ struct PackGrp {
   int32_t K;
 };
 
-// host-side record of one request slot (fq3_begin_request latches it; the kernels read it through KParams / SlotParams)
+// host-side record of one request slot (fq3_begin_request latches it; slot_params() hands it to the kernels)
 struct SlotHost {
   bool active = false;
   int prefill_len = 0, rope_delta = 0, n_left_pad = 0, max_new = 0, min_new = 0, trailing_len = 0;
@@ -86,7 +86,8 @@ struct fq3_engine {
   SlotParams* sl_host = nullptr;  // pinned
   // device buffers (slot-major: slot s starts at s * <per-slot size>)
   void *t_kc = nullptr, *t_vc = nullptr, *p_kc = nullptr, *p_vc = nullptr;
-  float *X = nullptr, *X1 = nullptr, *QKV = nullptr, *ATT = nullptr, *ACT = nullptr, *LOGITS = nullptr, *PART = nullptr;
+  float *X = nullptr, *X1 = nullptr, *QKV = nullptr, *ACT = nullptr, *LOGITS = nullptr, *PART = nullptr;
+  void* ATT = nullptr;  // model dtype
   unsigned* bar = nullptr;
   int* state = nullptr;
   int* state_host = nullptr;  // pinned
@@ -117,7 +118,6 @@ static size_t smem_bytes() { return sizeof(Smem); }
 // ------------------------------------------------------------------------------------------------------------
 // small kernels
 // ------------------------------------------------------------------------------------------------------------
-template <bool BF>
 __global__ void pack_kernel(const PackGrp* __restrict__ pg, int npg, const void* const* __restrict__ rowsrc,
                             uint8_t* __restrict__ tape) {
   for (int b = blockIdx.x; b < npg; b += gridDim.x) {
@@ -134,15 +134,7 @@ __global__ void pack_kernel(const PackGrp* __restrict__ pg, int npg, const void*
       const int t = (int)(rem / rows);
       const int kb = t * m + j;
       const uint8_t* src = reinterpret_cast<const uint8_t*>(rowsrc[g.rowsrc_idx + r]);
-      uint4 v;
-      if constexpr (BF) {
-        const uint2 a = *reinterpret_cast<const uint2*>(src + ((size_t)kb * 256 + lane * 4) * 2);
-        const uint2 c = *reinterpret_cast<const uint2*>(src + ((size_t)kb * 256 + 128 + lane * 4) * 2);
-        v = make_uint4(a.x, a.y, c.x, c.y);
-      } else {
-        v = *reinterpret_cast<const uint4*>(src + ((size_t)kb * 128 + lane * 4) * 4);
-      }
-      dst[q] = v;
+      dst[q] = *reinterpret_cast<const uint4*>(src + ((size_t)kb * 128 + lane * 4) * 4);
     }
   }
 }
@@ -307,7 +299,7 @@ extern "C" int fq3_engine_create(const fq3_config* cfg, fq3_engine** out) {
   const int ldATT = std::max(T.num_attention_heads, Pc.num_attention_heads) * 128;
   const int ldACT = std::max(T.intermediate_size, Pc.intermediate_size);
   CK(cudaMalloc(&e->X, 2 * ldX * sizeof(float))); CK(cudaMalloc(&e->X1, 2 * ldX * sizeof(float)));
-  CK(cudaMalloc(&e->QKV, 2 * ldQKV * sizeof(float))); CK(cudaMalloc(&e->ATT, 2 * ldATT * sizeof(float)));
+  CK(cudaMalloc(&e->QKV, 2 * ldQKV * sizeof(float))); CK(cudaMalloc(&e->ATT, ldATT * e->esz));
   CK(cudaMalloc(&e->ACT, 2 * ldACT * sizeof(float))); CK(cudaMalloc(&e->LOGITS, VMAX * sizeof(float)));
   CK(cudaMalloc(&e->bar, 32768)); CK(cudaMemset(e->bar, 0, 32768));
   CK(cudaMalloc(&e->PART, (size_t)T.num_attention_heads * 16 * PART_STRIDE * sizeof(float)));
@@ -343,18 +335,18 @@ extern "C" int fq3_engine_create(const fq3_config* cfg, fq3_engine** out) {
   }
   KParams& k = e->kp;
   memset(&k, 0, sizeof(k));
-  auto fill = [&](StackDev& s, const fq3_stack_config& c, void* kc, void* vc, int S) {
+  auto fill = [&](StackDev& s, const fq3_stack_config& c, int S) {
     s.H = c.hidden_size; s.I = c.intermediate_size; s.L = c.num_hidden_layers;
     s.nH = c.num_attention_heads; s.nKV = c.num_key_value_heads; s.V = c.vocab_size;
     s.qd = s.nH * 128; s.kd = s.nKV * 128; s.rep = s.nH / s.nKV; s.eps = c.rms_norm_eps;
-    s.kc = kc; s.vc = vc; s.S = S;
+    s.S = S;
   };
-  fill(k.t, T, e->t_kc, e->t_vc, cfg->max_seq_len);
-  fill(k.p, Pc, e->p_kc, e->p_vc, 32);
+  fill(k.t, T, cfg->max_seq_len);
+  fill(k.p, Pc, 32);
   k.ncta = e->ncta;
   k.X = e->X; k.X1 = e->X1; k.QKV = e->QKV; k.ATT = e->ATT; k.ACT = e->ACT; k.LOGITS = e->LOGITS;
   k.ldX = ldX; k.ldQKV = ldQKV; k.ldATT = ldATT; k.ldACT = ldACT;
-  k.bar = e->bar; k.state = e->state; k.past_hidden = e->past_hidden; k.seen = e->seen;
+  k.bar = e->bar;
   k.XB = e->XB; k.X1B = e->X1B; k.QKVB = e->QKVB; k.LOGB = e->LOGB;
   k.XNB = e->XNB; k.ATTB = e->ATTB; k.ACTB = e->ACTB; k.PINB = e->PINB; k.TOKB = e->TOKB;
   k.nslots = 0; k.sl = e->sl_dev;
@@ -370,8 +362,6 @@ extern "C" int fq3_engine_create(const fq3_config* cfg, fq3_engine** out) {
     k.PART = e->PART;
     k.attn_cnt = e->bar + 1024;
   }
-  k.sp_t = Sampling{1, 50, 0.9f, 1.0f, 1.05f};
-  k.sp_p = Sampling{1, 50, 0.9f, 1.0f, 1.0f};
   *out = e;
   return 0;
 }
@@ -727,7 +717,7 @@ extern "C" int fq3_engine_load_weights(fq3_engine* e, const fq3_tensor* tensors,
   {
     const int grid = (int)std::min<size_t>(pack.size(), 132 * 16);
     if (e->bf16) pack_mma_kernel<<<grid, 256, 0, stream>>>(d_pack, (int)pack.size(), (const void* const*)d_rowsrc, e->tape);
-    else pack_kernel<false><<<grid, 256, 0, stream>>>(d_pack, (int)pack.size(), (const void* const*)d_rowsrc, e->tape);
+    else pack_kernel<<<grid, 256, 0, stream>>>(d_pack, (int)pack.size(), (const void* const*)d_rowsrc, e->tape);
     e->launches++;
     CK(cudaGetLastError());
   }
@@ -753,13 +743,14 @@ extern "C" int fq3_engine_load_weights(fq3_engine* e, const fq3_tensor* tensors,
 // ------------------------------------------------------------------------------------------------------------
 // launches
 // ------------------------------------------------------------------------------------------------------------
+// one cooperative launch of a persistent decode kernel: the single-sequence kernel (kp.nslots == 0) or the batched
+// one, in the engine's dtype, with the grid-barrier and attention-split counters cleared first
 static int launch_decode(fq3_engine* e, const KParams& kp, cudaStream_t stream) {
+  const void* fn = kp.nslots == 0 ? (e->bf16 ? (const void*)fq3_decode_kernel<true> : (const void*)fq3_decode_kernel<false>)
+                                  : (e->bf16 ? (const void*)fq3_decode_batch_kernel<true> : (const void*)fq3_decode_batch_kernel<false>);
   CK(cudaMemsetAsync(e->bar, 0, 32768, stream));
   void* args[] = {(void*)&kp};
-  if (e->bf16)
-    CK(cudaLaunchCooperativeKernel((const void*)fq3_decode_kernel<true>, dim3(e->ncta), dim3(NTHREADS), args, smem_bytes(), stream));
-  else
-    CK(cudaLaunchCooperativeKernel((const void*)fq3_decode_kernel<false>, dim3(e->ncta), dim3(NTHREADS), args, smem_bytes(), stream));
+  CK(cudaLaunchCooperativeKernel(fn, dim3(e->ncta), dim3(NTHREADS), args, smem_bytes(), stream));
   e->launches++;
   return 0;
 }
@@ -780,18 +771,26 @@ static void* slot_tv(fq3_engine* e, int s) { return (uint8_t*)e->t_vc + (size_t)
 static void* slot_pk(fq3_engine* e, int s) { return (uint8_t*)e->p_kc + (size_t)s * e->pkv_slot; }
 static void* slot_pv(fq3_engine* e, int s) { return (uint8_t*)e->p_vc + (size_t)s * e->pkv_slot; }
 
-// kernel parameters of a single-sequence launch on slot s: the slot's caches / state + the request it latched
-static KParams kp_for_slot(fq3_engine* e, int s) {
-  KParams kp = e->kp;
+// the kernels' record of slot s: its caches and state, the request it latched, where its codes go
+static SlotParams slot_params(fq3_engine* e, int s, long long* codes_out) {
   const SlotHost& h = e->slots[s];
-  kp.t.kc = slot_tk(e, s); kp.t.vc = slot_tv(e, s); kp.p.kc = slot_pk(e, s); kp.p.vc = slot_pv(e, s);
-  kp.state = e->state + 8 * s;
-  kp.past_hidden = e->past_hidden + (size_t)s * HMAX;
-  kp.seen = e->seen + (size_t)s * (VMAX / 32);
-  kp.prefill_len = h.prefill_len; kp.rope_delta = h.rope_delta; kp.n_left_pad = h.n_left_pad;
-  kp.max_new = h.max_new; kp.min_new = h.min_new; kp.trailing_len = h.trailing_len;
-  kp.trailing = h.trailing; kp.tts_pad = h.tts_pad; kp.uniforms = h.uniforms;
-  kp.sp_t = h.sp_t; kp.sp_p = h.sp_p;
+  SlotParams p;
+  p.kc = slot_tk(e, s); p.vc = slot_tv(e, s); p.pkc = slot_pk(e, s); p.pvc = slot_pv(e, s);
+  p.state = e->state + 8 * s;
+  p.past_hidden = e->past_hidden + (size_t)s * HMAX;
+  p.seen = e->seen + (size_t)s * (VMAX / 32);
+  p.trailing = h.trailing; p.tts_pad = h.tts_pad; p.uniforms = h.uniforms;
+  p.codes_out = codes_out;
+  p.prefill_len = h.prefill_len; p.rope_delta = h.rope_delta; p.n_left_pad = h.n_left_pad;
+  p.max_new = h.max_new; p.min_new = h.min_new; p.trailing_len = h.trailing_len;
+  p.sp_t = h.sp_t; p.sp_p = h.sp_p;
+  return p;
+}
+
+// kernel parameters of a single-sequence launch on slot s
+static KParams kp_for_slot(fq3_engine* e, int s, long long* codes_out) {
+  KParams kp = e->kp;
+  kp.req = slot_params(e, s, codes_out);
   kp.nslots = 0;
   return kp;
 }
@@ -853,7 +852,7 @@ extern "C" int fq3_talker_step(fq3_engine* e, int32_t slot, const void* embeds_d
   if ((rc = check_slot(e, slot))) return rc;
   if (position < 0 || position >= e->cfg.max_seq_len) return fail(FQ3_ERR_INVALID, "position %d outside the cache", position);
   DevGuard dev_guard(e->dev);
-  KParams kp = kp_for_slot(e, slot);
+  KParams kp = kp_for_slot(e, slot, nullptr);
   kp.mode = MODE_TALKER_STEP;
   kp.in_embeds = embeds_dev; kp.hidden_out = hidden_out_dev; kp.position = position;
   kp.dbg_on = e->dbg_on;
@@ -868,10 +867,10 @@ extern "C" int fq3_predictor_run(fq3_engine* e, int32_t slot, const void* pred_i
   if ((rc = check_slot(e, slot))) return rc;
   if (sp->do_sample && !uniforms_dev) return fail(FQ3_ERR_INVALID, "do_sample needs uniforms");
   DevGuard dev_guard(e->dev);
-  KParams kp = kp_for_slot(e, slot);
+  KParams kp = kp_for_slot(e, slot, (long long*)codes_out_dev);
   kp.mode = MODE_PRED_RUN;
-  kp.pred_input = pred_input_dev; kp.pred_uniforms = uniforms_dev; kp.codes_out = (long long*)codes_out_dev;
-  kp.sp_p = to_sampling(sp);
+  kp.pred_input = pred_input_dev; kp.pred_uniforms = uniforms_dev;
+  kp.req.sp_p = to_sampling(sp);
   kp.dbg_on = e->dbg_on;
   return launch_decode(e, kp, (cudaStream_t)stream_);
 }
@@ -928,35 +927,15 @@ static int launch_decode_batch(fq3_engine* e, const int32_t* slots, int n, int n
                                cudaStream_t stream) {
   if (!e->sl_dev) return fail(FQ3_ERR_STATE, "engine was created with max_batch = 1");
   if (n > e->ncta) return fail(FQ3_ERR_INVALID, "%d slots need at least as many CTAs (engine has %d)", n, e->ncta);
-  for (int j = 0; j < n; ++j) {
-    const int s = slots[j];
-    const SlotHost& h = e->slots[s];
-    SlotParams& p = e->sl_host[j];
-    p.kc = slot_tk(e, s); p.vc = slot_tv(e, s); p.pkc = slot_pk(e, s); p.pvc = slot_pv(e, s);
-    p.state = e->state + 8 * s;
-    p.past_hidden = e->past_hidden + (size_t)s * HMAX;
-    p.seen = e->seen + (size_t)s * (VMAX / 32);
-    p.trailing = h.trailing; p.tts_pad = h.tts_pad; p.uniforms = h.uniforms;
-    p.codes_out = codes_out_dev + (size_t)j * n_frames * 16;
-    p.prefill_len = h.prefill_len; p.rope_delta = h.rope_delta; p.n_left_pad = h.n_left_pad;
-    p.max_new = h.max_new; p.min_new = h.min_new; p.trailing_len = h.trailing_len;
-    p.sp_t = h.sp_t; p.sp_p = h.sp_p;
-  }
+  for (int j = 0; j < n; ++j) e->sl_host[j] = slot_params(e, slots[j], codes_out_dev + (size_t)j * n_frames * 16);
   CK(cudaMemcpyAsync(e->sl_dev, e->sl_host, (size_t)n * sizeof(SlotParams), cudaMemcpyHostToDevice, stream));
-  CK(cudaMemsetAsync(e->bar, 0, 32768, stream));
   KParams kp = e->kp;
   kp.mode = MODE_FUSED;
   kp.nslots = n;
   kp.sl = e->sl_dev;
   kp.n_frames = n_frames;
   kp.dbg_on = e->dbg_on & 2;
-  void* args[] = {(void*)&kp};
-  if (e->bf16)
-    CK(cudaLaunchCooperativeKernel((const void*)fq3_decode_batch_kernel<true>, dim3(e->ncta), dim3(NTHREADS), args, smem_bytes(), stream));
-  else
-    CK(cudaLaunchCooperativeKernel((const void*)fq3_decode_batch_kernel<false>, dim3(e->ncta), dim3(NTHREADS), args, smem_bytes(), stream));
-  e->launches++;
-  return 0;
+  return launch_decode(e, kp, stream);
 }
 
 // numerics probe: ONE batched GEMV (the kernel the batched decode path is built from) over a weight segment
@@ -977,8 +956,6 @@ extern "C" int fq3_debug_gemv(fq3_engine* e, int32_t stack, int32_t layer, int32
     return fail(FQ3_ERR_INVALID, "which must be 0..4 (qkv, o, gate/up, down, head)");
   }
   DevGuard dev_guard(e->dev);
-  cudaStream_t stream = (cudaStream_t)stream_;
-  CK(cudaMemsetAsync(e->bar, 0, 32768, stream));
   KParams kp = e->kp;
   kp.mode = MODE_GEMV_TEST;
   kp.nslots = 1;
@@ -988,13 +965,7 @@ extern "C" int fq3_debug_gemv(fq3_engine* e, int32_t stack, int32_t layer, int32
   kp.gt_seg = sg; kp.gt_K = e->segs[sg].K; kp.gt_rows = e->segs[sg].rows; kp.gt_ncols = ncols;
   kp.gt_swiglu = which == 2 ? 1 : 0;
   kp.gt_x = x_dev; kp.gt_out = out_dev;
-  void* args[] = {(void*)&kp};
-  if (e->bf16)
-    CK(cudaLaunchCooperativeKernel((const void*)fq3_decode_batch_kernel<true>, dim3(e->ncta), dim3(NTHREADS), args, smem_bytes(), stream));
-  else
-    CK(cudaLaunchCooperativeKernel((const void*)fq3_decode_batch_kernel<false>, dim3(e->ncta), dim3(NTHREADS), args, smem_bytes(), stream));
-  e->launches++;
-  return 0;
+  return launch_decode(e, kp, (cudaStream_t)stream_);
 }
 
 extern "C" int fq3_decode_chunk(fq3_engine* e, const int32_t* slots, int32_t n_slots, int32_t n_frames,
@@ -1012,10 +983,9 @@ extern "C" int fq3_decode_chunk(fq3_engine* e, const int32_t* slots, int32_t n_s
   DevGuard dev_guard(e->dev);
   cudaStream_t stream = (cudaStream_t)stream_;
   if (n_slots == 1) {
-    KParams kp = kp_for_slot(e, slots[0]);
+    KParams kp = kp_for_slot(e, slots[0], (long long*)codes_out_dev);
     kp.mode = MODE_FUSED;
     kp.n_frames = n_frames;
-    kp.codes_out = (long long*)codes_out_dev;
     kp.dbg_on = e->dbg_on & 2;   // timing probes only; layer dumps belong to the step-wise entry points
     if ((rc = launch_decode(e, kp, stream))) return rc;
   } else {
