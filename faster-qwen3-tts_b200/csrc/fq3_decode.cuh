@@ -85,6 +85,7 @@ struct SlotParams {
   const float* uniforms;
   long long* codes_out; // [n_frames][16]
   int prefill_len, rope_delta, n_left_pad, max_new, min_new, trailing_len;
+  int text_open;        // more trailing rows may follow: a frame that would read row >= trailing_len waits (stops the slot)
   Sampling sp_t, sp_p;
 };
 
@@ -1845,6 +1846,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) fq3_decode_kernel(const __grid_co
         if (emitted >= P.n_frames) break;
         if (step >= rq.max_new) { finished = 1; break; }
         if (token == P.eos) { finished = 2; break; }
+        // open text: this frame's talker step reads trailing row gen_step; stop unfinished before touching any state
+        if (rq.text_open && gen_step >= rq.trailing_len) break;
         // predictor input: cat(past_hidden, codec_embedding(token))   generate.py:154-155
         for (int k = tid; k < Ht; k += NCT) {
           s.xin[0][k] = s.hid[k];

@@ -476,7 +476,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) fq3_decode_batch_kernel(const __g
         if (lane < B && s.bst[BS_FIN][lane] == 0 && s.bst[BS_EMIT][lane] < P.n_frames) {
           if (s.bst[BS_STEP][lane] >= P.sl[lane].max_new) s.bst[BS_FIN][lane] = 1;
           else if (s.bst[BS_TOK][lane] == P.eos) s.bst[BS_FIN][lane] = 2;
-          else r = true;
+          else r = !(P.sl[lane].text_open && s.bst[BS_GEN][lane] >= P.sl[lane].trailing_len);   // open text: wait for the row
         }
         const unsigned m = __ballot_sync(0xffffffffu, r);
         if (lane == 0) s.ibc[0] = (int)m;

@@ -62,6 +62,7 @@ struct PackGrp {
 struct SlotHost {
   bool active = false;
   int prefill_len = 0, rope_delta = 0, n_left_pad = 0, max_new = 0, min_new = 0, trailing_len = 0;
+  bool text_open = false, text_closed = false;   // fq3_set_text_rows: rows may still follow / the caller closed the text
   const void* trailing = nullptr;
   const void* tts_pad = nullptr;
   const float* uniforms = nullptr;
@@ -783,6 +784,7 @@ static SlotParams slot_params(fq3_engine* e, int s, long long* codes_out) {
   p.codes_out = codes_out;
   p.prefill_len = h.prefill_len; p.rope_delta = h.rope_delta; p.n_left_pad = h.n_left_pad;
   p.max_new = h.max_new; p.min_new = h.min_new; p.trailing_len = h.trailing_len;
+  p.text_open = h.text_open ? 1 : 0;
   p.sp_t = h.sp_t; p.sp_p = h.sp_p;
   return p;
 }
@@ -910,6 +912,7 @@ extern "C" int fq3_begin_request(fq3_engine* e, int32_t slot, const fq3_request*
   h.prefill_len = rq->prefill_len; h.rope_delta = rq->rope_delta; h.n_left_pad = rq->n_left_pad;
   h.max_new = rq->max_new_tokens; h.min_new = rq->min_new_tokens; h.trailing_len = rq->trailing_len;
   h.trailing = trailing_text_dev; h.tts_pad = tts_pad_dev; h.uniforms = uniforms_dev;
+  h.text_open = false; h.text_closed = false;
   h.sp_t = to_sampling(sp_talker); h.sp_p = to_sampling(sp_predictor);
   int* st = e->state + 8 * slot;
   float* ph = e->past_hidden + (size_t)slot * HMAX;
@@ -919,6 +922,25 @@ extern "C" int fq3_begin_request(fq3_engine* e, int32_t slot, const fq3_request*
   e->launches++;
   CK(cudaGetLastError());
   h.active = true;
+  return 0;
+}
+
+extern "C" int fq3_set_text_rows(fq3_engine* e, int32_t slot, int32_t trailing_len, int32_t open) {
+  if (!e) return fail(FQ3_ERR_INVALID, "null argument");
+  int rc;
+  if ((rc = check_slot(e, slot))) return rc;
+  SlotHost& h = e->slots[slot];
+  if (!h.active) return fail(FQ3_ERR_STATE, "fq3_begin_request has not been called for slot %d", slot);
+  if (trailing_len < h.trailing_len)
+    return fail(FQ3_ERR_INVALID, "slot %d: trailing_len %d < %d (rows already announced cannot be withdrawn)", slot, trailing_len, h.trailing_len);
+  if (open && h.text_closed) return fail(FQ3_ERR_STATE, "slot %d: the text was closed and cannot be reopened", slot);
+  // a closed slot may already have fed tts_pad past its last row: a row announced now would follow the end of the text
+  if (h.text_closed && trailing_len != h.trailing_len)
+    return fail(FQ3_ERR_STATE, "slot %d: the text was closed at %d rows; trailing_len cannot grow to %d", slot, h.trailing_len, trailing_len);
+  if (trailing_len > 0 && !h.trailing) return fail(FQ3_ERR_INVALID, "slot %d: trailing_len > 0 but fq3_begin_request latched no trailing text", slot);
+  h.trailing_len = trailing_len;
+  h.text_open = open != 0;
+  h.text_closed = open == 0;
   return 0;
 }
 

@@ -30,11 +30,25 @@ class SlotRequest:
     frames: int = 0
     finished: int = 0
     parts: List[torch.Tensor] = field(default_factory=list)
+    feed: Optional[object] = None   # text_stream.TextFeed of a text-fed request (rows announced before every step)
+    gen0: int = 0                   # generation_step at begin: the next frame reads trailing row gen0 + frames
+    rows_ahead: int = 1             # text-fed: trailing rows that must exist beyond gen0 + frames before a launch
+
+    def ready(self) -> bool:
+        """A text-fed request is launched once the rows of its next ``rows_ahead`` frames exist (fewer where
+        max_new_tokens ends it first), once its text is closed, or once it has reached max_new_tokens (the launch then
+        reports it finished)."""
+        if self.feed is None or self.feed.closed or self.frames >= self.max_new_tokens:
+            return True
+        need = min(self.gen0 + self.frames + self.rows_ahead, self.gen0 + self.max_new_tokens)
+        return self.feed.n_rows >= need
 
 
 class BatchScheduler:
     """Owns the engine's slots: ``submit`` prefills one request into a free slot and latches it, ``step`` advances
-    every active slot by up to ``n_frames`` frames with ONE launch and returns the new codes per request."""
+    every ready slot by up to ``n_frames`` frames with ONE launch and returns the new codes per request, ``cancel``
+    frees a slot.  A text-fed request (``feed``) is ready while its next trailing row exists or its text is closed; a
+    slot that waits for text costs the others nothing."""
 
     def __init__(self, engine, talker, config, predictor_graph, talker_graph):
         self.engine, self.talker, self.config = engine, talker, config
@@ -51,8 +65,11 @@ class BatchScheduler:
     @torch.inference_mode()
     def submit(self, tie, tam, tth, tpe, *, tag=None, max_new_tokens: int = 2048, min_new_tokens: int = 2,
                temperature: float = 0.9, top_k: int = 50, top_p: float = 1.0, do_sample: bool = True,
-               repetition_penalty: float = 1.05, uniforms: Optional[torch.Tensor] = None) -> SlotRequest:
-        """One request: tie [1,P,H], tam [1,P] (zeros = left padding), tth [1,Tt,H], tpe [1,1,H]."""
+               repetition_penalty: float = 1.05, uniforms: Optional[torch.Tensor] = None, feed=None,
+               rows_ahead: int = 1) -> SlotRequest:
+        """One request: tie [1,P,H], tam [1,P] (zeros = left padding), tth [1,Tt,H], tpe [1,1,H].  ``feed``: a
+        ``text_stream.TextFeed`` whose row buffer replaces ``tth``; ``rows_ahead``: rows it must hold beyond the next
+        frame's before the slot is launched (``n_frames`` of the steps keeps every launch a full chunk)."""
         if not self.free:
             raise RuntimeError(f"all {self.engine.max_batch} request slots are busy")
         slot = self.free.pop(0)
@@ -60,21 +77,27 @@ class BatchScheduler:
             begin_fused(self.engine, self.talker, tie, tam, tth, tpe, self.config, self.pg, self.tg,
                         max_new_tokens=max_new_tokens, min_new_tokens=min_new_tokens, temperature=temperature,
                         top_k=top_k, top_p=top_p, do_sample=do_sample, repetition_penalty=repetition_penalty,
-                        uniforms=uniforms, slot=slot)
+                        uniforms=uniforms, slot=slot, trailing_len=None if feed is None else 0)
+            if feed is not None:
+                self.engine.set_text_rows(slot, feed.update(), open=not feed.closed)
         except Exception:
             self.free.insert(0, slot)
             raise
-        rq = SlotRequest(slot=slot, tag=tag if tag is not None else slot, max_new_tokens=max_new_tokens)
+        rq = SlotRequest(slot=slot, tag=tag if tag is not None else slot, max_new_tokens=max_new_tokens, feed=feed,
+                         gen0=self.engine.gen_step0[slot], rows_ahead=max(1, int(rows_ahead)))
         self.active[slot] = rq
         return rq
 
     @torch.inference_mode()
     def step(self, n_frames: int) -> List[Tuple[SlotRequest, torch.Tensor]]:
-        """Advance all active slots; returns [(request, codes [n,16])] for every slot that was active (n may be 0 for a
+        """Advance all ready slots; returns [(request, codes [n,16])] for every slot that was launched (n may be 0 for a
         slot that stopped before emitting).  Finished slots are released."""
-        if not self.active:
+        for rq in self.active.values():
+            if rq.feed is not None:
+                self.engine.set_text_rows(rq.slot, rq.feed.update(), open=not rq.feed.closed)
+        slots = sorted(s for s, rq in self.active.items() if rq.ready())
+        if not slots:
             return []
-        slots = sorted(self.active)
         if len(slots) == 1:
             codes, res = self.engine.decode_chunk(n_frames, slot=slots[0])
             outs, ress = [codes], [res]
@@ -91,6 +114,12 @@ class BatchScheduler:
                 del self.active[s]
                 self.free.append(s)
         return done
+
+    def cancel(self, rq: SlotRequest) -> None:
+        """End a request now and free its slot (a client that went away)."""
+        if self.active.get(rq.slot) is rq:
+            del self.active[rq.slot]
+            self.free.append(rq.slot)
 
 
 def _rows(x: torch.Tensor, b: int) -> torch.Tensor:

@@ -60,7 +60,7 @@ class ChunkResult(C.Structure):
 EXPORTS = [
     "fq3_engine_create", "fq3_engine_load_weights", "fq3_engine_destroy", "fq3_import_kv", "fq3_export_kv",
     "fq3_set_generation_state", "fq3_talker_step", "fq3_predictor_run", "fq3_sample_logits", "fq3_begin_request",
-    "fq3_decode_chunk", "fq3_get_past_hidden", "fq3_debug_enable", "fq3_debug_read", "fq3_tape_bytes",
+    "fq3_decode_chunk", "fq3_set_text_rows", "fq3_get_past_hidden", "fq3_debug_enable", "fq3_debug_read", "fq3_tape_bytes",
     "fq3_num_ctas", "fq3_launch_count", "fq3_last_error", "fq3_version", "fq3_engine_set_prefill_weights", "fq3_prefill", "fq3_max_batch", "fq3_debug_gemv",
     "fq3_codec_create", "fq3_codec_load_weights", "fq3_codec_flops",
     "fq3_codec_load_frontend", "fq3_codec_decode_codes", "fq3_codec_frontend_flops",
@@ -117,6 +117,7 @@ def load_library() -> C.CDLL:
                                       C.c_void_p, C.POINTER(Sampling), C.POINTER(Sampling), C.c_void_p]
     lib.fq3_decode_chunk.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_int32, C.c_void_p,
                                      C.POINTER(ChunkResult), C.c_void_p]
+    lib.fq3_set_text_rows.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32]
     lib.fq3_get_past_hidden.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
     lib.fq3_max_batch.argtypes = [C.c_void_p]
     lib.fq3_debug_gemv.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -213,6 +214,7 @@ class Engine:
         self.h = h
         self.H = talker["hidden_size"]
         self._keep = {}  # slot -> tensors borrowed by the engine for the duration of that slot's request
+        self.gen_step0 = {}  # slot -> generation_step latched by begin_request (frame s reads trailing row gen_step0 + s)
         self.loaded = False
         self.has_prefill = False
         self._prefill_keep = None
@@ -327,7 +329,9 @@ class Engine:
     def begin_request(self, *, first_token: int, prefill_len: int, gen_step: int, past_hidden: torch.Tensor,
                       trailing_text: torch.Tensor, tts_pad: torch.Tensor, max_new_tokens: int, min_new_tokens: int,
                       sp_talker: SamplingParams, sp_predictor: SamplingParams, uniforms: Optional[torch.Tensor],
-                      rope_delta: int = 0, n_left_pad: int = 0, slot: int = 0):
+                      rope_delta: int = 0, n_left_pad: int = 0, slot: int = 0, trailing_len: Optional[int] = None):
+        """``trailing_len``: rows of ``trailing_text`` valid now (default: all of them); the rest of the buffer is for rows
+        announced later through ``set_text_rows``."""
         ph = self._t(past_hidden.reshape(-1))
         tt = self._t(trailing_text.reshape(-1, self.H)) if trailing_text is not None and trailing_text.numel() else None
         tp = self._t(tts_pad.reshape(-1))
@@ -338,12 +342,30 @@ class Engine:
         if u is not None and u.numel() < (max_new_tokens + 1) * 16:
             raise ValueError("uniforms must have (max_new_tokens + 1) * 16 elements")
         self._keep[int(slot)] = dict(ph=ph, tt=tt, tp=tp, u=u)
+        cap = 0 if tt is None else tt.shape[0]
+        if trailing_len is not None and tt is not None and tt.data_ptr() != trailing_text.data_ptr():
+            # rows written after the latch must reach the kernel: the engine has to borrow the caller's buffer itself
+            raise ValueError("a trailing text buffer filled later must be a contiguous tensor of the engine's dtype on "
+                             "its device (it would be copied)")
+        n_rows = cap if trailing_len is None else int(trailing_len)
+        if not 0 <= n_rows <= cap:
+            raise ValueError(f"trailing_len {n_rows} outside the {cap} rows of trailing_text")
         rq = Request(int(first_token), int(prefill_len), int(gen_step), int(rope_delta), int(n_left_pad),
-                     int(max_new_tokens), int(min_new_tokens), 0 if tt is None else tt.shape[0])
+                     int(max_new_tokens), int(min_new_tokens), n_rows)
         st, spd = sp_talker.c(), sp_predictor.c()
         _check(self.lib, self.lib.fq3_begin_request(
             self.h, int(slot), C.byref(rq), ph.data_ptr(), tt.data_ptr() if tt is not None else None, tp.data_ptr(),
             u.data_ptr() if u is not None else None, C.byref(st), C.byref(spd), self._stream()))
+        self.gen_step0[int(slot)] = int(gen_step)
+
+    def set_text_rows(self, slot: int, trailing_len: int, open: bool):
+        """Rows [0, trailing_len) of the slot's latched trailing buffer are valid; ``open``: more may follow, and a frame
+        that would need a missing row waits for it (the launch stops the slot unfinished)."""
+        tt = self._keep.get(int(slot), {}).get("tt")
+        cap = 0 if tt is None else tt.shape[0]
+        if trailing_len > cap:
+            raise ValueError(f"trailing_len {trailing_len} exceeds the {cap} rows latched for slot {slot}")
+        _check(self.lib, self.lib.fq3_set_text_rows(self.h, int(slot), int(trailing_len), int(bool(open))))
 
     def decode_chunk(self, n_frames: int, out: Optional[torch.Tensor] = None, slot: int = 0) -> Tuple[torch.Tensor, ChunkResult]:
         """Single-sequence launch on one slot: (codes [frames_emitted,16], result)."""

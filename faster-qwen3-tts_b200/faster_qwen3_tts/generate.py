@@ -38,9 +38,11 @@ def _prefill(talker, tie, tam, tth, tpe):
 
 
 def begin_fused(engine, talker, tie, tam, tth, tpe, config, predictor_graph, talker_graph, *, max_new_tokens,
-                min_new_tokens, temperature, top_k, top_p, do_sample, repetition_penalty, uniforms, slot=None):
+                min_new_tokens, temperature, top_k, top_p, do_sample, repetition_penalty, uniforms, slot=None,
+                trailing_len=None):
     """Prefill + first token + request latch (generate.py:104-140) for ONE row [1,P,H] into request slot `slot`
-    (default: the slot the graph handles drive).  Returns the first token id."""
+    (default: the slot the graph handles drive).  ``trailing_len``: rows of ``tth`` valid now (text-fed requests latch
+    a larger buffer and announce rows later, ``Engine.set_text_rows``).  Returns the first token id."""
     eos_id = config.codec_eos_token_id
     slot = int(getattr(talker_graph, "slot", 0) if slot is None else slot)
     native = getattr(engine, "has_prefill", False) and getattr(talker_graph, "use_native_prefill", True) \
@@ -79,7 +81,8 @@ def begin_fused(engine, talker, tie, tam, tth, tpe, config, predictor_graph, tal
     engine.begin_request(first_token=int(first.item()), prefill_len=prefill_len, gen_step=gen_step,
                          past_hidden=out.past_hidden, trailing_text=tth, tts_pad=tpe, max_new_tokens=max_new_tokens,
                          min_new_tokens=min_new_tokens, sp_talker=sp_t, sp_predictor=predictor_graph.sampling(),
-                         uniforms=uniforms, rope_delta=rope_delta, n_left_pad=n_left_pad, slot=slot)
+                         uniforms=uniforms, rope_delta=rope_delta, n_left_pad=n_left_pad, slot=slot,
+                         trailing_len=trailing_len)
     return first
 
 

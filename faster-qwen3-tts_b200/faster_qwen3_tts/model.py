@@ -117,6 +117,8 @@ class _StatefulWindow:
     reference's Phase-1 output continued for the whole utterance; Phase-2 chunks of the reference differ slightly because
     they see only 25 frames of context.  ICL reference frames warm the stream's state up front; no audio is made for them."""
 
+    any_chunking = True   # the PCM of a stream does not depend on how its frames are split into chunks
+
     def __init__(self, owner, speech_tokenizer, ref_codes, chunk_size, to_host=True):
         self.st = speech_tokenizer
         self.stream = speech_tokenizer.open_stream()
@@ -788,6 +790,84 @@ class FasterQwen3TTS:
                                            max_new_tokens=max_new_tokens, min_new_tokens=min_new_tokens,
                                            temperature=temperature, top_k=top_k, top_p=top_p, do_sample=do_sample,
                                            repetition_penalty=repetition_penalty)
+
+    # ------------------------------------------------------------------ incremental text input (text_stream.py)
+    def _text_streaming(self, text_stream, language, speaker, instruct, voice_clone_prompt, non_streaming_mode,
+                        chunk_size, gen):
+        """The one implementation behind the three ``*_text_streaming`` methods."""
+        from .text_stream import _refuse_unsupported, generate_text_streaming
+        _refuse_unsupported(voice_clone_prompt, non_streaming_mode)
+        instruct_ids = None
+        if instruct:
+            instruct_ids = self.model._tokenize_texts([self.model._build_instruct_text(instruct)])[0]
+        yield from generate_text_streaming(self, text_stream, language=language, speaker=speaker,
+                                           instruct_ids=instruct_ids, voice_clone_prompt=voice_clone_prompt,
+                                           chunk_size=chunk_size, **gen)
+
+    @torch.inference_mode()
+    def generate_custom_voice_text_streaming(self, text_stream, speaker: str, language: str,
+                                             instruct: Optional[str] = None, non_streaming_mode: Optional[bool] = None,
+                                             max_new_tokens: int = 2048, min_new_tokens: int = 2,
+                                             temperature: float = 0.9, top_k: int = 50, top_p: float = 1.0,
+                                             do_sample: bool = True, repetition_penalty: float = 1.05,
+                                             chunk_size: int = 12) -> Generator[Tuple[np.ndarray, int, dict], None, None]:
+        """``generate_custom_voice_streaming`` with the text fed while it is spoken: ``text_stream`` is any iterable of
+        ``str`` pieces (an LLM's reply token by token).  The audio equals that of the one-shot streaming request for the
+        same text, whatever the split and however fast the pieces come; generation waits where the text has not arrived
+        yet.  Timing dicts add ``text_wait_ms``, the time spent blocked on ``text_stream``."""
+        self._require_type("custom_voice", "Loaded model does not support custom voice generation")
+        self._validate(language, speaker, check_speaker=True)
+        instruct = self._drop_instruct_for_small_model(instruct)
+        yield from self._text_streaming(text_stream, language, speaker, instruct, None, non_streaming_mode, chunk_size,
+                                        self._text_gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p,
+                                                              do_sample, repetition_penalty))
+
+    @torch.inference_mode()
+    def generate_voice_design_text_streaming(self, text_stream, instruct: str, language: str,
+                                             non_streaming_mode: Optional[bool] = None, max_new_tokens: int = 2048,
+                                             min_new_tokens: int = 2, temperature: float = 0.9, top_k: int = 50,
+                                             top_p: float = 1.0, do_sample: bool = True,
+                                             repetition_penalty: float = 1.05, chunk_size: int = 12
+                                             ) -> Generator[Tuple[np.ndarray, int, dict], None, None]:
+        """``generate_voice_design_streaming`` with the text fed while it is spoken (see
+        ``generate_custom_voice_text_streaming``)."""
+        self._require_type("voice_design", "Loaded model does not support voice design generation")
+        self._validate(language)
+        yield from self._text_streaming(text_stream, language, None, instruct, None, non_streaming_mode, chunk_size,
+                                        self._text_gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p,
+                                                              do_sample, repetition_penalty))
+
+    @torch.inference_mode()
+    def generate_voice_clone_text_streaming(self, text_stream, language: str, ref_audio=None, ref_text: str = "",
+                                            max_new_tokens: int = 2048, min_new_tokens: int = 2,
+                                            temperature: float = 0.9, top_k: int = 50, top_p: float = 1.0,
+                                            do_sample: bool = True, repetition_penalty: float = 1.05,
+                                            chunk_size: int = 12, xvec_only: bool = True,
+                                            non_streaming_mode: Optional[bool] = None, append_silence: bool = True,
+                                            ref_spk=None, ref_rvq=None, ref_spk_emb=None, ref_codes=None,
+                                            voice_clone_prompt=None) -> Generator[Tuple[np.ndarray, int, dict], None, None]:
+        """``generate_voice_clone_streaming`` with the text fed while it is spoken, x-vector cloning only: ICL cloning
+        puts the target text under the reference codec frames inside the prompt, so it must be known before prefill
+        (ValueError)."""
+        self._reject_ggml_cached_reference_args(ref_spk, ref_rvq, ref_spk_emb, ref_codes)
+        voice_clone_prompt = self._cached_reference_prompt(ref_spk_emb, ref_codes, voice_clone_prompt)
+        from .text_stream import ICL_REFUSAL, _refuse_unsupported
+        _refuse_unsupported(None, non_streaming_mode)
+        if voice_clone_prompt is None and not xvec_only:
+            raise ValueError(ICL_REFUSAL)
+        # one request: only the length of input_ids is read while a prompt is resolved
+        vcp, _, _ = self._resolve_voice_clone_prompt(
+            input_ids=[None], ref_audio=ref_audio, ref_text=ref_text, xvec_only=True, append_silence=append_silence,
+            voice_clone_prompt=voice_clone_prompt)
+        _refuse_unsupported(vcp, non_streaming_mode)
+        yield from self._text_streaming(text_stream, language, None, None, vcp, non_streaming_mode, chunk_size,
+                                        self._text_gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p,
+                                                              do_sample, repetition_penalty))
+
+    @staticmethod
+    def _text_gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p, do_sample, repetition_penalty):
+        return dict(max_new_tokens=max_new_tokens, min_new_tokens=min_new_tokens, temperature=temperature, top_k=top_k,
+                    top_p=top_p, do_sample=do_sample, repetition_penalty=repetition_penalty)
 
     def _log_rtf(self, timing):
         n = timing["steps"]

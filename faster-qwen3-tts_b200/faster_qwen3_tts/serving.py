@@ -60,6 +60,11 @@ class Ticket:
     submitted_at: float = field(default_factory=time.time)
     first_chunk_at: Optional[float] = None
     frames: int = 0
+    cancelled: threading.Event = field(default_factory=threading.Event)
+
+    def cancel(self) -> None:
+        """End the request: the worker frees its slot (or drops it from the queue) and closes the ticket."""
+        self.cancelled.set()
 
     def __iter__(self) -> Iterator:
         while True:
@@ -75,22 +80,52 @@ class Ticket:
         return np.concatenate(parts) if parts else np.zeros(0, dtype=np.float32)
 
 
+@dataclass
+class TextTicket(Ticket):
+    """Ticket of a text-fed request: ``write`` text pieces as they arrive (an LLM's reply), ``close`` when the text is
+    complete.  Both are safe to call from any thread; the worker commits, embeds and announces the rows.  A client that
+    goes away before ``close`` must ``cancel``, or the request keeps its slot waiting for text."""
+    feed: Optional[object] = None
+    _pieces: List[str] = field(default_factory=list)
+    _closed: bool = False
+    _text_lock: threading.Lock = field(default_factory=threading.Lock)
+
+    def write(self, piece: str) -> None:
+        with self._text_lock:
+            if self._closed:
+                raise RuntimeError("text already closed")
+            self._pieces.append(piece)
+
+    def close(self) -> None:
+        with self._text_lock:
+            self._closed = True
+
+    def _take(self):
+        with self._text_lock:
+            pieces, self._pieces = self._pieces, []
+            return pieces, self._closed
+
+
 class ContinuousBatcher:
     """One worker thread, many clients.  ``scheduler_factory()`` -> object with ``has_capacity()``,
     ``submit(tie, tam, tth, tpe, tag=..., **gen) -> request``, ``step(n) -> [(request, codes)]`` and ``__len__`` (the
     ``BatchScheduler`` of batching.py); ``window_factory(ref_codes)`` -> object with ``push(codes) -> (pcm, sr)``
-    (``model._StreamWindow``)."""
+    (``model._StreamWindow``); ``feed_factory(max_rows)`` -> ``text_stream.TextFeed`` (text-fed requests)."""
 
     def __init__(self, scheduler, window_factory: Callable, chunk_size: int = 8, idle_sleep: float = 0.002,
-                 batch_decode: Optional[Callable] = None):
+                 batch_decode: Optional[Callable] = None, feed_factory: Optional[Callable] = None):
         self.sched, self.window_factory, self.chunk_size = scheduler, window_factory, chunk_size
         self.batch_decode = batch_decode   # (windows, code chunks) -> [(pcm, sr)]: one codec batch per window length
         self.idle_sleep = idle_sleep
         self.pending: "queue.Queue[Ticket]" = queue.Queue()
         self.live: Dict[int, tuple] = {}     # rid -> (ticket, window)
+        self.feed_factory = feed_factory
+        self.waiting: List[TextTicket] = []  # text-fed tickets whose first text id is not committed yet
+        self.requests: Dict[int, object] = {}   # rid -> scheduler request
         self._rid = 0
         self._lock = threading.Lock()
         self._stop = threading.Event()
+        self._queued: List[Ticket] = []      # ordinary tickets taken from `pending`, waiting for a slot
         self.steps = 0
         self.max_concurrent = 0
         self._thread = threading.Thread(target=self._run, name="fq3-batcher", daemon=True)
@@ -104,24 +139,93 @@ class ContinuousBatcher:
         self.pending.put(t)
         return t
 
+    def submit_text(self, prepare: Callable, **gen_kwargs) -> TextTicket:
+        """A text-fed request.  ``prepare(feed)`` -> (tie, tam, tpe, ref_codes) builds the prompt once the feed holds its
+        first committed id (``text_stream.TextFeed.prompt_ids``); it runs on the worker thread."""
+        if self.feed_factory is None:
+            raise RuntimeError("this batcher has no text feed factory")
+        with self._lock:
+            self._rid += 1
+            t = TextTicket(self._rid, prepare, gen_kwargs)
+        t.feed = self.feed_factory(int(gen_kwargs.get("max_new_tokens", 2048)))
+        self.pending.put(t)
+        return t
+
     def close(self):
         self._stop.set()
         self._thread.join(timeout=10)
 
     # ---- worker -----------------------------------------------------------------------------------------
+    @staticmethod
+    def _fail(t: Ticket, ex: BaseException):
+        t.out.put(ex)
+        t.out.put(_DONE)
+
+    def _drain_text(self):
+        """commit the text written since the last step (rows are embedded and announced by the scheduler's step)"""
+        for t in self.waiting + [t for t, _ in self.live.values() if isinstance(t, TextTicket)]:
+            pieces, closed = t._take()
+            try:
+                if pieces:   # one commit per drained batch: each commit re-tokenizes the text received so far
+                    t.feed.push("".join(pieces))
+                if closed and not t.feed.closed:
+                    t.feed.close()
+            except BaseException as ex:
+                t.cancel()
+                self._fail(t, ex)
+
+    def _reap_cancelled(self):
+        for t in [t for t in self.waiting if t.cancelled.is_set()]:
+            self.waiting.remove(t)
+            t.out.put(_DONE)
+        for rid, (t, _) in list(self.live.items()):
+            if t.cancelled.is_set():
+                self.sched.cancel(self.requests.pop(rid))
+                del self.live[rid]
+                t.out.put(_DONE)
+
+    def _start(self, t: Ticket):
+        if isinstance(t, TextTicket):
+            tie, tam, tpe, ref_codes = t.prepare(t.feed)
+            win = self.window_factory(ref_codes)
+            # a window whose audio depends on the chunking (the reference's window policy) must see the one-shot
+            # chunking: the slot is launched only when a full chunk of text rows exists, so every launch emits a full
+            # chunk or ends the request.  A stateful stream decodes to the same PCM in any chunking: one row suffices.
+            ahead = 1 if getattr(win, "any_chunking", False) else self.chunk_size
+            rq = self.sched.submit(tie, tam, t.feed.rows[None], tpe, tag=t.rid, feed=t.feed, rows_ahead=ahead,
+                                   **t.gen_kwargs)
+        else:
+            tie, tam, tth, tpe, ref_codes = t.prepare()
+            win = self.window_factory(ref_codes)
+            rq = self.sched.submit(tie, tam, tth, tpe, tag=t.rid, **t.gen_kwargs)
+        self.requests[t.rid] = rq
+        self.live[t.rid] = (t, win)
+
     def _admit(self):
-        while self.sched.has_capacity():
+        while True:
             try:
                 t = self.pending.get_nowait()
             except queue.Empty:
+                break
+            if isinstance(t, TextTicket):
+                self.waiting.append(t)
+            else:
+                self._queued.append(t)
+        self._reap_cancelled()
+        self._drain_text()
+        for t in [t for t in self._queued if t.cancelled.is_set()]:
+            self._queued.remove(t)
+            t.out.put(_DONE)
+        # text-fed requests enter once their first id is committed (the prompt holds it), in arrival order
+        ready = sorted([t for t in self.waiting if t.feed.n_ids] + self._queued, key=lambda t: t.rid)
+        for t in ready:
+            if not self.sched.has_capacity():
                 return
+            (self.waiting if isinstance(t, TextTicket) else self._queued).remove(t)
             try:
-                tie, tam, tth, tpe, ref_codes = t.prepare()
-                self.sched.submit(tie, tam, tth, tpe, tag=t.rid, **t.gen_kwargs)
-                self.live[t.rid] = (t, self.window_factory(ref_codes))
+                self._start(t)
             except BaseException as ex:   # a bad request must not take the worker down
-                t.out.put(ex)
-                t.out.put(_DONE)
+                self._fail(t, ex)
 
     def _run(self):
         while not self._stop.is_set():
@@ -137,6 +241,9 @@ class ContinuousBatcher:
                     t.out.put(ex)
                     t.out.put(_DONE)
                 self.live.clear()
+                continue
+            if not results:   # every active request is waiting for text
+                time.sleep(self.idle_sleep)
                 continue
             self.steps += 1
             live = [(rq, codes) for rq, codes in results if int(codes.shape[0])]
@@ -159,6 +266,7 @@ class ContinuousBatcher:
                 if rq.finished:
                     t.out.put(_DONE)
                     del self.live[rq.tag]
+                    self.requests.pop(rq.tag, None)
 
 
 def batcher_for_model(model, chunk_size: int = 8, to_host: bool = True) -> ContinuousBatcher:
@@ -177,7 +285,24 @@ def batcher_for_model(model, chunk_size: int = 8, to_host: bool = True) -> Conti
         return model._make_window(st, ref_codes, chunk_size, to_host) if st is not None else _CodesOnly()
 
     bd = (lambda wins, chunks: decode_windows_batched(st, wins, chunks)) if st is not None else None
-    return ContinuousBatcher(sched, window, chunk_size=chunk_size, batch_decode=bd)
+    from .text_stream import TextFeed
+    return ContinuousBatcher(sched, window, chunk_size=chunk_size, batch_decode=bd,
+                             feed_factory=lambda max_rows: TextFeed(model, max_rows))
+
+
+def custom_voice_text_request(model, speaker: str, language: str, instruct: Optional[str] = None):
+    """``prepare`` callable for ``ContinuousBatcher.submit_text``: the prompt of a text-fed custom-voice request, built
+    from the feed's first committed id exactly like ``generate_custom_voice_text_streaming`` builds it."""
+    from .text_stream import build_prompt
+    model._require_type("custom_voice", "Loaded model does not support custom voice generation")
+    model._validate(language, speaker, check_speaker=True)
+    instruct = model._drop_instruct_for_small_model(instruct)
+
+    def prepare(feed):
+        ins = model.model._tokenize_texts([model.model._build_instruct_text(instruct)])[0] if instruct else None
+        tie, tam, tpe = build_prompt(model, feed, language=language, speaker=speaker, instruct_ids=ins)
+        return tie, tam, tpe, None
+    return prepare
 
 
 def voice_clone_request(model, text: str, language: str, ref_audio, ref_text: str = "", xvec_only: bool = False,

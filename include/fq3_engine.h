@@ -105,6 +105,9 @@ typedef struct {
 /* Why the on-device loop stopped (generate.py:149-151,175-177 and the for-range bound). */
 enum fq3_finish { FQ3_RUNNING = 0, FQ3_FIN_MAX_NEW = 1, FQ3_FIN_EOS = 2, FQ3_FIN_MAX_SEQ = 3 };
 
+/* A slot whose text is open (fq3_set_text_rows) stops at the frame that would read trailing row >= trailing_len, with
+ * finished == FQ3_RUNNING: after a launch, finished == FQ3_RUNNING && frames_emitted < n_frames means "waiting for text".
+ * The slot's state is then exactly what it is at an n_frames boundary, so the next launch resumes it unchanged. */
 typedef struct {
   int32_t frames_emitted;   /* frames written by the last fq3_decode_chunk */
   int32_t finished;         /* fq3_finish */
@@ -169,6 +172,19 @@ int fq3_prefill(fq3_engine* e, int32_t slot, const void* embeds_dev, int32_t P, 
 int fq3_begin_request(fq3_engine* e, int32_t slot, const fq3_request* rq, const void* past_hidden_dev,
                       const void* trailing_text_dev, const void* tts_pad_dev, const float* uniforms_dev,
                       const fq3_sampling* sp_talker, const fq3_sampling* sp_predictor, void* stream);
+/* Incremental text input (the step-by-step text layout: frame s adds trailing row s to the talker input, tts_pad once
+ * the rows run out).  Announces that rows [0, trailing_len) of the buffer latched by fq3_begin_request are valid, and
+ * whether more may follow (open != 0).  While open, a frame that would read row >= trailing_len is not run: the slot
+ * stops there (see fq3_chunk_result) instead of feeding tts_pad, which would tell the model the text has ended, so a
+ * text-fed request sees exactly the inputs of the same request with all rows latched at once.  open == 0 closes the
+ * text: from then on the slot behaves like any other request, and its trailing_len is final (it may already have fed
+ * tts_pad past it).  fq3_begin_request resets the slot to closed-as-latched.
+ * Legal after fq3_begin_request and between launches.  The caller must have latched a buffer that holds every row it
+ * will ever announce, and writes new rows stream-ordered before the next fq3_decode_chunk on the same stream.
+ * Refused: inactive slot (FQ3_ERR_STATE), trailing_len smaller than before (FQ3_ERR_INVALID), open after a close
+ * (FQ3_ERR_STATE), a different trailing_len after a close (FQ3_ERR_STATE), trailing_len > 0 without a latched buffer
+ * (FQ3_ERR_INVALID). */
+int fq3_set_text_rows(fq3_engine* e, int32_t slot, int32_t trailing_len, int32_t open);
 /* generate.py:149-199 / streaming.py:106-173 for up to n_frames frames of every listed slot in ONE kernel launch.
  * slots[n_slots] distinct slot ids that have a latched request; codes_out_dev int64 [n_slots][n_frames][16];
  * res[n_slots] (host).  n_slots == 1: single-sequence kernel; n_slots >= 2: batched kernel, the slots advance in
