@@ -1069,3 +1069,27 @@ extern "C" int fq3_max_batch(fq3_engine* e) { return e ? e->max_batch : 0; }
 extern "C" const char* fq3_version(void) { return "fq3-h100 0.2.0 (sm_90a)"; }
 
 #include "fq3_prefill.cuh"
+
+// numerics probe: ONE launch of the dense-layer GEMM of K3 / K4 with the caller's arguments, unchanged.  Refused here:
+// only what would make the kernel divide by zero or dereference a missing parameter array, and operands the SwiGLU
+// epilogue would silently ignore.  Every shape and alignment rule is the kernel's own (fq3gemm::gemm refuses before it
+// launches anything).
+extern "C" int fq3_debug_conv_gemm(const fq3_conv_probe* p, void* stream) {
+  if (!p || !p->X || !p->W) return fail(FQ3_ERR_INVALID, "null argument");
+  if (p->T < 1 || p->Cin < 1 || p->N < 1 || p->taps < 1 || p->dil < 1 || p->batch < 0 || p->x_row0 < 0 || p->x_rows < 0)
+    return fail(FQ3_ERR_INVALID, "T, Cin, N, taps and dil must be positive; batch, x_row0 and x_rows non-negative");
+  if (p->mode < 0 || p->mode > 2) return fail(FQ3_ERR_INVALID, "mode must be 0 (general), 1 (SwiGLU) or 2 (GELU)");
+  if (!p->Yraw && !p->Yact) return fail(FQ3_ERR_INVALID, "no output");
+  if (p->mode == 1 && (p->Yact || p->R || p->bias || p->scale)) return fail(FQ3_ERR_INVALID, "the SwiGLU epilogue writes Yraw only");
+  if ((p->bias && p->bias_mod < 1) || (p->scale && p->scale_mod < 1)) return fail(FQ3_ERR_INVALID, "bias_mod / scale_mod < 1");
+  if (p->Yact && (!p->ea || !p->ib || p->act_mod < 1)) return fail(FQ3_ERR_INVALID, "Yact needs ea, ib and act_mod >= 1");
+  fq3gemm::ConvArgs a;
+  memset(&a, 0, sizeof(a));
+  a.X = (const __nv_bfloat16*)p->X; a.W = (const __nv_bfloat16*)p->W; a.bias = p->bias; a.R = (const __nv_bfloat16*)p->R;
+  a.Yraw = (__nv_bfloat16*)p->Yraw; a.Yact = (__nv_bfloat16*)p->Yact; a.ea = p->ea; a.ib = p->ib; a.scale = p->scale;
+  a.T = p->T; a.Cin = p->Cin; a.N = p->N; a.taps = p->taps; a.dil = p->dil; a.mode = p->mode;
+  a.bias_mod = p->bias ? p->bias_mod : 1; a.act_mod = p->Yact ? p->act_mod : 1; a.scale_mod = p->scale ? p->scale_mod : 1;
+  a.x_row0 = p->x_row0; a.x_rows = p->x_rows; a.batch = p->batch;
+  if (const char* err = fq3gemm::gemm(a, (cudaStream_t)stream)) return fail(FQ3_ERR_CUDA, "conv GEMM: %s", err);
+  return 0;
+}

@@ -52,6 +52,14 @@ class Request(C.Structure):
                 ("min_new_tokens", C.c_int32), ("trailing_len", C.c_int32)]
 
 
+class ConvProbe(C.Structure):
+    _fields_ = [("X", C.c_void_p), ("W", C.c_void_p), ("bias", C.c_void_p), ("R", C.c_void_p), ("Yraw", C.c_void_p),
+                ("Yact", C.c_void_p), ("ea", C.c_void_p), ("ib", C.c_void_p), ("scale", C.c_void_p),
+                ("T", C.c_int32), ("Cin", C.c_int32), ("N", C.c_int32), ("taps", C.c_int32), ("dil", C.c_int32),
+                ("mode", C.c_int32), ("bias_mod", C.c_int32), ("act_mod", C.c_int32), ("scale_mod", C.c_int32),
+                ("x_row0", C.c_int32), ("x_rows", C.c_int32), ("batch", C.c_int32)]
+
+
 class ChunkResult(C.Structure):
     _fields_ = [("frames_emitted", C.c_int32), ("finished", C.c_int32), ("total_frames", C.c_int32),
                 ("next_token", C.c_int32)]
@@ -62,6 +70,7 @@ EXPORTS = [
     "fq3_set_generation_state", "fq3_talker_step", "fq3_predictor_run", "fq3_sample_logits", "fq3_begin_request",
     "fq3_decode_chunk", "fq3_set_text_rows", "fq3_get_past_hidden", "fq3_debug_enable", "fq3_debug_read", "fq3_tape_bytes",
     "fq3_num_ctas", "fq3_launch_count", "fq3_last_error", "fq3_version", "fq3_engine_set_prefill_weights", "fq3_prefill", "fq3_max_batch", "fq3_debug_gemv",
+    "fq3_debug_conv_gemm",
     "fq3_codec_create", "fq3_codec_load_weights", "fq3_codec_flops",
     "fq3_codec_load_frontend", "fq3_codec_decode_codes", "fq3_codec_frontend_flops",
     "fq3_codec_stream_create", "fq3_codec_stream_reset", "fq3_codec_stream_destroy", "fq3_codec_stream_frames",
@@ -121,6 +130,7 @@ def load_library() -> C.CDLL:
     lib.fq3_get_past_hidden.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
     lib.fq3_max_batch.argtypes = [C.c_void_p]
     lib.fq3_debug_gemv.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.fq3_debug_conv_gemm.argtypes = [C.POINTER(ConvProbe), C.c_void_p]
     lib.fq3_debug_enable.argtypes = [C.c_void_p, C.c_int32]
     lib.fq3_debug_read.argtypes = [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p]
     lib.fq3_tape_bytes.argtypes = [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
@@ -165,6 +175,44 @@ def _check(lib, rc: int):
         if rc == -4:
             raise RuntimeError(msg)  # same type/message as talker_graph.py:163-167
         raise EngineError(f"fq3 error {rc}: {msg}")
+
+
+def debug_conv_gemm(X: torch.Tensor, W: torch.Tensor, *, mode: int = 0, dil: int = 1, T: Optional[int] = None,
+                    bias: Optional[torch.Tensor] = None, scale: Optional[torch.Tensor] = None,
+                    R: Optional[torch.Tensor] = None, ea: Optional[torch.Tensor] = None, ib: Optional[torch.Tensor] = None,
+                    raw: bool = True, act: bool = False, x_row0: int = 0,
+                    history: bool = False) -> Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]:
+    """One launch of the dense-layer GEMM of the prefill and the codec (numerics probe, fq3_debug_conv_gemm).
+    X bf16 [batch, rows, Cin] (or [rows, Cin]); W bf16 [N, taps, Cin]; bias / scale / ea / ib float32 (column n reads
+    element n % numel); R bf16 [batch, T, N].  With ``history`` the rows of X are [history ; new]: output row m reads
+    input rows x_row0 + m - shift and ``T`` new rows are produced; otherwise T = rows.  Returns (Yraw, Yact) as bf16
+    [batch, T, N] (Yraw [batch, T, N/2] in mode 1), None where not requested.  Operands are passed as they are, so an
+    unaligned view reaches the kernel's own check; they must be contiguous CUDA tensors of the stated dtype."""
+    def ptr(t, dtype, name):
+        if t is None:
+            return None
+        if not (t.is_cuda and t.dtype == dtype and t.is_contiguous()):
+            raise ValueError(f"{name} must be a contiguous CUDA {dtype} tensor")
+        return t.data_ptr()
+    lib = load_library()
+    X3 = X if X.dim() == 3 else X[None]
+    batch, rows, Cin = X3.shape
+    N, taps = W.shape[0], W.shape[1]
+    if W.shape[2] != Cin:
+        raise ValueError("W must be [N, taps, Cin]")
+    T = rows if T is None else int(T)
+    dev = X.device
+    Yraw = torch.empty(batch, T, N // 2 if mode == 1 else N, dtype=torch.bfloat16, device=dev) if raw else None
+    Yact = torch.empty(batch, T, N, dtype=torch.bfloat16, device=dev) if act else None
+    p = ConvProbe(ptr(X, torch.bfloat16, "X"), ptr(W, torch.bfloat16, "W"), ptr(bias, torch.float32, "bias"),
+                  ptr(R, torch.bfloat16, "R"), ptr(Yraw, torch.bfloat16, "Yraw"), ptr(Yact, torch.bfloat16, "Yact"),
+                  ptr(ea, torch.float32, "ea"), ptr(ib, torch.float32, "ib"), ptr(scale, torch.float32, "scale"),
+                  T, Cin, N, taps, int(dil), int(mode), bias.numel() if bias is not None else 1,
+                  ea.numel() if ea is not None else 1, scale.numel() if scale is not None else 1,
+                  int(x_row0), rows if history else 0, batch)
+    with torch.cuda.device(dev):
+        _check(lib, lib.fq3_debug_conv_gemm(C.byref(p), C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+    return Yraw, Yact
 
 
 @dataclass

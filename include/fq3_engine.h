@@ -210,6 +210,32 @@ int fq3_tape_bytes(fq3_engine* e, int64_t* talker_step_bytes, int64_t* predictor
 int fq3_num_ctas(fq3_engine* e);
 /* number of kernels launched by this engine since creation (bench.py "gpu_launches") */
 int64_t fq3_launch_count(fq3_engine* e);
+/* numerics probe of the dense-layer GEMM shared by K3 and K4 (fq3gemm::gemm, csrc/fq3_gemm.cuh: implicit-GEMM causal
+ * conv1d, taps = 1 is a linear layer, and its fused epilogues); needs no engine.  One launch with exactly these
+ * arguments; the fields mirror fq3gemm::ConvArgs.  Device pointers: X bf16 [batch][x_rows, or T when x_rows == 0][Cin];
+ * W bf16 [N][taps][Cin]; bias fp32 [bias_mod] or NULL; scale fp32 [scale_mod] or NULL; R bf16 [batch][T][N] or NULL;
+ * Yraw bf16 [batch][T][N] (mode 1: [batch][T][N/2]) or NULL; Yact bf16 [batch][T][N] (SnakeBeta of Yraw) or NULL;
+ * ea / ib fp32 [act_mod] (exp(alpha), 1 / (exp(beta) + 1e-9)), read when Yact is set.  batch 0 or 1 = one sequence.
+ * A shape or alignment the kernel refuses (Cin % 32, N % 8, SwiGLU N % 32, 16-byte operands) returns FQ3_ERR_CUDA with
+ * the kernel's message and launches nothing; a missing output or parameter array, a non-positive size or (mode 1) an
+ * operand the SwiGLU epilogue ignores returns FQ3_ERR_INVALID. */
+typedef struct {
+  const void* X;
+  const void* W;
+  const float* bias;
+  const void* R;
+  void* Yraw;
+  void* Yact;
+  const float* ea;
+  const float* ib;
+  const float* scale;
+  int32_t T, Cin, N, taps, dil;
+  int32_t mode;             /* 0 general, 1 SwiGLU on (gate, up) column pairs, 2 general with exact GELU */
+  int32_t bias_mod, act_mod, scale_mod;   /* column n reads bias[n % bias_mod], ea / ib [n % act_mod], scale[n % scale_mod] */
+  int32_t x_row0, x_rows;   /* output row m of a sequence reads input rows x_row0 + m - shift, zero outside [0, x_rows) */
+  int32_t batch;
+} fq3_conv_probe;
+int fq3_debug_conv_gemm(const fq3_conv_probe* p, void* stream);
 
 /* ---- K4: codec decoder (replaces the cuDNN path under speech_tokenizer.decode, model.py:924,1093,1122)
  * geom = {device, hidden_size, decoder_dim, n_blocks, rate_0..rate_{n-1}}; hidden_size and decoder_dim >> n_blocks must
