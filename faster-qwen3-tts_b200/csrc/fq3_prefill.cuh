@@ -7,27 +7,54 @@
 // causal GQA attention (eager semantics: bf16 scores, fp32 softmax rounded to bf16, bf16 P.V) -> o_proj GEMM with
 // fused residual -> RMSNorm rows -> gate/up GEMM with fused SwiGLU (interleaved columns) -> down GEMM with fused
 // residual.  GEMMs are the shared implicit-GEMM tensor-core kernel (fq3gemm::gemm, taps = 1).
+//
+// Several prompts go through one chain (fq3_prefill_batch; fq3_prefill is its n = 1 case): their rows are packed
+// row-major, [sum P_b][H], and the norms and GEMMs run on the packed rows as they are -- a row's result does not depend
+// on the rows next to it.  RoPE / KV append and the attention read the sequence table (by value, in the kernel
+// parameters) to map a packed row or a query block back to its sequence.  The attention's query blocks and key tiles
+// are aligned to each sequence's own row 0 and cache row 0, so every sequence sees exactly the tiles, masks and
+// online-softmax order of a launch with that sequence alone: the batch is bit-identical to one prefill per sequence.
 #pragma once
 #include "fq3_gemm.cuh"
 
 namespace pf {
 
+constexpr int MAXSEQ = 32;   // sequences of one chain (= the engine's request slots)
+
+struct SeqTab {
+  int n;                 // sequences
+  int row0[MAXSEQ];      // packed row of the sequence's row 0
+  int P[MAXSEQ];         // prompt rows
+  int pad[MAXSEQ];       // left pad (keys below it are masked, RoPE position = t - pad)
+  int slot[MAXSEQ];      // request slot whose KV cache receives rows [0, P)
+  int qb0[MAXSEQ + 1];   // first 32-query block of the sequence in the attention grid; qb0[n] = all blocks
+};
+
+// the sequence holding packed row r / attention block x (n <= 32: a scan of the parameter table)
+__device__ __forceinline__ int seq_of_row(const SeqTab& tab, int r) {
+  int b = 0;
+  while (b + 1 < tab.n && r >= tab.row0[b + 1]) ++b;
+  return b;
+}
+__device__ __forceinline__ int seq_of_qblock(const SeqTab& tab, int x) {
+  int b = 0;
+  while (b + 1 < tab.n && x >= tab.qb0[b + 1]) ++b;
+  return b;
+}
+
 __device__ __forceinline__ float rb(float x) { return __bfloat162float(__float2bfloat16_rn(x)); }
 
-// one block (256 threads) per row: Y = w * rnd(x * rsqrt(mean(x^2) + eps))
-__global__ void rmsnorm_rows_kernel(const __nv_bfloat16* __restrict__ X, const __nv_bfloat16* __restrict__ w, int H,
-                                    float eps, __nv_bfloat16* __restrict__ Y) {
+// one block (256 threads) per row: y = w * rnd(x * rsqrt(mean(x^2) + eps))
+__device__ __forceinline__ void rmsnorm_row(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ w, int H,
+                                            float eps, __nv_bfloat16* __restrict__ y) {
   __shared__ float red[8];
-  fq3gemm::pdl_launch();
-  fq3gemm::pdl_wait();
-  const size_t row = blockIdx.x;
   const int tid = threadIdx.x;
   float v[8];
   float ss = 0.f;
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
     const int k = tid + i * 256;
-    v[i] = k < H ? __bfloat162float(X[row * H + k]) : 0.f;
+    v[i] = k < H ? __bfloat162float(x[k]) : 0.f;
     ss += v[i] * v[i];
   }
 #pragma unroll
@@ -41,24 +68,45 @@ __global__ void rmsnorm_rows_kernel(const __nv_bfloat16* __restrict__ X, const _
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
     const int k = tid + i * 256;
-    if (k < H) Y[row * H + k] = __float2bfloat16_rn(__bfloat162float(w[k]) * rb(v[i] * r));
+    if (k < H) y[k] = __float2bfloat16_rn(__bfloat162float(w[k]) * rb(v[i] * r));
   }
 }
 
-// one warp per (token, vector) with vector in [q heads | k heads | v heads]: q/k RMSNorm + RoPE in place (q) or into
-// the KV cache (k, v).  QKV is [P][qd + 2 kd] bf16.
-__global__ void rope_kv_kernel(__nv_bfloat16* __restrict__ QKV, int P, int nH, int nKV, const __nv_bfloat16* qn,
+// Y[row] = norm(X[row]) for every packed row
+__global__ void rmsnorm_rows_kernel(const __nv_bfloat16* __restrict__ X, const __nv_bfloat16* __restrict__ w, int H,
+                                    float eps, __nv_bfloat16* __restrict__ Y) {
+  fq3gemm::pdl_launch();
+  fq3gemm::pdl_wait();
+  const size_t row = blockIdx.x;
+  rmsnorm_row(X + row * H, w, H, eps, Y + row * H);
+}
+
+// Y[b] = norm(last row of sequence b): the final norm, whose rows feed the head GEMM (M = n) and past_hidden
+__global__ void rmsnorm_last_rows_kernel(const __nv_bfloat16* __restrict__ X, const __nv_bfloat16* __restrict__ w, int H,
+                                         float eps, __nv_bfloat16* __restrict__ Y, const __grid_constant__ SeqTab tab) {
+  fq3gemm::pdl_launch();
+  fq3gemm::pdl_wait();
+  const int b = blockIdx.x;
+  rmsnorm_row(X + (size_t)(tab.row0[b] + tab.P[b] - 1) * H, w, H, eps, Y + (size_t)b * H);
+}
+
+// one warp per (packed row, vector) with vector in [q heads | k heads | v heads]: q/k RMSNorm + RoPE in place (q) or
+// into the KV cache of the row's sequence at its cache row t (k, v).  QKV is [rows][qd + 2 kd] bf16; kc / vc are one
+// layer of slot 0's caches, slot s starting `slot_stride` elements further.
+__global__ void rope_kv_kernel(__nv_bfloat16* __restrict__ QKV, int rows, int nH, int nKV, const __nv_bfloat16* qn,
                                const __nv_bfloat16* kn, const float* __restrict__ cosT, const float* __restrict__ sinT,
-                               int npos, int n_left_pad, float eps, __nv_bfloat16* __restrict__ kc,
-                               __nv_bfloat16* __restrict__ vc, int S) {
+                               int npos, float eps, __nv_bfloat16* __restrict__ kc, __nv_bfloat16* __restrict__ vc,
+                               size_t slot_stride, int S, const __grid_constant__ SeqTab tab) {
   fq3gemm::pdl_launch();
   fq3gemm::pdl_wait();
   const int gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   const int nvec = nH + 2 * nKV;
-  if (gw >= P * nvec) return;
-  const int t = gw / nvec, vi = gw % nvec;
+  if (gw >= rows * nvec) return;
+  const int row = gw / nvec, vi = gw % nvec;
+  const int sq = seq_of_row(tab, row);
+  const int t = row - tab.row0[sq], n_left_pad = tab.pad[sq];
   const int ld = (nH + 2 * nKV) * 128;
-  __nv_bfloat16* src = QKV + (size_t)t * ld + (size_t)vi * 128;
+  __nv_bfloat16* src = QKV + (size_t)row * ld + (size_t)vi * 128;
   float v[4];
 #pragma unroll
   for (int i = 0; i < 4; ++i) v[i] = __bfloat162float(src[lane + 32 * i]);
@@ -89,7 +137,7 @@ __global__ void rope_kv_kernel(__nv_bfloat16* __restrict__ QKV, int P, int nH, i
     for (int i = 0; i < 4; ++i) src[lane + 32 * i] = __float2bfloat16_rn(v[i]);
   } else {
     const int g = what == 1 ? vi - nH : vi - nH - nKV;
-    __nv_bfloat16* dst = (what == 1 ? kc : vc) + ((size_t)g * S + t) * 128;
+    __nv_bfloat16* dst = (what == 1 ? kc : vc) + (size_t)tab.slot[sq] * slot_stride + ((size_t)g * S + t) * 128;
 #pragma unroll
     for (int i = 0; i < 4; ++i) dst[lane + 32 * i] = __float2bfloat16_rn(v[i]);
   }
@@ -102,7 +150,9 @@ __global__ void rope_kv_kernel(__nv_bfloat16* __restrict__ QKV, int P, int nH, i
 // scores are rounded to bf16, scaled and rounded again; probabilities enter P.V as bf16; the output is bf16.  The
 // softmax is the online (running max / running sum) form in fp32, i.e. probabilities are rounded relative to the
 // running maximum instead of the final one -- within the bf16 envelope the parity test states.
-//   grid = (ceil(P / 32), nKV); keys below n_left_pad are masked; rows below n_left_pad produce zeros.
+//   grid = (tab.qb0[tab.n], nKV): blockIdx.x is query block qb of sequence b, qb0[b] + qb, whose rows are counted
+//   from the sequence's row 0 and whose key tiles from its cache row 0 -- the tiles of a launch with b alone.  Keys
+//   below the sequence's pad are masked; rows below it produce zeros.
 // ------------------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void ldsm_x4(uint32_t& a, uint32_t& b, uint32_t& c, uint32_t& d, const void* p) {
   asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
@@ -124,24 +174,29 @@ __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
 }
 
 template <int REP>
-__global__ void __launch_bounds__(128) attn_prefill_mma_kernel(const __nv_bfloat16* __restrict__ QKV, int P, int nH, int nKV,
+__global__ void __launch_bounds__(128) attn_prefill_mma_kernel(const __nv_bfloat16* __restrict__ QKVp, int nH, int nKV,
                                                               const __nv_bfloat16* __restrict__ kc,
-                                                              const __nv_bfloat16* __restrict__ vc, int S, int n_left_pad,
-                                                              __nv_bfloat16* __restrict__ OUT) {
+                                                              const __nv_bfloat16* __restrict__ vc, size_t slot_stride,
+                                                              int S, __nv_bfloat16* __restrict__ OUTp,
+                                                              const __grid_constant__ SeqTab tab) {
   constexpr int KT = 32;                                   // keys per staged tile
   __shared__ __align__(128) uint8_t sm[2][2][KT * 256];    // [buffer][K | V][key row x 256 B], 16-byte chunks XOR-swizzled
   fq3gemm::pdl_launch();
   fq3gemm::pdl_wait();
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int gq = lane >> 2, t = lane & 3;
-  const int g = blockIdx.y, qb = blockIdx.x;
+  const int sq = seq_of_qblock(tab, blockIdx.x);
+  const int g = blockIdx.y, qb = blockIdx.x - tab.qb0[sq];
+  const int P = tab.P[sq], n_left_pad = tab.pad[sq];
   const int ld = (nH + 2 * nKV) * 128;
+  const __nv_bfloat16* QKV = QKVp + (size_t)tab.row0[sq] * ld;
+  __nv_bfloat16* OUT = OUTp + (size_t)tab.row0[sq] * nH * 128;
   const bool active = warp < 2 * REP;
   const int h = g * REP + (warp % REP);
   const int q0 = qb * 32 + (warp / REP) * 16;
   const int i0 = q0 + gq, i1 = q0 + gq + 8;
-  const __nv_bfloat16* kb = kc + (size_t)g * S * 128;
-  const __nv_bfloat16* vb = vc + (size_t)g * S * 128;
+  const __nv_bfloat16* kb = kc + (size_t)tab.slot[sq] * slot_stride + (size_t)g * S * 128;
+  const __nv_bfloat16* vb = vc + (size_t)tab.slot[sq] * slot_stride + (size_t)g * S * 128;
   const int kt_first = n_left_pad / KT;
   const int kt_last = min(qb, (P - 1) / KT);
 
@@ -343,64 +398,104 @@ extern "C" int fq3_engine_set_prefill_weights(fq3_engine* e, const fq3_tensor* t
   return 0;
 }
 
-extern "C" int fq3_prefill(fq3_engine* e, int32_t slot, const void* embeds_dev, int32_t P, int32_t n_left_pad,
-                           void* logits_out_dev, void* hidden_out_dev, void* stream_) {
-  if (!e || !embeds_dev || !logits_out_dev || !hidden_out_dev) return fail(FQ3_ERR_INVALID, "null argument");
-  {
-    int rcs;
-    if ((rcs = check_slot(e, slot))) return rcs;
-  }
-  if (!e->pf_ready) return fail(FQ3_ERR_STATE, "fq3_engine_set_prefill_weights has not been called");
-  if ((uintptr_t)logits_out_dev & 15) return fail(FQ3_ERR_INVALID, "logits_out_dev must be 16-byte aligned");
-  if (P <= 0) return fail(FQ3_ERR_INVALID, "empty prompt");
-  if (P > e->cfg.max_seq_len)
-    return fail(FQ3_ERR_TOO_LONG, "Input is too long: prefill has %d tokens but max_seq_len=%d. Use shorter text or shorter reference audio.", P, e->cfg.max_seq_len);
-  DevGuard dev_guard(e->dev);
-  cudaStream_t stream = (cudaStream_t)stream_;
+// One chain of launches over the sequences of `tab` (sum of P <= max_seq_len rows): embeds [rows][H] packed as the table
+// says -> KV caches of the listed slots, logits [n][V], hidden [n][H].
+static int prefill_group(fq3_engine* e, const pf::SeqTab& tab, const void* embeds_dev, void* logits_out_dev,
+                         void* hidden_out_dev, cudaStream_t stream) {
   const fq3_stack_config& T = e->cfg.talker;
   const int L = T.num_hidden_layers, H = T.hidden_size, I = T.intermediate_size;
   const int nH = T.num_attention_heads, nKV = T.num_key_value_heads, qd = nH * 128, kd = nKV * 128, S = e->cfg.max_seq_len;
+  const int rows = tab.row0[tab.n - 1] + tab.P[tab.n - 1], n = tab.n;
   using bf = __nv_bfloat16;
   bf* x = (bf*)e->pf_buf[0];
   bf* x1 = (bf*)e->pf_buf[1];
   bf* hn = (bf*)e->pf_buf[2];
   bf* wide = (bf*)e->pf_buf[3];
   bf* att = (bf*)e->pf_buf[4];
-  CK(cudaMemcpyAsync(x, embeds_dev, (size_t)P * H * 2, cudaMemcpyDeviceToDevice, stream));
+  const size_t slot_stride = e->tkv_slot / sizeof(bf);
+  CK(cudaMemcpyAsync(x, embeds_dev, (size_t)rows * H * 2, cudaMemcpyDeviceToDevice, stream));
   const KParams& k = e->kp;
   int rc;
   for (int l = 0; l < L; ++l) {
-    FQ3_LAUNCH((pf::rmsnorm_rows_kernel), P, 256, 0, stream, x, (const bf*)k.t.ln_in + (size_t)l * H, H, T.rms_norm_eps, hn);
+    FQ3_LAUNCH((pf::rmsnorm_rows_kernel), rows, 256, 0, stream, x, (const bf*)k.t.ln_in + (size_t)l * H, H, T.rms_norm_eps, hn);
     e->launches++;
-    if ((rc = pf_gemm(e, hn, (const bf*)e->pf_qkv + (size_t)l * (qd + 2 * kd) * H, nullptr, wide, P, H, qd + 2 * kd, 0, stream))) return rc;
+    if ((rc = pf_gemm(e, hn, (const bf*)e->pf_qkv + (size_t)l * (qd + 2 * kd) * H, nullptr, wide, rows, H, qd + 2 * kd, 0, stream))) return rc;
+    bf* kl = (bf*)e->t_kc + (size_t)l * nKV * S * 128;   // layer l of slot 0; the kernels add slot * slot_stride
+    bf* vl = (bf*)e->t_vc + (size_t)l * nKV * S * 128;
     {
-      const int warps = P * (nH + 2 * nKV);
-      FQ3_LAUNCH((pf::rope_kv_kernel), (warps * 32 + 255) / 256, 256, 0, stream, 
-          wide, P, nH, nKV, (const bf*)k.t.qnorm + (size_t)l * 128, (const bf*)k.t.knorm + (size_t)l * 128, k.t.cos,
-          k.t.sin, k.t.npos, n_left_pad, T.rms_norm_eps, (bf*)slot_tk(e, slot) + (size_t)l * nKV * S * 128,
-          (bf*)slot_tv(e, slot) + (size_t)l * nKV * S * 128, S);
+      const int warps = rows * (nH + 2 * nKV);
+      FQ3_LAUNCH((pf::rope_kv_kernel), (warps * 32 + 255) / 256, 256, 0, stream,
+          wide, rows, nH, nKV, (const bf*)k.t.qnorm + (size_t)l * 128, (const bf*)k.t.knorm + (size_t)l * 128, k.t.cos,
+          k.t.sin, k.t.npos, T.rms_norm_eps, kl, vl, slot_stride, S, tab);
       e->launches++;
     }
-    {
-      const bf* kl = (const bf*)slot_tk(e, slot) + (size_t)l * nKV * S * 128;
-      const bf* vl = (const bf*)slot_tv(e, slot) + (size_t)l * nKV * S * 128;
-      if (nH == 2 * nKV)   // fq3_engine_set_prefill_weights admits GQA ratios 1 and 2 only
-        FQ3_LAUNCH((pf::attn_prefill_mma_kernel<2>), dim3((P + 31) / 32, nKV), 128, 0, stream, wide, P, nH, nKV, kl, vl, S, n_left_pad, att);
-      else
-        FQ3_LAUNCH((pf::attn_prefill_mma_kernel<1>), dim3((P + 31) / 32, nKV), 128, 0, stream, wide, P, nH, nKV, kl, vl, S, n_left_pad, att);
-    }
+    if (nH == 2 * nKV)   // fq3_engine_set_prefill_weights admits GQA ratios 1 and 2 only
+      FQ3_LAUNCH((pf::attn_prefill_mma_kernel<2>), dim3(tab.qb0[n], nKV), 128, 0, stream, wide, nH, nKV, kl, vl, slot_stride, S, att, tab);
+    else
+      FQ3_LAUNCH((pf::attn_prefill_mma_kernel<1>), dim3(tab.qb0[n], nKV), 128, 0, stream, wide, nH, nKV, kl, vl, slot_stride, S, att, tab);
     e->launches++;
-    if ((rc = pf_gemm(e, att, (const bf*)e->pf_o + (size_t)l * H * qd, x, x1, P, qd, H, 0, stream))) return rc;
-    FQ3_LAUNCH((pf::rmsnorm_rows_kernel), P, 256, 0, stream, x1, (const bf*)k.t.ln_post + (size_t)l * H, H, T.rms_norm_eps, hn);
+    if ((rc = pf_gemm(e, att, (const bf*)e->pf_o + (size_t)l * H * qd, x, x1, rows, qd, H, 0, stream))) return rc;
+    FQ3_LAUNCH((pf::rmsnorm_rows_kernel), rows, 256, 0, stream, x1, (const bf*)k.t.ln_post + (size_t)l * H, H, T.rms_norm_eps, hn);
     e->launches++;
-    if ((rc = pf_gemm(e, hn, (const bf*)e->pf_gu + (size_t)l * 2 * I * H, nullptr, wide, P, H, 2 * I, 1, stream))) return rc;
-    if ((rc = pf_gemm(e, wide, (const bf*)e->pf_down + (size_t)l * H * I, x1, x, P, I, H, 0, stream))) return rc;
+    if ((rc = pf_gemm(e, hn, (const bf*)e->pf_gu + (size_t)l * 2 * I * H, nullptr, wide, rows, H, 2 * I, 1, stream))) return rc;
+    if ((rc = pf_gemm(e, wide, (const bf*)e->pf_down + (size_t)l * H * I, x1, x, rows, I, H, 0, stream))) return rc;
   }
-  // final norm of the last row -> past_hidden; logits = codec_head(hidden)
-  FQ3_LAUNCH((pf::rmsnorm_rows_kernel), 1, 256, 0, stream, x + (size_t)(P - 1) * H, (const bf*)k.t.ln_f, H, T.rms_norm_eps, hn);
+  // final norm of every sequence's last row -> past_hidden; logits = codec_head(hidden), M = n
+  FQ3_LAUNCH((pf::rmsnorm_last_rows_kernel), n, 256, 0, stream, x, (const bf*)k.t.ln_f, H, T.rms_norm_eps, hn, tab);
   e->launches++;
-  CK(cudaMemcpyAsync(hidden_out_dev, hn, (size_t)H * 2, cudaMemcpyDeviceToDevice, stream));
-  if ((rc = pf_gemm(e, hn, (const bf*)e->pf_head, nullptr, (bf*)logits_out_dev, 1, H, T.vocab_size, 0, stream))) return rc;
+  CK(cudaMemcpyAsync(hidden_out_dev, hn, (size_t)n * H * 2, cudaMemcpyDeviceToDevice, stream));
+  if ((rc = pf_gemm(e, hn, (const bf*)e->pf_head, nullptr, (bf*)logits_out_dev, n, H, T.vocab_size, 0, stream))) return rc;
   CK(cudaGetLastError());
   return 0;
+}
+
+extern "C" int fq3_prefill_batch(fq3_engine* e, int32_t n, const int32_t* slots, const void* embeds_dev, const int32_t* P,
+                                 const int32_t* n_left_pad, void* logits_out_dev, void* hidden_out_dev, void* stream_) {
+  if (!e) return fail(FQ3_ERR_INVALID, "null argument");
+  if (n < 1 || n > e->max_batch) return fail(FQ3_ERR_INVALID, "n %d outside [1, max_batch=%d]", n, e->max_batch);
+  if (!slots || !embeds_dev || !P || !n_left_pad || !logits_out_dev || !hidden_out_dev) return fail(FQ3_ERR_INVALID, "null argument");
+  // every check before the first launch: a refused call leaves every slot as it was.  A row is named when n > 1.
+  char row[32] = "";
+  for (int i = 0; i < n; ++i) {
+    if (n > 1) snprintf(row, sizeof(row), " (row %d)", i);
+    if (slots[i] < 0 || slots[i] >= e->max_batch)
+      return fail(FQ3_ERR_INVALID, "slot %d outside [0, max_batch=%d)%s", slots[i], e->max_batch, row);
+    for (int j = 0; j < i; ++j)
+      if (slots[j] == slots[i]) return fail(FQ3_ERR_INVALID, "slot %d listed twice%s", slots[i], row);
+    if (P[i] <= 0) return fail(FQ3_ERR_INVALID, "empty prompt%s", row);
+    if (P[i] > e->cfg.max_seq_len)
+      return fail(FQ3_ERR_TOO_LONG, "Input is too long: prefill has %d tokens but max_seq_len=%d. Use shorter text or shorter reference audio.%s", P[i], e->cfg.max_seq_len, row);
+  }
+  if (!e->pf_ready) return fail(FQ3_ERR_STATE, "fq3_engine_set_prefill_weights has not been called");
+  if ((uintptr_t)logits_out_dev & 15) return fail(FQ3_ERR_INVALID, "logits_out_dev must be 16-byte aligned");
+  DevGuard dev_guard(e->dev);
+  cudaStream_t stream = (cudaStream_t)stream_;
+  const int H = e->cfg.talker.hidden_size, V = e->cfg.talker.vocab_size;
+  // consecutive groups in the caller's order, each as many sequences as fit the max_seq_len rows of scratch
+  size_t in_row = 0;
+  for (int b0 = 0; b0 < n;) {
+    pf::SeqTab tab;
+    memset(&tab, 0, sizeof(tab));
+    int rows = 0, qb = 0;
+    while (b0 + tab.n < n && rows + P[b0 + tab.n] <= e->cfg.max_seq_len) {
+      const int i = b0 + tab.n, j = tab.n++;
+      tab.row0[j] = rows; tab.P[j] = P[i]; tab.pad[j] = n_left_pad[i]; tab.slot[j] = slots[i]; tab.qb0[j] = qb;
+      rows += P[i];
+      qb += (P[i] + 31) / 32;
+    }
+    tab.qb0[tab.n] = qb;
+    int rc;
+    if ((rc = prefill_group(e, tab, (const __nv_bfloat16*)embeds_dev + in_row * H,
+                            (__nv_bfloat16*)logits_out_dev + (size_t)b0 * V, (__nv_bfloat16*)hidden_out_dev + (size_t)b0 * H,
+                            stream)))
+      return rc;
+    in_row += rows;
+    b0 += tab.n;
+  }
+  return 0;
+}
+
+extern "C" int fq3_prefill(fq3_engine* e, int32_t slot, const void* embeds_dev, int32_t P, int32_t n_left_pad,
+                           void* logits_out_dev, void* hidden_out_dev, void* stream) {
+  return fq3_prefill_batch(e, 1, &slot, embeds_dev, &P, &n_left_pad, logits_out_dev, hidden_out_dev, stream);
 }

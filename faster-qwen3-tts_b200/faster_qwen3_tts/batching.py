@@ -19,7 +19,7 @@ from typing import Dict, Generator, List, Optional, Tuple
 
 import torch
 
-from .generate import _sync, begin_fused, shared_engine
+from .generate import _sync, begin_fused, begin_fused_batch, shared_engine
 
 
 @dataclass
@@ -44,10 +44,15 @@ class SlotRequest:
         return self.feed.n_rows >= need
 
 
+# keyword defaults of BatchScheduler.submit, which submit_many applies to every request
+_SUBMIT_DEFAULTS = dict(max_new_tokens=2048, min_new_tokens=2, temperature=0.9, top_k=50, top_p=1.0, do_sample=True,
+                        repetition_penalty=1.05, uniforms=None)
+
+
 class BatchScheduler:
-    """Owns the engine's slots: ``submit`` prefills one request into a free slot and latches it, ``step`` advances
-    every ready slot by up to ``n_frames`` frames with ONE launch and returns the new codes per request, ``cancel``
-    frees a slot.  A text-fed request (``feed``) is ready while its next trailing row exists or its text is closed; a
+    """Owns the engine's slots: ``submit`` prefills one request into a free slot and latches it (``submit_many``:
+    several, with one batched prefill), ``step`` advances every ready slot by up to ``n_frames`` frames with ONE launch
+    and returns the new codes per request, ``cancel`` frees a slot.  A text-fed request (``feed``) is ready while its next trailing row exists or its text is closed; a
     slot that waits for text costs the others nothing."""
 
     def __init__(self, engine, talker, config, predictor_graph, talker_graph):
@@ -55,12 +60,17 @@ class BatchScheduler:
         self.pg, self.tg = predictor_graph, talker_graph
         self.free: List[int] = list(range(engine.max_batch))
         self.active: Dict[int, SlotRequest] = {}
+        self.max_seq_len = getattr(engine, "max_seq_len", None)   # longest prompt a slot takes
 
     def __len__(self) -> int:
         return len(self.active)
 
     def has_capacity(self) -> bool:
         return bool(self.free)
+
+    def capacity(self) -> int:
+        """free request slots"""
+        return len(self.free)
 
     @torch.inference_mode()
     def submit(self, tie, tam, tth, tpe, *, tag=None, max_new_tokens: int = 2048, min_new_tokens: int = 2,
@@ -87,6 +97,40 @@ class BatchScheduler:
                          gen0=self.engine.gen_step0[slot], rows_ahead=max(1, int(rows_ahead)))
         self.active[slot] = rq
         return rq
+
+    @torch.inference_mode()
+    def submit_many(self, requests: List[dict]) -> List[SlotRequest]:
+        """Several requests at once: ``requests[i]`` holds the arguments of one ``submit`` call by name (tie, tam, tth,
+        tpe, tag, the sampling keywords, uniforms, feed, rows_ahead).  They take the slots consecutive ``submit`` calls
+        would take and latch what those would latch, but on a K3 engine their prompts share ONE prefill launch chain
+        (``generate.begin_fused_batch``).  All or none: on an error every slot is released."""
+        n = len(requests)
+        if n > len(self.free):
+            raise RuntimeError(f"{n} requests but only {len(self.free)} of {self.engine.max_batch} request slots are free")
+        slots, self.free = self.free[:n], self.free[n:]
+        rows = []
+        for r in requests:
+            gen = dict(_SUBMIT_DEFAULTS)
+            gen.update({k: v for k, v in r.items() if k not in ("tag", "feed", "rows_ahead")})
+            gen["trailing_len"] = None if r.get("feed") is None else 0
+            rows.append(gen)
+        try:
+            if n:
+                begin_fused_batch(self.engine, self.talker, rows, self.config, self.pg, self.tg, slots)
+            for slot, r in zip(slots, requests):
+                if r.get("feed") is not None:
+                    self.engine.set_text_rows(slot, r["feed"].update(), open=not r["feed"].closed)
+        except Exception:
+            self.free = slots + self.free
+            raise
+        out = []
+        for slot, r, gen in zip(slots, requests, rows):
+            tag = r.get("tag")
+            rq = SlotRequest(slot=slot, tag=tag if tag is not None else slot, max_new_tokens=gen["max_new_tokens"],
+                             feed=r.get("feed"), gen0=self.engine.gen_step0[slot], rows_ahead=max(1, int(r.get("rows_ahead", 1))))
+            self.active[slot] = rq
+            out.append(rq)
+        return out
 
     @torch.inference_mode()
     def step(self, n_frames: int) -> List[Tuple[SlotRequest, torch.Tensor]]:
@@ -157,11 +201,11 @@ def fast_generate_streaming_batch(
     sched = BatchScheduler(engine, talker, config, predictor_graph, talker_graph)
     device = talker_input_embeds.device
     t0 = time.time()
-    for b in range(B):
-        sched.submit(_rows(talker_input_embeds, b), _rows(attention_mask, b), _rows(trailing_text_hiddens, b),
-                     tts_pad_embed, tag=b, max_new_tokens=max_new_tokens, min_new_tokens=min_new_tokens,
-                     temperature=temperature, top_k=top_k, top_p=top_p, do_sample=do_sample,
-                     repetition_penalty=repetition_penalty, uniforms=None if uniforms is None else uniforms[b])
+    sched.submit_many([dict(tie=_rows(talker_input_embeds, b), tam=_rows(attention_mask, b),
+                            tth=_rows(trailing_text_hiddens, b), tpe=tts_pad_embed, tag=b, max_new_tokens=max_new_tokens,
+                            min_new_tokens=min_new_tokens, temperature=temperature, top_k=top_k, top_p=top_p,
+                            do_sample=do_sample, repetition_penalty=repetition_penalty,
+                            uniforms=None if uniforms is None else uniforms[b]) for b in range(B)])
     _sync(device)
     t_prefill = time.time() - t0
     idx = 0

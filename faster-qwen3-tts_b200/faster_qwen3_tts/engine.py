@@ -69,7 +69,7 @@ EXPORTS = [
     "fq3_engine_create", "fq3_engine_load_weights", "fq3_engine_destroy", "fq3_import_kv", "fq3_export_kv",
     "fq3_set_generation_state", "fq3_talker_step", "fq3_predictor_run", "fq3_sample_logits", "fq3_begin_request",
     "fq3_decode_chunk", "fq3_set_text_rows", "fq3_get_past_hidden", "fq3_debug_enable", "fq3_debug_read", "fq3_tape_bytes",
-    "fq3_num_ctas", "fq3_launch_count", "fq3_last_error", "fq3_version", "fq3_engine_set_prefill_weights", "fq3_prefill", "fq3_max_batch", "fq3_debug_gemv",
+    "fq3_num_ctas", "fq3_launch_count", "fq3_last_error", "fq3_version", "fq3_engine_set_prefill_weights", "fq3_prefill", "fq3_prefill_batch", "fq3_max_batch", "fq3_debug_gemv",
     "fq3_debug_conv_gemm",
     "fq3_codec_create", "fq3_codec_load_weights", "fq3_codec_flops",
     "fq3_codec_load_frontend", "fq3_codec_decode_codes", "fq3_codec_frontend_flops",
@@ -138,6 +138,8 @@ def load_library() -> C.CDLL:
     lib.fq3_engine_set_prefill_weights.argtypes = [C.c_void_p, C.POINTER(Tensor), C.c_int32]
     lib.fq3_prefill.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
                                 C.c_void_p]
+    lib.fq3_prefill_batch.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.c_void_p, C.POINTER(C.c_int32),
+                                      C.POINTER(C.c_int32), C.c_void_p, C.c_void_p, C.c_void_p]
     lib.fq3_codec_create.argtypes = [C.POINTER(C.c_int32), C.c_int32, C.POINTER(C.c_void_p)]
     lib.fq3_codec_destroy.argtypes = [C.c_void_p]
     lib.fq3_codec_destroy.restype = None
@@ -315,6 +317,29 @@ class Engine:
         hidden = torch.empty(self.H, dtype=self.dtype, device=self.device)
         _check(self.lib, self.lib.fq3_prefill(self.h, int(slot), x.data_ptr(), x.shape[0], int(n_left_pad), logits.data_ptr(),
                                               hidden.data_ptr(), self._stream()))
+        return logits, hidden
+
+    def prefill_batch(self, rows, pads, slots) -> Tuple[torch.Tensor, torch.Tensor]:
+        """Several prompts into distinct request slots with one chain of launches: ``rows`` is a list of [P_b,H]
+        prompts (packed into one [sum P_b, H] tensor) or a left-padded [B,P,H] batch (packed by a reshape); ``pads[b]``
+        is the left pad of prompt b, ``slots[b]`` its slot.  Returns (logits [n,V], past_hidden [n,H]); row b and the
+        cache of ``slots[b]`` are bit-identical to ``prefill(rows[b], pads[b], slot=slots[b])``."""
+        if isinstance(rows, torch.Tensor):
+            x = self._t(rows.reshape(-1, self.H))
+            lens = [int(rows.shape[1])] * int(rows.shape[0])
+        else:
+            parts = [r.reshape(-1, self.H) for r in rows]
+            x = self._t(torch.cat(parts)) if parts else torch.empty(0, self.H, dtype=self.dtype, device=self.device)
+            lens = [int(r.shape[0]) for r in parts]
+        n = len(lens)
+        if len(pads) != n or len(slots) != n:
+            raise ValueError(f"{n} prompts but {len(pads)} pads and {len(slots)} slots")
+        logits = torch.empty(n, self.talker_cfg["vocab_size"], dtype=self.dtype, device=self.device)
+        hidden = torch.empty(n, self.H, dtype=self.dtype, device=self.device)
+        arr = C.c_int32 * n
+        _check(self.lib, self.lib.fq3_prefill_batch(self.h, n, arr(*[int(s) for s in slots]), x.data_ptr(), arr(*lens),
+                                                    arr(*[int(p) for p in pads]), logits.data_ptr(), hidden.data_ptr(),
+                                                    self._stream()))
         return logits, hidden
 
     # -- duck-type path ----------------------------------------------------------------------------------

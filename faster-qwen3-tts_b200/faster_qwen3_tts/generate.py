@@ -37,32 +37,35 @@ def _prefill(talker, tie, tam, tth, tpe):
                           past_hidden=None, past_key_values=None)
 
 
-def begin_fused(engine, talker, tie, tam, tth, tpe, config, predictor_graph, talker_graph, *, max_new_tokens,
-                min_new_tokens, temperature, top_k, top_p, do_sample, repetition_penalty, uniforms, slot=None,
-                trailing_len=None):
-    """Prefill + first token + request latch (generate.py:104-140) for ONE row [1,P,H] into request slot `slot`
-    (default: the slot the graph handles drive).  ``trailing_len``: rows of ``tth`` valid now (text-fed requests latch
-    a larger buffer and announce rows later, ``Engine.set_text_rows``).  Returns the first token id."""
-    eos_id = config.codec_eos_token_id
-    slot = int(getattr(talker_graph, "slot", 0) if slot is None else slot)
-    native = getattr(engine, "has_prefill", False) and getattr(talker_graph, "use_native_prefill", True) \
+def _native_prefill(engine, talker_graph, tie) -> bool:
+    """K3 (the hand-written prefill) serves a [1,P,H] row of a bf16 engine; fp32 engines, graphs that opt out and
+    multi-row inputs take the upstream ``talker.forward``."""
+    return getattr(engine, "has_prefill", False) and getattr(talker_graph, "use_native_prefill", True) \
         and tie.shape[0] == 1
-    pad = int((tam[0] == 0).sum().item()) if tam is not None else 0
-    if native:
-        # K3: hand-written prefill writes the KV cache directly (no talker.forward, no prefill_kv copies)
-        lg, ph = engine.prefill(tie[0], pad, slot=slot)
-        import types
-        out = types.SimpleNamespace(logits=lg.view(1, 1, -1), past_hidden=ph.view(1, 1, -1), generation_step=0,
-                                    past_key_values=None)
-    else:
-        out = _prefill(talker, tie, tam, tth, tpe)
-    sp_t = SamplingParams(do_sample=do_sample, top_k=top_k, temperature=temperature, top_p=top_p,
-                          repetition_penalty=repetition_penalty)
+
+
+def _native_out(logits, hidden):
+    import types
+    return types.SimpleNamespace(logits=logits.view(1, 1, -1), past_hidden=hidden.view(1, 1, -1), generation_step=0,
+                                 past_key_values=None)
+
+
+def _first_token(engine, out, config, uniforms, u0, *, min_new_tokens, temperature, top_k, top_p, do_sample, **_):
+    """first cb0 token of a prefilled row (generate.py:119-120), a device tensor [1]"""
+    return engine.sample_logits(out.logits[:, -1, :], SamplingParams(do_sample, top_k, temperature, top_p, 1.0), u=u0,
+                                suppress_special=True, eos_id=config.codec_eos_token_id, suppress_eos=min_new_tokens > 0)
+
+
+def _uniforms(engine, predictor_graph, uniforms, *, max_new_tokens, do_sample, **_):
     if (do_sample or predictor_graph.do_sample) and uniforms is None:
         uniforms = torch.rand(max_new_tokens + 1, 16, device=engine.device)
-    u0 = float(uniforms.reshape(-1)[0]) if (do_sample and uniforms is not None) else 0.0
-    first = engine.sample_logits(out.logits[:, -1, :], SamplingParams(do_sample, top_k, temperature, top_p, 1.0), u=u0,
-                                 suppress_special=True, eos_id=eos_id, suppress_eos=min_new_tokens > 0)
+    return uniforms
+
+
+def latch_fused(engine, talker, out, native, pad, tie, tth, tpe, predictor_graph, talker_graph, first, *, slot, uniforms,
+                trailing_len, max_new_tokens, min_new_tokens, temperature, top_k, top_p, do_sample, repetition_penalty):
+    """Latch half of ``begin_fused``: generation state and request of `slot` from a prefilled row ``out`` whose first
+    token ``first`` (int) is sampled (generate.py:120-140)."""
     if native:
         prefill_len = int(tie.shape[1])
         n_left_pad, rope_delta = pad, -pad   # rotary position = cache index - pad count (talker_graph.py:210-211)
@@ -78,12 +81,65 @@ def begin_fused(engine, talker, tie, tam, tth, tpe, config, predictor_graph, tal
     if slot == getattr(talker_graph, "slot", 0):
         talker_graph.prefill_len, talker_graph.n_left_pad, talker_graph.rope_delta = prefill_len, n_left_pad, rope_delta
     gen_step = int(out.generation_step) if out.generation_step is not None else 0
-    engine.begin_request(first_token=int(first.item()), prefill_len=prefill_len, gen_step=gen_step,
+    sp_t = SamplingParams(do_sample=do_sample, top_k=top_k, temperature=temperature, top_p=top_p,
+                          repetition_penalty=repetition_penalty)
+    engine.begin_request(first_token=int(first), prefill_len=prefill_len, gen_step=gen_step,
                          past_hidden=out.past_hidden, trailing_text=tth, tts_pad=tpe, max_new_tokens=max_new_tokens,
                          min_new_tokens=min_new_tokens, sp_talker=sp_t, sp_predictor=predictor_graph.sampling(),
                          uniforms=uniforms, rope_delta=rope_delta, n_left_pad=n_left_pad, slot=slot,
                          trailing_len=trailing_len)
+
+
+def begin_fused(engine, talker, tie, tam, tth, tpe, config, predictor_graph, talker_graph, *, max_new_tokens,
+                min_new_tokens, temperature, top_k, top_p, do_sample, repetition_penalty, uniforms, slot=None,
+                trailing_len=None):
+    """Prefill + first token + request latch (generate.py:104-140) for ONE row [1,P,H] into request slot `slot`
+    (default: the slot the graph handles drive).  ``trailing_len``: rows of ``tth`` valid now (text-fed requests latch
+    a larger buffer and announce rows later, ``Engine.set_text_rows``).  Returns the first token id."""
+    gen = dict(max_new_tokens=max_new_tokens, min_new_tokens=min_new_tokens, temperature=temperature, top_k=top_k,
+               top_p=top_p, do_sample=do_sample, repetition_penalty=repetition_penalty)
+    slot = int(getattr(talker_graph, "slot", 0) if slot is None else slot)
+    native = _native_prefill(engine, talker_graph, tie)
+    pad = int((tam[0] == 0).sum().item()) if tam is not None else 0
+    if native:
+        # K3: hand-written prefill writes the KV cache directly (no talker.forward, no prefill_kv copies)
+        out = _native_out(*engine.prefill(tie[0], pad, slot=slot))
+    else:
+        out = _prefill(talker, tie, tam, tth, tpe)
+    uniforms = _uniforms(engine, predictor_graph, uniforms, **gen)
+    u0 = float(uniforms.reshape(-1)[0]) if (do_sample and uniforms is not None) else 0.0
+    first = _first_token(engine, out, config, uniforms, u0, **gen)
+    latch_fused(engine, talker, out, native, pad, tie, tth, tpe, predictor_graph, talker_graph, first.item(), slot=slot,
+                uniforms=uniforms, trailing_len=trailing_len, **gen)
     return first
+
+
+def begin_fused_batch(engine, talker, rows, config, predictor_graph, talker_graph, slots):
+    """``begin_fused`` for several rows into distinct slots: ``rows[b]`` holds the arguments of one ``begin_fused`` call
+    (tie [1,P,H], tam, tth, tpe, the sampling keywords, uniforms, trailing_len).  On a K3 engine all prompts go through
+    ONE ``Engine.prefill_batch`` and the first tokens of all rows come back with one host synchronisation; every row
+    latches what ``begin_fused`` would latch.  Otherwise (fp32 engine, a graph that opts out of K3) each row takes
+    ``begin_fused``.  Returns the first token ids."""
+    if not all(_native_prefill(engine, talker_graph, r["tie"]) for r in rows):
+        return [int(begin_fused(engine, talker, r["tie"], r["tam"], r["tth"], r["tpe"], config, predictor_graph,
+                                talker_graph, slot=s, **{k: v for k, v in r.items() if k not in ("tie", "tam", "tth", "tpe")}))
+                for r, s in zip(rows, slots)]
+    gens = [{k: v for k, v in r.items() if k not in ("tie", "tam", "tth", "tpe", "uniforms", "trailing_len")} for r in rows]
+    n = len(rows)
+    uniforms = [_uniforms(engine, predictor_graph, r.get("uniforms"), **g) for r, g in zip(rows, gens)]
+    # pad counts (host arrays of the C call) and first-token draws of all rows: one transfer (float64 holds both exactly)
+    head = [torch.zeros(()) if r["tam"] is None else (r["tam"][0] == 0).sum() for r in rows] + \
+        [u.reshape(-1)[0] if (g["do_sample"] and u is not None) else torch.zeros(()) for u, g in zip(uniforms, gens)]
+    head = torch.stack([x.to(engine.device, torch.float64) for x in head]).tolist()
+    pads, u0 = [int(x) for x in head[:n]], head[n:]
+    logits, hidden = engine.prefill_batch([r["tie"][0] for r in rows], pads, slots)
+    outs = [_native_out(logits[b], hidden[b]) for b in range(n)]
+    firsts = torch.cat([_first_token(engine, o, config, u, x, **g) for o, u, x, g in zip(outs, uniforms, u0, gens)])
+    firsts = firsts.tolist()   # the one host synchronisation of the first tokens
+    for r, s, o, u, g, pad, first in zip(rows, slots, outs, uniforms, gens, pads, firsts):
+        latch_fused(engine, talker, o, True, pad, r["tie"], r["tth"], r["tpe"], predictor_graph, talker_graph, first,
+                    slot=int(s), uniforms=u, trailing_len=r.get("trailing_len"), **g)
+    return firsts
 
 
 def stepwise_frames(talker, tie, tam, tth, tpe, config, predictor_graph, talker_graph, *, max_new_tokens,

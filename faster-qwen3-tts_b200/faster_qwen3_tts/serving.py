@@ -109,8 +109,9 @@ class TextTicket(Ticket):
 class ContinuousBatcher:
     """One worker thread, many clients.  ``scheduler_factory()`` -> object with ``has_capacity()``,
     ``submit(tie, tam, tth, tpe, tag=..., **gen) -> request``, ``step(n) -> [(request, codes)]`` and ``__len__`` (the
-    ``BatchScheduler`` of batching.py); ``window_factory(ref_codes)`` -> object with ``push(codes) -> (pcm, sr)``
-    (``model._StreamWindow``); ``feed_factory(max_rows)`` -> ``text_stream.TextFeed`` (text-fed requests)."""
+    ``BatchScheduler`` of batching.py); with ``submit_many(list of submit arguments) -> [request]`` and ``capacity()``
+    the ready requests that fit the free slots are admitted together (one batched prefill); ``window_factory(ref_codes)``
+    -> object with ``push(codes) -> (pcm, sr)`` (``model._StreamWindow``); ``feed_factory(max_rows)`` -> ``text_stream.TextFeed`` (text-fed requests)."""
 
     def __init__(self, scheduler, window_factory: Callable, chunk_size: int = 8, idle_sleep: float = 0.002,
                  batch_decode: Optional[Callable] = None, feed_factory: Optional[Callable] = None):
@@ -184,7 +185,9 @@ class ContinuousBatcher:
                 del self.live[rid]
                 t.out.put(_DONE)
 
-    def _start(self, t: Ticket):
+    def _prepare(self, t: Ticket):
+        """-> (the ticket's ``submit`` arguments by name, its codec window); a prompt longer than the scheduler's
+        ``max_seq_len`` is refused here, with the reference's message (talker_graph.py:163-167)"""
         if isinstance(t, TextTicket):
             tie, tam, tpe, ref_codes = t.prepare(t.feed)
             win = self.window_factory(ref_codes)
@@ -192,12 +195,19 @@ class ContinuousBatcher:
             # chunking: the slot is launched only when a full chunk of text rows exists, so every launch emits a full
             # chunk or ends the request.  A stateful stream decodes to the same PCM in any chunking: one row suffices.
             ahead = 1 if getattr(win, "any_chunking", False) else self.chunk_size
-            rq = self.sched.submit(tie, tam, t.feed.rows[None], tpe, tag=t.rid, feed=t.feed, rows_ahead=ahead,
-                                   **t.gen_kwargs)
+            req = dict(tie=tie, tam=tam, tth=t.feed.rows[None], tpe=tpe, tag=t.rid, feed=t.feed, rows_ahead=ahead,
+                       **t.gen_kwargs)
         else:
             tie, tam, tth, tpe, ref_codes = t.prepare()
             win = self.window_factory(ref_codes)
-            rq = self.sched.submit(tie, tam, tth, tpe, tag=t.rid, **t.gen_kwargs)
+            req = dict(tie=tie, tam=tam, tth=tth, tpe=tpe, tag=t.rid, **t.gen_kwargs)
+        S = getattr(self.sched, "max_seq_len", None)
+        if S is not None and tie.shape[1] > S:
+            raise RuntimeError(f"Input is too long: prefill has {tie.shape[1]} tokens but max_seq_len={S}. "
+                               "Use shorter text or shorter reference audio.")
+        return req, win
+
+    def _live(self, t: Ticket, rq, win):
         self.requests[t.rid] = rq
         self.live[t.rid] = (t, win)
 
@@ -218,14 +228,29 @@ class ContinuousBatcher:
             t.out.put(_DONE)
         # text-fed requests enter once their first id is committed (the prompt holds it), in arrival order
         ready = sorted([t for t in self.waiting if t.feed.n_ids] + self._queued, key=lambda t: t.rid)
+        many = hasattr(self.sched, "submit_many")
+        batch = []   # (ticket, submit arguments, window) admitted together by one submit_many
         for t in ready:
-            if not self.sched.has_capacity():
-                return
+            if (len(batch) >= self.sched.capacity()) if many else not self.sched.has_capacity():
+                break
             (self.waiting if isinstance(t, TextTicket) else self._queued).remove(t)
-            try:
-                self._start(t)
-            except BaseException as ex:   # a bad request must not take the worker down
+            try:   # a bad request must not take the worker down, nor the requests admitted with it
+                req, win = self._prepare(t)
+                if many:
+                    batch.append((t, req, win))
+                else:
+                    self._live(t, self.sched.submit(**req), win)
+            except BaseException as ex:
                 self._fail(t, ex)
+        if batch:
+            try:
+                rqs = self.sched.submit_many([req for _, req, _ in batch])
+            except BaseException as ex:
+                for t, _, _ in batch:
+                    self._fail(t, ex)
+                return
+            for (t, _, win), rq in zip(batch, rqs):
+                self._live(t, rq, win)
 
     def _run(self):
         while not self._stop.is_set():

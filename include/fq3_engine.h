@@ -164,6 +164,21 @@ int fq3_engine_set_prefill_weights(fq3_engine* e, const fq3_tensor* tensors, int
  * cache index - n_left_pad (clamped at 0); keys below n_left_pad are masked. */
 int fq3_prefill(fq3_engine* e, int32_t slot, const void* embeds_dev, int32_t P, int32_t n_left_pad,
                 void* logits_out_dev, void* hidden_out_dev, void* stream);
+/* Batched prefill: n prompts into n distinct request slots with one chain of launches (fq3_prefill is the n = 1 case).
+ * slots[n], P[n], n_left_pad[n] are HOST arrays; embeds_dev [sum P_b][H] holds the prompts packed row-major in list
+ * order (prompt b at row P_0 + ... + P_{b-1}); logits_out_dev [n][V] (16-byte aligned) and hidden_out_dev [n][H] get
+ * row b for prompt b.  The norms and GEMMs run on the packed rows; RoPE, the KV append and the attention map every row
+ * and 32-query block back to its prompt, whose query blocks and key tiles start at its own row 0 / cache row 0.
+ * Bit-exactness: for every listed slot the KV cache rows [0, P_b), its logits row and its hidden row are bit-identical
+ * to fq3_prefill of that prompt into that slot alone; slots not listed are not touched.
+ * Scratch holds max_seq_len rows: when sum P_b exceeds it, the prompts run as consecutive groups in list order, each
+ * as many prompts as fit (one prompt of up to max_seq_len rows always does).  A group costs the launches of one
+ * fq3_prefill.
+ * Refused before anything is launched (no slot changes): n outside [1, max_batch], a slot listed twice, and per row
+ * what fq3_prefill refuses (slot out of range, P <= 0, P > max_seq_len = FQ3_ERR_TOO_LONG with the reference's
+ * message); the message names the row when n > 1. */
+int fq3_prefill_batch(fq3_engine* e, int32_t n, const int32_t* slots, const void* embeds_dev, const int32_t* P,
+                      const int32_t* n_left_pad, void* logits_out_dev, void* hidden_out_dev, void* stream);
 
 /* ---- fused path (the persistent on-device loop) ---------------------------------------------------------- */
 /* generate.py:120-147 / streaming.py:76-104: latch per-request state of `slot`.  past_hidden_dev [H] model dtype;
