@@ -1263,17 +1263,27 @@ __device__ __forceinline__ void small_kv_preload(Ctx& c, const StackDev& S, int 
   using Raw = typename SmallKV<BF>::Raw;
   const size_t esz = BF ? 2 : 4;
   const int g = c.warp < S.nKV ? c.warp : 0;
-  const uint8_t* kb = reinterpret_cast<const uint8_t*>(kc) + ((size_t)(layer * S.nKV + g) * S.S * 128) * esz;
-  const uint8_t* vb = reinterpret_cast<const uint8_t*>(vc) + ((size_t)(layer * S.nKV + g) * S.S * 128) * esz;
+  // `pre` lives in local memory (attention_small_all takes its address), and so does the Ctx: a store into `pre` may
+  // alias c.lane, so with the loads written straight into `pre` every load waited for the one before it (c.lane reloaded
+  // after each store, each store waiting for its load).  All loads go out first, into registers; then the copy.
+  const Raw* kp = reinterpret_cast<const Raw*>(reinterpret_cast<const uint8_t*>(kc) + ((size_t)(layer * S.nKV + g) * S.S * 128) * esz) + c.lane;
+  const Raw* vp = reinterpret_cast<const Raw*>(reinterpret_cast<const uint8_t*>(vc) + ((size_t)(layer * S.nKV + g) * S.S * 128) * esz) + c.lane;
+  constexpr int ROW = (int)(128 * (BF ? 2 : 4) / sizeof(Raw));   // Raw elements per cached row
+  Raw k[16], v[16];
 #pragma unroll
   for (int j = 0; j < 16; ++j) {
     if (j < slot0) {
-      pre.k[j] = __ldcg(reinterpret_cast<const Raw*>(kb + (size_t)j * 128 * esz) + c.lane);
-      pre.v[j] = __ldcg(reinterpret_cast<const Raw*>(vb + (size_t)j * 128 * esz) + c.lane);
+      k[j] = __ldcg(kp + j * ROW);
+      v[j] = __ldcg(vp + j * ROW);
     } else {
-      if constexpr (BF) { pre.k[j] = make_uint2(0, 0); pre.v[j] = make_uint2(0, 0); }
-      else { pre.k[j] = make_float4(0, 0, 0, 0); pre.v[j] = make_float4(0, 0, 0, 0); }
+      if constexpr (BF) { k[j] = make_uint2(0, 0); v[j] = make_uint2(0, 0); }
+      else { k[j] = make_float4(0, 0, 0, 0); v[j] = make_float4(0, 0, 0, 0); }
     }
+  }
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    pre.k[j] = k[j];
+    pre.v[j] = v[j];
   }
 }
 
