@@ -84,6 +84,7 @@ struct SlotParams {
   const void* tts_pad;
   const float* uniforms;
   long long* codes_out; // [n_frames][16]
+  float* logprob_out;   // [n_frames][16] or nullptr: col k >= 1 = codebook k of the frame, col 0 = the cb0 sampled after it
   int prefill_len, rope_delta, n_left_pad, max_new, min_new, trailing_len;
   int text_open;        // more trailing rows may follow: a frame that would read row >= trailing_len waits (stops the slot)
   Sampling sp_t, sp_p;
@@ -848,6 +849,7 @@ struct SampleArgs {
   int sup0;             // ids in [sup0, V) except eos are suppressed (V = none)   generate.py:46-50
   bool suppress_eos;
   int eos;
+  float* lp = nullptr;  // when set, thread 0 writes the log-probability of the drawn id here (DESIGN.md §4)
 };
 
 __device__ __forceinline__ uint32_t fkey(float f) {  // order-preserving float -> uint
@@ -892,6 +894,13 @@ __device__ int sample_block(Ctx& c, const SampleArgs& a) {
       const float om = SMEM().red[w];
       const int oi = SMEM().hist[w];
       if (om > m || (om == m && oi < bi2)) { m = om; bi2 = oi; }
+    }
+    if (a.lp) {  // log-softmax at the argmax, no temperature: (l_tok - m) - log(sum exp(l - m)) with l_tok == m
+      csync();   // every warp has read red[] / hist[] above before block_sum overwrites red[]
+      float se = 0.f;
+      for (int v = c.tid; v < V; v += NCT) se += expf(lg[v] - m);
+      se = block_sum(c, se);
+      if (c.tid == 0) *a.lp = -logf(se);
     }
     csync();
     return bi2;
@@ -980,6 +989,10 @@ __device__ int sample_block(Ctx& c, const SampleArgs& a) {
       if ((int)rk[v] >= keep) lg[v] = -INFINITY;
     csync();
   }
+  // the processed row the draw uses, kept for the log-probability (the softmax below overwrites lg; xin is free here)
+  float* lraw = &SMEM().xin[0][0];
+  if (a.lp)
+    for (int v = c.tid; v < V; v += NCT) lraw[v] = lg[v];
   // softmax -> probabilities in model dtype (F.softmax on a dtype tensor)
   float mx = -INFINITY;
   for (int v = c.tid; v < V; v += NCT) mx = fmaxf(mx, lg[v]);
@@ -1051,6 +1064,8 @@ __device__ int sample_block(Ctx& c, const SampleArgs& a) {
     for (int w = 1; w < NCW; ++w) tok = max(tok, SMEM().hist[w]);
     if (tok < 0) tok = 0;
   }
+  // fp32 log-softmax of the processed row at the drawn id, from the max and exp-sum the softmax reduced
+  if (a.lp && c.tid == 0) *a.lp = (lraw[tok] - mx) - logf(sm);
   csync();
   return tok;
 }
@@ -1700,9 +1715,9 @@ __device__ __forceinline__ void head_logits(Ctx& c, int seg, int H) {
 }
 
 // predictor: 15 passes (predictor_graph.py:115-167).  Inputs: s.xin[0] = past_hidden, s.xin[1] = embed(cb0 token).
-// Outputs s.codes[1..15].  u15: 15 uniforms.
+// Outputs s.codes[1..15].  u15: 15 uniforms.  lp_row: the frame's log-probability row (pass i -> column i + 1) or nullptr.
 template <bool BF>
-__device__ void predictor_frame(Ctx& c, const float* u15, bool dbg) {
+__device__ void predictor_frame(Ctx& c, const float* u15, bool dbg, float* lp_row) {
   const KParams& P = c.P;
   const StackDev& S = P.p;
   const int Ht = P.t.H;
@@ -1739,6 +1754,7 @@ __device__ void predictor_frame(Ctx& c, const float* u15, bool dbg) {
     SampleArgs sa;
     sa.logits = P.LOGITS; sa.V = S.V; sa.sp = P.req.sp_p; sa.u = u15 ? __ldg(u15 + i) : 0.f;
     sa.use_penalty = false; sa.sup0 = S.V; sa.suppress_eos = false; sa.eos = -1;
+    sa.lp = lp_row ? lp_row + 1 + i : nullptr;
     const int tok = sample_block<BF>(c, sa);
     if (c.tid == 0) SMEM().codes[i + 1] = tok;
     csync();
@@ -1844,7 +1860,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) fq3_decode_kernel(const __grid_co
     } else if (P.mode == MODE_PRED_RUN) {
       for (int k = tid; k < 2 * Ht; k += NCT) s.xin[k / Ht][k % Ht] = ldw<BF>(P.pred_input, k);
       csync();
-      predictor_frame<BF>(c, rq.sp_p.do_sample ? P.pred_uniforms : nullptr, P.dbg_on != 0);
+      predictor_frame<BF>(c, rq.sp_p.do_sample ? P.pred_uniforms : nullptr, P.dbg_on != 0, nullptr);
       if (cta == 0 && tid < P.ncb) rq.codes_out[tid] = (long long)s.codes[tid + 1];
     } else {
       // ---------------- fused frame loop: generate.py:149-199 / streaming.py:106-173 ----------------
@@ -1871,7 +1887,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) fq3_decode_kernel(const __grid_co
         const float* urow = rq.uniforms + (size_t)(step + 1) * 16;
         const int pslot = 2048 + 8 * (emitted & 63);
         probe_at(c, pslot + 0);
-        predictor_frame<BF>(c, rq.sp_p.do_sample ? urow + 1 : nullptr, false);
+        // CTA 0 writes the log-probabilities, as it writes the codes
+        float* lp_row = (rq.logprob_out && cta == 0) ? rq.logprob_out + (size_t)emitted * 16 : nullptr;
+        predictor_frame<BF>(c, rq.sp_p.do_sample ? urow + 1 : nullptr, false, lp_row);
         probe_at(c, pslot + 1);
         if (cta == 0 && tid < 16) rq.codes_out[(size_t)emitted * 16 + tid] = (long long)s.codes[tid];
         emitted++;
@@ -1899,6 +1917,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) fq3_decode_kernel(const __grid_co
         sa.logits = P.LOGITS; sa.V = P.t.V; sa.sp = rq.sp_t; sa.u = rq.sp_t.do_sample ? __ldg(urow) : 0.f;
         sa.use_penalty = true; sa.sup0 = P.t.V > 1024 ? P.t.V - 1024 : 0;
         sa.suppress_eos = (step + 1) < rq.min_new; sa.eos = P.eos;
+        sa.lp = lp_row;   // column 0: the cb0 that follows this frame (next frame's, or EOS)
         token = sample_block<BF>(c, sa);
         probe_at(c, pslot + 5);
         step++;

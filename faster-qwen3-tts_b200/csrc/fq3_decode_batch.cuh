@@ -543,6 +543,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) fq3_decode_batch_kernel(const __g
           sa.logits = P.LOGB + (size_t)v.b * VMAX; sa.V = Sp.V; sa.sp = me.sp_p;
           sa.u = (me.sp_p.do_sample && urow) ? __ldg(urow + 1 + i) : 0.f;
           sa.use_penalty = false; sa.sup0 = Sp.V; sa.suppress_eos = false; sa.eos = -1;
+          // the slot's rank-0 CTA writes the log-probabilities, as it writes the codes
+          if (me.logprob_out && v.rank == 0) sa.lp = me.logprob_out + (size_t)s.bst[BS_EMIT][v.b] * 16 + 1 + i;
           const int tok = sample_block<BF>(c, sa);
           if (tid == 0) s.codes[i + 1] = tok;
           csync();
@@ -605,6 +607,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) fq3_decode_batch_kernel(const __g
         sa.u = (me.sp_t.do_sample && urow) ? __ldg(urow) : 0.f;
         sa.use_penalty = true; sa.sup0 = P.t.V > 1024 ? P.t.V - 1024 : 0;
         sa.suppress_eos = (step + 1) < me.min_new; sa.eos = P.eos;
+        // column 0 of the frame just emitted (the bookkeeping above already counted it)
+        if (me.logprob_out && v.rank == 0) sa.lp = me.logprob_out + (size_t)(s.bst[BS_EMIT][v.b] - 1) * 16;
         const int tok = sample_block<BF>(c, sa);
         if (v.rank == 0 && tid == 0) P.TOKB[v.b] = tok;
       }

@@ -203,7 +203,7 @@ template <bool BF>
 __global__ void __launch_bounds__(NCT, 1)
     sample_kernel(const __grid_constant__ KParams P, const void* logits, int V, Sampling sp, float u,
                   const long long* hist, int n_hist, int suppress_special, int eos, int suppress_eos,
-                  long long* out) {
+                  long long* out, float* lp_out) {
   Smem& s = SMEM();
   const int tid = threadIdx.x;
   for (int i = tid; i < VMAX / 32; i += NCT) s.seen[i] = 0u;
@@ -222,6 +222,7 @@ __global__ void __launch_bounds__(NCT, 1)
   a.sup0 = suppress_special ? (V > 1024 ? V - 1024 : 0) : V;
   a.suppress_eos = suppress_eos != 0;
   a.eos = eos;
+  a.lp = lp_out;
   const int tok = sample_block<BF>(c, a);
   if (tid == 0) out[0] = tok;
 }
@@ -773,7 +774,7 @@ static void* slot_pk(fq3_engine* e, int s) { return (uint8_t*)e->p_kc + (size_t)
 static void* slot_pv(fq3_engine* e, int s) { return (uint8_t*)e->p_vc + (size_t)s * e->pkv_slot; }
 
 // the kernels' record of slot s: its caches and state, the request it latched, where its codes go
-static SlotParams slot_params(fq3_engine* e, int s, long long* codes_out) {
+static SlotParams slot_params(fq3_engine* e, int s, long long* codes_out, float* logprob_out) {
   const SlotHost& h = e->slots[s];
   SlotParams p;
   p.kc = slot_tk(e, s); p.vc = slot_tv(e, s); p.pkc = slot_pk(e, s); p.pvc = slot_pv(e, s);
@@ -782,6 +783,7 @@ static SlotParams slot_params(fq3_engine* e, int s, long long* codes_out) {
   p.seen = e->seen + (size_t)s * (VMAX / 32);
   p.trailing = h.trailing; p.tts_pad = h.tts_pad; p.uniforms = h.uniforms;
   p.codes_out = codes_out;
+  p.logprob_out = logprob_out;
   p.prefill_len = h.prefill_len; p.rope_delta = h.rope_delta; p.n_left_pad = h.n_left_pad;
   p.max_new = h.max_new; p.min_new = h.min_new; p.trailing_len = h.trailing_len;
   p.text_open = h.text_open ? 1 : 0;
@@ -790,9 +792,9 @@ static SlotParams slot_params(fq3_engine* e, int s, long long* codes_out) {
 }
 
 // kernel parameters of a single-sequence launch on slot s
-static KParams kp_for_slot(fq3_engine* e, int s, long long* codes_out) {
+static KParams kp_for_slot(fq3_engine* e, int s, long long* codes_out, float* logprob_out = nullptr) {
   KParams kp = e->kp;
-  kp.req = slot_params(e, s, codes_out);
+  kp.req = slot_params(e, s, codes_out, logprob_out);
   kp.nslots = 0;
   return kp;
 }
@@ -877,21 +879,28 @@ extern "C" int fq3_predictor_run(fq3_engine* e, int32_t slot, const void* pred_i
   return launch_decode(e, kp, (cudaStream_t)stream_);
 }
 
-extern "C" int fq3_sample_logits(fq3_engine* e, const void* logits_dev, int32_t V, const fq3_sampling* sp, float u,
-                                 const int64_t* history_dev, int32_t n_hist, int32_t suppress_special, int32_t eos_id,
-                                 int32_t suppress_eos, int64_t* token_out_dev, void* stream_) {
+extern "C" int fq3_sample_logits_lp(fq3_engine* e, const void* logits_dev, int32_t V, const fq3_sampling* sp, float u,
+                                    const int64_t* history_dev, int32_t n_hist, int32_t suppress_special, int32_t eos_id,
+                                    int32_t suppress_eos, int64_t* token_out_dev, float* logprob_out_dev, void* stream_) {
   if (!e || !logits_dev || !sp || !token_out_dev) return fail(FQ3_ERR_INVALID, "null argument");
   if (V <= 0 || V > VMAX) return fail(FQ3_ERR_INVALID, "V out of range");
   DevGuard dev_guard(e->dev);
   cudaStream_t stream = (cudaStream_t)stream_;
   const Sampling s = to_sampling(sp);
   if (e->bf16)
-    sample_kernel<true><<<1, NCT, smem_bytes(), stream>>>(e->kp, logits_dev, V, s, u, (const long long*)history_dev, history_dev ? n_hist : 0, suppress_special, eos_id, suppress_eos, (long long*)token_out_dev);
+    sample_kernel<true><<<1, NCT, smem_bytes(), stream>>>(e->kp, logits_dev, V, s, u, (const long long*)history_dev, history_dev ? n_hist : 0, suppress_special, eos_id, suppress_eos, (long long*)token_out_dev, logprob_out_dev);
   else
-    sample_kernel<false><<<1, NCT, smem_bytes(), stream>>>(e->kp, logits_dev, V, s, u, (const long long*)history_dev, history_dev ? n_hist : 0, suppress_special, eos_id, suppress_eos, (long long*)token_out_dev);
+    sample_kernel<false><<<1, NCT, smem_bytes(), stream>>>(e->kp, logits_dev, V, s, u, (const long long*)history_dev, history_dev ? n_hist : 0, suppress_special, eos_id, suppress_eos, (long long*)token_out_dev, logprob_out_dev);
   e->launches++;
   CK(cudaGetLastError());
   return 0;
+}
+
+extern "C" int fq3_sample_logits(fq3_engine* e, const void* logits_dev, int32_t V, const fq3_sampling* sp, float u,
+                                 const int64_t* history_dev, int32_t n_hist, int32_t suppress_special, int32_t eos_id,
+                                 int32_t suppress_eos, int64_t* token_out_dev, void* stream) {
+  return fq3_sample_logits_lp(e, logits_dev, V, sp, u, history_dev, n_hist, suppress_special, eos_id, suppress_eos,
+                              token_out_dev, nullptr, stream);
 }
 
 extern "C" int fq3_begin_request(fq3_engine* e, int32_t slot, const fq3_request* rq, const void* past_hidden_dev,
@@ -946,10 +955,12 @@ extern "C" int fq3_set_text_rows(fq3_engine* e, int32_t slot, int32_t trailing_l
 
 // batched launch: slots[0..n) become the columns of one pass over the weight tape
 static int launch_decode_batch(fq3_engine* e, const int32_t* slots, int n, int n_frames, long long* codes_out_dev,
-                               cudaStream_t stream) {
+                               float* logprob_out_dev, cudaStream_t stream) {
   if (!e->sl_dev) return fail(FQ3_ERR_STATE, "engine was created with max_batch = 1");
   if (n > e->ncta) return fail(FQ3_ERR_INVALID, "%d slots need at least as many CTAs (engine has %d)", n, e->ncta);
-  for (int j = 0; j < n; ++j) e->sl_host[j] = slot_params(e, slots[j], codes_out_dev + (size_t)j * n_frames * 16);
+  for (int j = 0; j < n; ++j)
+    e->sl_host[j] = slot_params(e, slots[j], codes_out_dev + (size_t)j * n_frames * 16,
+                                logprob_out_dev ? logprob_out_dev + (size_t)j * n_frames * 16 : nullptr);
   CK(cudaMemcpyAsync(e->sl_dev, e->sl_host, (size_t)n * sizeof(SlotParams), cudaMemcpyHostToDevice, stream));
   KParams kp = e->kp;
   kp.mode = MODE_FUSED;
@@ -990,8 +1001,8 @@ extern "C" int fq3_debug_gemv(fq3_engine* e, int32_t stack, int32_t layer, int32
   return launch_decode(e, kp, (cudaStream_t)stream_);
 }
 
-extern "C" int fq3_decode_chunk(fq3_engine* e, const int32_t* slots, int32_t n_slots, int32_t n_frames,
-                                int64_t* codes_out_dev, fq3_chunk_result* res, void* stream_) {
+extern "C" int fq3_decode_chunk_lp(fq3_engine* e, const int32_t* slots, int32_t n_slots, int32_t n_frames,
+                                   int64_t* codes_out_dev, float* logprob_out_dev, fq3_chunk_result* res, void* stream_) {
   if (!e || !slots || !codes_out_dev || !res) return fail(FQ3_ERR_INVALID, "null argument");
   if (n_slots <= 0 || n_slots > e->max_batch) return fail(FQ3_ERR_INVALID, "n_slots %d outside [1, max_batch=%d]", n_slots, e->max_batch);
   if (n_frames <= 0) return fail(FQ3_ERR_INVALID, "n_frames must be positive");
@@ -1005,13 +1016,13 @@ extern "C" int fq3_decode_chunk(fq3_engine* e, const int32_t* slots, int32_t n_s
   DevGuard dev_guard(e->dev);
   cudaStream_t stream = (cudaStream_t)stream_;
   if (n_slots == 1) {
-    KParams kp = kp_for_slot(e, slots[0], (long long*)codes_out_dev);
+    KParams kp = kp_for_slot(e, slots[0], (long long*)codes_out_dev, logprob_out_dev);
     kp.mode = MODE_FUSED;
     kp.n_frames = n_frames;
     kp.dbg_on = e->dbg_on & 2;   // timing probes only; layer dumps belong to the step-wise entry points
     if ((rc = launch_decode(e, kp, stream))) return rc;
   } else {
-    if ((rc = launch_decode_batch(e, slots, n_slots, n_frames, (long long*)codes_out_dev, stream))) return rc;
+    if ((rc = launch_decode_batch(e, slots, n_slots, n_frames, (long long*)codes_out_dev, logprob_out_dev, stream))) return rc;
   }
   for (int j = 0; j < n_slots; ++j)
     CK(cudaMemcpyAsync(e->state_host + 8 * j, e->state + 8 * slots[j], 32, cudaMemcpyDeviceToHost, stream));
@@ -1024,6 +1035,11 @@ extern "C" int fq3_decode_chunk(fq3_engine* e, const int32_t* slots, int32_t n_s
     res[j].frames_emitted = st[4];
   }
   return 0;
+}
+
+extern "C" int fq3_decode_chunk(fq3_engine* e, const int32_t* slots, int32_t n_slots, int32_t n_frames,
+                                int64_t* codes_out_dev, fq3_chunk_result* res, void* stream) {
+  return fq3_decode_chunk_lp(e, slots, n_slots, n_frames, codes_out_dev, nullptr, res, stream);
 }
 
 extern "C" int fq3_get_past_hidden(fq3_engine* e, int32_t slot, void* dst_dev, void* stream_) {

@@ -20,6 +20,7 @@ from typing import Dict, Generator, List, Optional, Tuple
 import torch
 
 from .generate import _sync, begin_fused, begin_fused_batch, shared_engine
+from .logprobs import FrameLogprobs
 
 
 @dataclass
@@ -33,6 +34,9 @@ class SlotRequest:
     feed: Optional[object] = None   # text_stream.TextFeed of a text-fed request (rows announced before every step)
     gen0: int = 0                   # generation_step at begin: the next frame reads trailing row gen0 + frames
     rows_ahead: int = 1             # text-fed: trailing rows that must exist beyond gen0 + frames before a launch
+    lp: Optional[FrameLogprobs] = None        # submit_many(logprobs=True): host assembly of the per-frame log-probabilities
+    chunk_logprobs: Optional[torch.Tensor] = None   # ... of the frames the last step returned, [n,16]
+    eos_logprob: Optional[float] = None       # ... of the EOS draw that ended the request
 
     def ready(self) -> bool:
         """A text-fed request is launched once the rows of its next ``rows_ahead`` frames exist (fewer where
@@ -99,11 +103,12 @@ class BatchScheduler:
         return rq
 
     @torch.inference_mode()
-    def submit_many(self, requests: List[dict]) -> List[SlotRequest]:
+    def submit_many(self, requests: List[dict], logprobs: bool = False) -> List[SlotRequest]:
         """Several requests at once: ``requests[i]`` holds the arguments of one ``submit`` call by name (tie, tam, tth,
         tpe, tag, the sampling keywords, uniforms, feed, rows_ahead).  They take the slots consecutive ``submit`` calls
         would take and latch what those would latch, but on a K3 engine their prompts share ONE prefill launch chain
-        (``generate.begin_fused_batch``).  All or none: on an error every slot is released."""
+        (``generate.begin_fused_batch``).  All or none: on an error every slot is released.  ``logprobs``: every
+        ``step`` also sets ``chunk_logprobs`` (and, at the end, ``eos_logprob``) of these requests (logprobs.py)."""
         n = len(requests)
         if n > len(self.free):
             raise RuntimeError(f"{n} requests but only {len(self.free)} of {self.engine.max_batch} request slots are free")
@@ -114,9 +119,14 @@ class BatchScheduler:
             gen.update({k: v for k, v in r.items() if k not in ("tag", "feed", "rows_ahead")})
             gen["trailing_len"] = None if r.get("feed") is None else 0
             rows.append(gen)
+        first_lps = [None] * n
         try:
             if n:
-                begin_fused_batch(self.engine, self.talker, rows, self.config, self.pg, self.tg, slots)
+                if logprobs:
+                    _, first_lps = begin_fused_batch(self.engine, self.talker, rows, self.config, self.pg, self.tg, slots,
+                                                     logprob=True)
+                else:   # the call of a scheduler without the option
+                    begin_fused_batch(self.engine, self.talker, rows, self.config, self.pg, self.tg, slots)
             for slot, r in zip(slots, requests):
                 if r.get("feed") is not None:
                     self.engine.set_text_rows(slot, r["feed"].update(), open=not r["feed"].closed)
@@ -124,10 +134,11 @@ class BatchScheduler:
             self.free = slots + self.free
             raise
         out = []
-        for slot, r, gen in zip(slots, requests, rows):
+        for slot, r, gen, flp in zip(slots, requests, rows, first_lps):
             tag = r.get("tag")
             rq = SlotRequest(slot=slot, tag=tag if tag is not None else slot, max_new_tokens=gen["max_new_tokens"],
-                             feed=r.get("feed"), gen0=self.engine.gen_step0[slot], rows_ahead=max(1, int(r.get("rows_ahead", 1))))
+                             feed=r.get("feed"), gen0=self.engine.gen_step0[slot], rows_ahead=max(1, int(r.get("rows_ahead", 1))),
+                             lp=FrameLogprobs(flp) if logprobs else None)
             self.active[slot] = rq
             out.append(rq)
         return out
@@ -142,17 +153,30 @@ class BatchScheduler:
         slots = sorted(s for s, rq in self.active.items() if rq.ready())
         if not slots:
             return []
-        if len(slots) == 1:
+        want_lp = any(self.active[s].lp is not None for s in slots)
+        lps = [None] * len(slots)
+        # off: the calls are exactly those of a scheduler without the option
+        if len(slots) == 1 and want_lp:
+            codes, lp, res = self.engine.decode_chunk(n_frames, slot=slots[0], logprobs=True)
+            outs, lps, ress = [codes], [lp], [res]
+        elif len(slots) == 1:
             codes, res = self.engine.decode_chunk(n_frames, slot=slots[0])
             outs, ress = [codes], [res]
         else:
-            buf, ress = self.engine.decode_chunk_batch(slots, n_frames)
+            if want_lp:
+                buf, lpb, ress = self.engine.decode_chunk_batch(slots, n_frames, logprobs=True)
+                lps = [lpb[j, : ress[j].frames_emitted] for j in range(len(slots))]
+            else:
+                buf, ress = self.engine.decode_chunk_batch(slots, n_frames)
             outs = [buf[j, : ress[j].frames_emitted] for j in range(len(slots))]
         done = []
-        for s, c, r in zip(slots, outs, ress):
+        for s, c, r, lp in zip(slots, outs, ress, lps):
             rq = self.active[s]
             rq.frames += int(r.frames_emitted)
             rq.finished = int(r.finished)
+            if rq.lp is not None:
+                rq.chunk_logprobs = rq.lp.push(lp)
+                rq.eos_logprob = rq.lp.eos_logprob(r.next_token, self.engine.eos)
             done.append((rq, c.clone()))
             if r.finished:
                 del self.active[s]
@@ -189,9 +213,11 @@ def fast_generate_streaming_batch(
     repetition_penalty: float = 1.05,
     chunk_size: int = 12,
     uniforms: Optional[torch.Tensor] = None,   # [B, max_new_tokens+1, 16]
+    return_logprobs: bool = False,
 ) -> Generator[List[Tuple[int, torch.Tensor, dict]], None, None]:
     """Batched counterpart of ``fast_generate_streaming`` (streaming.py:19-188): every yielded item is the list of
-    (row, codes [n,16], timing) of the rows that produced frames in that chunk; timing keys are the reference's."""
+    (row, codes [n,16], timing) of the rows that produced frames in that chunk; timing keys are the reference's, plus
+    with ``return_logprobs`` "logprobs" [n,16] and, on a row's last chunk, "eos_logprob" (as fast_generate_streaming)."""
     engine = shared_engine(predictor_graph, talker_graph)
     if engine is None:
         raise RuntimeError("batched decode needs graph handles backed by one loaded fq3 engine")
@@ -205,7 +231,8 @@ def fast_generate_streaming_batch(
                             tth=_rows(trailing_text_hiddens, b), tpe=tts_pad_embed, tag=b, max_new_tokens=max_new_tokens,
                             min_new_tokens=min_new_tokens, temperature=temperature, top_k=top_k, top_p=top_p,
                             do_sample=do_sample, repetition_penalty=repetition_penalty,
-                            uniforms=None if uniforms is None else uniforms[b]) for b in range(B)])
+                            uniforms=None if uniforms is None else uniforms[b]) for b in range(B)],
+                      logprobs=return_logprobs)
     _sync(device)
     t_prefill = time.time() - t0
     idx = 0
@@ -224,6 +251,10 @@ def fast_generate_streaming_batch(
                   "decode_ms": dt * 1000, "total_steps_so_far": totals[rq.tag], "is_final": n < chunk_size or rq.finished == 3}
             if engine.time_kernels:
                 tm["kernel_ms"] = engine.last_kernel_ms
+            if return_logprobs:
+                tm["logprobs"] = rq.chunk_logprobs
+                if rq.finished or rq.eos_logprob is not None:   # nothing follows this chunk
+                    tm["eos_logprob"] = rq.eos_logprob
             items.append((rq.tag, codes, tm))
         if items:
             yield items
@@ -235,24 +266,34 @@ def fast_generate_batch(talker, talker_input_embeds, attention_mask, trailing_te
                         predictor_graph, talker_graph, max_new_tokens: int = 2048, min_new_tokens: int = 2,
                         temperature: float = 0.9, top_k: int = 50, top_p: float = 1.0, do_sample: bool = True,
                         repetition_penalty: float = 1.05, uniforms: Optional[torch.Tensor] = None,
-                        launch_frames: int = 64) -> Tuple[List[Optional[torch.Tensor]], dict]:
+                        launch_frames: int = 64, return_logprobs: bool = False) -> Tuple[List[Optional[torch.Tensor]], dict]:
     """Batched counterpart of ``fast_generate`` (generate.py:16-215): (list of codes [steps_b,16] or None per row,
-    timing with the reference's keys; ``steps`` is the total over rows)."""
+    timing with the reference's keys; ``steps`` is the total over rows).  ``return_logprobs``: timing also holds
+    "logprobs" (per row float32 [steps_b,16]) and "eos_logprob" (per row, or None)."""
     B = talker_input_embeds.shape[0]
     parts: List[List[torch.Tensor]] = [[] for _ in range(B)]
+    lparts: List[List[torch.Tensor]] = [[] for _ in range(B)]
+    eos_lp: List[Optional[float]] = [None] * B
     t0 = time.time()
     prefill_ms = 0.0
     for items in fast_generate_streaming_batch(
             talker, talker_input_embeds, attention_mask, trailing_text_hiddens, tts_pad_embed, config, predictor_graph,
             talker_graph, max_new_tokens=max_new_tokens, min_new_tokens=min_new_tokens, temperature=temperature,
             top_k=top_k, top_p=top_p, do_sample=do_sample, repetition_penalty=repetition_penalty,
-            chunk_size=launch_frames, uniforms=uniforms):
+            chunk_size=launch_frames, uniforms=uniforms, return_logprobs=return_logprobs):
         for b, codes, tm in items:
             parts[b].append(codes)
+            if return_logprobs:
+                lparts[b].append(tm["logprobs"])
+                eos_lp[b] = tm.get("eos_logprob", eos_lp[b])
             prefill_ms = max(prefill_ms, tm["prefill_ms"])
     _sync(talker_input_embeds.device)
     dt = time.time() - t0 - prefill_ms / 1000
     out = [torch.cat(p) if p else None for p in parts]
     n = sum(int(c.shape[0]) for c in out if c is not None)
-    return out, {"prefill_ms": prefill_ms, "decode_s": dt, "steps": n, "ms_per_step": (dt / n * 1000) if n else 0,
-                 "steps_per_s": (n / dt) if dt > 0 else 0}
+    timing = {"prefill_ms": prefill_ms, "decode_s": dt, "steps": n, "ms_per_step": (dt / n * 1000) if n else 0,
+              "steps_per_s": (n / dt) if dt > 0 else 0}
+    if return_logprobs:
+        timing["logprobs"] = [torch.cat(p) if p else torch.zeros(0, 16) for p in lparts]
+        timing["eos_logprob"] = eos_lp
+    return out, timing

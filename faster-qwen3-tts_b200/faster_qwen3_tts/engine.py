@@ -67,8 +67,8 @@ class ChunkResult(C.Structure):
 
 EXPORTS = [
     "fq3_engine_create", "fq3_engine_load_weights", "fq3_engine_destroy", "fq3_import_kv", "fq3_export_kv",
-    "fq3_set_generation_state", "fq3_talker_step", "fq3_predictor_run", "fq3_sample_logits", "fq3_begin_request",
-    "fq3_decode_chunk", "fq3_set_text_rows", "fq3_get_past_hidden", "fq3_debug_enable", "fq3_debug_read", "fq3_tape_bytes",
+    "fq3_set_generation_state", "fq3_talker_step", "fq3_predictor_run", "fq3_sample_logits", "fq3_sample_logits_lp",
+    "fq3_begin_request", "fq3_decode_chunk", "fq3_decode_chunk_lp", "fq3_set_text_rows", "fq3_get_past_hidden", "fq3_debug_enable", "fq3_debug_read", "fq3_tape_bytes",
     "fq3_num_ctas", "fq3_launch_count", "fq3_last_error", "fq3_version", "fq3_engine_set_prefill_weights", "fq3_prefill", "fq3_prefill_batch", "fq3_max_batch", "fq3_debug_gemv",
     "fq3_debug_conv_gemm",
     "fq3_codec_create", "fq3_codec_load_weights", "fq3_codec_flops",
@@ -122,10 +122,14 @@ def load_library() -> C.CDLL:
                                       C.c_void_p]
     lib.fq3_sample_logits.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(Sampling), C.c_float, C.c_void_p,
                                       C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
+    lib.fq3_sample_logits_lp.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(Sampling), C.c_float, C.c_void_p,
+                                         C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.fq3_begin_request.argtypes = [C.c_void_p, C.c_int32, C.POINTER(Request), C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_void_p, C.POINTER(Sampling), C.POINTER(Sampling), C.c_void_p]
     lib.fq3_decode_chunk.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_int32, C.c_void_p,
                                      C.POINTER(ChunkResult), C.c_void_p]
+    lib.fq3_decode_chunk_lp.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                        C.POINTER(ChunkResult), C.c_void_p]
     lib.fq3_set_text_rows.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32]
     lib.fq3_get_past_hidden.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
     lib.fq3_max_batch.argtypes = [C.c_void_p]
@@ -387,16 +391,20 @@ class Engine:
 
     def sample_logits(self, logits: torch.Tensor, sp: SamplingParams, u: float = 0.0,
                       history: Optional[torch.Tensor] = None, suppress_special: bool = False, eos_id: int = -1,
-                      suppress_eos: bool = False) -> torch.Tensor:
+                      suppress_eos: bool = False, return_logprob: bool = False):
+        """token [1] (device); with ``return_logprob``: (token [1], float32 [1] log-probability of the draw,
+        fq3_decode_chunk_lp's definition)."""
         lg = self._t(logits.reshape(-1))
         out = torch.empty(1, dtype=torch.long, device=self.device)
+        lp = torch.empty(1, dtype=torch.float32, device=self.device) if return_logprob else None
         h = self._t(history.reshape(-1), torch.long) if history is not None and history.numel() else None
         s = sp.c()
-        _check(self.lib, self.lib.fq3_sample_logits(self.h, lg.data_ptr(), lg.numel(), C.byref(s), float(u),
-                                                     h.data_ptr() if h is not None else None,
-                                                     h.numel() if h is not None else 0, int(suppress_special), int(eos_id),
-                                                     int(suppress_eos), out.data_ptr(), self._stream()))
-        return out
+        _check(self.lib, self.lib.fq3_sample_logits_lp(self.h, lg.data_ptr(), lg.numel(), C.byref(s), float(u),
+                                                        h.data_ptr() if h is not None else None,
+                                                        h.numel() if h is not None else 0, int(suppress_special),
+                                                        int(eos_id), int(suppress_eos), out.data_ptr(),
+                                                        lp.data_ptr() if lp is not None else None, self._stream()))
+        return (out, lp) if return_logprob else out
 
     # -- fused path ----------------------------------------------------------------------------------------
     def begin_request(self, *, first_token: int, prefill_len: int, gen_step: int, past_hidden: torch.Tensor,
@@ -440,39 +448,63 @@ class Engine:
             raise ValueError(f"trailing_len {trailing_len} exceeds the {cap} rows latched for slot {slot}")
         _check(self.lib, self.lib.fq3_set_text_rows(self.h, int(slot), int(trailing_len), int(bool(open))))
 
-    def decode_chunk(self, n_frames: int, out: Optional[torch.Tensor] = None, slot: int = 0) -> Tuple[torch.Tensor, ChunkResult]:
-        """Single-sequence launch on one slot: (codes [frames_emitted,16], result)."""
+    def _logprob_buf(self, logprobs, shape):
+        """float32 device buffer for fq3_decode_chunk_lp: None = off, True = a new one, or the caller's tensor"""
+        if logprobs is None or logprobs is False:
+            return None
+        if logprobs is True:
+            return torch.empty(*shape, dtype=torch.float32, device=self.device)
+        if not (logprobs.device == self.device and logprobs.dtype == torch.float32 and logprobs.is_contiguous()
+                and tuple(logprobs.shape) == tuple(shape)):
+            raise ValueError(f"logprobs must be a contiguous float32 tensor of shape {tuple(shape)} on {self.device}")
+        return logprobs
+
+    def decode_chunk(self, n_frames: int, out: Optional[torch.Tensor] = None, slot: int = 0, logprobs=None):
+        """Single-sequence launch on one slot: (codes [frames_emitted,16], result).  ``logprobs`` (True or a float32
+        [n_frames,16] device tensor): also return the log-probability of every draw, (codes, logprobs
+        [frames_emitted,16], result) -- column 0 of a row is the cb0 sampled after that frame (fq3_decode_chunk_lp)."""
         if out is None:
             out = torch.empty(n_frames, 16, dtype=torch.long, device=self.device)
+        lp = self._logprob_buf(logprobs, (n_frames, 16))
         res = ChunkResult()
         sl = (C.c_int32 * 1)(int(slot))
         if self.time_kernels:
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
-        _check(self.lib, self.lib.fq3_decode_chunk(self.h, sl, 1, int(n_frames), out.data_ptr(), C.byref(res), self._stream()))
+        _check(self.lib, self.lib.fq3_decode_chunk_lp(self.h, sl, 1, int(n_frames), out.data_ptr(),
+                                                       lp.data_ptr() if lp is not None else None, C.byref(res),
+                                                       self._stream()))
         if self.time_kernels:
             e1.record()
             e1.synchronize()
             self.last_kernel_ms = e0.elapsed_time(e1)
+        if lp is not None:
+            return out[: res.frames_emitted], lp[: res.frames_emitted], res
         return out[: res.frames_emitted], res
 
-    def decode_chunk_batch(self, slots, n_frames: int, out: Optional[torch.Tensor] = None):
+    def decode_chunk_batch(self, slots, n_frames: int, out: Optional[torch.Tensor] = None, logprobs=None):
         """All listed slots advance up to n_frames frames in ONE launch sharing every pass over the weights.
-        Returns (codes [n_slots, n_frames, 16] -- row j valid up to results[j].frames_emitted --, [ChunkResult])."""
+        Returns (codes [n_slots, n_frames, 16] -- row j valid up to results[j].frames_emitted --, [ChunkResult]).
+        ``logprobs`` (True or a float32 [n_slots,n_frames,16] device tensor): (codes, logprobs, results), valid as the
+        codes are."""
         slots = [int(x) for x in slots]
         n = len(slots)
         if out is None:
             out = torch.empty(n, n_frames, 16, dtype=torch.long, device=self.device)
+        lp = self._logprob_buf(logprobs, (n, n_frames, 16))
         res = (ChunkResult * n)()
         sl = (C.c_int32 * n)(*slots)
         if self.time_kernels:
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
-        _check(self.lib, self.lib.fq3_decode_chunk(self.h, sl, n, int(n_frames), out.data_ptr(), res, self._stream()))
+        _check(self.lib, self.lib.fq3_decode_chunk_lp(self.h, sl, n, int(n_frames), out.data_ptr(),
+                                                       lp.data_ptr() if lp is not None else None, res, self._stream()))
         if self.time_kernels:
             e1.record()
             e1.synchronize()
             self.last_kernel_ms = e0.elapsed_time(e1)
+        if lp is not None:
+            return out, lp, list(res)
         return out, list(res)
 
     def past_hidden(self, slot: int = 0) -> torch.Tensor:

@@ -10,6 +10,7 @@ from typing import Optional, Tuple
 import torch
 
 from .engine import SamplingParams
+from .logprobs import FrameLogprobs
 from .sampling import apply_repetition_penalty, sample_logits
 
 _MAX_LAUNCH_FRAMES = 256
@@ -50,10 +51,13 @@ def _native_out(logits, hidden):
                                  past_key_values=None)
 
 
-def _first_token(engine, out, config, uniforms, u0, *, min_new_tokens, temperature, top_k, top_p, do_sample, **_):
-    """first cb0 token of a prefilled row (generate.py:119-120), a device tensor [1]"""
+def _first_token(engine, out, config, uniforms, u0, *, min_new_tokens, temperature, top_k, top_p, do_sample,
+                 logprob=False, **_):
+    """first cb0 token of a prefilled row (generate.py:119-120), a device tensor [1]; with ``logprob``: (token,
+    its log-probability float32 [1])"""
     return engine.sample_logits(out.logits[:, -1, :], SamplingParams(do_sample, top_k, temperature, top_p, 1.0), u=u0,
-                                suppress_special=True, eos_id=config.codec_eos_token_id, suppress_eos=min_new_tokens > 0)
+                                suppress_special=True, eos_id=config.codec_eos_token_id, suppress_eos=min_new_tokens > 0,
+                                return_logprob=logprob)
 
 
 def _uniforms(engine, predictor_graph, uniforms, *, max_new_tokens, do_sample, **_):
@@ -92,10 +96,11 @@ def latch_fused(engine, talker, out, native, pad, tie, tth, tpe, predictor_graph
 
 def begin_fused(engine, talker, tie, tam, tth, tpe, config, predictor_graph, talker_graph, *, max_new_tokens,
                 min_new_tokens, temperature, top_k, top_p, do_sample, repetition_penalty, uniforms, slot=None,
-                trailing_len=None):
+                trailing_len=None, logprob=False):
     """Prefill + first token + request latch (generate.py:104-140) for ONE row [1,P,H] into request slot `slot`
     (default: the slot the graph handles drive).  ``trailing_len``: rows of ``tth`` valid now (text-fed requests latch
-    a larger buffer and announce rows later, ``Engine.set_text_rows``).  Returns the first token id."""
+    a larger buffer and announce rows later, ``Engine.set_text_rows``).  Returns the first token id; with ``logprob``
+    (first token id, its log-probability as a float)."""
     gen = dict(max_new_tokens=max_new_tokens, min_new_tokens=min_new_tokens, temperature=temperature, top_k=top_k,
                top_p=top_p, do_sample=do_sample, repetition_penalty=repetition_penalty)
     slot = int(getattr(talker_graph, "slot", 0) if slot is None else slot)
@@ -108,22 +113,28 @@ def begin_fused(engine, talker, tie, tam, tth, tpe, config, predictor_graph, tal
         out = _prefill(talker, tie, tam, tth, tpe)
     uniforms = _uniforms(engine, predictor_graph, uniforms, **gen)
     u0 = float(uniforms.reshape(-1)[0]) if (do_sample and uniforms is not None) else 0.0
-    first = _first_token(engine, out, config, uniforms, u0, **gen)
+    first = _first_token(engine, out, config, uniforms, u0, logprob=logprob, **gen)
+    lp = None
+    if logprob:
+        first, lp = first
     latch_fused(engine, talker, out, native, pad, tie, tth, tpe, predictor_graph, talker_graph, first.item(), slot=slot,
                 uniforms=uniforms, trailing_len=trailing_len, **gen)
-    return first
+    return (first, float(lp.item())) if logprob else first
 
 
-def begin_fused_batch(engine, talker, rows, config, predictor_graph, talker_graph, slots):
+def begin_fused_batch(engine, talker, rows, config, predictor_graph, talker_graph, slots, logprob=False):
     """``begin_fused`` for several rows into distinct slots: ``rows[b]`` holds the arguments of one ``begin_fused`` call
     (tie [1,P,H], tam, tth, tpe, the sampling keywords, uniforms, trailing_len).  On a K3 engine all prompts go through
     ONE ``Engine.prefill_batch`` and the first tokens of all rows come back with one host synchronisation; every row
     latches what ``begin_fused`` would latch.  Otherwise (fp32 engine, a graph that opts out of K3) each row takes
-    ``begin_fused``.  Returns the first token ids."""
+    ``begin_fused``.  Returns the first token ids; with ``logprob`` (ids, their log-probabilities as floats)."""
     if not all(_native_prefill(engine, talker_graph, r["tie"]) for r in rows):
-        return [int(begin_fused(engine, talker, r["tie"], r["tam"], r["tth"], r["tpe"], config, predictor_graph,
-                                talker_graph, slot=s, **{k: v for k, v in r.items() if k not in ("tie", "tam", "tth", "tpe")}))
-                for r, s in zip(rows, slots)]
+        got = [begin_fused(engine, talker, r["tie"], r["tam"], r["tth"], r["tpe"], config, predictor_graph, talker_graph,
+                           slot=s, logprob=logprob, **{k: v for k, v in r.items() if k not in ("tie", "tam", "tth", "tpe")})
+               for r, s in zip(rows, slots)]
+        if logprob:
+            return [int(f) for f, _ in got], [lp for _, lp in got]
+        return [int(f) for f in got]
     gens = [{k: v for k, v in r.items() if k not in ("tie", "tam", "tth", "tpe", "uniforms", "trailing_len")} for r in rows]
     n = len(rows)
     uniforms = [_uniforms(engine, predictor_graph, r.get("uniforms"), **g) for r, g in zip(rows, gens)]
@@ -134,12 +145,15 @@ def begin_fused_batch(engine, talker, rows, config, predictor_graph, talker_grap
     pads, u0 = [int(x) for x in head[:n]], head[n:]
     logits, hidden = engine.prefill_batch([r["tie"][0] for r in rows], pads, slots)
     outs = [_native_out(logits[b], hidden[b]) for b in range(n)]
-    firsts = torch.cat([_first_token(engine, o, config, u, x, **g) for o, u, x, g in zip(outs, uniforms, u0, gens)])
-    firsts = firsts.tolist()   # the one host synchronisation of the first tokens
+    got = [_first_token(engine, o, config, u, x, logprob=logprob, **g) for o, u, x, g in zip(outs, uniforms, u0, gens)]
+    lps = None
+    if logprob:
+        got, lps = [t for t, _ in got], torch.cat([lp for _, lp in got]).tolist()
+    firsts = torch.cat(got).tolist()   # the one host synchronisation of the first tokens
     for r, s, o, u, g, pad, first in zip(rows, slots, outs, uniforms, gens, pads, firsts):
         latch_fused(engine, talker, o, True, pad, r["tie"], r["tth"], r["tpe"], predictor_graph, talker_graph, first,
                     slot=int(s), uniforms=u, trailing_len=r.get("trailing_len"), **g)
-    return firsts
+    return (firsts, lps) if logprob else firsts
 
 
 def stepwise_frames(talker, tie, tam, tth, tpe, config, predictor_graph, talker_graph, *, max_new_tokens,
@@ -213,26 +227,40 @@ def fast_generate(
     subtalker_temperature: Optional[float] = None,
     parity_mode: bool = False,
     uniforms: Optional[torch.Tensor] = None,
+    return_logprobs: bool = False,
 ) -> Tuple[Optional[torch.Tensor], dict]:
-    """Returns (codes LongTensor[steps,16] or None, timing dict with the reference's keys)."""
+    """Returns (codes LongTensor[steps,16] or None, timing dict with the reference's keys).  ``return_logprobs`` (fused
+    engine path only): the timing dict also holds "logprobs" (float32 [steps,16], the log-probability of every code;
+    see logprobs.py) and "eos_logprob" (the EOS draw that ended the request, or None)."""
     device = talker_input_embeds.device
     skw = dict(max_new_tokens=max_new_tokens, min_new_tokens=min_new_tokens, temperature=temperature, top_k=top_k,
                top_p=top_p, do_sample=do_sample, repetition_penalty=repetition_penalty)
     if parity_mode:
+        if return_logprobs:
+            raise ValueError("return_logprobs needs the fused decode path, not parity_mode")
         return _upstream_generate(talker, talker_input_embeds, attention_mask, trailing_text_hiddens, tts_pad_embed,
                                   config, subtalker_dosample, subtalker_top_k, subtalker_top_p,
                                   subtalker_temperature, **skw)
     engine = shared_engine(predictor_graph, talker_graph)
+    if return_logprobs and engine is None:
+        raise ValueError("return_logprobs needs graph handles backed by one loaded fq3 engine (the fused decode path)")
     t0 = time.time()
     if engine is not None:
-        begin_fused(engine, talker, talker_input_embeds, attention_mask, trailing_text_hiddens, tts_pad_embed, config,
-                    predictor_graph, talker_graph, uniforms=uniforms, **skw)
+        lkw = {"logprob": True} if return_logprobs else {}   # off: the calls are exactly those without the option
+        first = begin_fused(engine, talker, talker_input_embeds, attention_mask, trailing_text_hiddens, tts_pad_embed,
+                            config, predictor_graph, talker_graph, uniforms=uniforms, **lkw, **skw)
         _sync(device)
         t_prefill = time.time() - t0
         t1 = time.time()
         parts = []
+        lpa = FrameLogprobs(first[1]) if return_logprobs else None
         while True:
-            codes, res = engine.decode_chunk(_MAX_LAUNCH_FRAMES, slot=getattr(talker_graph, "slot", 0))
+            slot = getattr(talker_graph, "slot", 0)
+            if lpa is not None:
+                codes, lp, res = engine.decode_chunk(_MAX_LAUNCH_FRAMES, slot=slot, logprobs=True)
+                lpa.push(lp)
+            else:
+                codes, res = engine.decode_chunk(_MAX_LAUNCH_FRAMES, slot=slot)
             if res.frames_emitted:
                 parts.append(codes.clone())
             if res.finished:
@@ -260,6 +288,9 @@ def fast_generate(
         "ms_per_step": (t_decode / n * 1000) if n > 0 else 0,
         "steps_per_s": (n / t_decode) if t_decode > 0 else 0,
     }
+    if return_logprobs:
+        timing["logprobs"] = lpa.frames()
+        timing["eos_logprob"] = lpa.eos_logprob(res.next_token, engine.eos)
     return all_codes, timing
 
 

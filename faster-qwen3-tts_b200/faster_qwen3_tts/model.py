@@ -29,6 +29,13 @@ logger = logging.getLogger(__name__)
 CONTEXT_FRAMES = 25  # model.py:1056
 
 
+def take_uniforms(seed: int, max_new_tokens: int, device="cuda") -> torch.Tensor:
+    """The draws of one take (``*_takes``): [max_new_tokens + 1, 16] uniforms from a CPU generator seeded with ``seed``,
+    so a take can be re-rendered alone (``fast_generate(..., uniforms=take_uniforms(seed, n))``) on any device."""
+    g = torch.Generator(device="cpu").manual_seed(int(seed))
+    return torch.rand(int(max_new_tokens) + 1, 16, generator=g).to(device)
+
+
 class _StreamWindow:
     """Per-request state of the streaming codec-window policy (model.py:1052-1135), push-style so that several
     requests of a batch can each keep their own window while their code chunks arrive interleaved.
@@ -790,6 +797,121 @@ class FasterQwen3TTS:
                                            max_new_tokens=max_new_tokens, min_new_tokens=min_new_tokens,
                                            temperature=temperature, top_k=top_k, top_p=top_p, do_sample=do_sample,
                                            repetition_penalty=repetition_penalty)
+
+    # ------------------------------------------------------------------ several takes of one request
+    def _check_takes(self, n_takes, seeds):
+        """refusals of the ``*_takes`` calls, before anything is launched; returns the seeds"""
+        mb = getattr(self.engine, "max_batch", 1)
+        if mb < 2:
+            raise ValueError("takes need an engine built with max_batch >= 2 (they decode in one batched launch)")
+        if not 1 <= int(n_takes) <= mb:
+            raise ValueError(f"n_takes={n_takes} must be in [1, max_batch={mb}]")
+        if seeds is None:
+            seeds = torch.randint(0, 2 ** 62, (int(n_takes),)).tolist()
+        seeds = [int(s) for s in seeds]
+        if len(seeds) != int(n_takes):
+            raise ValueError(f"{len(seeds)} seeds for {n_takes} takes")
+        return seeds
+
+    def _takes(self, prep, ref_codes, seeds, gen, chunk_size=64):
+        """The one implementation behind the three ``*_takes`` methods: the prompt ``prep`` latched into one slot per take
+        with ONE batched prefill (``BatchScheduler.submit_many``), all takes decoded together (one launch per chunk),
+        their PCM decoded with one codec call per length.  Take i draws its uniforms from ``take_uniforms(seeds[i])``."""
+        from .batching import BatchScheduler
+        from .logprobs import score
+        m, talker, config, tie, tam, tth, tpe = prep
+        talker.rope_deltas = None
+        n = len(seeds)
+        sched = BatchScheduler(self.engine, talker, config, self.predictor_graph, self.talker_graph)
+        reqs = [dict(tie=tie, tam=tam, tth=tth, tpe=tpe, tag=i,
+                     uniforms=take_uniforms(seeds[i], gen["max_new_tokens"], self.engine.device), **gen) for i in range(n)]
+        sched.submit_many(reqs, logprobs=True)
+        parts, done = [[] for _ in range(n)], [None] * n
+        while len(sched):
+            for rq, codes in sched.step(chunk_size):
+                parts[rq.tag].append(codes)
+                if rq.finished:
+                    done[rq.tag] = rq
+        codes = [torch.cat(p) if p else None for p in parts]
+        scores = []
+        for i, rq in enumerate(done):
+            sc = score(rq.lp.frames(), rq.eos_logprob)
+            sc["seed"] = seeds[i]
+            scores.append(sc)
+        return self._decode_takes(m.speech_tokenizer, codes, ref_codes), self.sample_rate, scores
+
+    def _decode_takes(self, st, codes, ref_codes):
+        """``_decode_all`` of every take, takes of equal length in ONE codec call (the decoder's rows are independent)"""
+        out = [np.zeros(1, dtype=np.float32)] * len(codes)
+        groups = {}
+        for i, c in enumerate(codes):
+            if c is not None:
+                groups.setdefault(int(c.shape[0]), []).append(i)
+        ref_len = ref_codes.shape[0] if ref_codes is not None else 0
+        for T, idxs in groups.items():
+            batch = torch.stack([codes[i] if ref_codes is None else torch.cat([ref_codes.to(codes[i].device), codes[i]])
+                                 for i in idxs])
+            audio_list, _ = st.decode({"audio_codes": batch})
+            for i, a in zip(idxs, audio_list):
+                a = self._to_numpy(a)
+                if ref_len > 0:
+                    a = a[int(ref_len / max(batch.shape[1], 1) * len(a)):]
+                out[i] = a
+        return out
+
+    @torch.inference_mode()
+    def generate_voice_clone_takes(self, text: str, language: str, ref_audio=None, ref_text: str = "",
+                                   max_new_tokens: int = 2048, min_new_tokens: int = 2, temperature: float = 0.9,
+                                   top_k: int = 50, top_p: float = 1.0, do_sample: bool = True,
+                                   repetition_penalty: float = 1.05, xvec_only: bool = False,
+                                   non_streaming_mode: Optional[bool] = None, append_silence: bool = True,
+                                   instruct: Optional[str] = None, voice_clone_prompt=None, n_takes: int = 4,
+                                   seeds: Optional[List[int]] = None):
+        """``n_takes`` renderings of one ``generate_voice_clone`` request for the price of one batched decode: one prompt,
+        one batched prefill, one launch per chunk for all takes.  Take i is the request run alone with the uniforms of
+        ``take_uniforms(seeds[i], max_new_tokens)`` -- bit for bit while both run the per-head talker attention (a lone
+        request past 192 cached keys switches to the split-key path unless ``FQ3_ATTN_SPLIT=0``).  Returns (audios, sample_rate, scores): ``scores[i]``
+        holds "logprobs" (float32 [T,16], the log-probability of every code), "eos_logprob", "total_logprob" (their sum,
+        EOS term included), "frames" and "seed".  A log-probability says how likely the sampler found its draws, not
+        how good the audio is: the calls rank nothing and pick nothing."""
+        seeds = self._check_takes(n_takes, seeds)
+        nsm = self._resolve_non_streaming_mode(non_streaming_mode, default=False)
+        m, talker, config, tie, tam, tth, tpe, ref_codes = self._prepare_generation(
+            text=text, language=language, ref_audio=ref_audio, ref_text=ref_text, xvec_only=xvec_only,
+            non_streaming_mode=nsm, append_silence=append_silence, voice_clone_prompt=voice_clone_prompt,
+            instruct=instruct)
+        return self._takes((m, talker, config, tie, tam, tth, tpe), ref_codes, seeds,
+                           self._text_gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p, do_sample,
+                                                 repetition_penalty))
+
+    @torch.inference_mode()
+    def generate_custom_voice_takes(self, text: str, speaker: str, language: str, instruct: Optional[str] = None,
+                                    non_streaming_mode: Optional[bool] = None, max_new_tokens: int = 2048,
+                                    min_new_tokens: int = 2, temperature: float = 0.9, top_k: int = 50,
+                                    top_p: float = 1.0, do_sample: bool = True, repetition_penalty: float = 1.05,
+                                    n_takes: int = 4, seeds: Optional[List[int]] = None):
+        """``n_takes`` renderings of one ``generate_custom_voice`` request (see ``generate_voice_clone_takes``)."""
+        self._require_type("custom_voice", "Loaded model does not support custom voice generation")
+        self._validate(language, speaker, check_speaker=True)
+        seeds = self._check_takes(n_takes, seeds)
+        instruct = self._drop_instruct_for_small_model(instruct)
+        prep = self._simple(text, speaker, instruct, language, True, non_streaming_mode, None)
+        return self._takes(prep, None, seeds, self._text_gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k,
+                                                                     top_p, do_sample, repetition_penalty))
+
+    @torch.inference_mode()
+    def generate_voice_design_takes(self, text: str, instruct: str, language: str,
+                                    non_streaming_mode: Optional[bool] = None, max_new_tokens: int = 2048,
+                                    min_new_tokens: int = 2, temperature: float = 0.9, top_k: int = 50,
+                                    top_p: float = 1.0, do_sample: bool = True, repetition_penalty: float = 1.05,
+                                    n_takes: int = 4, seeds: Optional[List[int]] = None):
+        """``n_takes`` renderings of one ``generate_voice_design`` request (see ``generate_voice_clone_takes``)."""
+        self._require_type("voice_design", "Loaded model does not support voice design generation")
+        self._validate(language)
+        seeds = self._check_takes(n_takes, seeds)
+        prep = self._simple(text, None, instruct, language, True, non_streaming_mode, None)
+        return self._takes(prep, None, seeds, self._text_gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k,
+                                                                     top_p, do_sample, repetition_penalty))
 
     # ------------------------------------------------------------------ incremental text input (text_stream.py)
     def _text_streaming(self, text_stream, language, speaker, instruct, voice_clone_prompt, non_streaming_mode,

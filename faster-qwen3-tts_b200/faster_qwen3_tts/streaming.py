@@ -10,6 +10,7 @@ from typing import Generator, Optional, Tuple
 import torch
 
 from .generate import _sync, begin_fused, shared_engine, special_suppress_mask, stepwise_frames
+from .logprobs import FrameLogprobs
 from .sampling import apply_repetition_penalty, sample_logits
 
 
@@ -37,23 +38,34 @@ def fast_generate_streaming(
     repetition_penalty: float = 1.05,
     chunk_size: int = 12,
     uniforms: Optional[torch.Tensor] = None,
+    return_logprobs: bool = False,
 ) -> Generator[Tuple[torch.Tensor, dict], None, None]:
     """Yields (codes LongTensor[chunk_steps,16], timing); the last chunk may be short and has is_final=True
-    only when it is a partial chunk, exactly like the reference."""
+    only when it is a partial chunk, exactly like the reference.  ``return_logprobs`` (fused engine path only): every
+    timing dict also holds "logprobs" (float32 [chunk_steps,16], the log-probability of every code; see logprobs.py),
+    and the last chunk of the request "eos_logprob" (the EOS draw that ends it, or None)."""
     device = talker_input_embeds.device
     skw = dict(max_new_tokens=max_new_tokens, min_new_tokens=min_new_tokens, temperature=temperature, top_k=top_k,
                top_p=top_p, do_sample=do_sample, repetition_penalty=repetition_penalty)
     engine = shared_engine(predictor_graph, talker_graph)
+    if return_logprobs and engine is None:
+        raise ValueError("return_logprobs needs graph handles backed by one loaded fq3 engine (the fused decode path)")
     t0 = time.time()
     total = idx = 0
     if engine is not None:
-        begin_fused(engine, talker, talker_input_embeds, attention_mask, trailing_text_hiddens, tts_pad_embed, config,
-                    predictor_graph, talker_graph, uniforms=uniforms, **skw)
+        lkw = {"logprob": True} if return_logprobs else {}   # off: the calls are exactly those without the option
+        first = begin_fused(engine, talker, talker_input_embeds, attention_mask, trailing_text_hiddens, tts_pad_embed,
+                            config, predictor_graph, talker_graph, uniforms=uniforms, **lkw, **skw)
+        lpa = FrameLogprobs(first[1]) if return_logprobs else None
         _sync(device)
         t_prefill = time.time() - t0
         t1 = time.time()
         while True:
-            codes, res = engine.decode_chunk(chunk_size, slot=getattr(talker_graph, "slot", 0))
+            slot = getattr(talker_graph, "slot", 0)
+            if lpa is not None:
+                codes, lp, res = engine.decode_chunk(chunk_size, slot=slot, logprobs=True)
+            else:
+                codes, res = engine.decode_chunk(chunk_size, slot=slot)
             n = res.frames_emitted
             if n:
                 total += n
@@ -62,6 +74,10 @@ def fast_generate_streaming(
                 tm = _timing(idx, n, t_prefill, time.time() - t1, total, n < chunk_size or res.finished == 3)
                 if engine.time_kernels:
                     tm["kernel_ms"] = engine.last_kernel_ms
+                if lpa is not None:
+                    tm["logprobs"] = lpa.push(lp)
+                    if res.finished or res.next_token == engine.eos:   # nothing follows this chunk
+                        tm["eos_logprob"] = lpa.eos_logprob(res.next_token, engine.eos)
                 yield codes.clone(), tm
                 idx += 1
                 t1 = time.time()

@@ -152,6 +152,12 @@ int fq3_predictor_run(fq3_engine* e, int32_t slot, const void* pred_input_dev, c
 int fq3_sample_logits(fq3_engine* e, const void* logits_dev, int32_t V, const fq3_sampling* sp, float u,
                       const int64_t* history_dev, int32_t n_hist, int32_t suppress_special, int32_t eos_id,
                       int32_t suppress_eos, int64_t* token_out_dev, void* stream);
+/* fq3_sample_logits (its NULL case) that also writes the log-probability of the drawn id to logprob_out_dev float32[1]
+ * when it is not NULL, as fq3_decode_chunk_lp defines it; the first cb0 token of a request needs it.  The draw is
+ * bit-identical with and without it. */
+int fq3_sample_logits_lp(fq3_engine* e, const void* logits_dev, int32_t V, const fq3_sampling* sp, float u,
+                         const int64_t* history_dev, int32_t n_hist, int32_t suppress_special, int32_t eos_id,
+                         int32_t suppress_eos, int64_t* token_out_dev, float* logprob_out_dev, void* stream);
 
 /* ---- K3: hand-written prefill (bf16 engines) ------------------------------------------------------------------ */
 /* Borrow row-major weights for the prompt GEMMs (caller keeps them alive, 16-byte aligned): t.qkv [L,(nH+2nKV)*128,H]
@@ -206,6 +212,19 @@ int fq3_set_text_rows(fq3_engine* e, int32_t slot, int32_t trailing_len, int32_t
  * lock-step and stop independently (EOS / max_new_tokens / max_seq_len).  Synchronises the stream. */
 int fq3_decode_chunk(fq3_engine* e, const int32_t* slots, int32_t n_slots, int32_t n_frames, int64_t* codes_out_dev,
                      fq3_chunk_result* res, void* stream);
+/* fq3_decode_chunk (its NULL case) that also returns the log-probability of every code it draws: logprob_out_dev float32
+ * [n_slots][n_frames][16] or NULL.  Column k >= 1 of frame f is codebook k (predictor pass k); column 0 is the cb0 token
+ * sampled at the end of frame f, i.e. frame f + 1's cb0 or the EOS that ends the request (a frame cut off by max_seq_len
+ * samples none and leaves column 0 unwritten).  The first cb0 of a request comes from fq3_sample_logits_lp.
+ * Computed in fp32 from exactly the values the draw used:
+ *   sampling: l = the processed row (dtype-rounded logits, repetition penalty, suppressed ids at -inf, / temperature
+ *             rounded, top-k / top-p filtered); lp = (l_tok - max l) - log(sum exp(l - max l)), the max and sum the
+ *             softmax before the draw reduces;
+ *   greedy:   the log-softmax of the penalised, suppressed logits at the chosen id (no temperature).
+ * Codes are bit-identical with and without logprob_out_dev.  Rows at or past a slot's frames_emitted are not written;
+ * neither is anything of a slot not listed. */
+int fq3_decode_chunk_lp(fq3_engine* e, const int32_t* slots, int32_t n_slots, int32_t n_frames, int64_t* codes_out_dev,
+                        float* logprob_out_dev, fq3_chunk_result* res, void* stream);
 /* last post-norm talker hidden (generate.py:198 past_hidden) of `slot` -> dst_dev [H] model dtype */
 int fq3_get_past_hidden(fq3_engine* e, int32_t slot, void* dst_dev, void* stream);
 int fq3_max_batch(fq3_engine* e);
