@@ -4,7 +4,10 @@
 Same endpoint and wire format as the reference's example server (POST /v1/audio/speech, response_format wav | pcm,
 streaming WAV with an unknown-length header; the reference's examples/openai_server.py:91-118,215-263), but requests are
 not serialised behind a lock (:71,181): up to --max-batch requests share every pass over the model weights and new
-requests join between chunks (faster_qwen3_tts/serving.py).
+requests join between chunks (faster_qwen3_tts/serving.py).  A streamed response is a listener: it is paced at real time
+by default, so the engine, which makes audio several times faster than it is played, serves the clients closest to running
+dry first and holds up to --max-slots requests (each costs its KV cache) on --max-batch launch columns.  The request field
+"pace" overrides that: a number = playback speed relative to real time, null = as fast as possible.
 
     python examples/openai_server.py --model synthetic:1.7B --max-batch 16 --port 8000
     curl -s localhost:8000/v1/audio/speech -H 'Content-Type: application/json' \\
@@ -23,6 +26,7 @@ sys.path.insert(0, os.path.join(ROOT, "faster-qwen3-tts_b200"))
 def build_app(model, batcher, voices, default_voice):
     from fastapi import FastAPI, HTTPException
     from fastapi.responses import StreamingResponse
+    from typing import Optional
     from pydantic import BaseModel
     from faster_qwen3_tts.serving import to_pcm16, voice_clone_request, wav_header
 
@@ -34,6 +38,7 @@ def build_app(model, batcher, voices, default_voice):
         voice: str = "alloy"
         response_format: str = "wav"   # wav | pcm
         speed: float = 1.0             # accepted, not applied (as in the reference)
+        pace: Optional[float] = 1.0    # the client plays at pace x real time; null: everything as fast as possible
 
     @app.get("/health")
     async def health():
@@ -49,8 +54,11 @@ def build_app(model, batcher, voices, default_voice):
         fmt = req.response_format.lower()
         if fmt not in ("wav", "pcm"):
             raise HTTPException(status_code=400, detail=f"response_format {fmt!r} not supported. Use: wav, pcm")
+        if req.pace is not None and not req.pace > 0:
+            raise HTTPException(status_code=400, detail=f"'pace' must be a positive number or null, got {req.pace}")
         ticket = batcher.submit(voice_clone_request(model, req.input, v.get("language", "Auto"), v["ref_audio"],
-                                                    v.get("ref_text", "")), max_new_tokens=v.get("max_new_tokens", 2048))
+                                                    v.get("ref_text", "")), pace=req.pace,
+                                max_new_tokens=v.get("max_new_tokens", 2048))
         loop = asyncio.get_event_loop()
         it = iter(ticket)
 
@@ -75,7 +83,9 @@ def main():
     ap.add_argument("--ref-audio", default=os.environ.get("QWEN_TTS_REF_AUDIO", "ref_audio.wav"))
     ap.add_argument("--ref-text", default=os.environ.get("QWEN_TTS_REF_TEXT", ""))
     ap.add_argument("--language", default=os.environ.get("QWEN_TTS_LANGUAGE", "Auto"))
-    ap.add_argument("--max-batch", type=int, default=16)
+    ap.add_argument("--max-batch", type=int, default=16, help="requests one launch advances together (<= 32)")
+    ap.add_argument("--max-slots", type=int, default=None,
+                    help="resident requests (default: --max-batch); more serves more paced listeners, each costs its KV cache")
     ap.add_argument("--chunk-size", type=int, default=8)
     ap.add_argument("--streaming-codec", default="window", choices=["window", "stateful"],
                     help="window: the reference's two-phase window policy (sample-exact); stateful: one decoder stream per "
@@ -90,9 +100,10 @@ def main():
     from faster_qwen3_tts.serving import batcher_for_model
     if args.model.startswith("synthetic:"):
         model = FasterQwen3TTS.from_synthetic(args.model.split(":", 1)[1], device=args.device, dtype=torch.bfloat16,
-                                              max_batch=args.max_batch)
+                                              max_batch=args.max_batch, max_slots=args.max_slots)
     else:
-        model = FasterQwen3TTS.from_pretrained(args.model, device=args.device, max_batch=args.max_batch)
+        model = FasterQwen3TTS.from_pretrained(args.model, device=args.device, max_batch=args.max_batch,
+                                               max_slots=args.max_slots)
     model.streaming_codec = args.streaming_codec
     if args.voices:
         voices = json.load(open(args.voices))

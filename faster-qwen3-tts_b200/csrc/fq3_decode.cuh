@@ -87,6 +87,7 @@ struct SlotParams {
   float* logprob_out;   // [n_frames][16] or nullptr: col k >= 1 = codebook k of the frame, col 0 = the cb0 sampled after it
   int prefill_len, rope_delta, n_left_pad, max_new, min_new, trailing_len;
   int text_open;        // more trailing rows may follow: a frame that would read row >= trailing_len waits (stops the slot)
+  int n_frames;         // batched kernel: frames this slot may emit in the launch (the single-sequence one reads KParams::n_frames)
   Sampling sp_t, sp_p;
 };
 

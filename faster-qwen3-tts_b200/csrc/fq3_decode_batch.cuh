@@ -473,7 +473,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) fq3_decode_batch_kernel(const __g
       // ---- which slots run this frame (identical decision in every CTA)
       if (warp == 0) {
         bool r = false;
-        if (lane < B && s.bst[BS_FIN][lane] == 0 && s.bst[BS_EMIT][lane] < P.n_frames) {
+        if (lane < B && s.bst[BS_FIN][lane] == 0 && s.bst[BS_EMIT][lane] < P.sl[lane].n_frames) {   // the slot's own budget
           if (s.bst[BS_STEP][lane] >= P.sl[lane].max_new) s.bst[BS_FIN][lane] = 1;
           else if (s.bst[BS_TOK][lane] == P.eos) s.bst[BS_FIN][lane] = 2;
           else r = !(P.sl[lane].text_open && s.bst[BS_GEN][lane] >= P.sl[lane].trailing_len);   // open text: wait for the row

@@ -75,7 +75,8 @@ struct fq3_engine {
   size_t esz;
   int ncta;
   int dev;
-  int max_batch = 1;
+  int max_batch = 1;   // columns a launch may carry
+  int max_slots = 1;   // resident request slots (>= max_batch)
   bool loaded = false;
   std::vector<SlotHost> slots;
   size_t tkv_slot = 0, pkv_slot = 0;   // bytes of one slot's K (or V) cache: talker / predictor
@@ -242,10 +243,33 @@ static int check_stack(const fq3_stack_config& s, const char* nm, int nt) {
   return 0;
 }
 
+// bytes of one slot's talker / predictor K (or V) cache
+static size_t tkv_bytes(const fq3_config& c, size_t esz) {
+  return (size_t)c.talker.num_hidden_layers * c.talker.num_key_value_heads * c.max_seq_len * 128 * esz;
+}
+static size_t pkv_bytes(const fq3_config& c, size_t esz) {
+  return (size_t)c.predictor.num_hidden_layers * c.predictor.num_key_value_heads * 32 * 128 * esz;
+}
+constexpr size_t STATE_BYTES = 32;   // 8 ints per slot
+
+extern "C" int64_t fq3_slot_bytes(const fq3_config* cfg) {
+  if (!cfg) return fail(FQ3_ERR_INVALID, "null argument");
+  if (cfg->dtype != FQ3_F32 && cfg->dtype != FQ3_BF16) return fail(FQ3_ERR_INVALID, "dtype must be FQ3_F32 or FQ3_BF16");
+  const size_t esz = cfg->dtype == FQ3_BF16 ? 2 : 4;
+  return (int64_t)(2 * tkv_bytes(*cfg, esz) + 2 * pkv_bytes(*cfg, esz) + STATE_BYTES + HMAX * sizeof(float) + VMAX / 8);
+}
+
+static int engine_alloc(fq3_engine* e, const cudaDeviceProp& prop);
+
 extern "C" int fq3_engine_create(const fq3_config* cfg, fq3_engine** out) {
   if (!cfg || !out) return fail(FQ3_ERR_INVALID, "null argument");
   if (cfg->dtype != FQ3_F32 && cfg->dtype != FQ3_BF16) return fail(FQ3_ERR_INVALID, "dtype must be FQ3_F32 or FQ3_BF16");
   int rc;
+  const int max_batch = cfg->max_batch > 0 ? cfg->max_batch : 1;
+  const int max_slots = cfg->max_slots != 0 ? cfg->max_slots : max_batch;
+  if (max_batch > MAXB) return fail(FQ3_ERR_INVALID, "max_batch %d exceeds %d", cfg->max_batch, MAXB);
+  if (max_slots < max_batch) return fail(FQ3_ERR_INVALID, "max_slots %d is smaller than max_batch %d", cfg->max_slots, max_batch);
+  if (max_slots > FQ3_MAX_SLOTS) return fail(FQ3_ERR_INVALID, "max_slots %d exceeds %d", cfg->max_slots, FQ3_MAX_SLOTS);
   if ((rc = check_stack(cfg->talker, "talker", 1))) return rc;
   if ((rc = check_stack(cfg->predictor, "predictor", 2))) return rc;
   if (cfg->talker.hidden_size > HMAX) return fail(FQ3_ERR_INVALID, "talker hidden_size > %d", HMAX);
@@ -269,8 +293,22 @@ extern "C" int fq3_engine_create(const fq3_config* cfg, fq3_engine** out) {
   e->esz = e->bf16 ? 2 : 4;
   e->dev = cfg->device;
   e->ncta = cfg->num_ctas > 0 ? std::min(cfg->num_ctas, prop.multiProcessorCount) : prop.multiProcessorCount;
-  e->max_batch = cfg->max_batch > 0 ? cfg->max_batch : 1;
-  if (e->max_batch > MAXB) { delete e; return fail(FQ3_ERR_INVALID, "max_batch %d exceeds %d", cfg->max_batch, MAXB); }
+  e->max_batch = max_batch;
+  e->max_slots = max_slots;
+  if ((rc = engine_alloc(e, prop))) {
+    // the engine owns every pointer it got so far: destroy frees them.  An allocation that did not fit leaves a
+    // non-sticky error behind, which must not surface in the caller's next CUDA call
+    fq3_engine_destroy(e);
+    cudaGetLastError();
+    return rc;
+  }
+  *out = e;
+  return 0;
+}
+
+// kernel attributes, every device allocation (all of them before the first memset) and the kernel parameter template
+static int engine_alloc(fq3_engine* e, const cudaDeviceProp& prop) {
+  const fq3_config* cfg = &e->cfg;
   if (e->bf16) {
     CK(cudaFuncSetAttribute(fq3_decode_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes()));
     CK(cudaFuncSetAttribute(fq3_decode_batch_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes()));
@@ -283,18 +321,22 @@ extern "C" int fq3_engine_create(const fq3_config* cfg, fq3_engine** out) {
   int occ = 0;
   if (e->bf16) CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fq3_decode_kernel<true>, NTHREADS, smem_bytes()));
   else CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fq3_decode_kernel<false>, NTHREADS, smem_bytes()));
-  if (occ < 1) { delete e; return fail(FQ3_ERR_INVALID, "decode kernel does not fit on an SM (smem %zu)", smem_bytes()); }
+  if (occ < 1) return fail(FQ3_ERR_INVALID, "decode kernel does not fit on an SM (smem %zu)", smem_bytes());
 
   const fq3_stack_config &T = cfg->talker, &Pc = cfg->predictor;
-  const int MB = e->max_batch;
-  e->slots.assign(MB, SlotHost());
-  const size_t tkv = (size_t)T.num_hidden_layers * T.num_key_value_heads * cfg->max_seq_len * 128 * e->esz;
-  const size_t pkv = (size_t)Pc.num_hidden_layers * Pc.num_key_value_heads * 32 * 128 * e->esz;
+  const int MS = e->max_slots;   // per-slot storage; everything a launch needs per column is sized MAXB / MAXCOL below
+  e->slots.assign(MS, SlotHost());
+  const size_t tkv = tkv_bytes(*cfg, e->esz), pkv = pkv_bytes(*cfg, e->esz);
   e->tkv_slot = tkv; e->pkv_slot = pkv;
-  CK(cudaMalloc(&e->t_kc, tkv * MB)); CK(cudaMalloc(&e->t_vc, tkv * MB));
-  CK(cudaMalloc(&e->p_kc, pkv * MB)); CK(cudaMalloc(&e->p_vc, pkv * MB));
-  CK(cudaMemset(e->t_kc, 0, tkv * MB)); CK(cudaMemset(e->t_vc, 0, tkv * MB));
-  CK(cudaMemset(e->p_kc, 0, pkv * MB)); CK(cudaMemset(e->p_vc, 0, pkv * MB));
+  // buffers to clear, once every allocation has succeeded
+  std::vector<std::pair<void*, size_t>> zero;
+  auto zalloc = [&](void** p, size_t bytes) -> cudaError_t {
+    cudaError_t r = cudaMalloc(p, bytes);
+    if (r == cudaSuccess) zero.push_back({*p, bytes});
+    return r;
+  };
+  CK(zalloc(&e->t_kc, tkv * MS)); CK(zalloc(&e->t_vc, tkv * MS));
+  CK(zalloc(&e->p_kc, pkv * MS)); CK(zalloc(&e->p_vc, pkv * MS));
   const int ldX = std::max(T.hidden_size, Pc.hidden_size);
   const int ldQKV = std::max((T.num_attention_heads + 2 * T.num_key_value_heads) * 128,
                              (Pc.num_attention_heads + 2 * Pc.num_key_value_heads) * 128);
@@ -303,18 +345,15 @@ extern "C" int fq3_engine_create(const fq3_config* cfg, fq3_engine** out) {
   CK(cudaMalloc(&e->X, 2 * ldX * sizeof(float))); CK(cudaMalloc(&e->X1, 2 * ldX * sizeof(float)));
   CK(cudaMalloc(&e->QKV, 2 * ldQKV * sizeof(float))); CK(cudaMalloc(&e->ATT, ldATT * e->esz));
   CK(cudaMalloc(&e->ACT, 2 * ldACT * sizeof(float))); CK(cudaMalloc(&e->LOGITS, VMAX * sizeof(float)));
-  CK(cudaMalloc(&e->bar, 32768)); CK(cudaMemset(e->bar, 0, 32768));
+  CK(zalloc((void**)&e->bar, 32768));
   CK(cudaMalloc(&e->PART, (size_t)T.num_attention_heads * 16 * PART_STRIDE * sizeof(float)));
-  CK(cudaMalloc(&e->state, 32 * MB)); CK(cudaMemset(e->state, 0, 32 * MB));   // 8 ints per slot
-  CK(cudaMallocHost(&e->state_host, 32 * MB));
-  CK(cudaMalloc(&e->past_hidden, (size_t)MB * HMAX * sizeof(float))); CK(cudaMemset(e->past_hidden, 0, (size_t)MB * HMAX * sizeof(float)));
-  CK(cudaMalloc(&e->seen, (size_t)MB * (VMAX / 8))); CK(cudaMemset(e->seen, 0, (size_t)MB * (VMAX / 8)));
-  if (MB > 1) {
-    // batched decode: activation matrices [column][ld] (column = slot, predictor pass 0: token * B + slot)
-    auto zalloc = [&](void** p, size_t bytes) -> cudaError_t {
-      cudaError_t r = cudaMalloc(p, bytes);
-      return r != cudaSuccess ? r : cudaMemset(*p, 0, bytes);
-    };
+  CK(zalloc((void**)&e->state, STATE_BYTES * MS));
+  CK(cudaMallocHost(&e->state_host, STATE_BYTES * e->max_batch));   // results of one launch: a row per column
+  CK(zalloc((void**)&e->past_hidden, (size_t)MS * HMAX * sizeof(float)));
+  CK(zalloc((void**)&e->seen, (size_t)MS * (VMAX / 8)));
+  if (e->max_batch > 1) {
+    // batched decode: activation matrices [column][ld] (column = position in the launch's slot list, predictor pass 0:
+    // token * B + column)
     CK(zalloc((void**)&e->XB, (size_t)MAXCOL * ldX * sizeof(float)));
     CK(zalloc((void**)&e->X1B, (size_t)MAXCOL * ldX * sizeof(float)));
     CK(zalloc((void**)&e->QKVB, (size_t)MAXCOL * ldQKV * sizeof(float)));
@@ -332,9 +371,9 @@ extern "C" int fq3_engine_create(const fq3_config* cfg, fq3_engine** out) {
     const long long rec_p = 2LL * (Pc.num_attention_heads + 2 * Pc.num_key_value_heads) * 128 + 2LL * Pc.num_attention_heads * 128 + 4LL * Pc.hidden_size + 2LL * Pc.intermediate_size;
     e->dbg_stride = std::max(rec_t, rec_p);
     e->dbg_floats = (size_t)e->dbg_stride * std::max(T.num_hidden_layers, Pc.num_hidden_layers);
-    CK(cudaMalloc(&e->dbg, e->dbg_floats * sizeof(float)));
-    CK(cudaMemset(e->dbg, 0, e->dbg_floats * sizeof(float)));
+    CK(zalloc((void**)&e->dbg, e->dbg_floats * sizeof(float)));
   }
+  for (auto& z : zero) CK(cudaMemset(z.first, 0, z.second));
   KParams& k = e->kp;
   memset(&k, 0, sizeof(k));
   auto fill = [&](StackDev& s, const fq3_stack_config& c, int S) {
@@ -364,7 +403,6 @@ extern "C" int fq3_engine_create(const fq3_config* cfg, fq3_engine** out) {
     k.PART = e->PART;
     k.attn_cnt = e->bar + 1024;
   }
-  *out = e;
   return 0;
 }
 
@@ -764,8 +802,12 @@ static Sampling to_sampling(const fq3_sampling* s) {
   return r;
 }
 
+// the bound on slot ids by the name the engine's creator gave it: an engine created without max_slots has one number,
+// max_batch, and callers written for it read (and match) messages that name it
+static const char* slot_bound(const fq3_engine* e) { return e->max_slots == e->max_batch ? "max_batch" : "max_slots"; }
 static int check_slot(fq3_engine* e, int slot) {
-  if (slot < 0 || slot >= e->max_batch) return fail(FQ3_ERR_INVALID, "slot %d outside [0, max_batch=%d)", slot, e->max_batch);
+  if (slot < 0 || slot >= e->max_slots)
+    return fail(FQ3_ERR_INVALID, "slot %d outside [0, %s=%d)", slot, slot_bound(e), e->max_slots);
   return 0;
 }
 static void* slot_tk(fq3_engine* e, int s) { return (uint8_t*)e->t_kc + (size_t)s * e->tkv_slot; }
@@ -774,7 +816,7 @@ static void* slot_pk(fq3_engine* e, int s) { return (uint8_t*)e->p_kc + (size_t)
 static void* slot_pv(fq3_engine* e, int s) { return (uint8_t*)e->p_vc + (size_t)s * e->pkv_slot; }
 
 // the kernels' record of slot s: its caches and state, the request it latched, where its codes go
-static SlotParams slot_params(fq3_engine* e, int s, long long* codes_out, float* logprob_out) {
+static SlotParams slot_params(fq3_engine* e, int s, int n_frames, long long* codes_out, float* logprob_out) {
   const SlotHost& h = e->slots[s];
   SlotParams p;
   p.kc = slot_tk(e, s); p.vc = slot_tv(e, s); p.pkc = slot_pk(e, s); p.pvc = slot_pv(e, s);
@@ -787,6 +829,7 @@ static SlotParams slot_params(fq3_engine* e, int s, long long* codes_out, float*
   p.prefill_len = h.prefill_len; p.rope_delta = h.rope_delta; p.n_left_pad = h.n_left_pad;
   p.max_new = h.max_new; p.min_new = h.min_new; p.trailing_len = h.trailing_len;
   p.text_open = h.text_open ? 1 : 0;
+  p.n_frames = n_frames;
   p.sp_t = h.sp_t; p.sp_p = h.sp_p;
   return p;
 }
@@ -794,7 +837,7 @@ static SlotParams slot_params(fq3_engine* e, int s, long long* codes_out, float*
 // kernel parameters of a single-sequence launch on slot s
 static KParams kp_for_slot(fq3_engine* e, int s, long long* codes_out, float* logprob_out = nullptr) {
   KParams kp = e->kp;
-  kp.req = slot_params(e, s, codes_out, logprob_out);
+  kp.req = slot_params(e, s, 0, codes_out, logprob_out);   // the single-sequence kernel's budget is KParams::n_frames
   kp.nslots = 0;
   return kp;
 }
@@ -954,19 +997,20 @@ extern "C" int fq3_set_text_rows(fq3_engine* e, int32_t slot, int32_t trailing_l
 }
 
 // batched launch: slots[0..n) become the columns of one pass over the weight tape
-static int launch_decode_batch(fq3_engine* e, const int32_t* slots, int n, int n_frames, long long* codes_out_dev,
-                               float* logprob_out_dev, cudaStream_t stream) {
+// (column j emits up to n_frames[j] frames into row j of the [n][max_frames][16] outputs)
+static int launch_decode_batch(fq3_engine* e, const int32_t* slots, int n, const int32_t* n_frames, int max_frames,
+                               long long* codes_out_dev, float* logprob_out_dev, cudaStream_t stream) {
   if (!e->sl_dev) return fail(FQ3_ERR_STATE, "engine was created with max_batch = 1");
   if (n > e->ncta) return fail(FQ3_ERR_INVALID, "%d slots need at least as many CTAs (engine has %d)", n, e->ncta);
   for (int j = 0; j < n; ++j)
-    e->sl_host[j] = slot_params(e, slots[j], codes_out_dev + (size_t)j * n_frames * 16,
-                                logprob_out_dev ? logprob_out_dev + (size_t)j * n_frames * 16 : nullptr);
+    e->sl_host[j] = slot_params(e, slots[j], n_frames[j], codes_out_dev + (size_t)j * max_frames * 16,
+                                logprob_out_dev ? logprob_out_dev + (size_t)j * max_frames * 16 : nullptr);
   CK(cudaMemcpyAsync(e->sl_dev, e->sl_host, (size_t)n * sizeof(SlotParams), cudaMemcpyHostToDevice, stream));
   KParams kp = e->kp;
   kp.mode = MODE_FUSED;
   kp.nslots = n;
   kp.sl = e->sl_dev;
-  kp.n_frames = n_frames;
+  kp.n_frames = max_frames;   // the producer warp's bound: no slot runs longer
   kp.dbg_on = e->dbg_on & 2;
   return launch_decode(e, kp, stream);
 }
@@ -1001,13 +1045,16 @@ extern "C" int fq3_debug_gemv(fq3_engine* e, int32_t stack, int32_t layer, int32
   return launch_decode(e, kp, (cudaStream_t)stream_);
 }
 
-extern "C" int fq3_decode_chunk_lp(fq3_engine* e, const int32_t* slots, int32_t n_slots, int32_t n_frames,
-                                   int64_t* codes_out_dev, float* logprob_out_dev, fq3_chunk_result* res, void* stream_) {
-  if (!e || !slots || !codes_out_dev || !res) return fail(FQ3_ERR_INVALID, "null argument");
-  if (n_slots <= 0 || n_slots > e->max_batch) return fail(FQ3_ERR_INVALID, "n_slots %d outside [1, max_batch=%d]", n_slots, e->max_batch);
-  if (n_frames <= 0) return fail(FQ3_ERR_INVALID, "n_frames must be positive");
-  int rc;
+extern "C" int fq3_decode_chunk_n(fq3_engine* e, const int32_t* slots, int32_t n_slots, const int32_t* n_frames,
+                                  int64_t* codes_out_dev, float* logprob_out_dev, fq3_chunk_result* res, void* stream_) {
+  if (!e || !slots || !n_frames || !codes_out_dev || !res) return fail(FQ3_ERR_INVALID, "null argument");
+  if (n_slots <= 0 || n_slots > e->max_batch)
+    return fail(FQ3_ERR_INVALID, "n_slots %d outside [1, max_batch=%d] (columns of one launch; the engine holds %d slots)",
+                n_slots, e->max_batch, e->max_slots);
+  int rc, max_frames = 0;
   for (int j = 0; j < n_slots; ++j) {
+    if (n_frames[j] <= 0) return fail(FQ3_ERR_INVALID, "n_frames must be positive (slot %d: %d)", slots[j], n_frames[j]);
+    max_frames = std::max(max_frames, (int)n_frames[j]);
     if ((rc = check_slot(e, slots[j]))) return rc;
     if (!e->slots[slots[j]].active) return fail(FQ3_ERR_STATE, "fq3_begin_request has not been called for slot %d", slots[j]);
     for (int i = 0; i < j; ++i)
@@ -1018,11 +1065,11 @@ extern "C" int fq3_decode_chunk_lp(fq3_engine* e, const int32_t* slots, int32_t 
   if (n_slots == 1) {
     KParams kp = kp_for_slot(e, slots[0], (long long*)codes_out_dev, logprob_out_dev);
     kp.mode = MODE_FUSED;
-    kp.n_frames = n_frames;
+    kp.n_frames = n_frames[0];
     kp.dbg_on = e->dbg_on & 2;   // timing probes only; layer dumps belong to the step-wise entry points
     if ((rc = launch_decode(e, kp, stream))) return rc;
   } else {
-    if ((rc = launch_decode_batch(e, slots, n_slots, n_frames, (long long*)codes_out_dev, logprob_out_dev, stream))) return rc;
+    if ((rc = launch_decode_batch(e, slots, n_slots, n_frames, max_frames, (long long*)codes_out_dev, logprob_out_dev, stream))) return rc;
   }
   for (int j = 0; j < n_slots; ++j)
     CK(cudaMemcpyAsync(e->state_host + 8 * j, e->state + 8 * slots[j], 32, cudaMemcpyDeviceToHost, stream));
@@ -1035,6 +1082,13 @@ extern "C" int fq3_decode_chunk_lp(fq3_engine* e, const int32_t* slots, int32_t 
     res[j].frames_emitted = st[4];
   }
   return 0;
+}
+
+extern "C" int fq3_decode_chunk_lp(fq3_engine* e, const int32_t* slots, int32_t n_slots, int32_t n_frames,
+                                   int64_t* codes_out_dev, float* logprob_out_dev, fq3_chunk_result* res, void* stream) {
+  int32_t budgets[MAXB];
+  for (int j = 0; j < MAXB; ++j) budgets[j] = n_frames;
+  return fq3_decode_chunk_n(e, slots, n_slots, budgets, codes_out_dev, logprob_out_dev, res, stream);
 }
 
 extern "C" int fq3_decode_chunk(fq3_engine* e, const int32_t* slots, int32_t n_slots, int32_t n_frames,
@@ -1082,6 +1136,7 @@ extern "C" int fq3_num_ctas(fq3_engine* e) { return e ? e->ncta : 0; }
 extern "C" int64_t fq3_launch_count(fq3_engine* e) { return e ? e->launches : 0; }
 extern "C" const char* fq3_last_error(void) { return g_err; }
 extern "C" int fq3_max_batch(fq3_engine* e) { return e ? e->max_batch : 0; }
+extern "C" int fq3_max_slots(fq3_engine* e) { return e ? e->max_slots : 0; }
 extern "C" const char* fq3_version(void) { return "fq3-h100 0.2.0 (sm_90a)"; }
 
 #include "fq3_prefill.cuh"

@@ -452,14 +452,14 @@ static int prefill_group(fq3_engine* e, const pf::SeqTab& tab, const void* embed
 extern "C" int fq3_prefill_batch(fq3_engine* e, int32_t n, const int32_t* slots, const void* embeds_dev, const int32_t* P,
                                  const int32_t* n_left_pad, void* logits_out_dev, void* hidden_out_dev, void* stream_) {
   if (!e) return fail(FQ3_ERR_INVALID, "null argument");
-  if (n < 1 || n > e->max_batch) return fail(FQ3_ERR_INVALID, "n %d outside [1, max_batch=%d]", n, e->max_batch);
+  if (n < 1 || n > e->max_batch) return fail(FQ3_ERR_INVALID, "n %d outside [1, max_batch=%d] (prompts of one call)", n, e->max_batch);
   if (!slots || !embeds_dev || !P || !n_left_pad || !logits_out_dev || !hidden_out_dev) return fail(FQ3_ERR_INVALID, "null argument");
   // every check before the first launch: a refused call leaves every slot as it was.  A row is named when n > 1.
   char row[32] = "";
   for (int i = 0; i < n; ++i) {
     if (n > 1) snprintf(row, sizeof(row), " (row %d)", i);
-    if (slots[i] < 0 || slots[i] >= e->max_batch)
-      return fail(FQ3_ERR_INVALID, "slot %d outside [0, max_batch=%d)%s", slots[i], e->max_batch, row);
+    if (slots[i] < 0 || slots[i] >= e->max_slots)
+      return fail(FQ3_ERR_INVALID, "slot %d outside [0, %s=%d)%s", slots[i], slot_bound(e), e->max_slots, row);
     for (int j = 0; j < i; ++j)
       if (slots[j] == slots[i]) return fail(FQ3_ERR_INVALID, "slot %d listed twice%s", slots[i], row);
     if (P[i] <= 0) return fail(FQ3_ERR_INVALID, "empty prompt%s", row);

@@ -37,11 +37,24 @@ class SlotRequest:
     lp: Optional[FrameLogprobs] = None        # submit_many(logprobs=True): host assembly of the per-frame log-probabilities
     chunk_logprobs: Optional[torch.Tensor] = None   # ... of the frames the last step returned, [n,16]
     eos_logprob: Optional[float] = None       # ... of the EOS draw that ended the request
+    chunk_size: Optional[int] = None          # frames per launch of this request (default: the step's n_frames)
+    first_chunk: Optional[int] = None         # ... of its first launch only: a shorter one brings the first audio sooner
+    due: float = 0.0                          # urgency when more requests are ready than a launch has columns: smallest first
+    hold: bool = False                        # set by the caller between steps: not launched (a listener far enough ahead)
+    seq: int = 0                              # admission order, the tie-break of ``due``
+
+    def budget(self, n_frames: int) -> int:
+        """frames the next launch may emit for this request"""
+        if self.frames == 0 and self.first_chunk:
+            return self.first_chunk
+        return self.chunk_size or n_frames
 
     def ready(self) -> bool:
         """A text-fed request is launched once the rows of its next ``rows_ahead`` frames exist (fewer where
         max_new_tokens ends it first), once its text is closed, or once it has reached max_new_tokens (the launch then
-        reports it finished)."""
+        reports it finished).  A request on ``hold`` is not launched."""
+        if self.hold:
+            return False
         if self.feed is None or self.feed.closed or self.frames >= self.max_new_tokens:
             return True
         need = min(self.gen0 + self.frames + self.rows_ahead, self.gen0 + self.max_new_tokens)
@@ -53,17 +66,35 @@ _SUBMIT_DEFAULTS = dict(max_new_tokens=2048, min_new_tokens=2, temperature=0.9, 
                         repetition_penalty=1.05, uniforms=None)
 
 
+def _frames_arg(name: str, v) -> Optional[int]:
+    if v is None:
+        return None
+    if int(v) < 1:
+        raise ValueError(f"{name} must be at least 1 frame, got {v}")
+    return int(v)
+
+
 class BatchScheduler:
     """Owns the engine's slots: ``submit`` prefills one request into a free slot and latches it (``submit_many``:
-    several, with one batched prefill), ``step`` advances every ready slot by up to ``n_frames`` frames with ONE launch
+    several, with one batched prefill), ``step`` advances the ready slots by up to ``n_frames`` frames with ONE launch
     and returns the new codes per request, ``cancel`` frees a slot.  A text-fed request (``feed``) is ready while its next trailing row exists or its text is closed; a
-    slot that waits for text costs the others nothing."""
+    slot that waits for text costs the others nothing.
+
+    The engine holds ``max_slots`` requests and a launch carries ``max_batch`` of them.  While no more than that are
+    ready, ``step`` launches all of them.  When more are, it launches the ``max_batch`` with the smallest ``due``
+    (ties: the one admitted first); the others keep their slot and state and cost the launch nothing.  ``due`` and
+    ``hold`` belong to the caller, which sets them between steps (serving.ContinuousBatcher: the listener's playback
+    lead).  A request's ``chunk_size`` / ``first_chunk`` replace the step's ``n_frames`` for that request alone: its codes
+    do not depend on them, only how many frames each launch hands back."""
 
     def __init__(self, engine, talker, config, predictor_graph, talker_graph):
         self.engine, self.talker, self.config = engine, talker, config
         self.pg, self.tg = predictor_graph, talker_graph
-        self.free: List[int] = list(range(engine.max_batch))
+        self.max_slots = getattr(engine, "max_slots", engine.max_batch)
+        self.free: List[int] = list(range(self.max_slots))
+        self.max_prompts = engine.max_batch   # prompts one submit_many takes (one batched prefill)
         self.active: Dict[int, SlotRequest] = {}
+        self._seq = 0
         self.max_seq_len = getattr(engine, "max_seq_len", None)   # longest prompt a slot takes
 
     def __len__(self) -> int:
@@ -80,12 +111,14 @@ class BatchScheduler:
     def submit(self, tie, tam, tth, tpe, *, tag=None, max_new_tokens: int = 2048, min_new_tokens: int = 2,
                temperature: float = 0.9, top_k: int = 50, top_p: float = 1.0, do_sample: bool = True,
                repetition_penalty: float = 1.05, uniforms: Optional[torch.Tensor] = None, feed=None,
-               rows_ahead: int = 1) -> SlotRequest:
+               rows_ahead: int = 1, chunk_size: Optional[int] = None, first_chunk: Optional[int] = None) -> SlotRequest:
         """One request: tie [1,P,H], tam [1,P] (zeros = left padding), tth [1,Tt,H], tpe [1,1,H].  ``feed``: a
         ``text_stream.TextFeed`` whose row buffer replaces ``tth``; ``rows_ahead``: rows it must hold beyond the next
-        frame's before the slot is launched (``n_frames`` of the steps keeps every launch a full chunk)."""
+        frame's before the slot is launched (``n_frames`` of the steps keeps every launch a full chunk).
+        ``chunk_size`` / ``first_chunk``: this request's frames per launch / in its first launch."""
+        chunk_size, first_chunk = _frames_arg("chunk_size", chunk_size), _frames_arg("first_chunk", first_chunk)
         if not self.free:
-            raise RuntimeError(f"all {self.engine.max_batch} request slots are busy")
+            raise RuntimeError(f"all {self.max_slots} request slots are busy")
         slot = self.free.pop(0)
         try:
             begin_fused(self.engine, self.talker, tie, tam, tth, tpe, self.config, self.pg, self.tg,
@@ -98,25 +131,32 @@ class BatchScheduler:
             self.free.insert(0, slot)
             raise
         rq = SlotRequest(slot=slot, tag=tag if tag is not None else slot, max_new_tokens=max_new_tokens, feed=feed,
-                         gen0=self.engine.gen_step0[slot], rows_ahead=max(1, int(rows_ahead)))
+                         gen0=self.engine.gen_step0[slot], rows_ahead=max(1, int(rows_ahead)), chunk_size=chunk_size,
+                         first_chunk=first_chunk, seq=self._next_seq())
         self.active[slot] = rq
         return rq
+
+    def _next_seq(self) -> int:
+        self._seq += 1
+        return self._seq
 
     @torch.inference_mode()
     def submit_many(self, requests: List[dict], logprobs: bool = False) -> List[SlotRequest]:
         """Several requests at once: ``requests[i]`` holds the arguments of one ``submit`` call by name (tie, tam, tth,
-        tpe, tag, the sampling keywords, uniforms, feed, rows_ahead).  They take the slots consecutive ``submit`` calls
+        tpe, tag, the sampling keywords, uniforms, feed, rows_ahead, chunk_size, first_chunk).  They take the slots consecutive ``submit`` calls
         would take and latch what those would latch, but on a K3 engine their prompts share ONE prefill launch chain
         (``generate.begin_fused_batch``).  All or none: on an error every slot is released.  ``logprobs``: every
         ``step`` also sets ``chunk_logprobs`` (and, at the end, ``eos_logprob``) of these requests (logprobs.py)."""
         n = len(requests)
         if n > len(self.free):
-            raise RuntimeError(f"{n} requests but only {len(self.free)} of {self.engine.max_batch} request slots are free")
+            raise RuntimeError(f"{n} requests but only {len(self.free)} of {self.max_slots} request slots are free")
+        chunking = [(_frames_arg("chunk_size", r.get("chunk_size")), _frames_arg("first_chunk", r.get("first_chunk")))
+                    for r in requests]
         slots, self.free = self.free[:n], self.free[n:]
         rows = []
         for r in requests:
             gen = dict(_SUBMIT_DEFAULTS)
-            gen.update({k: v for k, v in r.items() if k not in ("tag", "feed", "rows_ahead")})
+            gen.update({k: v for k, v in r.items() if k not in ("tag", "feed", "rows_ahead", "chunk_size", "first_chunk")})
             gen["trailing_len"] = None if r.get("feed") is None else 0
             rows.append(gen)
         first_lps = [None] * n
@@ -134,25 +174,35 @@ class BatchScheduler:
             self.free = slots + self.free
             raise
         out = []
-        for slot, r, gen, flp in zip(slots, requests, rows, first_lps):
+        for slot, r, gen, flp, (chunk_size, first_chunk) in zip(slots, requests, rows, first_lps, chunking):
             tag = r.get("tag")
             rq = SlotRequest(slot=slot, tag=tag if tag is not None else slot, max_new_tokens=gen["max_new_tokens"],
                              feed=r.get("feed"), gen0=self.engine.gen_step0[slot], rows_ahead=max(1, int(r.get("rows_ahead", 1))),
-                             lp=FrameLogprobs(flp) if logprobs else None)
+                             lp=FrameLogprobs(flp) if logprobs else None, chunk_size=chunk_size, first_chunk=first_chunk,
+                             seq=self._next_seq())
             self.active[slot] = rq
             out.append(rq)
         return out
 
     @torch.inference_mode()
     def step(self, n_frames: int) -> List[Tuple[SlotRequest, torch.Tensor]]:
-        """Advance all ready slots; returns [(request, codes [n,16])] for every slot that was launched (n may be 0 for a
-        slot that stopped before emitting).  Finished slots are released."""
+        """Advance the ready slots -- all of them, or the ``max_batch`` most urgent (class docstring); returns [(request,
+        codes [n,16])] for every slot that was launched (n may be 0 for a slot that stopped before emitting).  Finished
+        slots are released."""
         for rq in self.active.values():
             if rq.feed is not None:
                 self.engine.set_text_rows(rq.slot, rq.feed.update(), open=not rq.feed.closed)
-        slots = sorted(s for s, rq in self.active.items() if rq.ready())
+        ready = [rq for rq in self.active.values() if rq.ready()]
+        if len(ready) > self.engine.max_batch:
+            ready = sorted(ready, key=lambda rq: (rq.due, rq.seq))[: self.engine.max_batch]
+        slots = sorted(rq.slot for rq in ready)
         if not slots:
             return []
+        budgets = [self.active[s].budget(n_frames) for s in slots]
+        if len(set(budgets)) > 1:
+            n_frames = budgets              # one budget per slot (fq3_decode_chunk_n)
+        else:
+            n_frames = budgets[0]           # without per-request chunking: the step's n_frames, the calls made without it
         want_lp = any(self.active[s].lp is not None for s in slots)
         lps = [None] * len(slots)
         # off: the calls are exactly those of a scheduler without the option
@@ -222,7 +272,7 @@ def fast_generate_streaming_batch(
     if engine is None:
         raise RuntimeError("batched decode needs graph handles backed by one loaded fq3 engine")
     B = talker_input_embeds.shape[0]
-    if B > engine.max_batch:
+    if B > engine.max_batch:   # one prefill call and lock-step launches: the rows are columns, whatever max_slots is
         raise ValueError(f"batch of {B} rows exceeds the engine's max_batch={engine.max_batch}")
     sched = BatchScheduler(engine, talker, config, predictor_graph, talker_graph)
     device = talker_input_embeds.device

@@ -8,6 +8,7 @@ constructors raise.
 from __future__ import annotations
 
 import ctypes as C
+import operator
 import os
 import subprocess
 from dataclasses import dataclass
@@ -34,7 +35,7 @@ class Config(C.Structure):
     _fields_ = [("dtype", C.c_int32), ("device", C.c_int32), ("max_seq_len", C.c_int32),
                 ("num_code_groups", C.c_int32), ("codec_eos_token_id", C.c_int32),
                 ("has_mtp_projection", C.c_int32), ("num_ctas", C.c_int32), ("rope_positions", C.c_int32),
-                ("talker", StackConfig), ("predictor", StackConfig), ("max_batch", C.c_int32)]
+                ("talker", StackConfig), ("predictor", StackConfig), ("max_batch", C.c_int32), ("max_slots", C.c_int32)]
 
 
 class Tensor(C.Structure):
@@ -68,7 +69,7 @@ class ChunkResult(C.Structure):
 EXPORTS = [
     "fq3_engine_create", "fq3_engine_load_weights", "fq3_engine_destroy", "fq3_import_kv", "fq3_export_kv",
     "fq3_set_generation_state", "fq3_talker_step", "fq3_predictor_run", "fq3_sample_logits", "fq3_sample_logits_lp",
-    "fq3_begin_request", "fq3_decode_chunk", "fq3_decode_chunk_lp", "fq3_set_text_rows", "fq3_get_past_hidden", "fq3_debug_enable", "fq3_debug_read", "fq3_tape_bytes",
+    "fq3_begin_request", "fq3_decode_chunk", "fq3_decode_chunk_lp", "fq3_decode_chunk_n", "fq3_max_slots", "fq3_slot_bytes", "fq3_set_text_rows", "fq3_get_past_hidden", "fq3_debug_enable", "fq3_debug_read", "fq3_tape_bytes",
     "fq3_num_ctas", "fq3_launch_count", "fq3_last_error", "fq3_version", "fq3_engine_set_prefill_weights", "fq3_prefill", "fq3_prefill_batch", "fq3_max_batch", "fq3_debug_gemv",
     "fq3_debug_conv_gemm",
     "fq3_codec_create", "fq3_codec_load_weights", "fq3_codec_flops",
@@ -130,6 +131,11 @@ def load_library() -> C.CDLL:
                                      C.POINTER(ChunkResult), C.c_void_p]
     lib.fq3_decode_chunk_lp.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
                                         C.POINTER(ChunkResult), C.c_void_p]
+    lib.fq3_decode_chunk_n.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.POINTER(C.c_int32), C.c_void_p,
+                                       C.c_void_p, C.POINTER(ChunkResult), C.c_void_p]
+    lib.fq3_max_slots.argtypes = [C.c_void_p]
+    lib.fq3_slot_bytes.argtypes = [C.POINTER(Config)]
+    lib.fq3_slot_bytes.restype = C.c_int64
     lib.fq3_set_text_rows.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32]
     lib.fq3_get_past_hidden.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
     lib.fq3_max_batch.argtypes = [C.c_void_p]
@@ -234,12 +240,31 @@ class SamplingParams:
                         float(self.repetition_penalty))
 
 
+def _stack_config(d: dict) -> StackConfig:
+    return StackConfig(d["hidden_size"], d["intermediate_size"], d["num_hidden_layers"], d["num_attention_heads"],
+                       d["num_key_value_heads"], d["vocab_size"], float(d.get("rms_norm_eps", 1e-6)))
+
+
+def slot_bytes(talker: dict, predictor: dict, dtype: torch.dtype, max_seq_len: int) -> int:
+    """Device bytes one resident request slot costs (fq3_slot_bytes): what ``max_slots`` multiplies.  Needs no GPU."""
+    lib = load_library()
+    cfg = Config(dtype=FQ3_BF16 if dtype == torch.bfloat16 else FQ3_F32, max_seq_len=int(max_seq_len),
+                 talker=_stack_config(talker), predictor=_stack_config(predictor))
+    n = lib.fq3_slot_bytes(C.byref(cfg))
+    if n < 0:
+        _check(lib, int(n))
+    return int(n)
+
+
 class Engine:
-    """One engine per device: packed weights, KV caches and the persistent decode kernel."""
+    """One engine per device: packed weights, KV caches and the persistent decode kernel.  ``max_batch`` is the number
+    of slots one launch may carry (<= 32), ``max_slots`` (default: ``max_batch``) the number of request slots that
+    exist; with more slots than columns the caller chooses which ones each launch advances."""
 
     def __init__(self, *, talker: dict, predictor: dict, dtype: torch.dtype, device="cuda", max_seq_len: int = 2048,
                  num_code_groups: int = 16, codec_eos_token_id: int = 2150, has_mtp_projection: bool = True,
-                 num_ctas: int = 0, rope_positions: Optional[int] = None, max_batch: int = 1):
+                 num_ctas: int = 0, rope_positions: Optional[int] = None, max_batch: int = 1,
+                 max_slots: Optional[int] = None):
         if not torch.cuda.is_available():
             raise RuntimeError("fq3 engine needs a CUDA device (sm_90a); no CPU fallback exists")
         self.lib = load_library()
@@ -254,18 +279,15 @@ class Engine:
         self.eos = codec_eos_token_id
         self.rope_positions = int(rope_positions or (self.max_seq_len + 64))
 
-        def sc(d):
-            return StackConfig(d["hidden_size"], d["intermediate_size"], d["num_hidden_layers"],
-                               d["num_attention_heads"], d["num_key_value_heads"], d["vocab_size"],
-                               float(d.get("rms_norm_eps", 1e-6)))
-
         cfg = Config(FQ3_BF16 if dtype == torch.bfloat16 else FQ3_F32, self.device.index, self.max_seq_len,
                      num_code_groups, codec_eos_token_id, int(bool(has_mtp_projection)), int(num_ctas),
-                     self.rope_positions, sc(talker), sc(predictor), int(max_batch))
+                     self.rope_positions, _stack_config(talker), _stack_config(predictor), int(max_batch),
+                     int(max_slots or 0))
         self.max_batch = int(max_batch)
         h = C.c_void_p()
         _check(self.lib, self.lib.fq3_engine_create(C.byref(cfg), C.byref(h)))
         self.h = h
+        self.max_slots = int(self.lib.fq3_max_slots(h))
         self.H = talker["hidden_size"]
         self._keep = {}  # slot -> tensors borrowed by the engine for the duration of that slot's request
         self.gen_step0 = {}  # slot -> generation_step latched by begin_request (frame s reads trailing row gen_step0 + s)
@@ -482,13 +504,22 @@ class Engine:
             return out[: res.frames_emitted], lp[: res.frames_emitted], res
         return out[: res.frames_emitted], res
 
-    def decode_chunk_batch(self, slots, n_frames: int, out: Optional[torch.Tensor] = None, logprobs=None):
-        """All listed slots advance up to n_frames frames in ONE launch sharing every pass over the weights.
-        Returns (codes [n_slots, n_frames, 16] -- row j valid up to results[j].frames_emitted --, [ChunkResult]).
-        ``logprobs`` (True or a float32 [n_slots,n_frames,16] device tensor): (codes, logprobs, results), valid as the
-        codes are."""
+    def decode_chunk_batch(self, slots, n_frames, out: Optional[torch.Tensor] = None, logprobs=None):
+        """All listed slots (at most ``max_batch`` of the ``max_slots`` resident ones) advance up to n_frames frames in
+        ONE launch sharing every pass over the weights; ``n_frames`` is an int or one budget per slot (below, n_frames
+        then stands for the largest).  Returns (codes [n_slots, n_frames, 16] -- row j valid up to
+        results[j].frames_emitted --, [ChunkResult]).  ``logprobs`` (True or a float32 [n_slots,n_frames,16] device
+        tensor): (codes, logprobs, results), valid as the codes are."""
         slots = [int(x) for x in slots]
         n = len(slots)
+        budgets = None
+        try:
+            n_frames = operator.index(n_frames)   # any integer scalar (int, numpy, 0-d torch): one budget for all
+        except TypeError:
+            budgets = [int(x) for x in n_frames]
+            if len(budgets) != n:
+                raise ValueError(f"{n} slots but {len(budgets)} frame budgets")
+            n_frames = max(max(budgets, default=0), 1)   # a budget <= 0 is the engine's to refuse
         if out is None:
             out = torch.empty(n, n_frames, 16, dtype=torch.long, device=self.device)
         lp = self._logprob_buf(logprobs, (n, n_frames, 16))
@@ -497,8 +528,10 @@ class Engine:
         if self.time_kernels:
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
-        _check(self.lib, self.lib.fq3_decode_chunk_lp(self.h, sl, n, int(n_frames), out.data_ptr(),
-                                                       lp.data_ptr() if lp is not None else None, res, self._stream()))
+        nf = int(n_frames) if budgets is None else (C.c_int32 * n)(*budgets)
+        call = self.lib.fq3_decode_chunk_lp if budgets is None else self.lib.fq3_decode_chunk_n
+        _check(self.lib, call(self.h, sl, n, nf, out.data_ptr(), lp.data_ptr() if lp is not None else None, res,
+                              self._stream()))
         if self.time_kernels:
             e1.record()
             e1.synchronize()

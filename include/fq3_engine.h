@@ -61,8 +61,14 @@ typedef struct {
   int32_t rope_positions;   /* rows of the talker cos/sin tables (>= max_seq_len + margin for rope deltas) */
   fq3_stack_config talker;
   fq3_stack_config predictor;
-  int32_t max_batch;        /* request slots (KV caches + per-request state); 0/1 = one sequence, <= 32 */
+  int32_t max_batch;        /* columns one launch may carry (slots that advance together); 0/1 = one sequence, <= 32 */
+  int32_t max_slots;        /* resident request slots (KV caches + per-request state); 0 = max_batch, else in
+                             * [max_batch, FQ3_MAX_SLOTS].  Memory is the bound: fq3_slot_bytes() per slot */
 } fq3_config;
+
+/* Most request slots an engine may hold.  Beyond its memory a slot costs one host record, so the cap follows what an
+ * 80 GB card holds: at the 1.7B geometry in bf16, 256 slots of max_seq_len 2048 are 60 GB of talker KV. */
+#define FQ3_MAX_SLOTS 256
 
 /* A named tensor handed to fq3_engine_load_weights.  Names (L = layers of that stack, stacked on dim 0):
  *   t.q [L,nH*128,H]  t.k [L,nKV*128,H]  t.v  t.o [L,H,nH*128]  t.gate [L,I,H]  t.up  t.down [L,H,I]
@@ -117,18 +123,27 @@ typedef struct {
 
 /* ---- lifecycle ------------------------------------------------------------------------------------------ */
 /* replaces TalkerGraph.__init__ / PredictorGraph.__init__ (talker_graph.py:27-59, predictor_graph.py:34-78):
- * allocates KV caches, scratch and tables.  */
+ * allocates KV caches, scratch and tables.  A configuration that cannot succeed (max_slots < max_batch, max_slots >
+ * FQ3_MAX_SLOTS, max_batch > 32, unsupported geometry) is refused with FQ3_ERR_INVALID before anything is allocated.
+ * Every allocation is made before the first memset: when one does not fit, the call returns FQ3_ERR_CUDA, has freed
+ * what it allocated, has launched nothing and leaves *out untouched. */
 int fq3_engine_create(const fq3_config* cfg, fq3_engine** out);
+/* Device bytes one resident request slot costs under `cfg` (talker and predictor K and V caches, loop state, past
+ * hidden, penalty bitmap): the part of fq3_engine_create's allocation that grows with max_slots.  Pure arithmetic, no
+ * device needed.  Negative fq3_status when cfg is NULL or its dtype is invalid. */
+int64_t fq3_slot_bytes(const fq3_config* cfg);
 /* replaces holding references to the upstream nn.Modules (predictor_graph.py:53-57, talker_graph.py:41):
  * copies norm/embedding tables and repacks every GEMV weight into the per-CTA streaming tape. */
 int fq3_engine_load_weights(fq3_engine* e, const fq3_tensor* tensors, int32_t n, void* stream);
 void fq3_engine_destroy(fq3_engine* e);
 
-/* Request slots.  The engine holds `max_batch` independent request slots (KV caches, predictor cache, penalty
- * bitmap, loop state).  Every per-request entry point names its slot; fq3_decode_chunk takes the list of slots
- * that advance together: one slot runs the single-sequence persistent kernel, several slots run the batched
- * kernel in which all of them share ONE pass over the weight tape per step (the reference batches left-padded
- * prompts, model.py:774-787, with per-row pad counts, talker_graph.py:177-187). */
+/* Request slots.  The engine holds `max_slots` independent request slots (KV caches, predictor cache, penalty
+ * bitmap, loop state).  Every per-request entry point names its slot, in [0, max_slots); fq3_decode_chunk takes the
+ * list of at most `max_batch` slots that advance together: one slot runs the single-sequence persistent kernel,
+ * several slots run the batched kernel in which all of them share ONE pass over the weight tape per step (the
+ * reference batches left-padded prompts, model.py:774-787, with per-row pad counts, talker_graph.py:177-187).  A
+ * column of a launch is a position in slots[], not a slot id: which resident slots a launch carries is the caller's
+ * choice from launch to launch, and a slot that is not listed is not touched. */
 
 /* ---- duck-type compatibility path (what the reference's own schedulers call) ----------------------------- */
 /* TalkerGraph.prefill_kv (talker_graph.py:153-170): k,v are [n_kv, P, 128] contiguous for one layer. */
@@ -180,7 +195,8 @@ int fq3_prefill(fq3_engine* e, int32_t slot, const void* embeds_dev, int32_t P, 
  * Scratch holds max_seq_len rows: when sum P_b exceeds it, the prompts run as consecutive groups in list order, each
  * as many prompts as fit (one prompt of up to max_seq_len rows always does).  A group costs the launches of one
  * fq3_prefill.
- * Refused before anything is launched (no slot changes): n outside [1, max_batch], a slot listed twice, and per row
+ * Refused before anything is launched (no slot changes): n outside [1, max_batch] (prompts per call, whatever
+ * max_slots is), a slot listed twice, and per row
  * what fq3_prefill refuses (slot out of range, P <= 0, P > max_seq_len = FQ3_ERR_TOO_LONG with the reference's
  * message); the message names the row when n > 1. */
 int fq3_prefill_batch(fq3_engine* e, int32_t n, const int32_t* slots, const void* embeds_dev, const int32_t* P,
@@ -225,9 +241,20 @@ int fq3_decode_chunk(fq3_engine* e, const int32_t* slots, int32_t n_slots, int32
  * neither is anything of a slot not listed. */
 int fq3_decode_chunk_lp(fq3_engine* e, const int32_t* slots, int32_t n_slots, int32_t n_frames, int64_t* codes_out_dev,
                         float* logprob_out_dev, fq3_chunk_result* res, void* stream);
+/* fq3_decode_chunk_lp with a frame budget per slot: n_frames[n_slots] (HOST array, every entry > 0) -- slot j emits at
+ * most n_frames[j] frames in this launch.  codes_out_dev int64 [n_slots][F][16] and logprob_out_dev float32
+ * [n_slots][F][16] or NULL, F = the largest budget.  A slot that has used its budget leaves the launch as a slot that
+ * waits for text does: the others go on, its state is what it is at a launch boundary, and the next launch resumes it
+ * unchanged, so its codes do not depend on the budgets it was given.  After the launch frames_emitted ==
+ * min(n_frames[j], frames to the request's end); rows at or past it are not written.  fq3_decode_chunk_lp is the case
+ * of equal budgets.  Refused before anything is launched: n_slots outside [1, max_batch], a slot outside
+ * [0, max_slots), a slot listed twice or without a request, a budget <= 0. */
+int fq3_decode_chunk_n(fq3_engine* e, const int32_t* slots, int32_t n_slots, const int32_t* n_frames,
+                       int64_t* codes_out_dev, float* logprob_out_dev, fq3_chunk_result* res, void* stream);
 /* last post-norm talker hidden (generate.py:198 past_hidden) of `slot` -> dst_dev [H] model dtype */
 int fq3_get_past_hidden(fq3_engine* e, int32_t slot, void* dst_dev, void* stream);
-int fq3_max_batch(fq3_engine* e);
+int fq3_max_batch(fq3_engine* e);   /* columns per launch */
+int fq3_max_slots(fq3_engine* e);   /* resident request slots (>= fq3_max_batch) */
 /* numerics probe of the batched GEMV: y[col][row] = W_seg[row,:] . x[col,:] for one weight segment of stack 0 (talker) /
  * 1 (predictor): which 0 qkv, 1 o_proj, 2 gate/up (out = model dtype [ncols][I] = silu(gate)*up), 3 down, 4 head
  * (predictor: layer = codebook).  x_dev model dtype [ncols][K]; out_dev float32 [ncols][rows] (which != 2). */
