@@ -1279,9 +1279,8 @@ __device__ __forceinline__ void small_kv_preload(Ctx& c, const StackDev& S, int 
   using Raw = typename SmallKV<BF>::Raw;
   const size_t esz = BF ? 2 : 4;
   const int g = c.warp < S.nKV ? c.warp : 0;
-  // `pre` lives in local memory (attention_small_all takes its address), and so does the Ctx: a store into `pre` may
-  // alias c.lane, so with the loads written straight into `pre` every load waited for the one before it (c.lane reloaded
-  // after each store, each store waiting for its load).  All loads go out first, into registers; then the copy.
+  // all loads go out before the first copy into `pre`: should `pre` ever land in local memory again, a store into it
+  // that may alias what a later load's address depends on would serialise the loads (one L2 round trip each)
   const Raw* kp = reinterpret_cast<const Raw*>(reinterpret_cast<const uint8_t*>(kc) + ((size_t)(layer * S.nKV + g) * S.S * 128) * esz) + c.lane;
   const Raw* vp = reinterpret_cast<const Raw*>(reinterpret_cast<const uint8_t*>(vc) + ((size_t)(layer * S.nKV + g) * S.S * 128) * esz) + c.lane;
   constexpr int ROW = (int)(128 * (BF ? 2 : 4) / sizeof(Raw));   // Raw elements per cached row
@@ -1588,7 +1587,8 @@ __device__ void run_layers(Ctx& c, const StackDev& S, int nt, int slot0, int rpo
                         [&](int row, int t, float v, float, float) { P.QKV[(size_t)t * P.ldQKV + row] = rnd<BF>(v); });
     probe(c, pi);  // 2: after QKV gemv
     const bool small_attn = !TALKER;   // geometry checked by fq3_engine_create (cache <= 32 slots, <= 2 q-heads per kv head)
-    const bool kv_pre = small_attn && nt == 1 && S.nKV <= NCW;
+    // a warp preloads its own kv group (warp < nKV); attention_small_all reads further groups (nKV > NCW) itself
+    const bool kv_pre = small_attn && nt == 1;
     SmallKV<BF> skv;
     grid_arrive(c);
     if (kv_pre) small_kv_preload<BF>(c, S, l, slot0, kc, vc, skv);  // cached keys/values do not depend on this layer's QKV
@@ -1602,7 +1602,9 @@ __device__ void run_layers(Ctx& c, const StackDev& S, int nt, int slot0, int rpo
     if constexpr (!TALKER) {
       // ---- P2+P3 fused: redundant small attention straight into the staging vector (no exchange, no barrier)
       auto to_xs = [&](int t, int i, float v) { xs_put<BF>(c, t * S.qd + i, v); };
-      if (nt == 1) attention_small_all<BF, 1>(c, S, l, slot0, rpos0, P.QKV, P.ldQKV, kc, vc, cta0, kv_pre ? &skv : nullptr, to_xs);
+      // &skv unconditionally (nt == 1 always preloads): a pointer chosen at run time between skv and nullptr would
+      // keep skv in local memory, so that every preloaded row took an STL and an LDL
+      if (nt == 1) attention_small_all<BF, 1>(c, S, l, slot0, rpos0, P.QKV, P.ldQKV, kc, vc, cta0, &skv, to_xs);
       else attention_small_all<BF, 2>(c, S, l, slot0, rpos0, P.QKV, P.ldQKV, kc, vc, cta0, nullptr, to_xs);
       probe(c, pi);  // 4
       probe(c, pi);  // 5
@@ -1679,9 +1681,24 @@ __device__ void run_layers(Ctx& c, const StackDev& S, int nt, int slot0, int rpo
     probe(c, pi);  // 8: after GU gemv
     grid_sync(c);
     probe(c, pi);  // 9: after B4
-    // ---- P5: down rows + residual
-    for (int t = 0; t < nt; ++t)
-      for (int k = c.tid; k < S.I; k += NCT) xs_put<BF>(c, t * S.I + k, __ldcg(P.ACT + (size_t)t * P.ldACT + k));
+    // ---- P5: down rows + residual.  ACT -> staging vector with all of a thread's loads in flight before its first
+    //      store (one L2 round trip instead of one per element)
+    for (int t = 0; t < nt; ++t) {
+      constexpr int U = 12;
+      for (int k0 = 0; k0 < S.I; k0 += U * NCT) {
+        float v[U];
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+          const int k = k0 + u * NCT + c.tid;
+          v[u] = k < S.I ? __ldcg(P.ACT + (size_t)t * P.ldACT + k) : 0.f;
+        }
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+          const int k = k0 + u * NCT + c.tid;
+          if (k < S.I) xs_put<BF>(c, t * S.I + k, v[u]);
+        }
+      }
+    }
     csync();
     if (dbg && cta0) {
       float* d = P.dbg + (size_t)l * P.dbg_stride_layer + (size_t)2 * (S.qd + 2 * S.kd) + 2 * S.qd + 2 * S.H;
@@ -1717,25 +1734,20 @@ __device__ __forceinline__ void head_logits(Ctx& c, int seg, int H) {
 
 // predictor: 15 passes (predictor_graph.py:115-167).  Inputs: s.xin[0] = past_hidden, s.xin[1] = embed(cb0 token).
 // Outputs s.codes[1..15].  u15: 15 uniforms.  lp_row: the frame's log-probability row (pass i -> column i + 1) or nullptr.
+// A real function that works on a private copy of the caller's Ctx and hands the advanced counters back at the end.
+// The caller's Ctx has its address taken and lives in local memory; used directly, every c.lane, c.warp and
+// c.tile_ctr of the predictor was an LDL, reloaded after each store the compiler could not prove disjoint from the
+// stack (every global store of a GEMV epilogue or a K/V append).  The copy's address is never taken: registers.
+// (The caller keeps its own Ctx in memory on purpose: promoted to registers, it adds spills to the talker's path.)
 template <bool BF>
-__device__ void predictor_frame(Ctx& c, const float* u15, bool dbg, float* lp_row) {
+__device__ void predictor_frame(Ctx& cio, const float* u15, bool dbg, float* lp_row) {
+  Ctx c = cio;
   const KParams& P = c.P;
   const StackDev& S = P.p;
   const int Ht = P.t.H;
   for (int i = 0; i < P.ncb; ++i) {
     const int nt = (i == 0) ? 2 : 1;
     probe_at(c, 1024 + 8 * i + 0);
-    if (i > 0) {
-      const int prev = SMEM().codes[i];  // code sampled by pass i-1
-      if (P.has_mtp) {  // small_to_mtp_projection(codec_embedding[i-1](prev)) was tabulated when the weights were loaded
-        for (int k = c.tid; k < S.H; k += NCT)
-          SMEM().xin[0][k] = ldw<BF>(P.mtp_tab, ((size_t)(i - 1) * S.V + prev) * S.H + k);
-      } else {
-        for (int k = c.tid; k < Ht; k += NCT)
-          SMEM().xin[0][k] = ldw<BF>(P.p_embeds, ((size_t)(i - 1) * S.V + prev) * Ht + k);
-      }
-      csync();
-    }
     // pass 0 projects cat(past_hidden, cb0 embedding), which the table does not cover
     const bool project = i == 0 && P.has_mtp;
     if (project) {
@@ -1758,9 +1770,29 @@ __device__ void predictor_frame(Ctx& c, const float* u15, bool dbg, float* lp_ro
     sa.lp = lp_row ? lp_row + 1 + i : nullptr;
     const int tok = sample_block<BF>(c, sa);
     if (c.tid == 0) SMEM().codes[i + 1] = tok;
+    if (i + 1 < P.ncb) {
+      // the next pass's input row, fetched as soon as the code is known (sample_block is done with xin[0]), all of a
+      // thread's loads in flight together.  With the projection: small_to_mtp_projection(codec_embedding[i](tok)),
+      // tabulated when the weights were loaded
+      const void* tab = P.has_mtp ? P.mtp_tab : P.p_embeds;
+      const int n = P.has_mtp ? S.H : Ht;
+      float r[NORM_E];
+#pragma unroll
+      for (int e = 0; e < NORM_E; ++e) {
+        const int k = c.tid + e * NCT;
+        r[e] = k < n ? ldw<BF>(tab, ((size_t)i * S.V + tok) * n + k) : 0.f;
+      }
+#pragma unroll
+      for (int e = 0; e < NORM_E; ++e) {
+        const int k = c.tid + e * NCT;
+        if (k < n) SMEM().xin[0][k] = r[e];
+      }
+    }
     csync();
     probe_at(c, 1024 + 8 * i + 4);
   }
+  cio.tile_ctr = c.tile_ctr;
+  cio.bar_target = c.bar_target;
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -1898,10 +1930,26 @@ __global__ void __launch_bounds__(NTHREADS, 1) fq3_decode_kernel(const __grid_co
         {
           const void* extra = gen_step < rq.trailing_len ? rq.trailing : rq.tts_pad;
           const size_t eoff = gen_step < rq.trailing_len ? (size_t)gen_step * Ht : 0;
-          for (int k = tid; k < Ht; k += NCT) {
-            float sm = ldw<BF>(P.t_embed, (size_t)token * Ht + k);
-            for (int i = 0; i < P.ncb; ++i) sm += ldw<BF>(P.p_embeds, ((size_t)i * P.p.V + s.codes[i + 1]) * Ht + k);
-            s.xin[0][k] = rnd<BF>(rnd<BF>(sm) + ldw<BF>(extra, eoff + k));
+          // a thread's NORM_E elements advance through the rows together, so each row is one round of independent
+          // loads (not one dependent chain of 16 loads per element); every element still adds its rows in order
+          float sm[NORM_E];
+#pragma unroll
+          for (int e = 0; e < NORM_E; ++e) {
+            const int k = tid + e * NCT;
+            sm[e] = k < Ht ? ldw<BF>(P.t_embed, (size_t)token * Ht + k) : 0.f;
+          }
+          for (int i = 0; i < P.ncb; ++i) {
+            const size_t row = ((size_t)i * P.p.V + s.codes[i + 1]) * Ht;
+#pragma unroll
+            for (int e = 0; e < NORM_E; ++e) {
+              const int k = tid + e * NCT;
+              if (k < Ht) sm[e] += ldw<BF>(P.p_embeds, row + k);
+            }
+          }
+#pragma unroll
+          for (int e = 0; e < NORM_E; ++e) {
+            const int k = tid + e * NCT;
+            if (k < Ht) s.xin[0][k] = rnd<BF>(rnd<BF>(sm[e]) + ldw<BF>(extra, eoff + k));
           }
           csync();
         }
