@@ -87,11 +87,13 @@ class BatchScheduler:
     lead).  A request's ``chunk_size`` / ``first_chunk`` replace the step's ``n_frames`` for that request alone: its codes
     do not depend on them, only how many frames each launch hands back."""
 
-    def __init__(self, engine, talker, config, predictor_graph, talker_graph):
+    def __init__(self, engine, talker, config, predictor_graph, talker_graph, slots=None):
+        """``slots``: the engine's request slots this scheduler hands out (default: all of them)."""
         self.engine, self.talker, self.config = engine, talker, config
         self.pg, self.tg = predictor_graph, talker_graph
-        self.max_slots = getattr(engine, "max_slots", engine.max_batch)
-        self.free: List[int] = list(range(self.max_slots))
+        self.free: List[int] = list(range(getattr(engine, "max_slots", engine.max_batch))) if slots is None \
+            else [int(s) for s in slots]
+        self.max_slots = len(self.free)
         self.max_prompts = engine.max_batch   # prompts one submit_many takes (one batched prefill)
         self.active: Dict[int, SlotRequest] = {}
         self._seq = 0
@@ -116,25 +118,11 @@ class BatchScheduler:
         ``text_stream.TextFeed`` whose row buffer replaces ``tth``; ``rows_ahead``: rows it must hold beyond the next
         frame's before the slot is launched (``n_frames`` of the steps keeps every launch a full chunk).
         ``chunk_size`` / ``first_chunk``: this request's frames per launch / in its first launch."""
-        chunk_size, first_chunk = _frames_arg("chunk_size", chunk_size), _frames_arg("first_chunk", first_chunk)
-        if not self.free:
-            raise RuntimeError(f"all {self.max_slots} request slots are busy")
-        slot = self.free.pop(0)
-        try:
-            begin_fused(self.engine, self.talker, tie, tam, tth, tpe, self.config, self.pg, self.tg,
-                        max_new_tokens=max_new_tokens, min_new_tokens=min_new_tokens, temperature=temperature,
-                        top_k=top_k, top_p=top_p, do_sample=do_sample, repetition_penalty=repetition_penalty,
-                        uniforms=uniforms, slot=slot, trailing_len=None if feed is None else 0)
-            if feed is not None:
-                self.engine.set_text_rows(slot, feed.update(), open=not feed.closed)
-        except Exception:
-            self.free.insert(0, slot)
-            raise
-        rq = SlotRequest(slot=slot, tag=tag if tag is not None else slot, max_new_tokens=max_new_tokens, feed=feed,
-                         gen0=self.engine.gen_step0[slot], rows_ahead=max(1, int(rows_ahead)), chunk_size=chunk_size,
-                         first_chunk=first_chunk, seq=self._next_seq())
-        self.active[slot] = rq
-        return rq
+        return self.submit_many([dict(tie=tie, tam=tam, tth=tth, tpe=tpe, tag=tag, max_new_tokens=max_new_tokens,
+                                      min_new_tokens=min_new_tokens, temperature=temperature, top_k=top_k, top_p=top_p,
+                                      do_sample=do_sample, repetition_penalty=repetition_penalty, uniforms=uniforms,
+                                      feed=feed, rows_ahead=rows_ahead, chunk_size=chunk_size,
+                                      first_chunk=first_chunk)])[0]
 
     def _next_seq(self) -> int:
         self._seq += 1
@@ -160,13 +148,17 @@ class BatchScheduler:
             gen["trailing_len"] = None if r.get("feed") is None else 0
             rows.append(gen)
         first_lps = [None] * n
+        lkw = {"logprob": True} if logprobs else {}   # off: the calls of a scheduler without the option
         try:
-            if n:
-                if logprobs:
-                    _, first_lps = begin_fused_batch(self.engine, self.talker, rows, self.config, self.pg, self.tg, slots,
-                                                     logprob=True)
-                else:   # the call of a scheduler without the option
-                    begin_fused_batch(self.engine, self.talker, rows, self.config, self.pg, self.tg, slots)
+            if n == 1:   # one request: ``begin_fused``, the one-row case of ``begin_fused_batch``
+                r = rows[0]
+                got = begin_fused(self.engine, self.talker, r["tie"], r["tam"], r["tth"], r["tpe"], self.config, self.pg,
+                                  self.tg, slot=slots[0], **{k: v for k, v in r.items() if k not in ("tie", "tam", "tth", "tpe")},
+                                  **lkw)
+                first_lps = [got[1]] if logprobs else first_lps
+            elif n:
+                got = begin_fused_batch(self.engine, self.talker, rows, self.config, self.pg, self.tg, slots, **lkw)
+                first_lps = got[1] if logprobs else first_lps
             for slot, r in zip(slots, requests):
                 if r.get("feed") is not None:
                     self.engine.set_text_rows(slot, r["feed"].update(), open=not r["feed"].closed)
@@ -240,6 +232,51 @@ class BatchScheduler:
             self.free.append(rq.slot)
 
 
+def _single(engine, talker, config, predictor_graph, talker_graph, request: dict, logprobs: bool = False):
+    """The one request of a single-request driver (``submit_many`` arguments), admitted to a scheduler that owns only
+    the slot the graph handles drive.  -> (scheduler, request, prefill seconds)"""
+    sched = BatchScheduler(engine, talker, config, predictor_graph, talker_graph,
+                           slots=[getattr(talker_graph, "slot", 0)])
+    t0 = time.time()
+    rq = sched.submit_many([request], logprobs=logprobs)[0]
+    _sync(request["tie"].device)
+    return sched, rq, time.time() - t0
+
+
+def _chunks(sched: BatchScheduler, chunk_size: int, t_prefill: float, before_step=None):
+    """The launch loop of the fused drivers: ``sched.step(chunk_size)`` until no request is left.  Yields, per step that
+    produced frames, [(request, codes [n,16], timing)] with the reference's per-chunk timing keys, "kernel_ms" when the
+    engine times its kernels, and for a request admitted with log-probabilities "logprobs" [n,16] and, on its last
+    chunk, "eos_logprob".  ``before_step`` runs before every step, inside its "decode_ms"."""
+    engine, idx = sched.engine, 0
+    while len(sched):
+        t1 = time.time()
+        if before_step is not None:
+            before_step()
+        out = sched.step(chunk_size)
+        dt = time.time() - t1
+        items = []
+        for rq, codes in out:
+            n = int(codes.shape[0])
+            if not n:
+                continue
+            # the reference flags the trailing partial chunk -- and a full chunk cut off by the cache limit, which
+            # leaves its loop before the "buffer full" check (streaming.py:130-132 vs :158-173)
+            tm = {"chunk_index": idx, "chunk_steps": n, "prefill_ms": t_prefill * 1000 if idx == 0 else 0,
+                  "decode_ms": dt * 1000, "total_steps_so_far": rq.frames,
+                  "is_final": n < chunk_size or rq.finished == 3}
+            if engine.time_kernels:
+                tm["kernel_ms"] = engine.last_kernel_ms
+            if rq.lp is not None:
+                tm["logprobs"] = rq.chunk_logprobs
+                if rq.finished or rq.eos_logprob is not None:   # nothing follows this chunk
+                    tm["eos_logprob"] = rq.eos_logprob
+            items.append((rq, codes, tm))
+        if items:
+            yield items
+            idx += 1
+
+
 def _rows(x: torch.Tensor, b: int) -> torch.Tensor:
     return x[b:b + 1]
 
@@ -284,31 +321,8 @@ def fast_generate_streaming_batch(
                             uniforms=None if uniforms is None else uniforms[b]) for b in range(B)],
                       logprobs=return_logprobs)
     _sync(device)
-    t_prefill = time.time() - t0
-    idx = 0
-    totals = [0] * B
-    while len(sched):
-        t1 = time.time()
-        out = sched.step(chunk_size)
-        dt = time.time() - t1
-        items = []
-        for rq, codes in out:
-            n = int(codes.shape[0])
-            if not n:
-                continue
-            totals[rq.tag] += n
-            tm = {"chunk_index": idx, "chunk_steps": n, "prefill_ms": t_prefill * 1000 if idx == 0 else 0,
-                  "decode_ms": dt * 1000, "total_steps_so_far": totals[rq.tag], "is_final": n < chunk_size or rq.finished == 3}
-            if engine.time_kernels:
-                tm["kernel_ms"] = engine.last_kernel_ms
-            if return_logprobs:
-                tm["logprobs"] = rq.chunk_logprobs
-                if rq.finished or rq.eos_logprob is not None:   # nothing follows this chunk
-                    tm["eos_logprob"] = rq.eos_logprob
-            items.append((rq.tag, codes, tm))
-        if items:
-            yield items
-            idx += 1
+    for items in _chunks(sched, chunk_size, time.time() - t0):
+        yield [(rq.tag, codes, tm) for rq, codes, tm in items]
 
 
 @torch.inference_mode()

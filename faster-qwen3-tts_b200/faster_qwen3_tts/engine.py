@@ -355,7 +355,10 @@ class Engine:
             lens = [int(rows.shape[1])] * int(rows.shape[0])
         else:
             parts = [r.reshape(-1, self.H) for r in rows]
-            x = self._t(torch.cat(parts)) if parts else torch.empty(0, self.H, dtype=self.dtype, device=self.device)
+            if len(parts) == 1:   # one prompt needs no packing copy
+                x = self._t(parts[0])
+            else:
+                x = self._t(torch.cat(parts)) if parts else torch.empty(0, self.H, dtype=self.dtype, device=self.device)
             lens = [int(r.shape[0]) for r in parts]
         n = len(lens)
         if len(pads) != n or len(slots) != n:

@@ -1,6 +1,7 @@
 """Non-streaming generation: same signature, return value and timing keys as the reference's ``fast_generate``
 (faster_qwen3_tts/generate.py:16-215).  When both graph objects are backed by one fq3 engine the whole decode
-loop runs on device (one persistent-kernel launch per <=256 frames); otherwise a step-wise loop drives any
+loop runs on device (one persistent-kernel launch per <=256 frames, issued by the launch loop of the batched drivers
+on the graph's slot, batching.py); otherwise a step-wise loop drives any
 duck-typed ``PredictorGraph`` / ``TalkerGraph`` (the contract of the reference's tests/test_sampling.py:79-93)."""
 from __future__ import annotations
 
@@ -10,7 +11,6 @@ from typing import Optional, Tuple
 import torch
 
 from .engine import SamplingParams
-from .logprobs import FrameLogprobs
 from .sampling import apply_repetition_penalty, sample_logits
 
 _MAX_LAUNCH_FRAMES = 256
@@ -98,44 +98,54 @@ def begin_fused(engine, talker, tie, tam, tth, tpe, config, predictor_graph, tal
                 min_new_tokens, temperature, top_k, top_p, do_sample, repetition_penalty, uniforms, slot=None,
                 trailing_len=None, logprob=False):
     """Prefill + first token + request latch (generate.py:104-140) for ONE row [1,P,H] into request slot `slot`
-    (default: the slot the graph handles drive).  ``trailing_len``: rows of ``tth`` valid now (text-fed requests latch
-    a larger buffer and announce rows later, ``Engine.set_text_rows``).  Returns the first token id; with ``logprob``
-    (first token id, its log-probability as a float)."""
-    gen = dict(max_new_tokens=max_new_tokens, min_new_tokens=min_new_tokens, temperature=temperature, top_k=top_k,
-               top_p=top_p, do_sample=do_sample, repetition_penalty=repetition_penalty)
+    (default: the slot the graph handles drive): the one-row case of ``begin_fused_batch``.  ``trailing_len``: rows of
+    ``tth`` valid now (text-fed requests latch a larger buffer and announce rows later, ``Engine.set_text_rows``).
+    Returns the first token id; with ``logprob`` (first token id, its log-probability as a float)."""
+    row = dict(tie=tie, tam=tam, tth=tth, tpe=tpe, max_new_tokens=max_new_tokens, min_new_tokens=min_new_tokens,
+               temperature=temperature, top_k=top_k, top_p=top_p, do_sample=do_sample,
+               repetition_penalty=repetition_penalty, uniforms=uniforms, trailing_len=trailing_len)
     slot = int(getattr(talker_graph, "slot", 0) if slot is None else slot)
-    native = _native_prefill(engine, talker_graph, tie)
-    pad = int((tam[0] == 0).sum().item()) if tam is not None else 0
-    if native:
-        # K3: hand-written prefill writes the KV cache directly (no talker.forward, no prefill_kv copies)
-        out = _native_out(*engine.prefill(tie[0], pad, slot=slot))
-    else:
-        out = _prefill(talker, tie, tam, tth, tpe)
-    uniforms = _uniforms(engine, predictor_graph, uniforms, **gen)
-    u0 = float(uniforms.reshape(-1)[0]) if (do_sample and uniforms is not None) else 0.0
+    got = begin_fused_batch(engine, talker, [row], config, predictor_graph, talker_graph, [slot], logprob=logprob)
+    return (got[0][0], got[1][0]) if logprob else got[0]
+
+
+def _gen(row):
+    """the sampling keywords of a ``begin_fused_batch`` row"""
+    return {k: v for k, v in row.items() if k not in ("tie", "tam", "tth", "tpe", "uniforms", "trailing_len")}
+
+
+def _begin_upstream(engine, talker, row, config, predictor_graph, talker_graph, slot, logprob):
+    """One row prefilled by the upstream ``talker.forward`` (fp32 engine, a graph that opts out of K3) and latched into
+    `slot`, its KV cache imported: -> (first token id, its log-probability as a float or None)."""
+    gen = _gen(row)
+    pad = int((row["tam"][0] == 0).sum().item()) if row["tam"] is not None else 0
+    out = _prefill(talker, row["tie"], row["tam"], row["tth"], row["tpe"])
+    uniforms = _uniforms(engine, predictor_graph, row.get("uniforms"), **gen)
+    u0 = float(uniforms.reshape(-1)[0]) if (gen["do_sample"] and uniforms is not None) else 0.0
     first = _first_token(engine, out, config, uniforms, u0, logprob=logprob, **gen)
     lp = None
     if logprob:
         first, lp = first
-    latch_fused(engine, talker, out, native, pad, tie, tth, tpe, predictor_graph, talker_graph, first.item(), slot=slot,
-                uniforms=uniforms, trailing_len=trailing_len, **gen)
-    return (first, float(lp.item())) if logprob else first
+        lp = float(lp.item())
+    first = int(first.item())
+    latch_fused(engine, talker, out, False, pad, row["tie"], row["tth"], row["tpe"], predictor_graph, talker_graph, first,
+                slot=slot, uniforms=uniforms, trailing_len=row.get("trailing_len"), **gen)
+    return first, lp
 
 
 def begin_fused_batch(engine, talker, rows, config, predictor_graph, talker_graph, slots, logprob=False):
-    """``begin_fused`` for several rows into distinct slots: ``rows[b]`` holds the arguments of one ``begin_fused`` call
-    (tie [1,P,H], tam, tth, tpe, the sampling keywords, uniforms, trailing_len).  On a K3 engine all prompts go through
-    ONE ``Engine.prefill_batch`` and the first tokens of all rows come back with one host synchronisation; every row
-    latches what ``begin_fused`` would latch.  Otherwise (fp32 engine, a graph that opts out of K3) each row takes
-    ``begin_fused``.  Returns the first token ids; with ``logprob`` (ids, their log-probabilities as floats)."""
+    """Prefill + first token + request latch for several rows into distinct slots: ``rows[b]`` holds the arguments of
+    one ``begin_fused`` call (tie [1,P,H], tam, tth, tpe, the sampling keywords, uniforms, trailing_len).  On a K3
+    engine all prompts go through ONE ``Engine.prefill_batch`` and the first tokens of all rows come back with one host
+    synchronisation.  Otherwise (fp32 engine, a graph that opts out of K3) each row is prefilled by the upstream
+    ``talker.forward`` in turn.  Returns the first token ids; with ``logprob`` (ids, their log-probabilities as
+    floats)."""
     if not all(_native_prefill(engine, talker_graph, r["tie"]) for r in rows):
-        got = [begin_fused(engine, talker, r["tie"], r["tam"], r["tth"], r["tpe"], config, predictor_graph, talker_graph,
-                           slot=s, logprob=logprob, **{k: v for k, v in r.items() if k not in ("tie", "tam", "tth", "tpe")})
+        got = [_begin_upstream(engine, talker, r, config, predictor_graph, talker_graph, int(s), logprob)
                for r, s in zip(rows, slots)]
-        if logprob:
-            return [int(f) for f, _ in got], [lp for _, lp in got]
-        return [int(f) for f in got]
-    gens = [{k: v for k, v in r.items() if k not in ("tie", "tam", "tth", "tpe", "uniforms", "trailing_len")} for r in rows]
+        firsts, lps = [f for f, _ in got], [lp for _, lp in got]
+        return (firsts, lps) if logprob else firsts
+    gens = [_gen(r) for r in rows]
     n = len(rows)
     uniforms = [_uniforms(engine, predictor_graph, r.get("uniforms"), **g) for r, g in zip(rows, gens)]
     # pad counts (host arrays of the C call) and first-token draws of all rows: one transfer (float64 holds both exactly)
@@ -246,25 +256,12 @@ def fast_generate(
         raise ValueError("return_logprobs needs graph handles backed by one loaded fq3 engine (the fused decode path)")
     t0 = time.time()
     if engine is not None:
-        lkw = {"logprob": True} if return_logprobs else {}   # off: the calls are exactly those without the option
-        first = begin_fused(engine, talker, talker_input_embeds, attention_mask, trailing_text_hiddens, tts_pad_embed,
-                            config, predictor_graph, talker_graph, uniforms=uniforms, **lkw, **skw)
-        _sync(device)
-        t_prefill = time.time() - t0
+        from .batching import _chunks, _single
+        sched, rq, t_prefill = _single(engine, talker, config, predictor_graph, talker_graph,
+                                       dict(tie=talker_input_embeds, tam=attention_mask, tth=trailing_text_hiddens,
+                                            tpe=tts_pad_embed, uniforms=uniforms, **skw), return_logprobs)
         t1 = time.time()
-        parts = []
-        lpa = FrameLogprobs(first[1]) if return_logprobs else None
-        while True:
-            slot = getattr(talker_graph, "slot", 0)
-            if lpa is not None:
-                codes, lp, res = engine.decode_chunk(_MAX_LAUNCH_FRAMES, slot=slot, logprobs=True)
-                lpa.push(lp)
-            else:
-                codes, res = engine.decode_chunk(_MAX_LAUNCH_FRAMES, slot=slot)
-            if res.frames_emitted:
-                parts.append(codes.clone())
-            if res.finished:
-                break
+        parts = [codes for items in _chunks(sched, _MAX_LAUNCH_FRAMES, t_prefill) for _, codes, _ in items]
         t_decode = time.time() - t1
         all_codes = torch.cat(parts) if parts else None
     else:
@@ -289,8 +286,8 @@ def fast_generate(
         "steps_per_s": (n / t_decode) if t_decode > 0 else 0,
     }
     if return_logprobs:
-        timing["logprobs"] = lpa.frames()
-        timing["eos_logprob"] = lpa.eos_logprob(res.next_token, engine.eos)
+        timing["logprobs"] = rq.lp.frames()
+        timing["eos_logprob"] = rq.eos_logprob
     return all_codes, timing
 
 

@@ -9,8 +9,8 @@ from typing import Generator, Optional, Tuple
 
 import torch
 
-from .generate import _sync, begin_fused, shared_engine, special_suppress_mask, stepwise_frames
-from .logprobs import FrameLogprobs
+from .batching import _chunks, _single
+from .generate import _sync, shared_engine, special_suppress_mask, stepwise_frames
 from .sampling import apply_repetition_penalty, sample_logits
 
 
@@ -50,43 +50,17 @@ def fast_generate_streaming(
     engine = shared_engine(predictor_graph, talker_graph)
     if return_logprobs and engine is None:
         raise ValueError("return_logprobs needs graph handles backed by one loaded fq3 engine (the fused decode path)")
-    t0 = time.time()
-    total = idx = 0
     if engine is not None:
-        lkw = {"logprob": True} if return_logprobs else {}   # off: the calls are exactly those without the option
-        first = begin_fused(engine, talker, talker_input_embeds, attention_mask, trailing_text_hiddens, tts_pad_embed,
-                            config, predictor_graph, talker_graph, uniforms=uniforms, **lkw, **skw)
-        lpa = FrameLogprobs(first[1]) if return_logprobs else None
-        _sync(device)
-        t_prefill = time.time() - t0
-        t1 = time.time()
-        while True:
-            slot = getattr(talker_graph, "slot", 0)
-            if lpa is not None:
-                codes, lp, res = engine.decode_chunk(chunk_size, slot=slot, logprobs=True)
-            else:
-                codes, res = engine.decode_chunk(chunk_size, slot=slot)
-            n = res.frames_emitted
-            if n:
-                total += n
-                # the reference flags the trailing partial chunk -- and a full chunk cut off by the cache limit, which
-                # leaves its loop before the "buffer full" check (streaming.py:130-132 vs :158-173)
-                tm = _timing(idx, n, t_prefill, time.time() - t1, total, n < chunk_size or res.finished == 3)
-                if engine.time_kernels:
-                    tm["kernel_ms"] = engine.last_kernel_ms
-                if lpa is not None:
-                    tm["logprobs"] = lpa.push(lp)
-                    if res.finished or res.next_token == engine.eos:   # nothing follows this chunk
-                        tm["eos_logprob"] = lpa.eos_logprob(res.next_token, engine.eos)
-                yield codes.clone(), tm
-                idx += 1
-                t1 = time.time()
-            if res.finished:
-                return
+        sched, _, t_prefill = _single(engine, talker, config, predictor_graph, talker_graph,
+                                      dict(tie=talker_input_embeds, tam=attention_mask, tth=trailing_text_hiddens,
+                                           tpe=tts_pad_embed, uniforms=uniforms, **skw), return_logprobs)
+        for items in _chunks(sched, chunk_size, t_prefill):
+            for _, codes, tm in items:
+                yield codes, tm
     else:
         yield from _chunked(stepwise_frames(talker, talker_input_embeds, attention_mask, trailing_text_hiddens,
                                             tts_pad_embed, config, predictor_graph, talker_graph, **skw),
-                            device, chunk_size, t0)
+                            device, chunk_size, time.time())
 
 
 def _chunked(frames, device, chunk_size, t0):

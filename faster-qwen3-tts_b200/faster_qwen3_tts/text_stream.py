@@ -189,13 +189,15 @@ def generate_text_streaming(model, text_stream: Iterable[str], *, language: str,
                             ) -> Iterator:
     """Yields (pcm, sample_rate, timing) like the ``*_streaming`` methods.  Prefills once the first text id is
     committed, then per launch: pull text until the next chunk's rows exist (window codec policy) or one more row
-    exists (stateful codec), or the text closes; announce the rows; decode one chunk.
+    exists (stateful codec), or the text closes; announce the rows; decode one chunk.  The request is the one request of
+    a ``BatchScheduler`` on the graph's slot: its ``rows_ahead`` rule (``SlotRequest.ready``) says when to launch.
 
     The window policy gets only full ``chunk_size`` chunks plus the final partial one, exactly the chunking of the
     one-shot request, so its PCM is identical.  The stateful codec decodes whatever frames exist at once: a stream equals
     the one-shot decode whatever the chunking.  ``timing`` has the reference's keys plus ``text_wait_ms``, the time this
     chunk spent blocked on ``text_stream``."""
-    from .generate import _sync, begin_fused, shared_engine
+    from .batching import _chunks, _single
+    from .generate import shared_engine
     engine = shared_engine(model.predictor_graph, model.talker_graph)
     if engine is None:
         raise RuntimeError("text streaming needs graph handles backed by one loaded fq3 engine")
@@ -223,47 +225,28 @@ def generate_text_streaming(model, text_stream: Iterable[str], *, language: str,
         feed.close()   # raises: no text at all
     tie, tam, tpe = build_prompt(model, feed, language=language, speaker=speaker, instruct_ids=instruct_ids,
                                  voice_clone_prompt=voice_clone_prompt)
-    slot = int(getattr(model.talker_graph, "slot", 0))
-    t0 = time.time()
-    begin_fused(engine, m.talker, tie, tam, feed.rows[None], tpe, m.config.talker_config, model.predictor_graph,
-                model.talker_graph, max_new_tokens=max_new_tokens, min_new_tokens=min_new_tokens,
-                temperature=temperature, top_k=top_k, top_p=top_p, do_sample=do_sample,
-                repetition_penalty=repetition_penalty, uniforms=uniforms, slot=slot, trailing_len=0)
-    _sync(tie.device)
-    t_prefill = time.time() - t0
-    gen0 = engine.gen_step0[slot]
     win = model._make_window(st, None, chunk_size, to_host) if st is not None else None
     # the window policy's PCM depends on the chunking: launch only when a full chunk of rows exists, so that every launch
     # emits a full chunk or ends the request.  A stateful stream (or codes only) is the same in any chunking.
     ahead = 1 if win is None or getattr(win, "any_chunking", False) else chunk_size
+    sched, rq, t_prefill = _single(
+        engine, m.talker, m.config.talker_config, model.predictor_graph, model.talker_graph,
+        dict(tie=tie, tam=tam, tth=feed.rows[None], tpe=tpe, max_new_tokens=max_new_tokens,
+             min_new_tokens=min_new_tokens, temperature=temperature, top_k=top_k, top_p=top_p, do_sample=do_sample,
+             repetition_penalty=repetition_penalty, uniforms=uniforms, feed=feed, rows_ahead=ahead))
     wait_before = wait[0]   # text wait before the prefill: reported with the first chunk, outside its decode window
     wait[0] = 0.0
-    total = idx = 0
-    finished = False
-    t1 = time.time()
-    while not finished:
-        # frames at or past max_new_tokens never run, so rows past it are never needed
-        need = min(gen0 + total + ahead, feed.max_rows)
-        pull(lambda: feed.update() >= need)
+
+    def rows_ready() -> bool:
         feed.update()
-        engine.set_text_rows(slot, feed.n_rows, open=not feed.closed)
-        codes, res = engine.decode_chunk(chunk_size, slot=slot)
-        n = int(res.frames_emitted)
-        finished = bool(res.finished)
-        if not n:
-            continue
-        total += n
-        chunk = codes.clone()
-        tm = {"chunk_index": idx, "chunk_steps": n,
-              "prefill_ms": t_prefill * 1000 if idx == 0 else 0, "decode_ms": (time.time() - t1 - wait[0]) * 1000,
-              "total_steps_so_far": total, "is_final": finished, "text_wait_ms": (wait[0] + wait_before) * 1000}
-        if engine.time_kernels:
-            tm["kernel_ms"] = engine.last_kernel_ms
+        return rq.ready()
+
+    for (_, codes, tm), in _chunks(sched, chunk_size, t_prefill, before_step=lambda: pull(rows_ready)):
+        tm.update(decode_ms=tm["decode_ms"] - wait[0] * 1000, is_final=bool(rq.finished),
+                  text_wait_ms=(wait[0] + wait_before) * 1000)
         wait[0] = wait_before = 0.0
         if win is None:
-            yield (chunk.cpu().numpy() if to_host else chunk), model.sample_rate, tm
+            yield (codes.cpu().numpy() if to_host else codes), model.sample_rate, tm
         else:
-            pcm, sr = win.push(chunk)
+            pcm, sr = win.push(codes)
             yield pcm, sr, tm
-        idx += 1
-        t1 = time.time()

@@ -110,8 +110,8 @@ tpe = prompts[0][3]
 many = batching.BatchScheduler.submit_many
 
 
-def one_by_one(self, requests):
-    return [self.submit(**r) for r in requests]
+def one_by_one(self, requests, logprobs=False):
+    return [many(self, [r], logprobs=logprobs)[0] for r in requests]
 
 
 def burst(mode):
