@@ -522,7 +522,7 @@ extern "C" int fq3_codec_load_weights(fq3_codec* c, const fq3_tensor* tensors, i
 }
 
 static int launch_conv(fq3_codec* c, const Layer& L, const __nv_bfloat16* X, const __nv_bfloat16* R, __nv_bfloat16* Yraw,
-                       __nv_bfloat16* Yact, int T, int batch, cudaStream_t stream, int x_row0 = 0, int x_rows = 0) {
+                       __nv_bfloat16* Yact, int T, int batch, cudaStream_t stream, int x_row0, int x_rows) {
   ConvArgs a;
   a.X = X; a.W = L.W; a.bias = L.bias; a.R = R; a.Yraw = Yraw; a.Yact = Yact; a.ea = L.ea; a.ib = L.ib;
   a.T = T; a.Cin = L.Cin; a.N = L.N; a.taps = L.taps; a.dil = L.dil; a.bias_mod = L.bias_mod; a.act_mod = L.act_mod;
@@ -535,64 +535,8 @@ static int launch_conv(fq3_codec* c, const Layer& L, const __nv_bfloat16* X, con
   return 0;
 }
 
-// the waveform stack on a channels-last bf16 input xcl [batch][T4][hidden]; pcm_out_dev float32 [batch][T4 * prod(rates)]
-static int stack_reserve(fq3_codec* c, int batch, int T4) {
-  // largest tensor: [T_final][C_final * 2] worth of bf16 at the widest level; size every buffer for the maximum
-  size_t need = (size_t)T4 * c->hidden;
-  {
-    size_t T = T4;
-    int C = c->decoder_dim;
-    need = std::max(need, T * (size_t)C);
-    for (int bi = 0; bi < c->n_blocks; ++bi) {
-      T *= c->rates[bi];
-      C /= 2;
-      need = std::max(need, T * (size_t)C);
-    }
-  }
-  need *= (size_t)batch;
-  if (need > c->cap) {
-    for (auto*& b : c->buf) { if (b) cudaFree(b); b = nullptr; }
-    for (auto*& b : c->buf) CCK(cudaMalloc(&b, need * 2));
-    c->cap = need;
-  }
-  return 0;
-}
-
-static int stack_run(fq3_codec* c, const __nv_bfloat16* xcl, int batch, int T4, float* pcm_out_dev, cudaStream_t stream) {
-  int rc;
-  int T = T4;
-  size_t li = 0;
-  // four ping-pong buffers.  `cur` always holds the activated input of the next layer; the other three are free.
-  __nv_bfloat16* cur = c->buf[1];
-  if ((rc = launch_conv(c, c->layers[li++], xcl, nullptr, nullptr, cur, T, batch, stream))) return rc;
-  for (int bi = 0; bi < c->n_blocks; ++bi) {
-    __nv_bfloat16* f[3];
-    int k = 0;
-    for (auto* b : c->buf)
-      if (b != cur) f[k++] = b;
-    __nv_bfloat16 *x = f[0], *a1 = f[1], *a2 = f[2], *y = cur;  // cur is free once the up-conv has consumed it
-    const Layer& U = c->layers[li++];
-    if ((rc = launch_conv(c, U, cur, nullptr, x, a1, T, batch, stream))) return rc;  // raw -> x, SnakeBeta(raw) -> a1
-    T *= U.upsample;
-    for (int j = 0; j < 3; ++j) {
-      const Layer& C1 = c->layers[li++];
-      const Layer& C2 = c->layers[li++];
-      if ((rc = launch_conv(c, C1, a1, nullptr, nullptr, a2, T, batch, stream))) return rc;  // a2 = act2(conv7(a1))
-      // y = conv1(a2) + x ; a1 <- SnakeBeta_next(y)   (conv7 has consumed a1, so it can be overwritten)
-      if ((rc = launch_conv(c, C2, a2, x, C2.write_raw ? y : nullptr, a1, T, batch, stream))) return rc;
-      std::swap(x, y);
-    }
-    cur = a1;
-  }
-  __nv_bfloat16* act = cur;
-  FQ3_LAUNCH((conv_out_kernel), dim3((T + 255) / 256, batch), 256, 0, stream, act, c->w_out, c->b_out, T, c->c_out, 7, pcm_out_dev, 0, T);
-  c->launches++;
-  CCK(cudaGetLastError());
-  return 0;
-}
-
 // ------------------------------------------------------------------------------------------------------------
-// front end: weights + the codes -> PCM entry point
+// front end weights
 // ------------------------------------------------------------------------------------------------------------
 // dst[(n * dmul + dadd) * K + k] = bf16(src[off + n * sn + k * sk])   (weight repacking on device)
 static __global__ void cast_strided_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ dst, long long N,
@@ -736,76 +680,6 @@ static int fe_gemm(fq3_codec* c, const __nv_bfloat16* X, const __nv_bfloat16* W,
   return 0;
 }
 
-/* speech_tokenizer.decode (model.py:924,1093,1122) in one call: codes int64 [batch][T][Q] (device) -> PCM float32
- * [batch][T * total_upsample], clamped to [-1, 1].  `batch` windows of equal length share every launch. */
-extern "C" int fq3_codec_decode_codes(fq3_codec* c, const int64_t* codes_dev, int32_t batch, int32_t T, float* pcm_out_dev,
-                                      void* stream_) {
-  if (!c || !codes_dev || !pcm_out_dev || T <= 0 || batch <= 0) return cfail(FQ3_ERR_INVALID, "null argument");
-  if (c->layers.empty()) return cfail(FQ3_ERR_STATE, "codec weights not loaded");
-  FrontEnd& f = c->fe;
-  if (!f.ready) return cfail(FQ3_ERR_STATE, "fq3_codec_load_frontend has not been called");
-  CodecDevGuard dev_guard(c->dev);
-  cudaStream_t stream = (cudaStream_t)stream_;
-  const int H = f.H, I = f.I, hd = H / f.nh;
-  const size_t rows0 = (size_t)batch * T;
-  size_t up = 1;
-  for (auto& u : f.ups) up *= (size_t)u.r;
-  const size_t rowsU = rows0 * up;
-  if (rowsU > f.cap_rows) {
-    for (auto*& b : f.buf) { if (b) cudaFree(b); b = nullptr; }
-    const size_t wide = std::max(rows0 * (size_t)std::max(3 * H, I), rowsU * (size_t)4 * H);
-    for (int i = 0; i < 5; ++i) CCK(cudaMalloc(&f.buf[i], (i == 3 ? wide : rowsU * (size_t)H) * 2));
-    f.cap_rows = rowsU;
-  }
-  int rc;
-  if ((rc = stack_reserve(c, batch, (int)(T * up)))) return rc;
-  __nv_bfloat16 *A = f.buf[0], *Bx = f.buf[1], *Cn = f.buf[2], *D = f.buf[3], *E = f.buf[4];
-  const int R0 = (int)rows0;
-  FQ3_LAUNCH((fe::embed_mean_kernel), R0, 256, 0, stream, (const long long*)codes_dev, f.emb, f.Q, f.codebook, H, A);
-  c->launches++;
-  const int Wpad = (f.window + 31) & ~31;
-  const size_t swa_smem = (size_t)(8 * Wpad + 8 * hd) * sizeof(float);
-  if (swa_smem > 96 * 1024) return cfail(FQ3_ERR_INVALID, "sliding window too large");
-  for (int l = 0; l < f.L; ++l) {
-    const FeLayer& y = f.layers[l];
-    FQ3_LAUNCH((fe::rmsnorm_rows_kernel), R0, 256, 0, stream, A, y.ln1, H, f.eps, Cn);
-    if ((rc = fe_gemm(c, Cn, y.qkv, nullptr, nullptr, nullptr, D, R0, H, 3 * H, 1, 0, stream))) return rc;
-    {
-      const long long warps = (long long)R0 * f.nh * 2;
-      FQ3_LAUNCH((fe::rope_qk_kernel), (unsigned)((warps * 32 + 255) / 256), 256, 0, stream, D, R0, T, f.nh, hd, f.inv_freq, nullptr);
-    }
-    {
-      dim3 g((T + 7) / 8, f.nh, batch);
-      if (hd == 64) FQ3_LAUNCH((fe::swa_kernel<64>), g, 256, swa_smem, stream, D, T, f.nh, f.window, E, T, 0, nullptr);
-      else FQ3_LAUNCH((fe::swa_kernel<128>), g, 256, swa_smem, stream, D, T, f.nh, f.window, E, T, 0, nullptr);
-    }
-    if ((rc = fe_gemm(c, E, y.o, nullptr, y.s1, A, Bx, R0, H, H, 1, 0, stream))) return rc;
-    FQ3_LAUNCH((fe::rmsnorm_rows_kernel), R0, 256, 0, stream, Bx, y.ln2, H, f.eps, Cn);
-    if ((rc = fe_gemm(c, Cn, y.gu, nullptr, nullptr, nullptr, D, R0, H, 2 * I, 1, 1, stream))) return rc;
-    if ((rc = fe_gemm(c, D, y.down, nullptr, y.s2, Bx, A, R0, I, H, 1, 0, stream))) return rc;
-    c->launches += 4;
-  }
-  FQ3_LAUNCH((fe::rmsnorm_rows_kernel), R0, 256, 0, stream, A, f.norm, H, f.eps, Cn);
-  c->launches++;
-  __nv_bfloat16* cur = Cn;
-  int rows = R0, Tc = T;
-  for (size_t u = 0; u < f.ups.size(); ++u) {
-    const FeUp& y = f.ups[u];
-    __nv_bfloat16* out = (cur == Cn) ? E : Cn;
-    // ConvTranspose1d(k = s = r) as a GEMM onto r*H phase channels: [rows][r*H] IS [rows*r][H]
-    if ((rc = fe_gemm(c, cur, y.ct, y.ct_b, nullptr, nullptr, A, rows, H, y.r * H, H, 0, stream))) return rc;
-    rows *= y.r;
-    Tc *= y.r;
-    FQ3_LAUNCH((fe::dwconv_ln_kernel), rows, 256, 0, stream, A, Tc, H, y.dw_w, y.dw_b, y.ln_w, y.ln_b, 1e-6f, Bx, 0, Tc);
-    c->launches++;
-    if ((rc = fe_gemm(c, Bx, y.pw1, y.pw1_b, nullptr, nullptr, D, rows, H, 4 * H, 4 * H, 2, stream))) return rc;
-    if ((rc = fe_gemm(c, D, y.pw2, y.pw2_b, y.gamma, A, out, rows, 4 * H, H, H, 0, stream))) return rc;
-    cur = out;
-  }
-  CCK(cudaGetLastError());
-  return stack_run(c, cur, batch, Tc, pcm_out_dev, stream);
-}
-
 
 // ------------------------------------------------------------------------------------------------------------
 // Stateful streaming decode (SURVEY 8(f) item 2): instead of re-decoding a window of old frames for every chunk
@@ -813,7 +687,8 @@ extern "C" int fq3_codec_decode_codes(fq3_codec* c, const int64_t* codes_dev, in
 // keeps the tail of its own input -- (k-1)*dilation rows for a causal conv, 1 row for a transposed conv, the last
 // window-1 (k, v) rows for the sliding-window attention -- and a chunk costs only its own frames.  Each output row is
 // computed by exactly the arithmetic of a one-shot decode of the whole sequence (the model is causal), so the PCM of a
-// stream equals the non-streaming decode of the same codes.
+// stream equals the non-streaming decode of the same codes.  The one-shot decode is the same forward (codec_forward)
+// without history.
 // ------------------------------------------------------------------------------------------------------------
 static __global__ void ext_build_kernel(const __nv_bfloat16* const* __restrict__ tails, size_t off,
                                         const __nv_bfloat16* __restrict__ X, int h, int T, int C8,
@@ -854,6 +729,164 @@ static int stream_sites(fq3_codec* c) {
   add(6, c->c_out);
   c->tail_elems = off;
   return 0;
+}
+
+// front-end and waveform-stack activations of `batch` sequences of T code frames (grown on demand)
+static int reserve(fq3_codec* c, int batch, int T) {
+  FrontEnd& f = c->fe;
+  const size_t rows0 = (size_t)batch * T;
+  size_t up = 1;
+  for (auto& u : f.ups) up *= (size_t)u.r;
+  const size_t rowsU = rows0 * up;
+  if (rowsU > f.cap_rows) {
+    for (auto*& b : f.buf) { if (b) cudaFree(b); b = nullptr; }
+    const size_t wide = std::max(rows0 * (size_t)std::max(3 * f.H, f.I), rowsU * (size_t)4 * f.H);
+    for (int i = 0; i < 5; ++i) CCK(cudaMalloc(&f.buf[i], (i == 3 ? wide : rowsU * (size_t)f.H) * 2));
+    f.cap_rows = rowsU;
+  }
+  // waveform stack: largest tensor [T_final][C_final * 2] worth of bf16 at the widest level; every buffer sized for it
+  size_t Tl = (size_t)T * up;
+  int C = c->decoder_dim;
+  size_t need = std::max(Tl * c->hidden, Tl * (size_t)C);
+  for (int bi = 0; bi < c->n_blocks; ++bi) {
+    Tl *= c->rates[bi];
+    C /= 2;
+    need = std::max(need, Tl * (size_t)C);
+  }
+  need *= (size_t)batch;
+  if (need > c->cap) {
+    for (auto*& b : c->buf) { if (b) cudaFree(b); b = nullptr; }
+    for (auto*& b : c->buf) CCK(cudaMalloc(&b, need * 2));
+    c->cap = need;
+  }
+  return 0;
+}
+
+/* The codec forward of both entry points: codes int64 [batch][T][Q] (device) -> PCM float32 [batch][T * total_upsample]
+ * clamped to [-1, 1]; conv_out is skipped when pcm_out_dev is NULL.  history = true: every causal site reads the
+ * streams' tails in front of its new rows, through the per-call tables (d_tailptr, d_pos0, d_valid) and c->ext that
+ * fq3_codec_stream_decode has set up, and saves its new tail.  history = false: the one-shot decode, the same launches
+ * without the history copies -- no site has rows in front, no sequence has earlier positions. */
+static int codec_forward(fq3_codec* c, const int64_t* codes_dev, int batch, int T, float* pcm_out_dev, bool history,
+                         cudaStream_t stream) {
+  FrontEnd& f = c->fe;
+  const int H = f.H, I = f.I, hd = H / f.nh;
+  const int Wpad = (f.window + 31) & ~31;
+  const size_t swa_smem = (size_t)(8 * Wpad + 8 * hd) * sizeof(float);
+  if (swa_smem > 96 * 1024) return cfail(FQ3_ERR_INVALID, "sliding window too large");
+  int rc;
+  if ((rc = reserve(c, batch, T))) return rc;
+  const int* pos0 = history ? c->d_pos0 : nullptr;
+  const int* valid = history ? c->d_valid : nullptr;
+  size_t site = 0;
+  // input X [batch][Tn][C] of the next causal site with its h history rows in front -> c->ext [batch][h + Tn][C], the
+  // streams' tails updated; X itself when h = 0
+  auto with_history = [&](const __nv_bfloat16* X, int Tn, int& h) -> const __nv_bfloat16* {
+    h = 0;
+    if (!history) return X;
+    const fq3_codec::Site& st = c->sites[site++];
+    if (st.h == 0) return X;
+    h = st.h;
+    const int C8 = st.C / 8;
+    const long long n = (long long)(st.h + Tn) * C8;
+    dim3 g((unsigned)std::min<long long>((n + 255) / 256, 1024), batch);
+    FQ3_LAUNCH((ext_build_kernel), g, 256, 0, stream, (const __nv_bfloat16* const*)c->d_tailptr, st.off, X, st.h, Tn, C8, c->ext);
+    dim3 g2((unsigned)std::min<long long>(((long long)st.h * C8 + 255) / 256, 256), batch);
+    FQ3_LAUNCH((tail_save_kernel), g2, 256, 0, stream, (__nv_bfloat16* const*)c->d_tailptr, st.off, c->ext, st.h, Tn, C8);
+    c->launches += 2;
+    return c->ext;
+  };
+  int h;
+  // ---- front end
+  __nv_bfloat16 *A = f.buf[0], *Bx = f.buf[1], *Cn = f.buf[2], *D = f.buf[3], *E = f.buf[4];
+  const int R0 = batch * T;
+  FQ3_LAUNCH((fe::embed_mean_kernel), R0, 256, 0, stream, (const long long*)codes_dev, f.emb, f.Q, f.codebook, H, A);
+  c->launches++;
+  for (int l = 0; l < f.L; ++l) {
+    const FeLayer& y = f.layers[l];
+    FQ3_LAUNCH((fe::rmsnorm_rows_kernel), R0, 256, 0, stream, A, y.ln1, H, f.eps, Cn);
+    if ((rc = fe_gemm(c, Cn, y.qkv, nullptr, nullptr, nullptr, D, R0, H, 3 * H, 1, 0, stream))) return rc;
+    {
+      const long long warps = (long long)R0 * f.nh * 2;
+      FQ3_LAUNCH((fe::rope_qk_kernel), (unsigned)((warps * 32 + 255) / 256), 256, 0, stream, D, R0, T, f.nh, hd, f.inv_freq, pos0);
+    }
+    const __nv_bfloat16* qkv = with_history(D, T, h);
+    {
+      dim3 g((T + 7) / 8, f.nh, batch);
+      if (hd == 64) FQ3_LAUNCH((fe::swa_kernel<64>), g, 256, swa_smem, stream, qkv, T, f.nh, f.window, E, h + T, h, valid);
+      else FQ3_LAUNCH((fe::swa_kernel<128>), g, 256, swa_smem, stream, qkv, T, f.nh, f.window, E, h + T, h, valid);
+    }
+    if ((rc = fe_gemm(c, E, y.o, nullptr, y.s1, A, Bx, R0, H, H, 1, 0, stream))) return rc;
+    FQ3_LAUNCH((fe::rmsnorm_rows_kernel), R0, 256, 0, stream, Bx, y.ln2, H, f.eps, Cn);
+    if ((rc = fe_gemm(c, Cn, y.gu, nullptr, nullptr, nullptr, D, R0, H, 2 * I, 1, 1, stream))) return rc;
+    if ((rc = fe_gemm(c, D, y.down, nullptr, y.s2, Bx, A, R0, I, H, 1, 0, stream))) return rc;
+    c->launches += 4;
+  }
+  FQ3_LAUNCH((fe::rmsnorm_rows_kernel), R0, 256, 0, stream, A, f.norm, H, f.eps, Cn);
+  c->launches++;
+  __nv_bfloat16* cur = Cn;
+  int rows = R0, Ts = T;
+  for (size_t u = 0; u < f.ups.size(); ++u) {
+    const FeUp& y = f.ups[u];
+    __nv_bfloat16* out = (cur == Cn) ? E : Cn;
+    // ConvTranspose1d(k = s = r) as a GEMM onto r*H phase channels: [rows][r*H] IS [rows*r][H]
+    if ((rc = fe_gemm(c, cur, y.ct, y.ct_b, nullptr, nullptr, A, rows, H, y.r * H, H, 0, stream))) return rc;
+    rows *= y.r;
+    Ts *= y.r;
+    const __nv_bfloat16* xin = with_history(A, Ts, h);
+    FQ3_LAUNCH((fe::dwconv_ln_kernel), rows, 256, 0, stream, xin, Ts, H, y.dw_w, y.dw_b, y.ln_w, y.ln_b, 1e-6f, Bx, h, h + Ts);
+    c->launches++;
+    if ((rc = fe_gemm(c, Bx, y.pw1, y.pw1_b, nullptr, nullptr, D, rows, H, 4 * H, 4 * H, 2, stream))) return rc;
+    if ((rc = fe_gemm(c, D, y.pw2, y.pw2_b, y.gamma, A, out, rows, 4 * H, H, H, 0, stream))) return rc;
+    cur = out;
+  }
+  CCK(cudaGetLastError());
+  // ---- waveform stack
+  size_t li = 0;
+  auto conv = [&](const Layer& L, const __nv_bfloat16* X, const __nv_bfloat16* R, __nv_bfloat16* Yraw, __nv_bfloat16* Yact) -> int {
+    const __nv_bfloat16* xin = with_history(X, Ts, h);
+    return launch_conv(c, L, xin, R, Yraw, Yact, Ts, batch, stream, h, h + Ts);
+  };
+  // four ping-pong buffers.  `act` always holds the activated input of the next layer; the other three are free.
+  __nv_bfloat16* act = c->buf[1];
+  if ((rc = conv(c->layers[li++], cur, nullptr, nullptr, act))) return rc;
+  for (int bi = 0; bi < c->n_blocks; ++bi) {
+    __nv_bfloat16* fr[3];
+    int k = 0;
+    for (auto* b : c->buf)
+      if (b != act) fr[k++] = b;
+    __nv_bfloat16 *x = fr[0], *a1 = fr[1], *a2 = fr[2], *y = act;  // act is free once the up-conv has consumed it
+    const Layer& U = c->layers[li++];
+    if ((rc = conv(U, act, nullptr, x, a1))) return rc;  // raw -> x, SnakeBeta(raw) -> a1
+    Ts *= U.upsample;
+    for (int j = 0; j < 3; ++j) {
+      const Layer& C1 = c->layers[li++];
+      const Layer& C2 = c->layers[li++];
+      if ((rc = conv(C1, a1, nullptr, nullptr, a2))) return rc;  // a2 = act2(conv7(a1))
+      // y = conv1(a2) + x ; a1 <- SnakeBeta_next(y)   (conv7 has consumed a1, so it can be overwritten)
+      if ((rc = conv(C2, a2, x, C2.write_raw ? y : nullptr, a1))) return rc;
+      std::swap(x, y);
+    }
+    act = a1;
+  }
+  const __nv_bfloat16* xin = with_history(act, Ts, h);   // conv_out's history advances even when no PCM is wanted
+  if (pcm_out_dev) {
+    FQ3_LAUNCH((conv_out_kernel), dim3((Ts + 255) / 256, batch), 256, 0, stream, xin, c->w_out, c->b_out, Ts, c->c_out, 7, pcm_out_dev, h, h + Ts);
+    c->launches++;
+  }
+  CCK(cudaGetLastError());
+  return 0;
+}
+
+/* speech_tokenizer.decode (model.py:924,1093,1122) in one call: codes int64 [batch][T][Q] (device) -> PCM float32
+ * [batch][T * total_upsample], clamped to [-1, 1].  `batch` windows of equal length share every launch. */
+extern "C" int fq3_codec_decode_codes(fq3_codec* c, const int64_t* codes_dev, int32_t batch, int32_t T, float* pcm_out_dev,
+                                      void* stream_) {
+  if (!c || !codes_dev || !pcm_out_dev || T <= 0 || batch <= 0) return cfail(FQ3_ERR_INVALID, "null argument");
+  if (c->layers.empty()) return cfail(FQ3_ERR_STATE, "codec weights not loaded");
+  if (!c->fe.ready) return cfail(FQ3_ERR_STATE, "fq3_codec_load_frontend has not been called");
+  CodecDevGuard dev_guard(c->dev);
+  return codec_forward(c, codes_dev, batch, T, pcm_out_dev, false, (cudaStream_t)stream_);
 }
 
 extern "C" int fq3_codec_stream_create(fq3_codec* c, fq3_codec_stream** out) {
@@ -909,8 +942,7 @@ extern "C" int fq3_codec_stream_decode(fq3_codec* c, fq3_codec_stream* const* st
   CodecDevGuard dev_guard(c->dev);
   cudaStream_t stream = (cudaStream_t)stream_;
   stream_sites(c);
-  const int batch = n_streams;
-  const int H = f.H, I = f.I, hd = H / f.nh, W1 = f.window - 1;
+  const int batch = n_streams, W1 = f.window - 1;
   // ---- per-call stream tables
   if (batch > c->tab_cap) {
     if (c->d_tailptr) { cudaFree(c->d_tailptr); cudaFree(c->d_pos0); cudaFree(c->d_valid); }
@@ -932,19 +964,7 @@ extern "C" int fq3_codec_stream_decode(fq3_codec* c, fq3_codec_stream* const* st
     CCK(cudaMemcpyAsync(c->d_valid, vd.data(), batch * sizeof(int), cudaMemcpyHostToDevice, stream));
     // pageable sources: cudaMemcpyAsync returns once they have been staged, so the vectors may go out of scope here
   }
-  // ---- buffers
-  const size_t rows0 = (size_t)batch * T;
-  size_t up = 1;
-  for (auto& u : f.ups) up *= (size_t)u.r;
-  const size_t rowsU = rows0 * up;
-  if (rowsU > f.cap_rows) {
-    for (auto*& b : f.buf) { if (b) cudaFree(b); b = nullptr; }
-    const size_t wide = std::max(rows0 * (size_t)std::max(3 * H, I), rowsU * (size_t)4 * H);
-    for (int i = 0; i < 5; ++i) CCK(cudaMalloc(&f.buf[i], (i == 3 ? wide : rowsU * (size_t)H) * 2));
-    f.cap_rows = rowsU;
-  }
-  int rc;
-  if ((rc = stack_reserve(c, batch, (int)(T * up)))) return rc;
+  // ---- c->ext: the largest site input with its history rows in front
   {
     size_t need = 0, Tl = T;
     size_t si = 0;
@@ -960,104 +980,8 @@ extern "C" int fq3_codec_stream_decode(fq3_codec* c, fq3_codec_stream* const* st
       c->ext_cap = need;
     }
   }
-  size_t site = 0;
-  // history rows of site `site` in front of the new rows X [batch][Tn][C]  ->  c->ext [batch][h + Tn][C]; state updated
-  auto with_history = [&](const __nv_bfloat16* X, int Tn) -> const __nv_bfloat16* {
-    const fq3_codec::Site& st = c->sites[site++];
-    if (st.h == 0) return X;
-    const int C8 = st.C / 8;
-    const long long n = (long long)(st.h + Tn) * C8;
-    dim3 g((unsigned)std::min<long long>((n + 255) / 256, 1024), batch);
-    FQ3_LAUNCH((ext_build_kernel), g, 256, 0, stream, (const __nv_bfloat16* const*)c->d_tailptr, st.off, X, st.h, Tn, C8, c->ext);
-    dim3 g2((unsigned)std::min<long long>(((long long)st.h * C8 + 255) / 256, 256), batch);
-    FQ3_LAUNCH((tail_save_kernel), g2, 256, 0, stream, (__nv_bfloat16* const*)c->d_tailptr, st.off, c->ext, st.h, Tn, C8);
-    c->launches += 2;
-    return c->ext;
-  };
-  auto hist = [&](size_t i) { return c->sites[i].h; };
-  // ---- front end
-  __nv_bfloat16 *A = f.buf[0], *Bx = f.buf[1], *Cn = f.buf[2], *D = f.buf[3], *E = f.buf[4];
-  const int R0 = (int)rows0;
-  FQ3_LAUNCH((fe::embed_mean_kernel), R0, 256, 0, stream, (const long long*)codes_dev, f.emb, f.Q, f.codebook, H, A);
-  c->launches++;
-  const int Wpad = (f.window + 31) & ~31;
-  const size_t swa_smem = (size_t)(8 * Wpad + 8 * hd) * sizeof(float);
-  for (int l = 0; l < f.L; ++l) {
-    const FeLayer& y = f.layers[l];
-    FQ3_LAUNCH((fe::rmsnorm_rows_kernel), R0, 256, 0, stream, A, y.ln1, H, f.eps, Cn);
-    if ((rc = fe_gemm(c, Cn, y.qkv, nullptr, nullptr, nullptr, D, R0, H, 3 * H, 1, 0, stream))) return rc;
-    {
-      const long long warps = (long long)R0 * f.nh * 2;
-      FQ3_LAUNCH((fe::rope_qk_kernel), (unsigned)((warps * 32 + 255) / 256), 256, 0, stream, D, R0, T, f.nh, hd, f.inv_freq, c->d_pos0);
-    }
-    const int h = hist(site);
-    const __nv_bfloat16* qkv = with_history(D, T);
-    {
-      dim3 g((T + 7) / 8, f.nh, batch);
-      if (hd == 64) FQ3_LAUNCH((fe::swa_kernel<64>), g, 256, swa_smem, stream, qkv, T, f.nh, f.window, E, h + T, h, c->d_valid);
-      else FQ3_LAUNCH((fe::swa_kernel<128>), g, 256, swa_smem, stream, qkv, T, f.nh, f.window, E, h + T, h, c->d_valid);
-    }
-    if ((rc = fe_gemm(c, E, y.o, nullptr, y.s1, A, Bx, R0, H, H, 1, 0, stream))) return rc;
-    FQ3_LAUNCH((fe::rmsnorm_rows_kernel), R0, 256, 0, stream, Bx, y.ln2, H, f.eps, Cn);
-    if ((rc = fe_gemm(c, Cn, y.gu, nullptr, nullptr, nullptr, D, R0, H, 2 * I, 1, 1, stream))) return rc;
-    if ((rc = fe_gemm(c, D, y.down, nullptr, y.s2, Bx, A, R0, I, H, 1, 0, stream))) return rc;
-    c->launches += 4;
-  }
-  FQ3_LAUNCH((fe::rmsnorm_rows_kernel), R0, 256, 0, stream, A, f.norm, H, f.eps, Cn);
-  c->launches++;
-  __nv_bfloat16* cur = Cn;
-  int rows = R0, Tc = T;
-  for (size_t u = 0; u < f.ups.size(); ++u) {
-    const FeUp& y = f.ups[u];
-    __nv_bfloat16* out = (cur == Cn) ? E : Cn;
-    if ((rc = fe_gemm(c, cur, y.ct, y.ct_b, nullptr, nullptr, A, rows, H, y.r * H, H, 0, stream))) return rc;
-    rows *= y.r;
-    Tc *= y.r;
-    const int h = hist(site);
-    const __nv_bfloat16* xin = with_history(A, Tc);
-    FQ3_LAUNCH((fe::dwconv_ln_kernel), rows, 256, 0, stream, xin, Tc, H, y.dw_w, y.dw_b, y.ln_w, y.ln_b, 1e-6f, Bx, h, h + Tc);
-    c->launches++;
-    if ((rc = fe_gemm(c, Bx, y.pw1, y.pw1_b, nullptr, nullptr, D, rows, H, 4 * H, 4 * H, 2, stream))) return rc;
-    if ((rc = fe_gemm(c, D, y.pw2, y.pw2_b, y.gamma, A, out, rows, 4 * H, H, H, 0, stream))) return rc;
-    cur = out;
-  }
-  // ---- waveform stack (stack_run with the history detours)
-  int Ts = Tc;
-  size_t li = 0;
-  auto conv = [&](const Layer& L, const __nv_bfloat16* X, const __nv_bfloat16* R, __nv_bfloat16* Yraw, __nv_bfloat16* Yact) -> int {
-    const int h = hist(site);
-    const __nv_bfloat16* xin = with_history(X, Ts);
-    return launch_conv(c, L, xin, R, Yraw, Yact, Ts, batch, stream, h, h + Ts);
-  };
-  __nv_bfloat16* act = c->buf[1];
-  if ((rc = conv(c->layers[li++], cur, nullptr, nullptr, act))) return rc;
-  for (int bi = 0; bi < c->n_blocks; ++bi) {
-    __nv_bfloat16* fr[3];
-    int k = 0;
-    for (auto* b : c->buf)
-      if (b != act) fr[k++] = b;
-    __nv_bfloat16 *x = fr[0], *a1 = fr[1], *a2 = fr[2], *y = act;
-    const Layer& U = c->layers[li++];
-    if ((rc = conv(U, act, nullptr, x, a1))) return rc;
-    Ts *= U.upsample;
-    for (int j = 0; j < 3; ++j) {
-      const Layer& C1 = c->layers[li++];
-      const Layer& C2 = c->layers[li++];
-      if ((rc = conv(C1, a1, nullptr, nullptr, a2))) return rc;
-      if ((rc = conv(C2, a2, x, C2.write_raw ? y : nullptr, a1))) return rc;
-      std::swap(x, y);
-    }
-    act = a1;
-  }
-  {
-    const int h = hist(site);
-    const __nv_bfloat16* xin = with_history(act, Ts);
-    if (pcm_out_dev) {
-      FQ3_LAUNCH((conv_out_kernel), dim3((Ts + 255) / 256, batch), 256, 0, stream, xin, c->w_out, c->b_out, Ts, c->c_out, 7, pcm_out_dev, h, h + Ts);
-      c->launches++;
-    }
-  }
-  CCK(cudaGetLastError());
+  int rc;
+  if ((rc = codec_forward(c, codes_dev, batch, T, pcm_out_dev, true, stream))) return rc;
   for (int b = 0; b < batch; ++b) streams[b]->frames += T;
   return 0;
 }

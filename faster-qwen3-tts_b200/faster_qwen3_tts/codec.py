@@ -323,24 +323,31 @@ class SpeechTokenizer:
         except Exception:
             pass
 
+    def _engine_call(self, codes: torch.Tensor, want_pcm: bool, call):
+        """What every engine codec call shares: codes [B, n, Q] as int64 on the codec's device, the code-group check, the
+        PCM buffer, the device context and the error check.  ``call(codes_ptr, B, n, pcm_ptr, stream)`` makes the C ABI
+        call (pcm_ptr None without PCM).  Returns the B PCM rows, or None."""
+        import ctypes as C
+        codes = codes.to(device=self._dev, dtype=torch.long).contiguous()
+        B, n, Q = codes.shape
+        if Q != self.decoder.config.num_quantizers:
+            raise ValueError(f"audio_codes must have {self.decoder.config.num_quantizers} code groups, got {Q}")
+        pcm = torch.empty(B, n * self.decoder.config.total_upsample, dtype=torch.float32, device=self._dev) if want_pcm else None
+        with torch.cuda.device(self._dev):
+            rc = call(C.c_void_p(codes.data_ptr()), B, n, C.c_void_p(pcm.data_ptr()) if want_pcm else None,
+                      C.c_void_p(torch.cuda.current_stream(self._dev).cuda_stream))
+        if rc:
+            raise RuntimeError(self._lib.fq3_codec_last_error().decode())
+        self.launches = int(self._lib.fq3_codec_launch_count(self._h))
+        return [pcm[b] for b in range(B)] if want_pcm else None
+
     @torch.inference_mode()
     def decode(self, payload) -> Tuple[List[torch.Tensor], int]:
         codes = payload["audio_codes"]  # [B, T, Q]
-        dev = next(self.decoder.parameters()).device
         if self.backend == "engine":
-            import ctypes as C
-            codes = codes.to(device=dev, dtype=torch.long).contiguous()
-            B, T, Q = codes.shape
-            if Q != self.decoder.config.num_quantizers:
-                raise ValueError(f"audio_codes must have {self.decoder.config.num_quantizers} code groups, got {Q}")
-            pcm = torch.empty(B, T * self.decoder.config.total_upsample, dtype=torch.float32, device=dev)
-            with torch.cuda.device(dev):
-                rc = self._lib.fq3_codec_decode_codes(self._h, C.c_void_p(codes.data_ptr()), B, T, C.c_void_p(pcm.data_ptr()),
-                                                      C.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
-            if rc:
-                raise RuntimeError(self._lib.fq3_codec_last_error().decode())
-            self.launches = int(self._lib.fq3_codec_launch_count(self._h))
-            return [pcm[b] for b in range(B)], self.sample_rate
+            pcm = self._engine_call(codes, True, lambda *a: self._lib.fq3_codec_decode_codes(self._h, *a))
+            return pcm, self.sample_rate
+        dev = next(self.decoder.parameters()).device
         wav = self.decoder(codes.to(dev).transpose(1, 2).contiguous())
         self.launches += 1
         return [w.reshape(-1).float() for w in wav], self.sample_rate
@@ -394,20 +401,11 @@ class SpeechTokenizer:
         """The next n frames of several streams in ONE set of launches: codes [B, n, 16] -> list of B PCM tensors
         (or None with want_pcm=False: state warm-up, e.g. the ICL reference frames)."""
         import ctypes as C
-        codes = codes.to(device=self._dev, dtype=torch.long).contiguous()
-        B, n, Q = codes.shape
-        if B != len(streams):
+        if codes.shape[0] != len(streams):
             raise ValueError("one row of codes per stream")
-        pcm = torch.empty(B, n * self.decoder.config.total_upsample, dtype=torch.float32, device=self._dev) if want_pcm else None
-        arr = (C.c_void_p * B)(*[s._h for s in streams])
-        with torch.cuda.device(self._dev):
-            rc = self._lib.fq3_codec_stream_decode(self._h, arr, B, C.c_void_p(codes.data_ptr()), n,
-                                                   C.c_void_p(pcm.data_ptr()) if want_pcm else None,
-                                                   C.c_void_p(torch.cuda.current_stream(self._dev).cuda_stream))
-        if rc:
-            raise RuntimeError(self._lib.fq3_codec_last_error().decode())
-        self.launches = int(self._lib.fq3_codec_launch_count(self._h))
-        return [pcm[b] for b in range(B)] if want_pcm else None
+        arr = (C.c_void_p * len(streams))(*[s._h for s in streams])
+        return self._engine_call(codes, want_pcm, lambda codes_p, B, n, pcm_p, stream:
+                                 self._lib.fq3_codec_stream_decode(self._h, arr, B, codes_p, n, pcm_p, stream))
 
     def flops(self, T: int) -> float:
         """dense-layer FLOPs of the waveform stack for T code frames"""

@@ -110,11 +110,7 @@ class _StreamWindow:
         return audio[int(round(n_ctx * self.spf)):] if n_ctx > 0 else audio
 
     def push(self, codec_chunk):
-        codes, meta = self.window(codec_chunk)
-        if meta[0] == "phase1_stream":
-            return self.finish(self.p1.push(codes), meta), self.st.sample_rate
-        audio_list, sr = self.st.decode({"audio_codes": codes.unsqueeze(0)})
-        return self.finish(audio_list[0], meta), sr
+        return decode_windows_batched(self.st, [self], [codec_chunk])[0]
 
 
 class _StatefulWindow:
@@ -134,7 +130,7 @@ class _StatefulWindow:
             self.stream.warm(ref_codes)   # 174 reference frames: ~3 ms once, instead of re-decoding them for four chunks
 
     def push(self, codec_chunk):
-        return self.conv(self.stream.push(codec_chunk)), self.st.sample_rate
+        return decode_windows_batched(self.st, [self], [codec_chunk])[0]
 
 
 def decode_windows_batched(speech_tokenizer, wins, chunks):
@@ -516,19 +512,7 @@ class FasterQwen3TTS:
 
     def _decode_all(self, speech_tokenizer, codec_ids, ref_codes):
         """Non-streaming decode + proportional reference trim (model.py:918-938)."""
-        if ref_codes is not None:
-            codes = torch.cat([ref_codes.to(codec_ids.device), codec_ids], dim=0)
-        else:
-            codes = codec_ids
-        audio_list, sr = speech_tokenizer.decode({"audio_codes": codes.unsqueeze(0)})
-        ref_len = ref_codes.shape[0] if ref_codes is not None else 0
-        out = []
-        for a in audio_list:
-            a = self._to_numpy(a)
-            if ref_len > 0:
-                a = a[int(ref_len / max(codes.shape[0], 1) * len(a)):]
-            out.append(a)
-        return out, sr
+        return self._decode_takes(speech_tokenizer, [codec_ids], ref_codes)
 
     def _stream_audio(self, chunks, speech_tokenizer, ref_codes, chunk_size, to_host=True):
         """The reference's hybrid streaming decode (model.py:1052-1135): Phase 1 re-decodes everything so far
@@ -841,11 +825,14 @@ class FasterQwen3TTS:
             sc = score(rq.lp.frames(), rq.eos_logprob)
             sc["seed"] = seeds[i]
             scores.append(sc)
-        return self._decode_takes(m.speech_tokenizer, codes, ref_codes), self.sample_rate, scores
+        audio, _ = self._decode_takes(m.speech_tokenizer, codes, ref_codes)
+        return audio, self.sample_rate, scores
 
     def _decode_takes(self, st, codes, ref_codes):
-        """``_decode_all`` of every take, takes of equal length in ONE codec call (the decoder's rows are independent)"""
+        """Non-streaming decode + proportional reference trim of every take, takes of equal length in ONE codec call (the
+        decoder's rows are independent).  Returns (audio per take, the sample rate the codec returned)."""
         out = [np.zeros(1, dtype=np.float32)] * len(codes)
+        sr = self.sample_rate
         groups = {}
         for i, c in enumerate(codes):
             if c is not None:
@@ -854,13 +841,13 @@ class FasterQwen3TTS:
         for T, idxs in groups.items():
             batch = torch.stack([codes[i] if ref_codes is None else torch.cat([ref_codes.to(codes[i].device), codes[i]])
                                  for i in idxs])
-            audio_list, _ = st.decode({"audio_codes": batch})
+            audio_list, sr = st.decode({"audio_codes": batch})
             for i, a in zip(idxs, audio_list):
                 a = self._to_numpy(a)
                 if ref_len > 0:
                     a = a[int(ref_len / max(batch.shape[1], 1) * len(a)):]
                 out[i] = a
-        return out
+        return out, sr
 
     @torch.inference_mode()
     def generate_voice_clone_takes(self, text: str, language: str, ref_audio=None, ref_text: str = "",

@@ -119,6 +119,86 @@ def test_engine_decode_launches_no_library_kernel(full_codec):
     assert not foreign, foreign
 
 
+def _kernels_in_start_order(fn):
+    """names of the kernels fn() launches, in start-time order (torch profiler, CUPTI); skips when CUDA cannot be traced"""
+    torch.cuda.synchronize()
+    try:
+        from torch.profiler import ProfilerActivity, profile
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            fn()
+            torch.cuda.synchronize()
+        ev = [e for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA
+              and not e.name.startswith(("Memcpy", "Memset"))]
+    except Exception as ex:  # pragma: no cover
+        pytest.skip(f"CUDA profiling unavailable: {ex!r}")
+    if not ev:
+        pytest.skip("profiler returned no kernel records")
+    return [e.name for e in sorted(ev, key=lambda e: e.time_range.start)]
+
+
+def _launch_geometry(st):
+    """(launches of one decode, causal sites with history rows) of the codec geometry"""
+    c = st.decoder.config
+    L, U, nb = c.num_hidden_layers, len(c.upsampling_ratios), len(c.upsample_rates)
+    # embedding mean; per pre-transformer layer 2 norms, 4 GEMMs, RoPE, attention; final norm; per upsampler
+    # ConvTranspose GEMM, dwconv + LayerNorm, 2 GEMMs; conv_in; per decoder block ConvTranspose, 3 x (conv7, conv1); conv_out
+    n_decode = 1 + 8 * L + 1 + 4 * U + 1 + 7 * nb + 1
+    # sites with history: attention, dwconv, conv_in, per decoder block the ConvTranspose and the 3 conv7, conv_out
+    return n_decode, L + U + 1 + 4 * nb + 1
+
+
+def test_decode_launch_count_follows_the_codec_geometry(full_codec):
+    """a decode of [2, 33, 16] makes the launches the codec geometry gives; push_streams on two fresh streams with the same
+    codes makes those plus two history copies per causal site, and returns the same PCM"""
+    st = full_codec
+    n_decode, n_sites = _launch_geometry(st)
+    assert (n_decode, n_sites) == (104, 28)
+    codes = torch.randint(0, 2048, (2, 33, 16), generator=torch.Generator().manual_seed(41)).cuda()
+    n0 = int(st._lib.fq3_codec_launch_count(st._h))
+    one_shot, _ = st.decode({"audio_codes": codes})
+    assert st.launches - n0 == n_decode
+    streams = [st.open_stream() for _ in range(2)]
+    n0 = st.launches
+    streamed = st.push_streams(streams, codes)
+    assert st.launches - n0 == n_decode + 2 * n_sites
+    for a, b in zip(one_shot, streamed):
+        assert torch.equal(a, b)
+    for s in streams:
+        s.close()
+
+
+def test_one_shot_decode_is_the_stream_decode_without_history_copies(full_codec):
+    """The one-shot decode and the stream decode run one codec forward: a decode of [2, 33, 16] launches the kernels of
+    push_streams on two fresh streams with the same codes, in the same order, once the stream's history copies are
+    removed."""
+    st = full_codec
+    n_decode, n_sites = _launch_geometry(st)
+    codes = torch.randint(0, 2048, (2, 33, 16), generator=torch.Generator().manual_seed(42)).cuda()
+    streams = [st.open_stream() for _ in range(2)]
+    st.decode({"audio_codes": codes})
+    st.push_streams(streams, codes)
+    for s in streams:
+        s.reset()
+    one_shot = _kernels_in_start_order(lambda: st.decode({"audio_codes": codes}))
+    streamed = _kernels_in_start_order(lambda: st.push_streams(streams, codes))
+    copies = ("ext_build_kernel", "tail_save_kernel")
+    assert len(one_shot) == n_decode and len(streamed) == n_decode + 2 * n_sites
+    assert sum(any(k in n for k in copies) for n in streamed) == 2 * n_sites
+    assert [n for n in streamed if not any(k in n for k in copies)] == one_shot
+    for s in streams:
+        s.close()
+
+
+def test_push_streams_refuses_a_wrong_code_group_count_before_launching(full_codec):
+    st = full_codec
+    s = st.open_stream()
+    n0 = int(st._lib.fq3_codec_launch_count(st._h))
+    with pytest.raises(ValueError, match="16 code groups"):
+        st.push_streams([s], torch.zeros(1, 4, 15, dtype=torch.long, device="cuda"))
+    assert int(st._lib.fq3_codec_launch_count(st._h)) == n0 and s.frames == 0
+    s.close()
+
+
 # ---------------------------------------------------------------------------------------------------------------------
 # stateful streaming codec (SURVEY 8(f) item 2): a stream's PCM equals the one-shot decode of the same codes
 # ---------------------------------------------------------------------------------------------------------------------
