@@ -67,15 +67,34 @@ struct StackDev {
   int seg_base;        // segment id of layer 0 / QKV; layer l uses seg_base + 4*l + {0:QKV,1:O,2:GU,3:DN}
   int seg_head;        // first head segment
   const void *ln_in, *ln_post, *qnorm, *knorm, *ln_f;
-  int S;               // cache slots per kv head: the request's caches are [L][nKV][S][128] model dtype
+  int S;               // predictor: cache rows per kv head, [L][nKV][S][128] model dtype (the talker's cache is paged)
   const float *cos, *sin;  // [npos][128] fp32
   int npos;
 };
 
+// ---- talker KV cache: pages of KV_PAGE rows from one engine-wide pool.  Page p is ONE contiguous block
+// {K [L][nKV][KV_PAGE][128], V [L][nKV][KV_PAGE][128]} in model dtype, so the KV_PAGE rows of one (layer, kv head) are
+// contiguous.  A slot's page table maps its row block t / KV_PAGE to a page (-1 = unmapped; the engine refuses work
+// that would touch such a row before launching it).  kv_row() is the only code that turns a cache row into an address:
+// every reader and writer, device (decode, prefill) and host (import / export), goes through it.
+constexpr int KV_PAGE = 64;
+__host__ __device__ __forceinline__ size_t kv_half_bytes(int L, int nKV, size_t esz) {   // K (or V) part of a page
+  return (size_t)L * nKV * KV_PAGE * 128 * esz;
+}
+// which: 0 = K, 1 = V; row t of (layer, kv head g) of the slot whose table is `pages`
+__host__ __device__ __forceinline__ uint8_t* kv_row(void* pool, int L, int nKV, size_t esz, const int* pages, int which,
+                                                    int layer, int g, int t) {
+  const int page = pages[t / KV_PAGE];   // the kernels pass their copy in shared memory (Smem::kvtab)
+  const size_t half = kv_half_bytes(L, nKV, esz);
+  return reinterpret_cast<uint8_t*>(pool) + (size_t)page * 2 * half + (size_t)which * half +
+         ((size_t)(layer * nKV + g) * KV_PAGE + t % KV_PAGE) * 128 * esz;
+}
+
 // one request: its caches, decode state and parameters.  The single-sequence kernel reads it from KParams::req, the
 // batched kernel one per column from KParams::sl.
 struct SlotParams {
-  void *kc, *vc;        // talker KV cache of this slot   [L][nKV][S][128]
+  void* kv;             // the engine's talker KV page pool (kv_row)
+  const int* kv_pages;  // this slot's page table [ceil(max_seq_len / KV_PAGE)]
   void *pkc, *pvc;      // predictor KV cache of this slot [Lp][nKVp][32][128]
   int* state;           // [0] token [1] step [2] gen_step [3] finished [4] emitted(last launch)
   float* past_hidden;   // [HMAX] fp32 holding dtype-rounded values
@@ -231,6 +250,8 @@ struct __align__(128) Smem {
   int bst[5][32];           // batched kernel: replicated per-column loop state (token, step, gen_step, finished, emitted)
   long long prof[12];       // batched kernel, CTA 0 / thread 0: [0] last clock [1] current category [2..] cycles per category
   int runl[36];             // batched kernel: columns running in the current (sub)frame, ascending; [32] = their number
+  int kvtab[SEQMAX / KV_PAGE];   // page table of the request being attended to: the single-sequence kernel's, read
+                                 // once per launch; the batched kernel's current column, read once per attention item
 };
 
 // All dynamic shared memory of the kernel is one Smem; going through this accessor (instead of a reference carried
@@ -459,11 +480,11 @@ struct Producer {
     if (b >= S.nH * Sx) return;
     const int h = b / Sx, sp = b - h * Sx, g = h / S.rep;
     const KvSlice sl = kv_slice(slot0 - kv_start, Sx, sp);
-    const size_t row0 = (size_t)(layer * S.nKV + g) * S.S + kv_start + sl.j0;
-    const uint8_t* kb = reinterpret_cast<const uint8_t*>(P.req.kc) + row0 * 256;
-    const uint8_t* vb = reinterpret_cast<const uint8_t*>(P.req.vc) + row0 * 256;
     for (int tl = 0; tl < sl.ntile; ++tl) {
-      const uint32_t bytes = (uint32_t)min(KVT_KEYS, sl.n - KVT_KEYS * tl) * 256u;
+      // a slice starts at a multiple of 8 keys, so a tile may straddle two pages: then it is two copies per matrix
+      const int r0 = kv_start + sl.j0 + KVT_KEYS * tl;
+      const int n = min(KVT_KEYS, sl.n - KVT_KEYS * tl), n1 = min(n, KV_PAGE - r0 % KV_PAGE);
+      const uint32_t bytes = (uint32_t)n * 256u, b1 = (uint32_t)n1 * 256u;
       const int stage = (int)(ctr % NS);
       const uint32_t par = ((ctr / NS) & 1u) ^ 1u;
       while (!mbar_try_wait(&s.empty[stage], par)) {
@@ -473,8 +494,15 @@ struct Producer {
         }
       }
       mbar_expect_tx(&s.full[stage], 2 * bytes);
-      bulk_g2s(s.ring[stage], kb + (size_t)tl * KVT_KEYS * 256, bytes, &s.full[stage]);
-      bulk_g2s(s.ring[stage] + KVT_VOFF, vb + (size_t)tl * KVT_KEYS * 256, bytes, &s.full[stage]);
+      bulk_g2s(s.ring[stage], kv_row(P.req.kv, S.L, S.nKV, 2, s.kvtab, 0, layer, g, r0), b1, &s.full[stage]);
+      bulk_g2s(s.ring[stage] + KVT_VOFF, kv_row(P.req.kv, S.L, S.nKV, 2, s.kvtab, 1, layer, g, r0), b1,
+               &s.full[stage]);
+      if (n1 < n) {
+        bulk_g2s(s.ring[stage] + b1, kv_row(P.req.kv, S.L, S.nKV, 2, s.kvtab, 0, layer, g, r0 + n1), bytes - b1,
+                 &s.full[stage]);
+        bulk_g2s(s.ring[stage] + KVT_VOFF + b1, kv_row(P.req.kv, S.L, S.nKV, 2, s.kvtab, 1, layer, g, r0 + n1),
+                 bytes - b1, &s.full[stage]);
+      }
       ++ctr;
     }
   }
@@ -498,7 +526,8 @@ struct Producer {
 // ------------------------------------------------------------------------------------------------------------
 template <bool BF>
 __device__ __forceinline__ void head_qkv(Ctx& c, const StackDev& S, int layer, int h, const float* qkv, int rpos,
-                                         float* qs, float* ks, float* vs, void* kc, void* vc, int slot, bool append) {
+                                         float* qs, float* ks, float* vs, void* kv, const int* pages, int slot,
+                                         bool append) {
   if (c.warp < 3) {
     const int what = c.warp, g = h / S.rep;
     const float* src = qkv + (what == 0 ? h * 128 : (what == 1 ? S.qd + g * 128 : S.qd + S.kd + g * 128));
@@ -537,8 +566,7 @@ __device__ __forceinline__ void head_qkv(Ctx& c, const StackDev& S, int layer, i
 #pragma unroll
     for (int i = 0; i < 4; ++i) dst[c.lane + 32 * i] = v[i];
     if (what > 0 && append) {
-      uint8_t* cb = reinterpret_cast<uint8_t*>(what == 1 ? kc : vc) +
-                    ((size_t)(layer * S.nKV + g) * S.S + slot) * 128 * (BF ? 2 : 4);
+      uint8_t* cb = kv_row(kv, S.L, S.nKV, BF ? 2 : 4, pages, what - 1, layer, g, slot);
 #pragma unroll
       for (int i = 0; i < 4; ++i) stw<BF>(cb, c.lane + 32 * i, v[i]);
       asm volatile("fence.proxy.async.global;" ::: "memory");
@@ -549,12 +577,13 @@ __device__ __forceinline__ void head_qkv(Ctx& c, const StackDev& S, int layer, i
 
 // ------------------------------------------------------------------------------------------------------------
 // Talker attention of one new token for one q-head over the KV cache (transformers eager_attention_forward semantics,
-// GQA by repeat_kv): cache slot slot0, rotary position rpos0, keys from kv_start on.  qkv: the token's QKV row; kc / vc:
-// the request's caches; the head's output goes to att[h*128 .. h*128+128) in model dtype.  Both kernels run it.
+// GQA by repeat_kv): cache slot slot0, rotary position rpos0, keys from kv_start on.  qkv: the token's QKV row; pool /
+// pages: the page pool and the request's page table; the head's output goes to att[h*128 .. h*128+128) in model dtype.
+// Both kernels run it.
 // ------------------------------------------------------------------------------------------------------------
 template <bool BF>
-__device__ void attention_head(Ctx& c, const StackDev& S, int layer, int h, const float* __restrict__ qkv, void* kc, void* vc,
-                               void* att, int slot0, int rpos0, int kv_start) {
+__device__ void attention_head(Ctx& c, const StackDev& S, int layer, int h, const float* __restrict__ qkv, void* pool,
+                               const int* pages, void* att, int slot0, int rpos0, int kv_start) {
   float* sc = SMEM().xs;            // scores [SEQMAX]
   float* qs = SMEM().xs + SEQMAX;   // [128]
   float* ks = qs + 128;             // [128]
@@ -562,10 +591,8 @@ __device__ void attention_head(Ctx& c, const StackDev& S, int layer, int h, cons
   float* opart = vs + 128;          // [8][128]
   const int g = h / S.rep;
   const size_t esz = BF ? 2 : 4;
-  const uint8_t* kbase = reinterpret_cast<const uint8_t*>(kc) + ((size_t)(layer * S.nKV + g) * S.S * 128) * esz;
-  const uint8_t* vbase = reinterpret_cast<const uint8_t*>(vc) + ((size_t)(layer * S.nKV + g) * S.S * 128) * esz;
   // --- a. q/k norm + rope, v copy; the first q-head of each kv group appends the new row
-  head_qkv<BF>(c, S, layer, h, qkv, rpos0, qs, ks, vs, kc, vc, slot0, (h % S.rep) == 0);
+  head_qkv<BF>(c, S, layer, h, qkv, rpos0, qs, ks, vs, pool, pages, slot0, (h % S.rep) == 0);
   const float scale = 0.08838834764831845f;  // 128^-0.5
   const int nk = slot0 + 1 - kv_start;       // visible keys
   const int nold = slot0 - kv_start;         // keys that live in the global cache
@@ -585,7 +612,7 @@ __device__ void attention_head(Ctx& c, const StackDev& S, int layer, int h, cons
       for (int u = 0; u < U; ++u) {
         const int jj = base + (u * NCW + c.warp) * KPW + kin;
         if (jj < nold)
-          kv[u] = __ldcg(reinterpret_cast<const uint4*>(kbase + ((size_t)(kv_start + jj) * 128) * esz) + sub);
+          kv[u] = __ldcg(reinterpret_cast<const uint4*>(kv_row(pool, S.L, S.nKV, esz, pages, 0, layer, g, kv_start + jj)) + sub);
         else
           kv[u] = make_uint4(0, 0, 0, 0);
       }
@@ -647,7 +674,7 @@ __device__ void attention_head(Ctx& c, const StackDev& S, int layer, int h, cons
       for (int u = 0; u < U; ++u) {
         const int jj = base + (u * NCW + c.warp) * KPW + kin;
         if (jj < nold) {
-          vv[u] = __ldcg(reinterpret_cast<const uint4*>(vbase + ((size_t)(kv_start + jj) * 128) * esz) + sub);
+          vv[u] = __ldcg(reinterpret_cast<const uint4*>(kv_row(pool, S.L, S.nKV, esz, pages, 1, layer, g, kv_start + jj)) + sub);
           pv[u] = sc[jj];
         } else {
           vv[u] = make_uint4(0, 0, 0, 0);
@@ -713,7 +740,7 @@ __device__ void attention_split(Ctx& c, const StackDev& S, int layer, int slot0,
   float* vs = ks + 128;            // [128]
   float* opart = vs + 128;         // [8][128]
   // --- a. q/k norm + rope, v copy; one CTA per kv group appends the new row
-  head_qkv<BF>(c, S, layer, h, P.QKV, rpos0, qs, ks, vs, P.req.kc, P.req.vc, slot0, sp == 0 && (h % S.rep) == 0);
+  head_qkv<BF>(c, S, layer, h, P.QKV, rpos0, qs, ks, vs, P.req.kv, SMEM().kvtab, slot0, sp == 0 && (h % S.rep) == 0);
   const KvSlice sl = kv_slice(slot0 - kv_start, Sx, sp);
   const bool has_new = sp == Sx - 1;
   const int nloc = sl.n + (has_new ? 1 : 0);
@@ -1568,8 +1595,8 @@ __device__ void run_layers(Ctx& c, const StackDev& S, int nt, int slot0, int rpo
   constexpr bool is_talker = TALKER;
   const KParams& P = c.P;
   const bool cta0 = blockIdx.x == 0;
-  void* kc = TALKER ? P.req.kc : P.req.pkc;  // the request's caches of this stack
-  void* vc = TALKER ? P.req.vc : P.req.pvc;
+  void* kc = P.req.pkc;  // the request's predictor caches (the talker's are paged: P.req.kv / kv_pages)
+  void* vc = P.req.pvc;
   int pi = 0;
   dbg = dbg && (P.dbg_on & 1);
   auto nopre = [](int, int) { return 0.f; };
@@ -1615,7 +1642,7 @@ __device__ void run_layers(Ctx& c, const StackDev& S, int nt, int slot0, int rpo
       if (split) attention_split<BF>(c, S, l, slot0, rpos0, kv_start);
       else
         for (int h = blockIdx.x; h < S.nH; h += gridDim.x)
-          attention_head<BF>(c, S, l, h, P.QKV, kc, vc, P.ATT, slot0, rpos0, kv_start);
+          attention_head<BF>(c, S, l, h, P.QKV, P.req.kv, SMEM().kvtab, P.ATT, slot0, rpos0, kv_start);
       if (!split && is_talker && (int)blockIdx.x >= S.nH && slot0 - kv_start > 64) {
         // idle CTAs pull the NEXT layer's keys/values into L2 (evict_last) so the attention CTAs see L2 latency
         const int ln = (l + 1) % S.L;
@@ -1631,8 +1658,8 @@ __device__ void run_layers(Ctx& c, const StackDev& S, int nt, int slot0, int rpo
           r /= lines_per_row;
           const int j = (int)(r % nk);
           const int g = (int)(r / nk);
-          const uint8_t* base = reinterpret_cast<const uint8_t*>(which ? vc : kc) +
-                                (((size_t)(ln * S.nKV + g) * S.S + kv_start + j) * 128) * esz + (size_t)ln_i * 128;
+          const uint8_t* base = kv_row(P.req.kv, S.L, S.nKV, esz, SMEM().kvtab, which, ln, g, kv_start + j) +
+                                (size_t)ln_i * 128;
           asm volatile("prefetch.global.L2::evict_last [%0];" ::"l"(base));
         }
       }
@@ -1875,6 +1902,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) fq3_decode_kernel(const __grid_co
   const int cta = blockIdx.x;
 
   cta_prologue(P, P.mode == MODE_FUSED ? P.req.seen : nullptr);
+  for (int i = tid; i < (P.max_seq_len + KV_PAGE - 1) / KV_PAGE; i += NTHREADS) s.kvtab[i] = P.req.kv_pages[i];
   __syncthreads();
 
   if (warp == NCW) {

@@ -342,7 +342,11 @@ __device__ void stack_b(Ctx& c, const StackDev& S, const BView& v, int nt, uint3
         const int b = SMEM().runl[idx / S.nH], h = idx % S.nH;
         const SlotParams& sp = P.sl[b];
         const int pos = sp.prefill_len + SMEM().bst[BS_STEP][b];
-        attention_head<BF>(c, S, l, h, P.QKVB + (size_t)b * P.ldQKV, sp.kc, sp.vc,
+        // the column's page table into shared memory for the item's key loops (the previous item's last barrier
+        // freed it; this one publishes it)
+        for (int i = c.tid; i < (P.max_seq_len + KV_PAGE - 1) / KV_PAGE; i += NCT) SMEM().kvtab[i] = sp.kv_pages[i];
+        csync();
+        attention_head<BF>(c, S, l, h, P.QKVB + (size_t)b * P.ldQKV, sp.kv, SMEM().kvtab,
                            reinterpret_cast<uint8_t*>(P.ATTB) + (size_t)b * P.ldATT * (BF ? 2 : 4), pos,
                            pos + sp.rope_delta, sp.n_left_pad);
       }

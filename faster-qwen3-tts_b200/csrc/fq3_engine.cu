@@ -63,6 +63,7 @@ struct SlotHost {
   bool active = false;
   int prefill_len = 0, rope_delta = 0, n_left_pad = 0, max_new = 0, min_new = 0, trailing_len = 0;
   bool text_open = false, text_closed = false;   // fq3_set_text_rows: rows may still follow / the caller closed the text
+  int step = 0;   // frames since fq3_begin_request (state[1] after the slot's last launch): where its next row goes
   const void* trailing = nullptr;
   const void* tts_pad = nullptr;
   const float* uniforms = nullptr;
@@ -79,7 +80,16 @@ struct fq3_engine {
   int max_slots = 1;   // resident request slots (>= max_batch)
   bool loaded = false;
   std::vector<SlotHost> slots;
-  size_t tkv_slot = 0, pkv_slot = 0;   // bytes of one slot's K (or V) cache: talker / predictor
+  size_t pkv_slot = 0;   // bytes of one slot's predictor K (or V) cache
+  // paged talker KV cache (kv_row): kv_npages pages of kv_page_bytes; slot s's device page table is kv_tab + s * kv_npt.
+  // The host copy of the tables, the owner of every page and the pages a slot maps are what the refusals check.
+  void* kv = nullptr;
+  int* kv_tab = nullptr;
+  int kv_npt = 0, kv_npages = 0;
+  size_t kv_page_bytes = 0;
+  std::vector<int> kv_tab_host, kv_owner, kv_nmapped;
+  int* kv_stage = nullptr;               // pinned: one slot's table on its way to the device
+  cudaStream_t kv_stream = nullptr;      // private stream of the table uploads
   // batched decode: activation matrices + per-launch slot table
   float *XB = nullptr, *X1B = nullptr, *QKVB = nullptr, *LOGB = nullptr;
   void *XNB = nullptr, *ATTB = nullptr, *ACTB = nullptr, *PINB = nullptr;
@@ -87,7 +97,7 @@ struct fq3_engine {
   SlotParams* sl_dev = nullptr;
   SlotParams* sl_host = nullptr;  // pinned
   // device buffers (slot-major: slot s starts at s * <per-slot size>)
-  void *t_kc = nullptr, *t_vc = nullptr, *p_kc = nullptr, *p_vc = nullptr;
+  void *p_kc = nullptr, *p_vc = nullptr;
   float *X = nullptr, *X1 = nullptr, *QKV = nullptr, *ACT = nullptr, *LOGITS = nullptr, *PART = nullptr;
   void* ATT = nullptr;  // model dtype
   unsigned* bar = nullptr;
@@ -243,10 +253,12 @@ static int check_stack(const fq3_stack_config& s, const char* nm, int nt) {
   return 0;
 }
 
-// bytes of one slot's talker / predictor K (or V) cache
-static size_t tkv_bytes(const fq3_config& c, size_t esz) {
-  return (size_t)c.talker.num_hidden_layers * c.talker.num_key_value_heads * c.max_seq_len * 128 * esz;
+// bytes of one talker KV page (K and V of KV_PAGE rows of every layer and kv head), pages of max_seq_len rows, and one
+// slot's predictor K (or V) cache
+static size_t page_bytes(const fq3_config& c, size_t esz) {
+  return 2 * kv_half_bytes(c.talker.num_hidden_layers, c.talker.num_key_value_heads, esz);
 }
+static int pages_per_seq(const fq3_config& c) { return (c.max_seq_len + KV_PAGE - 1) / KV_PAGE; }
 static size_t pkv_bytes(const fq3_config& c, size_t esz) {
   return (size_t)c.predictor.num_hidden_layers * c.predictor.num_key_value_heads * 32 * 128 * esz;
 }
@@ -256,7 +268,14 @@ extern "C" int64_t fq3_slot_bytes(const fq3_config* cfg) {
   if (!cfg) return fail(FQ3_ERR_INVALID, "null argument");
   if (cfg->dtype != FQ3_F32 && cfg->dtype != FQ3_BF16) return fail(FQ3_ERR_INVALID, "dtype must be FQ3_F32 or FQ3_BF16");
   const size_t esz = cfg->dtype == FQ3_BF16 ? 2 : 4;
-  return (int64_t)(2 * tkv_bytes(*cfg, esz) + 2 * pkv_bytes(*cfg, esz) + STATE_BYTES + HMAX * sizeof(float) + VMAX / 8);
+  return (int64_t)(pages_per_seq(*cfg) * page_bytes(*cfg, esz) + 2 * pkv_bytes(*cfg, esz) + STATE_BYTES +
+                   HMAX * sizeof(float) + VMAX / 8);
+}
+
+extern "C" int64_t fq3_kv_page_bytes(const fq3_config* cfg) {
+  if (!cfg) return fail(FQ3_ERR_INVALID, "null argument");
+  if (cfg->dtype != FQ3_F32 && cfg->dtype != FQ3_BF16) return fail(FQ3_ERR_INVALID, "dtype must be FQ3_F32 or FQ3_BF16");
+  return (int64_t)page_bytes(*cfg, cfg->dtype == FQ3_BF16 ? 2 : 4);
 }
 
 static int engine_alloc(fq3_engine* e, const cudaDeviceProp& prop);
@@ -277,6 +296,9 @@ extern "C" int fq3_engine_create(const fq3_config* cfg, fq3_engine** out) {
   if (cfg->max_seq_len < 8 || cfg->max_seq_len > SEQMAX) return fail(FQ3_ERR_INVALID, "max_seq_len must be in [8,%d]", SEQMAX);
   if (cfg->num_code_groups < 2 || cfg->num_code_groups > 16) return fail(FQ3_ERR_INVALID, "num_code_groups must be in [2,16]");
   if (cfg->rope_positions < cfg->max_seq_len) return fail(FQ3_ERR_INVALID, "rope_positions < max_seq_len");
+  if (cfg->kv_pages < 0 || (cfg->kv_pages > 0 && cfg->kv_pages < pages_per_seq(*cfg)))
+    return fail(FQ3_ERR_INVALID, "kv_pages %d: a pool must hold one request of max_seq_len=%d rows (%d pages of %d rows)",
+                cfg->kv_pages, cfg->max_seq_len, pages_per_seq(*cfg), KV_PAGE);
   int ndev = 0;
   CK(cudaGetDeviceCount(&ndev));
   if (cfg->device < 0 || cfg->device >= ndev) return fail(FQ3_ERR_INVALID, "device %d out of range", cfg->device);
@@ -326,8 +348,24 @@ static int engine_alloc(fq3_engine* e, const cudaDeviceProp& prop) {
   const fq3_stack_config &T = cfg->talker, &Pc = cfg->predictor;
   const int MS = e->max_slots;   // per-slot storage; everything a launch needs per column is sized MAXB / MAXCOL below
   e->slots.assign(MS, SlotHost());
-  const size_t tkv = tkv_bytes(*cfg, e->esz), pkv = pkv_bytes(*cfg, e->esz);
-  e->tkv_slot = tkv; e->pkv_slot = pkv;
+  const size_t pkv = pkv_bytes(*cfg, e->esz);
+  e->pkv_slot = pkv;
+  // talker KV pool: kv_pages = 0 is one max_seq_len run of pages per slot, slot s mapped to its own run for good;
+  // a pool of kv_pages > 0 starts with every slot unmapped
+  e->kv_npt = pages_per_seq(*cfg);
+  e->kv_npages = cfg->kv_pages > 0 ? cfg->kv_pages : MS * e->kv_npt;
+  e->kv_page_bytes = page_bytes(*cfg, e->esz);
+  e->kv_tab_host.assign((size_t)MS * e->kv_npt, -1);
+  e->kv_owner.assign(e->kv_npages, -1);
+  e->kv_nmapped.assign(MS, 0);
+  if (cfg->kv_pages == 0)
+    for (int sl = 0; sl < MS; ++sl) {
+      for (int i = 0; i < e->kv_npt; ++i) {
+        e->kv_tab_host[(size_t)sl * e->kv_npt + i] = sl * e->kv_npt + i;
+        e->kv_owner[sl * e->kv_npt + i] = sl;
+      }
+      e->kv_nmapped[sl] = e->kv_npt;
+    }
   // buffers to clear, once every allocation has succeeded
   std::vector<std::pair<void*, size_t>> zero;
   auto zalloc = [&](void** p, size_t bytes) -> cudaError_t {
@@ -335,7 +373,10 @@ static int engine_alloc(fq3_engine* e, const cudaDeviceProp& prop) {
     if (r == cudaSuccess) zero.push_back({*p, bytes});
     return r;
   };
-  CK(zalloc(&e->t_kc, tkv * MS)); CK(zalloc(&e->t_vc, tkv * MS));
+  CK(zalloc(&e->kv, e->kv_page_bytes * e->kv_npages));
+  CK(cudaMalloc(&e->kv_tab, e->kv_tab_host.size() * sizeof(int)));
+  CK(cudaMallocHost(&e->kv_stage, e->kv_npt * sizeof(int)));
+  CK(cudaStreamCreateWithFlags(&e->kv_stream, cudaStreamNonBlocking));
   CK(zalloc(&e->p_kc, pkv * MS)); CK(zalloc(&e->p_vc, pkv * MS));
   const int ldX = std::max(T.hidden_size, Pc.hidden_size);
   const int ldQKV = std::max((T.num_attention_heads + 2 * T.num_key_value_heads) * 128,
@@ -374,6 +415,7 @@ static int engine_alloc(fq3_engine* e, const cudaDeviceProp& prop) {
     CK(zalloc((void**)&e->dbg, e->dbg_floats * sizeof(float)));
   }
   for (auto& z : zero) CK(cudaMemset(z.first, 0, z.second));
+  CK(cudaMemcpy(e->kv_tab, e->kv_tab_host.data(), e->kv_tab_host.size() * sizeof(int), cudaMemcpyHostToDevice));
   KParams& k = e->kp;
   memset(&k, 0, sizeof(k));
   auto fill = [&](StackDev& s, const fq3_stack_config& c, int S) {
@@ -409,7 +451,7 @@ static int engine_alloc(fq3_engine* e, const cudaDeviceProp& prop) {
 extern "C" void fq3_engine_destroy(fq3_engine* e) {
   if (!e) return;
   cudaSetDevice(e->dev);
-  void* ptrs[] = {e->t_kc, e->t_vc, e->p_kc, e->p_vc, e->X, e->X1, e->QKV, e->ATT, e->ACT, e->LOGITS, e->PART, e->bar,
+  void* ptrs[] = {e->kv, e->kv_tab, e->p_kc, e->p_vc, e->X, e->X1, e->QKV, e->ATT, e->ACT, e->LOGITS, e->PART, e->bar,
                   e->state, e->past_hidden, e->seen, e->dbg, e->tape, e->grps, e->segtab, e->cta_grp_off,
                   e->XB, e->X1B, e->QKVB, e->LOGB, e->XNB, e->ATTB, e->ACTB, e->PINB, e->TOKB, e->sl_dev};
   for (void* p : ptrs)
@@ -420,6 +462,8 @@ extern "C" void fq3_engine_destroy(fq3_engine* e) {
     if (p) cudaFree(p);
   if (e->state_host) cudaFreeHost(e->state_host);
   if (e->sl_host) cudaFreeHost(e->sl_host);
+  if (e->kv_stage) cudaFreeHost(e->kv_stage);
+  if (e->kv_stream) cudaStreamDestroy(e->kv_stream);
   delete e;
 }
 
@@ -810,8 +854,14 @@ static int check_slot(fq3_engine* e, int slot) {
     return fail(FQ3_ERR_INVALID, "slot %d outside [0, %s=%d)", slot, slot_bound(e), e->max_slots);
   return 0;
 }
-static void* slot_tk(fq3_engine* e, int s) { return (uint8_t*)e->t_kc + (size_t)s * e->tkv_slot; }
-static void* slot_tv(fq3_engine* e, int s) { return (uint8_t*)e->t_vc + (size_t)s * e->tkv_slot; }
+// cache rows slot s has pages for; the refusals below keep every kernel inside them
+static int kv_rows(const fq3_engine* e, int s) { return e->kv_nmapped[s] * KV_PAGE; }
+static int check_rows(fq3_engine* e, int slot, long long rows, const char* what) {
+  if (rows > kv_rows(e, slot))
+    return fail(FQ3_ERR_INVALID, "slot %d: %s needs cache rows [0, %lld) but its pages map %d rows", slot, what, rows,
+                kv_rows(e, slot));
+  return 0;
+}
 static void* slot_pk(fq3_engine* e, int s) { return (uint8_t*)e->p_kc + (size_t)s * e->pkv_slot; }
 static void* slot_pv(fq3_engine* e, int s) { return (uint8_t*)e->p_vc + (size_t)s * e->pkv_slot; }
 
@@ -819,7 +869,7 @@ static void* slot_pv(fq3_engine* e, int s) { return (uint8_t*)e->p_vc + (size_t)
 static SlotParams slot_params(fq3_engine* e, int s, int n_frames, long long* codes_out, float* logprob_out) {
   const SlotHost& h = e->slots[s];
   SlotParams p;
-  p.kc = slot_tk(e, s); p.vc = slot_tv(e, s); p.pkc = slot_pk(e, s); p.pvc = slot_pv(e, s);
+  p.kv = e->kv; p.kv_pages = e->kv_tab + (size_t)s * e->kv_npt; p.pkc = slot_pk(e, s); p.pvc = slot_pv(e, s);
   p.state = e->state + 8 * s;
   p.past_hidden = e->past_hidden + (size_t)s * HMAX;
   p.seen = e->seen + (size_t)s * (VMAX / 32);
@@ -842,6 +892,25 @@ static KParams kp_for_slot(fq3_engine* e, int s, long long* codes_out, float* lo
   return kp;
 }
 
+// rows [0,P) of one layer between the caller's k,v [n_kv, P, 128] and the slot's pages: per page, one 2-D copy of the
+// page's rows of every kv head (they are KV_PAGE rows apart in the page, P rows apart in the caller's tensor)
+static int copy_kv(fq3_engine* e, int slot, int layer, void* k, void* v, int P, bool to_cache, cudaStream_t stream) {
+  const int L = e->cfg.talker.num_hidden_layers, nKV = e->cfg.talker.num_key_value_heads;
+  const int* pages = e->kv_tab_host.data() + (size_t)slot * e->kv_npt;
+  const size_t rowb = 128 * e->esz, pitch = (size_t)P * rowb;
+  for (int t0 = 0; t0 < P; t0 += KV_PAGE) {
+    const size_t w = (size_t)std::min(KV_PAGE, P - t0) * rowb;
+    for (int which = 0; which < 2; ++which) {
+      uint8_t* c = kv_row(e->kv, L, nKV, e->esz, pages, which, layer, 0, t0);
+      const size_t cp = kv_row(e->kv, L, nKV, e->esz, pages, which, layer, 1, t0) - c;   // kv head to kv head
+      uint8_t* u = (uint8_t*)(which ? v : k) + (size_t)t0 * rowb;
+      if (to_cache) CK(cudaMemcpy2DAsync(c, cp, u, pitch, w, nKV, cudaMemcpyDeviceToDevice, stream));
+      else CK(cudaMemcpy2DAsync(u, pitch, c, cp, w, nKV, cudaMemcpyDeviceToDevice, stream));
+    }
+  }
+  return 0;
+}
+
 extern "C" int fq3_import_kv(fq3_engine* e, int32_t slot, int32_t layer, const void* k_dev, const void* v_dev, int32_t P,
                              void* stream_) {
   if (!e || !k_dev || !v_dev) return fail(FQ3_ERR_INVALID, "null argument");
@@ -850,17 +919,9 @@ extern "C" int fq3_import_kv(fq3_engine* e, int32_t slot, int32_t layer, const v
   if (P > e->cfg.max_seq_len)
     return fail(FQ3_ERR_TOO_LONG, "Input is too long: prefill has %d tokens but max_seq_len=%d. Use shorter text or shorter reference audio.", P, e->cfg.max_seq_len);
   if (layer < 0 || layer >= e->cfg.talker.num_hidden_layers) return fail(FQ3_ERR_INVALID, "layer out of range");
+  if ((rc = check_rows(e, slot, P, "fq3_import_kv"))) return rc;
   DevGuard dev_guard(e->dev);
-  cudaStream_t stream = (cudaStream_t)stream_;
-  const int nKV = e->cfg.talker.num_key_value_heads, S = e->cfg.max_seq_len;
-  const size_t row = (size_t)P * 128 * e->esz, pitch = (size_t)S * 128 * e->esz;
-  uint8_t* kd = (uint8_t*)slot_tk(e, slot) + (size_t)layer * nKV * pitch;
-  uint8_t* vd = (uint8_t*)slot_tv(e, slot) + (size_t)layer * nKV * pitch;
-  if (P > 0) {
-    CK(cudaMemcpy2DAsync(kd, pitch, k_dev, row, row, nKV, cudaMemcpyDeviceToDevice, stream));
-    CK(cudaMemcpy2DAsync(vd, pitch, v_dev, row, row, nKV, cudaMemcpyDeviceToDevice, stream));
-  }
-  return 0;
+  return copy_kv(e, slot, layer, (void*)k_dev, (void*)v_dev, P, true, (cudaStream_t)stream_);
 }
 
 extern "C" int fq3_export_kv(fq3_engine* e, int32_t slot, int32_t layer, void* k_dev, void* v_dev, int32_t P, void* stream_) {
@@ -869,17 +930,9 @@ extern "C" int fq3_export_kv(fq3_engine* e, int32_t slot, int32_t layer, void* k
   if ((rc = check_slot(e, slot))) return rc;
   if (P < 0 || P > e->cfg.max_seq_len) return fail(FQ3_ERR_INVALID, "P outside the cache");
   if (layer < 0 || layer >= e->cfg.talker.num_hidden_layers) return fail(FQ3_ERR_INVALID, "layer out of range");
+  if ((rc = check_rows(e, slot, P, "fq3_export_kv"))) return rc;
   DevGuard dev_guard(e->dev);
-  cudaStream_t stream = (cudaStream_t)stream_;
-  const int nKV = e->cfg.talker.num_key_value_heads, S = e->cfg.max_seq_len;
-  const size_t row = (size_t)P * 128 * e->esz, pitch = (size_t)S * 128 * e->esz;
-  const uint8_t* ks = (const uint8_t*)slot_tk(e, slot) + (size_t)layer * nKV * pitch;
-  const uint8_t* vs = (const uint8_t*)slot_tv(e, slot) + (size_t)layer * nKV * pitch;
-  if (P > 0) {
-    CK(cudaMemcpy2DAsync(k_dev, row, ks, pitch, row, nKV, cudaMemcpyDeviceToDevice, stream));
-    CK(cudaMemcpy2DAsync(v_dev, row, vs, pitch, row, nKV, cudaMemcpyDeviceToDevice, stream));
-  }
-  return 0;
+  return copy_kv(e, slot, layer, k_dev, v_dev, P, false, (cudaStream_t)stream_);
 }
 
 extern "C" int fq3_set_generation_state(fq3_engine* e, int32_t slot, int32_t n_left_pad, int32_t rope_delta) {
@@ -898,6 +951,7 @@ extern "C" int fq3_talker_step(fq3_engine* e, int32_t slot, const void* embeds_d
   int rc;
   if ((rc = check_slot(e, slot))) return rc;
   if (position < 0 || position >= e->cfg.max_seq_len) return fail(FQ3_ERR_INVALID, "position %d outside the cache", position);
+  if ((rc = check_rows(e, slot, (long long)position + 1, "fq3_talker_step"))) return rc;
   DevGuard dev_guard(e->dev);
   KParams kp = kp_for_slot(e, slot, nullptr);
   kp.mode = MODE_TALKER_STEP;
@@ -965,6 +1019,7 @@ extern "C" int fq3_begin_request(fq3_engine* e, int32_t slot, const fq3_request*
   h.max_new = rq->max_new_tokens; h.min_new = rq->min_new_tokens; h.trailing_len = rq->trailing_len;
   h.trailing = trailing_text_dev; h.tts_pad = tts_pad_dev; h.uniforms = uniforms_dev;
   h.text_open = false; h.text_closed = false;
+  h.step = 0;
   h.sp_t = to_sampling(sp_talker); h.sp_p = to_sampling(sp_predictor);
   int* st = e->state + 8 * slot;
   float* ph = e->past_hidden + (size_t)slot * HMAX;
@@ -1059,6 +1114,10 @@ extern "C" int fq3_decode_chunk_n(fq3_engine* e, const int32_t* slots, int32_t n
     if (!e->slots[slots[j]].active) return fail(FQ3_ERR_STATE, "fq3_begin_request has not been called for slot %d", slots[j]);
     for (int i = 0; i < j; ++i)
       if (slots[i] == slots[j]) return fail(FQ3_ERR_INVALID, "slot %d listed twice", slots[j]);
+    // frame s writes cache row prefill_len + s unless that row is the last one (the max_seq_len rule)
+    const SlotHost& h = e->slots[slots[j]];
+    const long long rows = std::min((long long)h.prefill_len + h.step + n_frames[j], (long long)e->cfg.max_seq_len - 1);
+    if ((rc = check_rows(e, slots[j], rows, "a frame budget"))) return rc;
   }
   DevGuard dev_guard(e->dev);
   cudaStream_t stream = (cudaStream_t)stream_;
@@ -1080,6 +1139,7 @@ extern "C" int fq3_decode_chunk_n(fq3_engine* e, const int32_t* slots, int32_t n
     res[j].total_frames = st[1];
     res[j].finished = st[3];
     res[j].frames_emitted = st[4];
+    e->slots[slots[j]].step = st[1];
   }
   return 0;
 }
@@ -1132,12 +1192,75 @@ extern "C" int fq3_tape_bytes(fq3_engine* e, int64_t* talker_step_bytes, int64_t
   return 0;
 }
 
+// ---- paged talker KV cache
+extern "C" int fq3_map_kv_pages(fq3_engine* e, int32_t slot, const int32_t* pages, int32_t n) {
+  if (!e || (n > 0 && !pages)) return fail(FQ3_ERR_INVALID, "null argument");
+  int rc;
+  if ((rc = check_slot(e, slot))) return rc;
+  if (n < 0 || n > e->kv_npt)
+    return fail(FQ3_ERR_INVALID, "slot %d: %d pages outside [0, %d] (max_seq_len=%d rows)", slot, n, e->kv_npt, e->cfg.max_seq_len);
+  for (int i = 0; i < n; ++i) {
+    if (pages[i] < 0 || pages[i] >= e->kv_npages)
+      return fail(FQ3_ERR_INVALID, "slot %d: page %d outside [0, %d)", slot, pages[i], e->kv_npages);
+    for (int j = 0; j < i; ++j)
+      if (pages[j] == pages[i]) return fail(FQ3_ERR_INVALID, "slot %d: page %d listed twice", slot, pages[i]);
+    const int o = e->kv_owner[pages[i]];
+    if (o >= 0 && o != slot) return fail(FQ3_ERR_INVALID, "slot %d: page %d is mapped to slot %d", slot, pages[i], o);
+  }
+  DevGuard dev_guard(e->dev);
+  int* tab = e->kv_tab_host.data() + (size_t)slot * e->kv_npt;
+  for (int i = 0; i < e->kv_npt; ++i) {
+    if (tab[i] >= 0) e->kv_owner[tab[i]] = -1;
+    tab[i] = i < n ? pages[i] : -1;
+  }
+  for (int i = 0; i < n; ++i) e->kv_owner[pages[i]] = slot;
+  e->kv_nmapped[slot] = n;
+  memcpy(e->kv_stage, tab, e->kv_npt * sizeof(int));
+  CK(cudaMemcpyAsync(e->kv_tab + (size_t)slot * e->kv_npt, e->kv_stage, e->kv_npt * sizeof(int), cudaMemcpyHostToDevice,
+                     e->kv_stream));
+  CK(cudaStreamSynchronize(e->kv_stream));
+  return 0;
+}
+
+extern "C" int fq3_slot_kv_rows(fq3_engine* e, int32_t slot) {
+  if (!e) return fail(FQ3_ERR_INVALID, "null argument");
+  int rc;
+  if ((rc = check_slot(e, slot))) return rc;
+  return kv_rows(e, slot);
+}
+
+extern "C" int fq3_kv_pool_pages(fq3_engine* e) { return e ? e->kv_npages : 0; }
+
+static int copy_pages(fq3_engine* e, const int32_t* pages, int32_t n, void* mem, bool out, void* stream_) {
+  if (!e || (n > 0 && (!pages || !mem))) return fail(FQ3_ERR_INVALID, "null argument");
+  if (n < 0) return fail(FQ3_ERR_INVALID, "n %d < 0", n);
+  for (int i = 0; i < n; ++i) {
+    if (pages[i] < 0 || pages[i] >= e->kv_npages) return fail(FQ3_ERR_INVALID, "page %d outside [0, %d)", pages[i], e->kv_npages);
+    for (int j = 0; j < i; ++j)
+      if (pages[j] == pages[i]) return fail(FQ3_ERR_INVALID, "page %d listed twice", pages[i]);
+  }
+  DevGuard dev_guard(e->dev);
+  const int L = e->cfg.talker.num_hidden_layers, nKV = e->cfg.talker.num_key_value_heads;
+  for (int i = 0; i < n; ++i) {
+    uint8_t* pg = kv_row(e->kv, L, nKV, e->esz, &pages[i], 0, 0, 0, 0);   // a page is one block: its first row
+    uint8_t* m = (uint8_t*)mem + (size_t)i * e->kv_page_bytes;
+    CK(cudaMemcpyAsync(out ? m : pg, out ? pg : m, e->kv_page_bytes, cudaMemcpyDefault, (cudaStream_t)stream_));
+  }
+  return 0;
+}
+extern "C" int fq3_kv_pages_to(fq3_engine* e, const int32_t* pages, int32_t n, void* dst, void* stream) {
+  return copy_pages(e, pages, n, dst, true, stream);
+}
+extern "C" int fq3_kv_pages_from(fq3_engine* e, const int32_t* pages, int32_t n, const void* src, void* stream) {
+  return copy_pages(e, pages, n, (void*)src, false, stream);
+}
+
 extern "C" int fq3_num_ctas(fq3_engine* e) { return e ? e->ncta : 0; }
 extern "C" int64_t fq3_launch_count(fq3_engine* e) { return e ? e->launches : 0; }
 extern "C" const char* fq3_last_error(void) { return g_err; }
 extern "C" int fq3_max_batch(fq3_engine* e) { return e ? e->max_batch : 0; }
 extern "C" int fq3_max_slots(fq3_engine* e) { return e ? e->max_slots : 0; }
-extern "C" const char* fq3_version(void) { return "fq3-h100 0.2.0 (sm_90a)"; }
+extern "C" const char* fq3_version(void) { return "fq3-h100 0.3.0 (sm_90a)"; }
 
 #include "fq3_prefill.cuh"
 

@@ -2,8 +2,8 @@
 //
 // Replaces the variable-length prompt forward the reference delegates to upstream HF eager code
 // (faster_qwen3_tts/generate.py:107-118, streaming.py:63-74) and the 56 index_copy_ calls of
-// TalkerGraph.prefill_kv (talker_graph.py:153-170): K and V are written straight into the engine's
-// [layer][kv_head][slot][128] cache.  Per layer: RMSNorm rows -> QKV GEMM -> q/k-norm + RoPE + KV append ->
+// TalkerGraph.prefill_kv (talker_graph.py:153-170): K and V are written straight into the request's pages of the
+// engine's paged talker cache (fq3::kv_row).  Per layer: RMSNorm rows -> QKV GEMM -> q/k-norm + RoPE + KV append ->
 // causal GQA attention (eager semantics: bf16 scores, fp32 softmax rounded to bf16, bf16 P.V) -> o_proj GEMM with
 // fused residual -> RMSNorm rows -> gate/up GEMM with fused SwiGLU (interleaved columns) -> down GEMM with fused
 // residual.  GEMMs are the shared implicit-GEMM tensor-core kernel (fq3gemm::gemm, taps = 1).
@@ -91,12 +91,12 @@ __global__ void rmsnorm_last_rows_kernel(const __nv_bfloat16* __restrict__ X, co
 }
 
 // one warp per (packed row, vector) with vector in [q heads | k heads | v heads]: q/k RMSNorm + RoPE in place (q) or
-// into the KV cache of the row's sequence at its cache row t (k, v).  QKV is [rows][qd + 2 kd] bf16; kc / vc are one
-// layer of slot 0's caches, slot s starting `slot_stride` elements further.
+// into the KV cache of the row's sequence at its cache row t (k, v).  QKV is [rows][qd + 2 kd] bf16; kv is the page
+// pool of the L-layer cache, slot s's page table starts at tabs + s * npt (kv_row).
 __global__ void rope_kv_kernel(__nv_bfloat16* __restrict__ QKV, int rows, int nH, int nKV, const __nv_bfloat16* qn,
                                const __nv_bfloat16* kn, const float* __restrict__ cosT, const float* __restrict__ sinT,
-                               int npos, float eps, __nv_bfloat16* __restrict__ kc, __nv_bfloat16* __restrict__ vc,
-                               size_t slot_stride, int S, const __grid_constant__ SeqTab tab) {
+                               int npos, float eps, void* kv, const int* __restrict__ tabs, int npt, int L, int layer,
+                               const __grid_constant__ SeqTab tab) {
   fq3gemm::pdl_launch();
   fq3gemm::pdl_wait();
   const int gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
@@ -137,7 +137,8 @@ __global__ void rope_kv_kernel(__nv_bfloat16* __restrict__ QKV, int rows, int nH
     for (int i = 0; i < 4; ++i) src[lane + 32 * i] = __float2bfloat16_rn(v[i]);
   } else {
     const int g = what == 1 ? vi - nH : vi - nH - nKV;
-    __nv_bfloat16* dst = (what == 1 ? kc : vc) + (size_t)tab.slot[sq] * slot_stride + ((size_t)g * S + t) * 128;
+    __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(
+        fq3::kv_row(kv, L, nKV, 2, tabs + (size_t)tab.slot[sq] * npt, what - 1, layer, g, t));
 #pragma unroll
     for (int i = 0; i < 4; ++i) dst[lane + 32 * i] = __float2bfloat16_rn(v[i]);
   }
@@ -175,9 +176,8 @@ __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
 
 template <int REP>
 __global__ void __launch_bounds__(128) attn_prefill_mma_kernel(const __nv_bfloat16* __restrict__ QKVp, int nH, int nKV,
-                                                              const __nv_bfloat16* __restrict__ kc,
-                                                              const __nv_bfloat16* __restrict__ vc, size_t slot_stride,
-                                                              int S, __nv_bfloat16* __restrict__ OUTp,
+                                                              void* kv, const int* __restrict__ tabs, int npt, int L,
+                                                              int layer, __nv_bfloat16* __restrict__ OUTp,
                                                               const __grid_constant__ SeqTab tab) {
   constexpr int KT = 32;                                   // keys per staged tile
   __shared__ __align__(128) uint8_t sm[2][2][KT * 256];    // [buffer][K | V][key row x 256 B], 16-byte chunks XOR-swizzled
@@ -195,8 +195,7 @@ __global__ void __launch_bounds__(128) attn_prefill_mma_kernel(const __nv_bfloat
   const int h = g * REP + (warp % REP);
   const int q0 = qb * 32 + (warp / REP) * 16;
   const int i0 = q0 + gq, i1 = q0 + gq + 8;
-  const __nv_bfloat16* kb = kc + (size_t)tab.slot[sq] * slot_stride + (size_t)g * S * 128;
-  const __nv_bfloat16* vb = vc + (size_t)tab.slot[sq] * slot_stride + (size_t)g * S * 128;
+  const int* pages = tabs + (size_t)tab.slot[sq] * npt;
   const int kt_first = n_left_pad / KT;
   const int kt_last = min(qb, (P - 1) / KT);
 
@@ -208,7 +207,9 @@ __global__ void __launch_bounds__(128) attn_prefill_mma_kernel(const __nv_bfloat
       const int mat = idx >> 9, r = (idx & 511) >> 4, ch = idx & 15;
       const int key = k0 + r;
       const bool ok = key < P;
-      const __nv_bfloat16* src = (mat ? vb : kb) + (size_t)(ok ? key : 0) * 128 + ch * 8;
+      // a 32-key tile never straddles a KV_PAGE-row page
+      const __nv_bfloat16* src =
+          reinterpret_cast<const __nv_bfloat16*>(fq3::kv_row(kv, L, nKV, 2, pages, mat, layer, g, ok ? key : 0)) + ch * 8;
       fq3gemm::cp_async16(&sm[buf][mat][r * 256 + ((ch ^ (r & 7)) << 4)], src, ok);
     }
   };
@@ -404,7 +405,7 @@ static int prefill_group(fq3_engine* e, const pf::SeqTab& tab, const void* embed
                          void* hidden_out_dev, cudaStream_t stream) {
   const fq3_stack_config& T = e->cfg.talker;
   const int L = T.num_hidden_layers, H = T.hidden_size, I = T.intermediate_size;
-  const int nH = T.num_attention_heads, nKV = T.num_key_value_heads, qd = nH * 128, kd = nKV * 128, S = e->cfg.max_seq_len;
+  const int nH = T.num_attention_heads, nKV = T.num_key_value_heads, qd = nH * 128, kd = nKV * 128;
   const int rows = tab.row0[tab.n - 1] + tab.P[tab.n - 1], n = tab.n;
   using bf = __nv_bfloat16;
   bf* x = (bf*)e->pf_buf[0];
@@ -412,7 +413,6 @@ static int prefill_group(fq3_engine* e, const pf::SeqTab& tab, const void* embed
   bf* hn = (bf*)e->pf_buf[2];
   bf* wide = (bf*)e->pf_buf[3];
   bf* att = (bf*)e->pf_buf[4];
-  const size_t slot_stride = e->tkv_slot / sizeof(bf);
   CK(cudaMemcpyAsync(x, embeds_dev, (size_t)rows * H * 2, cudaMemcpyDeviceToDevice, stream));
   const KParams& k = e->kp;
   int rc;
@@ -420,19 +420,17 @@ static int prefill_group(fq3_engine* e, const pf::SeqTab& tab, const void* embed
     FQ3_LAUNCH((pf::rmsnorm_rows_kernel), rows, 256, 0, stream, x, (const bf*)k.t.ln_in + (size_t)l * H, H, T.rms_norm_eps, hn);
     e->launches++;
     if ((rc = pf_gemm(e, hn, (const bf*)e->pf_qkv + (size_t)l * (qd + 2 * kd) * H, nullptr, wide, rows, H, qd + 2 * kd, 0, stream))) return rc;
-    bf* kl = (bf*)e->t_kc + (size_t)l * nKV * S * 128;   // layer l of slot 0; the kernels add slot * slot_stride
-    bf* vl = (bf*)e->t_vc + (size_t)l * nKV * S * 128;
     {
       const int warps = rows * (nH + 2 * nKV);
       FQ3_LAUNCH((pf::rope_kv_kernel), (warps * 32 + 255) / 256, 256, 0, stream,
           wide, rows, nH, nKV, (const bf*)k.t.qnorm + (size_t)l * 128, (const bf*)k.t.knorm + (size_t)l * 128, k.t.cos,
-          k.t.sin, k.t.npos, T.rms_norm_eps, kl, vl, slot_stride, S, tab);
+          k.t.sin, k.t.npos, T.rms_norm_eps, e->kv, e->kv_tab, e->kv_npt, L, l, tab);
       e->launches++;
     }
     if (nH == 2 * nKV)   // fq3_engine_set_prefill_weights admits GQA ratios 1 and 2 only
-      FQ3_LAUNCH((pf::attn_prefill_mma_kernel<2>), dim3(tab.qb0[n], nKV), 128, 0, stream, wide, nH, nKV, kl, vl, slot_stride, S, att, tab);
+      FQ3_LAUNCH((pf::attn_prefill_mma_kernel<2>), dim3(tab.qb0[n], nKV), 128, 0, stream, wide, nH, nKV, e->kv, e->kv_tab, e->kv_npt, L, l, att, tab);
     else
-      FQ3_LAUNCH((pf::attn_prefill_mma_kernel<1>), dim3(tab.qb0[n], nKV), 128, 0, stream, wide, nH, nKV, kl, vl, slot_stride, S, att, tab);
+      FQ3_LAUNCH((pf::attn_prefill_mma_kernel<1>), dim3(tab.qb0[n], nKV), 128, 0, stream, wide, nH, nKV, e->kv, e->kv_tab, e->kv_npt, L, l, att, tab);
     e->launches++;
     if ((rc = pf_gemm(e, att, (const bf*)e->pf_o + (size_t)l * H * qd, x, x1, rows, qd, H, 0, stream))) return rc;
     FQ3_LAUNCH((pf::rmsnorm_rows_kernel), rows, 256, 0, stream, x1, (const bf*)k.t.ln_post + (size_t)l * H, H, T.rms_norm_eps, hn);
@@ -465,6 +463,8 @@ extern "C" int fq3_prefill_batch(fq3_engine* e, int32_t n, const int32_t* slots,
     if (P[i] <= 0) return fail(FQ3_ERR_INVALID, "empty prompt%s", row);
     if (P[i] > e->cfg.max_seq_len)
       return fail(FQ3_ERR_TOO_LONG, "Input is too long: prefill has %d tokens but max_seq_len=%d. Use shorter text or shorter reference audio.%s", P[i], e->cfg.max_seq_len, row);
+    int rc;
+    if ((rc = check_rows(e, slots[i], P[i], "the prompt"))) return rc;
   }
   if (!e->pf_ready) return fail(FQ3_ERR_STATE, "fq3_engine_set_prefill_weights has not been called");
   if ((uintptr_t)logits_out_dev & 15) return fail(FQ3_ERR_INVALID, "logits_out_dev must be 16-byte aligned");

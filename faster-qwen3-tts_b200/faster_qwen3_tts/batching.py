@@ -19,6 +19,7 @@ from typing import Dict, Generator, List, Optional, Tuple
 
 import torch
 
+from .engine import KV_PAGE
 from .generate import _sync, begin_fused, begin_fused_batch, shared_engine
 from .logprobs import FrameLogprobs
 
@@ -42,6 +43,8 @@ class SlotRequest:
     due: float = 0.0                          # urgency when more requests are ready than a launch has columns: smallest first
     hold: bool = False                        # set by the caller between steps: not launched (a listener far enough ahead)
     seq: int = 0                              # admission order, the tie-break of ``due``
+    prompt_rows: int = 0                      # cache rows of the prompt: frame s writes row prompt_rows + s
+    parked: Optional[torch.Tensor] = None     # paged engine: the request's KV pages while parked in host memory
 
     def budget(self, n_frames: int) -> int:
         """frames the next launch may emit for this request"""
@@ -66,6 +69,67 @@ _SUBMIT_DEFAULTS = dict(max_new_tokens=2048, min_new_tokens=2, temperature=0.9, 
                         repetition_penalty=1.05, uniforms=None)
 
 
+class KvPager:
+    """The talker KV pages of a paged engine (``Engine(kv_pages=N)``) as one scheduler hands them to its slots.  A slot
+    maps the pages of the rows it has written and of its next launch; a parked request's pages wait in pinned host
+    memory (``park`` / ``restore``), its slot keeping everything else.  ``peak``: most pages in use at once."""
+
+    def __init__(self, engine):
+        self.engine = engine
+        self.free: List[int] = list(range(engine.kv_pages))
+        self.mapped: Dict[int, List[int]] = {}
+        self.peak = 0
+        self.parks = 0
+
+    @staticmethod
+    def pages(rows: int) -> int:
+        return -(-int(rows) // KV_PAGE)
+
+    def in_use(self) -> int:
+        return self.engine.kv_pages - len(self.free)
+
+    def rows(self, slot: int) -> int:
+        return KV_PAGE * len(self.mapped.get(slot, ()))
+
+    def grow(self, slot: int, rows: int) -> int:
+        """map pages for the slot's rows [0, rows) as far as free pages go; -> the rows it maps"""
+        have = self.mapped.setdefault(slot, [])
+        n = min(self.pages(rows) - len(have), len(self.free))
+        if n > 0:
+            self.engine.map_kv_pages(slot, have + self.free[:n])
+            have += self.free[:n]
+            del self.free[:n]
+            self.peak = max(self.peak, self.in_use())
+        return self.rows(slot)
+
+    def release(self, slot: int) -> None:
+        pages = self.mapped.pop(slot, [])
+        if pages:
+            self.engine.map_kv_pages(slot, [])
+            self.free += pages
+
+    def park(self, slot: int, rows: int) -> torch.Tensor:
+        """copy the pages of the slot's rows [0, rows) to pinned host memory and free all its pages"""
+        pages = self.mapped.get(slot, [])[: self.pages(rows)]
+        host = torch.empty(len(pages), self.engine.kv_page_bytes, dtype=torch.uint8,
+                           pin_memory=torch.cuda.is_available())
+        self.engine.kv_pages_to(pages, host)
+        self.release(slot)
+        self.parks += 1
+        return host
+
+    def restore(self, slot: int, host: torch.Tensor, rows: int) -> bool:
+        """once free pages cover rows [0, rows): map them and copy the parked pages back into the first ones"""
+        if self.pages(rows) > len(self.free) or self.mapped.get(slot):
+            return False
+        n = int(host.shape[0])
+        self.grow(slot, n * KV_PAGE)
+        self.engine.kv_pages_from(self.mapped[slot], host)
+        if torch.cuda.is_available():   # the host buffer is dropped after this
+            torch.cuda.current_stream(getattr(self.engine, "device", None)).synchronize()
+        return True
+
+
 def _frames_arg(name: str, v) -> Optional[int]:
     if v is None:
         return None
@@ -85,7 +149,24 @@ class BatchScheduler:
     (ties: the one admitted first); the others keep their slot and state and cost the launch nothing.  ``due`` and
     ``hold`` belong to the caller, which sets them between steps (serving.ContinuousBatcher: the listener's playback
     lead).  A request's ``chunk_size`` / ``first_chunk`` replace the step's ``n_frames`` for that request alone: its codes
-    do not depend on them, only how many frames each launch hands back."""
+    do not depend on them, only how many frames each launch hands back.
+
+    Paged engines (``Engine(kv_pages=N)``, a pool smaller than ``max_slots x max_seq_len`` rows) get their talker KV
+    pages through ``pager`` (``KvPager``); with the default pool it is None and the scheduler makes no page calls.
+    Admission (``submit_many``) needs a free slot and free pages for each prompt plus one chunk (the frames of the last
+    step), else ``has_capacity()`` is false and it raises as when slots run out.  Before each step every launched
+    request maps pages for its position plus budget (at most ``max_seq_len`` rows).  One that cannot get them all is
+    launched only if its pages hold all the frames it has left, for those; otherwise it is not launched, like a request
+    waiting for text.  A launch thus never ends inside a chunk, so every request's chunks (and under the codec's window
+    policy its audio) are those it gets when pages are plenty.  When no ready
+    request can advance one frame, the resident request with the largest ``due`` (ties: the latest admitted) other
+    than the most urgent ready one is *parked*: its pages go to pinned host memory and are freed, its slot and the rest
+    of its state stay.  It is restored into whatever pages are free, before it is next launched, once they cover its
+    rows plus one chunk.  Parking is exact: a page comes back with the bytes it left with.
+    Progress: the pool holds at least one request of ``max_seq_len`` rows (the engine refuses a smaller one), so after
+    parking every other resident request the most urgent ready one has all the pages it can use and advances.  A
+    request parks only while another is launched instead, so, as for starvation above, it runs again once its
+    ``due`` is the smallest.  Pages are freed when a request finishes or is cancelled, parked or not."""
 
     def __init__(self, engine, talker, config, predictor_graph, talker_graph, slots=None):
         """``slots``: the engine's request slots this scheduler hands out (default: all of them)."""
@@ -98,12 +179,28 @@ class BatchScheduler:
         self.active: Dict[int, SlotRequest] = {}
         self._seq = 0
         self.max_seq_len = getattr(engine, "max_seq_len", None)   # longest prompt a slot takes
+        self.pager = KvPager(engine) if getattr(engine, "paged", False) else None
+        self._chunk = 1   # frames of the last step: the chunk a paged admission reserves pages for
 
     def __len__(self) -> int:
         return len(self.active)
 
     def has_capacity(self) -> bool:
-        return bool(self.free)
+        return bool(self.free) and (self.pager is None or bool(self.pager.free))
+
+    def _admit_rows(self, r: dict) -> int:
+        """cache rows a request needs at admission: its prompt plus one chunk (a frame at row max_seq_len - 1 writes
+        none)"""
+        chunk = r.get("first_chunk") or r.get("chunk_size") or self._chunk
+        P = int(r["tie"].shape[1])
+        return max(P, min(P + int(chunk), self.max_seq_len - 1))
+
+    def admits(self, requests: List[dict]) -> bool:
+        """whether ``submit_many(requests)`` finds the slots and KV pages it needs"""
+        if len(requests) > len(self.free):
+            return False
+        return self.pager is None or \
+            sum(KvPager.pages(self._admit_rows(r)) for r in requests) <= len(self.pager.free)
 
     def capacity(self) -> int:
         """free request slots"""
@@ -138,6 +235,9 @@ class BatchScheduler:
         n = len(requests)
         if n > len(self.free):
             raise RuntimeError(f"{n} requests but only {len(self.free)} of {self.max_slots} request slots are free")
+        if not self.admits(requests):
+            raise RuntimeError(f"{n} requests need more KV pages than the {len(self.pager.free)} of "
+                               f"{self.engine.kv_pages} that are free")
         chunking = [(_frames_arg("chunk_size", r.get("chunk_size")), _frames_arg("first_chunk", r.get("first_chunk")))
                     for r in requests]
         slots, self.free = self.free[:n], self.free[n:]
@@ -150,6 +250,9 @@ class BatchScheduler:
         first_lps = [None] * n
         lkw = {"logprob": True} if logprobs else {}   # off: the calls of a scheduler without the option
         try:
+            if self.pager is not None:
+                for slot, r in zip(slots, requests):
+                    self.pager.grow(slot, self._admit_rows(r))
             if n == 1:   # one request: ``begin_fused``, the one-row case of ``begin_fused_batch``
                 r = rows[0]
                 got = begin_fused(self.engine, self.talker, r["tie"], r["tam"], r["tth"], r["tpe"], self.config, self.pg,
@@ -163,6 +266,9 @@ class BatchScheduler:
                 if r.get("feed") is not None:
                     self.engine.set_text_rows(slot, r["feed"].update(), open=not r["feed"].closed)
         except Exception:
+            if self.pager is not None:
+                for slot in slots:
+                    self.pager.release(slot)
             self.free = slots + self.free
             raise
         out = []
@@ -171,7 +277,8 @@ class BatchScheduler:
             rq = SlotRequest(slot=slot, tag=tag if tag is not None else slot, max_new_tokens=gen["max_new_tokens"],
                              feed=r.get("feed"), gen0=self.engine.gen_step0[slot], rows_ahead=max(1, int(r.get("rows_ahead", 1))),
                              lp=FrameLogprobs(flp) if logprobs else None, chunk_size=chunk_size, first_chunk=first_chunk,
-                             seq=self._next_seq())
+                             seq=self._next_seq(),
+                             prompt_rows=int(r["tie"].shape[1]) if self.pager is not None else 0)
             self.active[slot] = rq
             out.append(rq)
         return out
@@ -185,12 +292,17 @@ class BatchScheduler:
             if rq.feed is not None:
                 self.engine.set_text_rows(rq.slot, rq.feed.update(), open=not rq.feed.closed)
         ready = [rq for rq in self.active.values() if rq.ready()]
-        if len(ready) > self.engine.max_batch:
-            ready = sorted(ready, key=lambda rq: (rq.due, rq.seq))[: self.engine.max_batch]
-        slots = sorted(rq.slot for rq in ready)
+        self._chunk = n_frames
+        if self.pager is not None:
+            budget_of = self._page_budgets(ready, n_frames)
+        else:
+            if len(ready) > self.engine.max_batch:
+                ready = sorted(ready, key=lambda rq: (rq.due, rq.seq))[: self.engine.max_batch]
+            budget_of = {rq.slot: rq.budget(n_frames) for rq in ready}
+        slots = sorted(budget_of)
         if not slots:
             return []
-        budgets = [self.active[s].budget(n_frames) for s in slots]
+        budgets = [budget_of[s] for s in slots]
         if len(set(budgets)) > 1:
             n_frames = budgets              # one budget per slot (fq3_decode_chunk_n)
         else:
@@ -221,15 +333,65 @@ class BatchScheduler:
                 rq.eos_logprob = rq.lp.eos_logprob(r.next_token, self.engine.eos)
             done.append((rq, c.clone()))
             if r.finished:
-                del self.active[s]
-                self.free.append(s)
+                self._end(rq)
         return done
+
+    def _end(self, rq: SlotRequest) -> None:
+        del self.active[rq.slot]
+        rq.parked = None
+        if self.pager is not None:
+            self.pager.release(rq.slot)
+        self.free.append(rq.slot)
+
+    def _fit(self, rq: SlotRequest, budget: int) -> int:
+        """paged engine: restore a parked request and map pages for its next ``budget`` frames; -> the budget of its
+        launch (0: not launched)"""
+        pos = rq.prompt_rows + rq.frames                      # the row its next frame writes
+        want = min(pos + budget, self.max_seq_len - 1)        # a frame at row max_seq_len - 1 writes nothing
+        if rq.parked is not None:
+            if not self.pager.restore(rq.slot, rq.parked, want):
+                return 0
+            rq.parked = None
+        got = self.pager.grow(rq.slot, want)
+        if got >= want:
+            return budget
+        # short of pages: only the frames the request has left, never part of a chunk, so that its launches end where
+        # they end when pages are plenty (a window policy's audio depends on where its chunks end)
+        left = rq.max_new_tokens - rq.frames
+        return left if 0 < left and min(pos + left, self.max_seq_len - 1) <= got else 0
+
+    def _page_budgets(self, ready: List[SlotRequest], n_frames: int) -> Dict[int, int]:
+        """paged engine: {slot: budget} of the next launch, parking requests while none can advance (class docstring)"""
+        order = sorted(ready, key=lambda rq: (rq.due, rq.seq))
+        parked = set()   # parked by this step: not restored in it, or the pages would cycle
+        while True:
+            out = {}
+            for rq in order:
+                if len(out) == self.engine.max_batch:
+                    break
+                if rq.slot in parked:
+                    continue
+                b = self._fit(rq, rq.budget(n_frames))
+                if b > 0:
+                    out[rq.slot] = b
+            if out or not order:
+                return out
+            victims = [rq for rq in self.active.values()
+                       if rq is not order[0] and rq.parked is None and self.pager.rows(rq.slot)]
+            if not victims:
+                return out
+            victim = max(victims, key=lambda rq: (rq.due, rq.seq))
+            self.park(victim)
+            parked.add(victim.slot)
+
+    def park(self, rq: SlotRequest) -> None:
+        """paged engine: move the request's KV pages to host memory; it is restored before it is next launched"""
+        rq.parked = self.pager.park(rq.slot, min(rq.prompt_rows + rq.frames, self.max_seq_len))
 
     def cancel(self, rq: SlotRequest) -> None:
         """End a request now and free its slot (a client that went away)."""
         if self.active.get(rq.slot) is rq:
-            del self.active[rq.slot]
-            self.free.append(rq.slot)
+            self._end(rq)
 
 
 def _single(engine, talker, config, predictor_graph, talker_graph, request: dict, logprobs: bool = False):

@@ -35,7 +35,8 @@ class Config(C.Structure):
     _fields_ = [("dtype", C.c_int32), ("device", C.c_int32), ("max_seq_len", C.c_int32),
                 ("num_code_groups", C.c_int32), ("codec_eos_token_id", C.c_int32),
                 ("has_mtp_projection", C.c_int32), ("num_ctas", C.c_int32), ("rope_positions", C.c_int32),
-                ("talker", StackConfig), ("predictor", StackConfig), ("max_batch", C.c_int32), ("max_slots", C.c_int32)]
+                ("talker", StackConfig), ("predictor", StackConfig), ("kv_pages", C.c_int32), ("max_batch", C.c_int32),
+                ("max_slots", C.c_int32)]
 
 
 class Tensor(C.Structure):
@@ -71,7 +72,8 @@ EXPORTS = [
     "fq3_set_generation_state", "fq3_talker_step", "fq3_predictor_run", "fq3_sample_logits", "fq3_sample_logits_lp",
     "fq3_begin_request", "fq3_decode_chunk", "fq3_decode_chunk_lp", "fq3_decode_chunk_n", "fq3_max_slots", "fq3_slot_bytes", "fq3_set_text_rows", "fq3_get_past_hidden", "fq3_debug_enable", "fq3_debug_read", "fq3_tape_bytes",
     "fq3_num_ctas", "fq3_launch_count", "fq3_last_error", "fq3_version", "fq3_engine_set_prefill_weights", "fq3_prefill", "fq3_prefill_batch", "fq3_max_batch", "fq3_debug_gemv",
-    "fq3_debug_conv_gemm",
+    "fq3_debug_conv_gemm", "fq3_kv_page_bytes", "fq3_map_kv_pages", "fq3_slot_kv_rows", "fq3_kv_pool_pages",
+    "fq3_kv_pages_to", "fq3_kv_pages_from",
     "fq3_codec_create", "fq3_codec_load_weights", "fq3_codec_flops",
     "fq3_codec_load_frontend", "fq3_codec_decode_codes", "fq3_codec_frontend_flops",
     "fq3_codec_stream_create", "fq3_codec_stream_reset", "fq3_codec_stream_destroy", "fq3_codec_stream_frames",
@@ -136,6 +138,13 @@ def load_library() -> C.CDLL:
     lib.fq3_max_slots.argtypes = [C.c_void_p]
     lib.fq3_slot_bytes.argtypes = [C.POINTER(Config)]
     lib.fq3_slot_bytes.restype = C.c_int64
+    lib.fq3_kv_page_bytes.argtypes = [C.POINTER(Config)]
+    lib.fq3_kv_page_bytes.restype = C.c_int64
+    lib.fq3_map_kv_pages.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.c_int32]
+    lib.fq3_slot_kv_rows.argtypes = [C.c_void_p, C.c_int32]
+    lib.fq3_kv_pool_pages.argtypes = [C.c_void_p]
+    lib.fq3_kv_pages_to.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_void_p, C.c_void_p]
+    lib.fq3_kv_pages_from.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_void_p, C.c_void_p]
     lib.fq3_set_text_rows.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32]
     lib.fq3_get_past_hidden.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
     lib.fq3_max_batch.argtypes = [C.c_void_p]
@@ -256,15 +265,32 @@ def slot_bytes(talker: dict, predictor: dict, dtype: torch.dtype, max_seq_len: i
     return int(n)
 
 
+def kv_page_bytes(talker: dict, predictor: dict, dtype: torch.dtype) -> int:
+    """Device bytes of one talker KV page (fq3_kv_page_bytes): 64 cache rows of every layer and kv head, K and V.
+    Needs no GPU."""
+    lib = load_library()
+    cfg = Config(dtype=FQ3_BF16 if dtype == torch.bfloat16 else FQ3_F32, max_seq_len=64,
+                 talker=_stack_config(talker), predictor=_stack_config(predictor))
+    n = lib.fq3_kv_page_bytes(C.byref(cfg))
+    if n < 0:
+        _check(lib, int(n))
+    return int(n)
+
+
+KV_PAGE = 64   # cache rows per talker KV page
+
+
 class Engine:
     """One engine per device: packed weights, KV caches and the persistent decode kernel.  ``max_batch`` is the number
     of slots one launch may carry (<= 32), ``max_slots`` (default: ``max_batch``) the number of request slots that
-    exist; with more slots than columns the caller chooses which ones each launch advances."""
+    exist; with more slots than columns the caller chooses which ones each launch advances.  ``kv_pages`` (default 0:
+    every slot owns ceil(max_seq_len / 64) pages for good) makes the talker cache a pool of that many 64-row pages that
+    slots map with ``map_kv_pages`` as their rows are written."""
 
     def __init__(self, *, talker: dict, predictor: dict, dtype: torch.dtype, device="cuda", max_seq_len: int = 2048,
                  num_code_groups: int = 16, codec_eos_token_id: int = 2150, has_mtp_projection: bool = True,
                  num_ctas: int = 0, rope_positions: Optional[int] = None, max_batch: int = 1,
-                 max_slots: Optional[int] = None):
+                 max_slots: Optional[int] = None, kv_pages: int = 0):
         if not torch.cuda.is_available():
             raise RuntimeError("fq3 engine needs a CUDA device (sm_90a); no CPU fallback exists")
         self.lib = load_library()
@@ -281,13 +307,16 @@ class Engine:
 
         cfg = Config(FQ3_BF16 if dtype == torch.bfloat16 else FQ3_F32, self.device.index, self.max_seq_len,
                      num_code_groups, codec_eos_token_id, int(bool(has_mtp_projection)), int(num_ctas),
-                     self.rope_positions, _stack_config(talker), _stack_config(predictor), int(max_batch),
-                     int(max_slots or 0))
+                     self.rope_positions, _stack_config(talker), _stack_config(predictor), kv_pages=int(kv_pages),
+                     max_batch=int(max_batch), max_slots=int(max_slots or 0))
         self.max_batch = int(max_batch)
         h = C.c_void_p()
         _check(self.lib, self.lib.fq3_engine_create(C.byref(cfg), C.byref(h)))
         self.h = h
         self.max_slots = int(self.lib.fq3_max_slots(h))
+        self.kv_pages = int(self.lib.fq3_kv_pool_pages(h))   # pages in the pool
+        self.paged = int(kv_pages) > 0                       # slots start unmapped: the caller maps their pages
+        self.kv_page_bytes = kv_page_bytes(talker, predictor, dtype)
         self.H = talker["hidden_size"]
         self._keep = {}  # slot -> tensors borrowed by the engine for the duration of that slot's request
         self.gen_step0 = {}  # slot -> generation_step latched by begin_request (frame s reads trailing row gen_step0 + s)
@@ -370,6 +399,37 @@ class Engine:
                                                     arr(*[int(p) for p in pads]), logits.data_ptr(), hidden.data_ptr(),
                                                     self._stream()))
         return logits, hidden
+
+    # -- paged talker KV cache --------------------------------------------------------------------------------
+    def map_kv_pages(self, slot: int, pages):
+        """Set slot's page table: ``pages[i]`` holds its cache rows [64 i, 64 i + 64); an empty list unmaps it."""
+        pages = [int(p) for p in pages]
+        arr = (C.c_int32 * max(len(pages), 1))(*pages)
+        _check(self.lib, self.lib.fq3_map_kv_pages(self.h, int(slot), arr, len(pages)))
+
+    def slot_kv_rows(self, slot: int) -> int:
+        """cache rows slot's pages map"""
+        n = self.lib.fq3_slot_kv_rows(self.h, int(slot))
+        if n < 0:
+            _check(self.lib, n)
+        return n
+
+    def kv_pages_to(self, pages, dst: torch.Tensor):
+        """copy whole pages into ``dst`` (uint8 [len(pages), kv_page_bytes], device or pinned host), stream-ordered"""
+        self._page_copy(self.lib.fq3_kv_pages_to, pages, dst)
+
+    def kv_pages_from(self, pages, src: torch.Tensor):
+        """copy ``src`` (uint8 [len(pages), kv_page_bytes], device or pinned host) into whole pages, stream-ordered"""
+        self._page_copy(self.lib.fq3_kv_pages_from, pages, src)
+
+    def _page_copy(self, fn, pages, mem: torch.Tensor):
+        pages = [int(p) for p in pages]
+        if not (mem.dtype == torch.uint8 and mem.is_contiguous() and mem.numel() == len(pages) * self.kv_page_bytes
+                and (mem.is_cuda or mem.is_pinned())):
+            raise ValueError(f"page memory must be a contiguous uint8 tensor of {len(pages)} x {self.kv_page_bytes} bytes "
+                             "on the device or in pinned host memory")
+        arr = (C.c_int32 * max(len(pages), 1))(*pages)
+        _check(self.lib, fn(self.h, arr, len(pages), mem.data_ptr(), self._stream()))
 
     # -- duck-type path ----------------------------------------------------------------------------------
     def import_kv(self, layer: int, k: torch.Tensor, v: torch.Tensor, slot: int = 0):

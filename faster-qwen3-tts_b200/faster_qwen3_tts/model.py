@@ -256,11 +256,12 @@ class FasterQwen3TTS:
                         quant: str = "BF16", gguf_talker_path=None, gguf_codec_path=None, qwentts_library_path=None,
                         qwentts_use_fa: bool = True, qwentts_clamp_fp16: bool = False, qwentts_ref_cache_dir=None,
                         cache_dir=None, local_files_only: bool = False, max_batch: int = 1,
-                        max_slots: Optional[int] = None):
+                        max_slots: Optional[int] = None, kv_pages: int = 0):
         """Same arguments as the reference (model.py:106-124); trailing and engine-specific: ``max_batch`` = requests one
         launch advances together (> 1 enables the batched persistent kernel / continuous batching, serving.py; <= 32),
         ``max_slots`` = request slots that exist (default ``max_batch``; more serves more paced listeners than a launch
-        has columns, each slot costing its KV cache)."""
+        has columns, each slot costing its KV cache), ``kv_pages`` = a pool of that many 64-row talker KV pages that
+        requests map as they grow, instead of max_seq_len rows reserved per slot (0: the reservation)."""
         if backend not in ("torch", "ggml", "qwentts"):
             raise ValueError(f"Unsupported backend {backend!r}. Expected 'torch', 'ggml', or 'qwentts'.")
         if backend in ("ggml", "qwentts"):
@@ -272,7 +273,7 @@ class FasterQwen3TTS:
             raise ValueError("CUDA graphs require CUDA device")
         if str(model_name).startswith("synthetic:"):
             return cls.from_synthetic(str(model_name).split(":", 1)[1], device=device, dtype=dtype, max_seq_len=max_seq_len,
-                                      max_batch=max_batch, max_slots=max_slots)
+                                      max_batch=max_batch, max_slots=max_slots, kv_pages=kv_pages)
         try:
             from qwen_tts import Qwen3TTSModel
         except ImportError as ex:
@@ -280,17 +281,18 @@ class FasterQwen3TTS:
                               "for random-init weights of the real geometry") from ex
         base = Qwen3TTSModel.from_pretrained(model_name, device_map=device, torch_dtype=dtype,
                                              attn_implementation=attn_implementation)
-        return cls._wrap(base, device, dtype, max_seq_len, max_batch=max_batch, max_slots=max_slots)
+        return cls._wrap(base, device, dtype, max_seq_len, max_batch=max_batch, max_slots=max_slots, kv_pages=kv_pages)
 
     @classmethod
-    def _wrap(cls, base_model, device, dtype, max_seq_len, num_ctas: int = 0, max_batch: int = 1, max_slots=None):
+    def _wrap(cls, base_model, device, dtype, max_seq_len, num_ctas: int = 0, max_batch: int = 1, max_slots=None,
+              kv_pages: int = 0):
         from .predictor_graph import PredictorGraph
         from .talker_graph import TalkerGraph
         from .weights import engine_for_talker
         talker = base_model.model.talker
         tcfg = base_model.model.config.talker_config
         engine = engine_for_talker(talker, dtype=dtype, device=device, max_seq_len=max_seq_len, num_ctas=num_ctas,
-                                   max_batch=max_batch, max_slots=max_slots)
+                                   max_batch=max_batch, max_slots=max_slots, kv_pages=kv_pages)
         pg = PredictorGraph(talker.code_predictor, talker.code_predictor.model.config, tcfg.hidden_size, device=device,
                             dtype=dtype, do_sample=True, top_k=50, temperature=0.9, engine=engine)
         tg = TalkerGraph(talker.model, tcfg, device=device, dtype=dtype, max_seq_len=max_seq_len, engine=engine)
@@ -299,7 +301,8 @@ class FasterQwen3TTS:
     @classmethod
     def from_synthetic(cls, size: str = "1.7B", device: str = "cuda", dtype: torch.dtype = torch.bfloat16,
                        max_seq_len: int = 2048, seed: int = 0, num_ctas: int = 0, with_codec: bool = True,
-                       codec_config=None, max_batch: int = 1, max_slots: Optional[int] = None):
+                       codec_config=None, max_batch: int = 1, max_slots: Optional[int] = None,
+                       kv_pages: int = 0):
         """Random-init weights at the real geometry (no checkpoint exists offline)."""
         from . import synthetic
         from .codec import build_codec
@@ -311,7 +314,7 @@ class FasterQwen3TTS:
         st = build_codec(codec_config, seed=seed + 1, dtype=dtype, device=device) if with_codec else None
         base = synthetic.build_base_model(cfg, None, seed=seed, dtype=dtype, device=device, speech_tokenizer=st)
         base.syn_cfg = cfg
-        m = cls._wrap(base, device, dtype, max_seq_len, num_ctas=num_ctas, max_batch=max_batch, max_slots=max_slots)
+        m = cls._wrap(base, device, dtype, max_seq_len, num_ctas=num_ctas, max_batch=max_batch, max_slots=max_slots, kv_pages=kv_pages)
         return m
 
     def warmup(self, prefill_len: int = 100) -> None:

@@ -64,6 +64,7 @@ class Ticket:
     pace: Optional[float] = None          # a listener playing at pace x real time; None: wants the audio as fast as possible
     lead_s: float = 0.0                   # paced: audio seconds handed over minus seconds played, as of the last step
     underruns: int = 0                    # paced: chunks delivered after the listener had run dry (lead < 0)
+    prepared: Optional[tuple] = None      # (submit arguments, window) of a ticket waiting for KV pages
 
     def cancel(self) -> None:
         """End the request: the worker frees its slot (or drops it from the queue) and closes the ticket."""
@@ -274,13 +275,19 @@ class ContinuousBatcher:
         # text-fed requests enter once their first id is committed (the prompt holds it), in arrival order
         ready = sorted([t for t in self.waiting if t.feed.n_ids] + self._queued, key=lambda t: t.rid)
         many = hasattr(self.sched, "submit_many")
+        admits = getattr(self.sched, "admits", None)   # a paged scheduler: do the prompts' KV pages fit as well
         batch = []   # (ticket, submit arguments, window) admitted together by one submit_many
         for t in ready:
             if (len(batch) >= self.sched.capacity()) if many else not self.sched.has_capacity():
                 break
-            (self.waiting if isinstance(t, TextTicket) else self._queued).remove(t)
+            queue_of = self.waiting if isinstance(t, TextTicket) else self._queued
+            queue_of.remove(t)
             try:   # a bad request must not take the worker down, nor the requests admitted with it
-                req, win = self._prepare(t)
+                req, win = t.prepared or self._prepare(t)
+                if many and admits is not None and not admits([r for _, r, _ in batch] + [req]):
+                    t.prepared = (req, win)   # waits, prompt built, until finished requests free pages
+                    queue_of.append(t)
+                    break
                 if many:
                     batch.append((t, req, win))
                 else:

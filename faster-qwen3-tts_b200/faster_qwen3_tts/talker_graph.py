@@ -48,7 +48,9 @@ class TalkerGraph:
         eng = self._need_engine()
         x = torch.zeros(self.hidden_size, dtype=eng.dtype, device=eng.device)
         pos = min(max(int(prefill_len), 0), self.max_seq_len - 1)
-        for _ in range(max(1, min(int(num_warmup), 1))):
+        # a slot of a paged engine (kv_pages > 0) has no cache rows until a request maps them: its first request loads
+        # the modules instead
+        for _ in range(max(1, min(int(num_warmup), 1)) if not getattr(eng, "paged", False) else 0):
             eng.talker_step(x, pos)
         torch.cuda.synchronize()
         self.captured = True

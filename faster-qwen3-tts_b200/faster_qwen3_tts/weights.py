@@ -99,7 +99,8 @@ def engine_tensors(talker, talker_cfg: dict, pred_cfg: dict, dtype, device, rope
 
 
 def engine_for_talker(talker, dtype=torch.bfloat16, device="cuda", max_seq_len: int = 2048, num_ctas: int = 0,
-                      native_prefill: bool = True, max_batch: int = 1, max_slots=None):
+                      native_prefill: bool = True, max_batch: int = 1, max_slots=None,
+                      kv_pages: int = 0):
     """Build and load an fq3 Engine from the upstream talker module (``base_model.model.talker``)."""
     from .engine import Engine
 
@@ -111,7 +112,7 @@ def engine_for_talker(talker, dtype=torch.bfloat16, device="cuda", max_seq_len: 
                  num_code_groups=int(_cfg_get(tcfg_obj, "num_code_groups", 16)),
                  codec_eos_token_id=int(_cfg_get(tcfg_obj, "codec_eos_token_id")),
                  has_mtp_projection=has_mtp_projection(talker.code_predictor), num_ctas=num_ctas,
-                 max_batch=max_batch, max_slots=max_slots)
+                 max_batch=max_batch, max_slots=max_slots, kv_pages=kv_pages)
     tensors = engine_tensors(talker, tcfg, pcfg, dtype, eng.device, eng.rope_positions)
     eng.load_weights(tensors)
     if dtype == torch.bfloat16 and native_prefill:

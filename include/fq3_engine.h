@@ -61,13 +61,17 @@ typedef struct {
   int32_t rope_positions;   /* rows of the talker cos/sin tables (>= max_seq_len + margin for rope deltas) */
   fq3_stack_config talker;
   fq3_stack_config predictor;
+  int32_t kv_pages;         /* talker KV page pool (see "Paged talker KV cache" below).  0 = max_slots *
+                             * ceil(max_seq_len / 64) pages, slot s mapped for good to its own consecutive run; > 0 = a
+                             * pool of that many pages, every slot unmapped; at least ceil(max_seq_len / 64) */
   int32_t max_batch;        /* columns one launch may carry (slots that advance together); 0/1 = one sequence, <= 32 */
   int32_t max_slots;        /* resident request slots (KV caches + per-request state); 0 = max_batch, else in
                              * [max_batch, FQ3_MAX_SLOTS].  Memory is the bound: fq3_slot_bytes() per slot */
 } fq3_config;
 
 /* Most request slots an engine may hold.  Beyond its memory a slot costs one host record, so the cap follows what an
- * 80 GB card holds: at the 1.7B geometry in bf16, 256 slots of max_seq_len 2048 are 60 GB of talker KV. */
+ * 80 GB card holds: at the 1.7B geometry in bf16, 256 slots of max_seq_len 2048 are 60 GB of talker KV with the
+ * default pool (a smaller kv_pages pool is what a slot then shares). */
 #define FQ3_MAX_SLOTS 256
 
 /* A named tensor handed to fq3_engine_load_weights.  Names (L = layers of that stack, stacked on dim 0):
@@ -132,6 +136,9 @@ int fq3_engine_create(const fq3_config* cfg, fq3_engine** out);
  * hidden, penalty bitmap): the part of fq3_engine_create's allocation that grows with max_slots.  Pure arithmetic, no
  * device needed.  Negative fq3_status when cfg is NULL or its dtype is invalid. */
 int64_t fq3_slot_bytes(const fq3_config* cfg);
+/* Bytes of one talker KV page under `cfg` (2 * L * nKV * 64 * 128 * element size).  Pure arithmetic like
+ * fq3_slot_bytes. */
+int64_t fq3_kv_page_bytes(const fq3_config* cfg);
 /* replaces holding references to the upstream nn.Modules (predictor_graph.py:53-57, talker_graph.py:41):
  * copies norm/embedding tables and repacks every GEMV weight into the per-CTA streaming tape. */
 int fq3_engine_load_weights(fq3_engine* e, const fq3_tensor* tensors, int32_t n, void* stream);
@@ -144,6 +151,25 @@ void fq3_engine_destroy(fq3_engine* e);
  * reference batches left-padded prompts, model.py:774-787, with per-row pad counts, talker_graph.py:177-187).  A
  * column of a launch is a position in slots[], not a slot id: which resident slots a launch carries is the caller's
  * choice from launch to launch, and a slot that is not listed is not touched. */
+
+/* Paged talker KV cache.  The talker's K/V rows live in pages of 64 rows taken from one engine-wide pool of
+ * fq3_kv_pool_pages() pages.  A page is one contiguous block {K [L][nKV][64][128], V [L][nKV][64][128]} in model dtype.
+ * Each slot has a page table: entry i is the page of its cache rows [64 i, 64 i + 64).  With the default pool
+ * (kv_pages = 0) every slot is mapped to its own pages from creation on and nothing below is needed.
+ * fq3_map_kv_pages sets slot's table to pages[0..n) (n <= ceil(max_seq_len / 64); n = 0 unmaps it).  Rows keep their
+ * contents only where an entry keeps its page.  Refused before anything changes: a page outside the pool, a page listed
+ * twice, a page mapped to another slot.  Returns once the table is on the device; no launch that reads the slot may
+ * be in flight.  fq3_slot_kv_rows: the rows the slot's pages map (64 n).
+ * No kernel touches an unmapped row: fq3_prefill[_batch] refuses P beyond the slot's rows, fq3_decode_chunk* a frame
+ * budget whose frames would write past them, fq3_import_kv / fq3_export_kv P beyond them and fq3_talker_step a
+ * position at or beyond them, all with FQ3_ERR_INVALID before launching anything. */
+int fq3_map_kv_pages(fq3_engine* e, int32_t slot, const int32_t* pages, int32_t n);
+int fq3_slot_kv_rows(fq3_engine* e, int32_t slot);
+int fq3_kv_pool_pages(fq3_engine* e);
+/* Whole pages pages[0..n) to / from caller memory (device or pinned host) [n][fq3_kv_page_bytes], stream-ordered,
+ * one copy per page (parking a request's cache off the device).  Refused: a page outside the pool or listed twice. */
+int fq3_kv_pages_to(fq3_engine* e, const int32_t* pages, int32_t n, void* dst, void* stream);
+int fq3_kv_pages_from(fq3_engine* e, const int32_t* pages, int32_t n, const void* src, void* stream);
 
 /* ---- duck-type compatibility path (what the reference's own schedulers call) ----------------------------- */
 /* TalkerGraph.prefill_kv (talker_graph.py:153-170): k,v are [n_kv, P, 128] contiguous for one layer. */

@@ -9,6 +9,8 @@ mean number of slots; a step that finds every listener held launches nothing and
 (wall time of the launches, prefills and codec decodes over the run's wall time) and where the worker's time went.  One
 JSON record per run, each with the card's name, power limit and SM clock read in this process.  Besides the paced runs,
 N = 32 unpaced requests (pace = None: the engine calls of a build without paced listeners) give the reference point.
+``--kv-pages N`` serves the listeners from a pool of N 64-row talker KV pages instead of max_seq_len rows per slot: the
+records then also hold the parks and the most pages in use at once.
 
     python tools/paced_serving_bench.py --listeners 32,64,96,128,160,192 --codec window,stateful --repeats 2 \\
         --out profiles/h100_paced_serving.jsonl
@@ -99,7 +101,8 @@ def run(model, n, codec, first_chunk, seed, stagger_s, chunk, pace=1.0):
             "slots_per_launch_mean": round(step.items / max(step.n, 1), 2),
             "slot_chunks_per_launch_s": round(step.items / max(step.s, 1e-9), 1),
             "decode_step_s": round(step.s, 2), "prefill_s": round(admit.s, 2), "codec_s": round(decode.s, 2),
-            "gpu_busy": round((step.s + admit.s + decode.s) / wall, 3), "max_concurrent": b.max_concurrent}
+            "gpu_busy": round((step.s + admit.s + decode.s) / wall, 3), "max_concurrent": b.max_concurrent,
+            **({"parks": b.sched.pager.parks, "peak_pages": b.sched.pager.peak} if b.sched.pager else {})}
 
 
 def main():
@@ -111,19 +114,26 @@ def main():
     ap.add_argument("--stagger-s", type=float, default=3.0)
     ap.add_argument("--chunk", type=int, default=8)
     ap.add_argument("--size", default="1.7B")
+    ap.add_argument("--kv-pages", type=int, default=0, help="talker KV page pool (0: max_seq_len rows per slot)")
     ap.add_argument("--out", default=os.path.join(ROOT, "profiles", "h100_paced_serving.jsonl"))
     args = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit("paced_serving_bench needs the GPU: a CPU run would measure nothing")
     from faster_qwen3_tts import FasterQwen3TTS
+    from faster_qwen3_tts.batching import KvPager
     from faster_qwen3_tts.engine import slot_bytes
     ns = [int(x) for x in args.listeners.split(",")]
     model = FasterQwen3TTS.from_synthetic(args.size, dtype=torch.bfloat16, max_seq_len=args.max_seq_len, max_batch=32,
-                                          max_slots=max(max(ns), 32))
+                                          max_slots=max(max(ns), 32), kv_pages=args.kv_pages)
     eng = model.engine
     base = {"model": f"synthetic:{args.size} bf16", "max_batch": eng.max_batch, "max_slots": eng.max_slots,
             "max_seq_len": args.max_seq_len,
             "kv_gb": round(eng.max_slots * slot_bytes(eng.talker_cfg, eng.pred_cfg, torch.bfloat16, args.max_seq_len) / 2 ** 30, 2)}
+    if args.kv_pages:   # the talker pool replaces the slots' talker caches
+        talker_kv = KvPager.pages(args.max_seq_len) * eng.kv_page_bytes
+        base.update(kv_pages=eng.kv_pages, kv_gb=round((eng.max_slots * (
+            slot_bytes(eng.talker_cfg, eng.pred_cfg, torch.bfloat16, args.max_seq_len) - talker_kv) +
+            eng.kv_pages * eng.kv_page_bytes) / 2 ** 30, 2))
     run(model, 8, "stateful", None, 0, 0.5, args.chunk)   # warm-up: modules, codec shapes, the prefill path
     run(model, 8, "window", None, 0, 0.5, args.chunk)
     os.makedirs(os.path.dirname(args.out), exist_ok=True)
