@@ -213,18 +213,6 @@ class FasterQwen3TTS:
     def _resolve_non_streaming_mode(non_streaming_mode: Optional[bool], *, default: bool) -> bool:
         return default if non_streaming_mode is None else non_streaming_mode
 
-    @staticmethod
-    def _reject_ggml_cached_reference_args(ref_spk, ref_rvq, ref_spk_emb, ref_codes) -> None:
-        """``.spk`` / ``.rvq`` FILES are qwentts.cpp's own on-disk formats (read by qwentts-cpp-python,
-        ggml_backend.py:476-509): like the reference's torch backend they are refused here with the reference's message
-        (tests/test_voice_clone_prompt_api.py:116-134).  The DECODED form of such a cached reference -- ``ref_spk_emb`` (the
-        speaker vector) and ``ref_codes`` (the reference's codec frames) as arrays -- is accepted, see
-        ``_cached_reference_prompt``."""
-        if any(v is not None for v in (ref_spk, ref_rvq)):
-            raise NotImplementedError(
-                "ref_spk/ref_rvq cached qwentts.cpp references require backend='ggml'. "
-                "Use voice_clone_prompt for precomputed prompts with the torch backend.")
-
     def _cached_reference_prompt(self, ref_spk_emb, ref_codes, voice_clone_prompt):
         """SURVEY 8(f) item 4, in-memory half: a cached reference in decoded form -> the voice_clone_prompt dict the prompt
         builder consumes (what ggml_backend.py:476-509 hands to qwentts.cpp).  ref_spk_emb: [H_talker] floats; ref_codes:
@@ -491,15 +479,21 @@ class FasterQwen3TTS:
         return m, talker, m.config.talker_config, tie, tam, tth, tpe, ref_codes
 
     def _prepare_generation_custom(self, text, language, speaker, instruct=None, non_streaming_mode=True):
-        """Inputs for custom-voice / voice-design requests (model.py:545-581)."""
+        """Inputs for one custom-voice / voice-design request (model.py:545-581): the one-row call of
+        ``_prepare_generation_custom_batch``; voice design has speaker None."""
+        return self._prepare_generation_custom_batch([text], [language], [speaker], [instruct], non_streaming_mode)
+
+    def _prepare_generation_custom_batch(self, texts, languages, speakers, instructs, non_streaming_mode):
+        """Inputs for custom-voice / voice-design requests, one row per text, left-padded like the reference's builder
+        pads a list of requests (model.py:583-805)."""
         from .prompt import build_talker_inputs
-        input_ids = self.model._tokenize_texts([self.model._build_assistant_text(text)])
-        instruct_ids = [None if instruct is None or instruct == "" else
-                        self.model._tokenize_texts([self.model._build_instruct_text(instruct)])[0]]
+        input_ids = self.model._tokenize_texts([self.model._build_assistant_text(t) for t in texts])
+        instruct_ids = [self.model._tokenize_texts([self.model._build_instruct_text(i)])[0] if i else None
+                        for i in instructs]
         m = self.model.model
         tie, tam, tth, tpe = build_talker_inputs(
-            m, input_ids=input_ids, ref_ids=[None], voice_clone_prompt=None,
-            languages=[language] if language is not None else ["Auto"], speakers=[speaker],
+            m, input_ids=input_ids, ref_ids=[None] * len(texts), voice_clone_prompt=None,
+            languages=[l if l is not None else "Auto" for l in languages], speakers=list(speakers),
             non_streaming_mode=non_streaming_mode, instruct_ids=instruct_ids)
         if not self._warmed_up:
             self.warmup(tie.shape[1])
@@ -533,10 +527,10 @@ class FasterQwen3TTS:
             raise ValueError("streaming_codec must be 'window' or 'stateful'")
         return _StreamWindow(self, speech_tokenizer, ref_codes, chunk_size, to_host)
 
-    def _gen_kwargs(self, max_new_tokens, min_new_tokens, temperature, top_k, top_p, do_sample, repetition_penalty):
+    @staticmethod
+    def _gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p, do_sample, repetition_penalty):
         return dict(max_new_tokens=max_new_tokens, min_new_tokens=min_new_tokens, temperature=temperature, top_k=top_k,
-                    top_p=top_p, do_sample=do_sample, repetition_penalty=repetition_penalty,
-                    predictor_graph=self.predictor_graph, talker_graph=self.talker_graph)
+                    top_p=top_p, do_sample=do_sample, repetition_penalty=repetition_penalty)
 
     # ------------------------------------------------------------------ the embeddings-in entry (bench / servers)
     @torch.inference_mode()
@@ -551,6 +545,7 @@ class FasterQwen3TTS:
         chunks = fast_generate_streaming(
             talker=m.talker, talker_input_embeds=tie, attention_mask=tam, trailing_text_hiddens=tth, tts_pad_embed=tpe,
             config=m.config.talker_config, chunk_size=chunk_size, uniforms=uniforms,
+            predictor_graph=self.predictor_graph, talker_graph=self.talker_graph,
             **self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p, do_sample, repetition_penalty))
         st = m.speech_tokenizer
         if st is None:
@@ -579,7 +574,8 @@ class FasterQwen3TTS:
         kw = self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p, do_sample, repetition_penalty)
         for items in fast_generate_streaming_batch(
                 talker=m.talker, talker_input_embeds=tie, attention_mask=tam, trailing_text_hiddens=tth,
-                tts_pad_embed=tpe, config=m.config.talker_config, chunk_size=chunk_size, uniforms=uniforms, **kw):
+                tts_pad_embed=tpe, config=m.config.talker_config, chunk_size=chunk_size, uniforms=uniforms,
+                predictor_graph=self.predictor_graph, talker_graph=self.talker_graph, **kw):
             if wins is None:
                 yield [(b, codes.cpu().numpy() if to_host else codes, self.sample_rate, timing) for b, codes, timing in items]
                 continue
@@ -595,32 +591,13 @@ class FasterQwen3TTS:
         """Concurrent custom-voice requests (BASELINE config 4) sharing every pass over the weights: the prompts are
         batched and left-padded exactly like the reference's builder does for a list of requests (model.py:583-805),
         then decoded together.  Returns ([audio per request], sample_rate)."""
-        from .prompt import build_talker_inputs
-        self._require_type("custom_voice", "Loaded model does not support custom voice generation")
-        n = len(texts)
-        if not (len(speakers) == n and len(languages) == n):
-            raise ValueError("texts, speakers and languages must have the same length")
-        for lang, spk in zip(languages, speakers):
-            self._validate(lang, spk, check_speaker=True)
-        nsm = self._resolve_non_streaming_mode(non_streaming_mode, default=True)
-        instructs = instructs or [None] * n
-        ids = self.model._tokenize_texts([self.model._build_assistant_text(t) for t in texts])
-        ins = []
-        for i in instructs:
-            i = self._drop_instruct_for_small_model(i)
-            ins.append(None if not i else self.model._tokenize_texts([self.model._build_instruct_text(i)])[0])
-        m = self.model.model
-        tie, tam, tth, tpe = build_talker_inputs(m, input_ids=ids, ref_ids=[None] * n, voice_clone_prompt=None,
-                                                 languages=[l if l is not None else "Auto" for l in languages],
-                                                 speakers=list(speakers), non_streaming_mode=nsm, instruct_ids=ins)
-        if not self._warmed_up:
-            self.warmup(tie.shape[1])
-        parts = [[] for _ in range(n)]
+        instructs, nsm = self._custom_voice_rules(texts, languages, speakers, instructs or [None] * len(texts),
+                                                  non_streaming_mode)
+        _, _, _, tie, tam, tth, tpe = self._prepare_generation_custom_batch(texts, languages, speakers, instructs, nsm)
+        parts = [[] for _ in texts]
         sr = self.sample_rate
-        for items in self.stream_batch_from_embeds(tie, tam, tth, tpe, chunk_size=chunk_size,
-                                                   max_new_tokens=max_new_tokens, min_new_tokens=min_new_tokens,
-                                                   temperature=temperature, top_k=top_k, top_p=top_p,
-                                                   do_sample=do_sample, repetition_penalty=repetition_penalty):
+        for items in self.stream_batch_from_embeds(tie, tam, tth, tpe, chunk_size=chunk_size, **self._gen_kwargs(
+                max_new_tokens, min_new_tokens, temperature, top_k, top_p, do_sample, repetition_penalty)):
             for b, audio, sr, _ in items:
                 parts[b].append(audio)
         return [np.concatenate(p) if p else np.zeros(0, dtype=np.float32) for p in parts], sr
@@ -634,24 +611,14 @@ class FasterQwen3TTS:
                              non_streaming_mode: Optional[bool] = None, append_silence: bool = True,
                              instruct: Optional[str] = None, ref_spk=None, ref_rvq=None, ref_spk_emb=None,
                              ref_codes=None, voice_clone_prompt=None) -> Tuple[list, int]:
-        self._reject_ggml_cached_reference_args(ref_spk, ref_rvq, ref_spk_emb, ref_codes)
-        voice_clone_prompt = self._cached_reference_prompt(ref_spk_emb, ref_codes, voice_clone_prompt)
-        from .generate import fast_generate
-        nsm = self._resolve_non_streaming_mode(non_streaming_mode, default=False)
-        m, talker, config, tie, tam, tth, tpe, ref_codes = self._prepare_generation(
+        voice_clone_prompt, nsm = self._voice_clone_rules(voice_clone_prompt, non_streaming_mode, ref_spk, ref_rvq,
+                                                          ref_spk_emb, ref_codes)
+        *prep, ref_codes = self._prepare_generation(
             text=text, language=language, ref_audio=ref_audio, ref_text=ref_text, xvec_only=xvec_only,
             non_streaming_mode=nsm, append_silence=append_silence, voice_clone_prompt=voice_clone_prompt,
             instruct=instruct)
-        codec_ids, timing = fast_generate(
-            talker=talker, talker_input_embeds=tie, attention_mask=tam, trailing_text_hiddens=tth, tts_pad_embed=tpe,
-            config=config, **self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p, do_sample,
-                                              repetition_penalty))
-        if codec_ids is None:
-            logger.warning("Generation returned no tokens")
-            return [np.zeros(1, dtype=np.float32)], self.sample_rate
-        audio, sr = self._decode_all(m.speech_tokenizer, codec_ids, ref_codes)
-        self._log_rtf(timing)
-        return audio, sr
+        return self._one_shot(prep, ref_codes, self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k,
+                                                                top_p, do_sample, repetition_penalty))
 
     @torch.inference_mode()
     def generate_voice_clone_streaming(self, text: str, language: str, ref_audio=None, ref_text: str = "",
@@ -663,25 +630,38 @@ class FasterQwen3TTS:
                                        instruct: Optional[str] = None, ref_spk=None, ref_rvq=None, ref_spk_emb=None,
                                        ref_codes=None, voice_clone_prompt=None
                                        ) -> Generator[Tuple[np.ndarray, int, dict], None, None]:
-        self._reject_ggml_cached_reference_args(ref_spk, ref_rvq, ref_spk_emb, ref_codes)
-        voice_clone_prompt = self._cached_reference_prompt(ref_spk_emb, ref_codes, voice_clone_prompt)
-        nsm = self._resolve_non_streaming_mode(non_streaming_mode, default=False)
+        voice_clone_prompt, nsm = self._voice_clone_rules(voice_clone_prompt, non_streaming_mode, ref_spk, ref_rvq,
+                                                          ref_spk_emb, ref_codes)
         m, talker, config, tie, tam, tth, tpe, ref_codes = self._prepare_generation(
             text=text, language=language, ref_audio=ref_audio, ref_text=ref_text, xvec_only=xvec_only,
             non_streaming_mode=nsm, append_silence=append_silence, voice_clone_prompt=voice_clone_prompt,
             instruct=instruct)
+        gen = self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p, do_sample, repetition_penalty)
         if parity_mode:   # the reference's dynamic-cache baseline (model.py:1064-1077 -> streaming.py:192-359)
             from .streaming import parity_generate_streaming
             chunks = parity_generate_streaming(
                 talker=talker, talker_input_embeds=tie, attention_mask=tam, trailing_text_hiddens=tth, tts_pad_embed=tpe,
-                config=config, max_new_tokens=max_new_tokens, min_new_tokens=min_new_tokens, temperature=temperature,
-                top_k=top_k, top_p=top_p, do_sample=do_sample, repetition_penalty=repetition_penalty, chunk_size=chunk_size)
+                config=config, chunk_size=chunk_size, **gen)
             yield from self._stream_audio(chunks, m.speech_tokenizer, ref_codes, chunk_size)
             return
-        yield from self.stream_from_embeds(tie, tam, tth, tpe, ref_codes=ref_codes, chunk_size=chunk_size,
-                                           max_new_tokens=max_new_tokens, min_new_tokens=min_new_tokens,
-                                           temperature=temperature, top_k=top_k, top_p=top_p, do_sample=do_sample,
-                                           repetition_penalty=repetition_penalty)
+        yield from self.stream_from_embeds(tie, tam, tth, tpe, ref_codes=ref_codes, chunk_size=chunk_size, **gen)
+
+    def _voice_clone_rules(self, voice_clone_prompt, non_streaming_mode, ref_spk=None, ref_rvq=None, ref_spk_emb=None,
+                           ref_codes=None):
+        """What every voice-clone request checks before anything is tokenized -> (voice_clone_prompt, non_streaming_mode
+        with the voice-clone default False).
+
+        ``.spk`` / ``.rvq`` FILES are qwentts.cpp's own on-disk formats (read by qwentts-cpp-python,
+        ggml_backend.py:476-509): like the reference's torch backend they are refused here with the reference's message
+        (tests/test_voice_clone_prompt_api.py:116-134).  The DECODED form of such a cached reference -- ``ref_spk_emb`` (the
+        speaker vector) and ``ref_codes`` (the reference's codec frames) as arrays -- is accepted and becomes the
+        ``voice_clone_prompt``, see ``_cached_reference_prompt``."""
+        if any(v is not None for v in (ref_spk, ref_rvq)):
+            raise NotImplementedError(
+                "ref_spk/ref_rvq cached qwentts.cpp references require backend='ggml'. "
+                "Use voice_clone_prompt for precomputed prompts with the torch backend.")
+        return (self._cached_reference_prompt(ref_spk_emb, ref_codes, voice_clone_prompt),
+                self._resolve_non_streaming_mode(non_streaming_mode, default=False))
 
     # ------------------------------------------------------------------ custom voice / voice design
     def _require_type(self, kind: str, msg: str):
@@ -702,37 +682,50 @@ class FasterQwen3TTS:
             if v is not None:
                 v([speaker])
 
-    def _drop_instruct_for_small_model(self, instruct):
-        """model.py:1166-1167,1251-1252: the 0.6B custom-voice checkpoint ignores instructions"""
+    def _custom_voice_rules(self, texts, languages, speakers, instructs, non_streaming_mode):
+        """What every custom-voice request checks before anything is tokenized: the model type, one speaker and language
+        per text and upstream's validators.  -> (instructs, non_streaming_mode with the custom-voice default True); the
+        0.6B custom-voice checkpoint ignores instructions, so they are dropped (model.py:1166-1167,1251-1252)."""
+        self._require_type("custom_voice", "Loaded model does not support custom voice generation")
+        if not (len(speakers) == len(texts) and len(languages) == len(texts)):
+            raise ValueError("texts, speakers and languages must have the same length")
+        for language, speaker in zip(languages, speakers):
+            self._validate(language, speaker, check_speaker=True)
         size = getattr(self.model.model, "tts_model_size", None)
-        return None if size is not None and size in "0b6" else instruct
+        if size is not None and size in "0b6":
+            instructs = [None] * len(instructs)
+        return instructs, self._resolve_non_streaming_mode(non_streaming_mode, default=True)
 
-    def _simple(self, prep_text, speaker, instruct, language, nsm_default, non_streaming_mode, gen):
-        nsm = self._resolve_non_streaming_mode(non_streaming_mode, default=nsm_default)
-        m, talker, config, tie, tam, tth, tpe = self._prepare_generation_custom(
-            text=prep_text, language=language, speaker=speaker, instruct=instruct, non_streaming_mode=nsm)
-        return m, talker, config, tie, tam, tth, tpe
+    def _voice_design_rules(self, language, non_streaming_mode):
+        """What every voice-design request checks before anything is tokenized -> non_streaming_mode with the
+        voice-design default True."""
+        self._require_type("voice_design", "Loaded model does not support voice design generation")
+        self._validate(language)
+        return self._resolve_non_streaming_mode(non_streaming_mode, default=True)
+
+    def _one_shot(self, prep, ref_codes, gen):
+        """The delivery of the three one-shot methods: generate, then decode every frame at once (model.py:893-947)."""
+        from .generate import fast_generate
+        m, talker, config, tie, tam, tth, tpe = prep
+        codec_ids, timing = fast_generate(
+            talker=talker, talker_input_embeds=tie, attention_mask=tam, trailing_text_hiddens=tth, tts_pad_embed=tpe,
+            config=config, predictor_graph=self.predictor_graph, talker_graph=self.talker_graph, **gen)
+        if codec_ids is None:
+            logger.warning("Generation returned no tokens")
+            return [np.zeros(1, dtype=np.float32)], self.sample_rate
+        audio, sr = self._decode_all(m.speech_tokenizer, codec_ids, ref_codes)
+        self._log_rtf(timing)
+        return audio, sr
 
     @torch.inference_mode()
     def generate_custom_voice(self, text: str, speaker: str, language: str, instruct: Optional[str] = None,
                               non_streaming_mode: Optional[bool] = None, max_new_tokens: int = 2048,
                               min_new_tokens: int = 2, temperature: float = 0.9, top_k: int = 50, top_p: float = 1.0,
                               do_sample: bool = True, repetition_penalty: float = 1.05) -> Tuple[list, int]:
-        self._require_type("custom_voice", "Loaded model does not support custom voice generation")
-        self._validate(language, speaker, check_speaker=True)
-        instruct = self._drop_instruct_for_small_model(instruct)
-        from .generate import fast_generate
-        m, talker, config, tie, tam, tth, tpe = self._simple(text, speaker, instruct, language, True,
-                                                              non_streaming_mode, None)
-        codec_ids, timing = fast_generate(
-            talker=talker, talker_input_embeds=tie, attention_mask=tam, trailing_text_hiddens=tth, tts_pad_embed=tpe,
-            config=config, **self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p, do_sample,
-                                              repetition_penalty))
-        if codec_ids is None:
-            return [np.zeros(1, dtype=np.float32)], self.sample_rate
-        audio, sr = self._decode_all(m.speech_tokenizer, codec_ids, None)
-        self._log_rtf(timing)
-        return audio, sr
+        (instruct,), nsm = self._custom_voice_rules([text], [language], [speaker], [instruct], non_streaming_mode)
+        prep = self._prepare_generation_custom(text, language, speaker, instruct, nsm)
+        return self._one_shot(prep, None, self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p,
+                                                           do_sample, repetition_penalty))
 
     @torch.inference_mode()
     def generate_custom_voice_streaming(self, text: str, speaker: str, language: str, instruct: Optional[str] = None,
@@ -740,38 +733,20 @@ class FasterQwen3TTS:
                                         min_new_tokens: int = 2, temperature: float = 0.9, top_k: int = 50,
                                         top_p: float = 1.0, do_sample: bool = True, repetition_penalty: float = 1.05,
                                         chunk_size: int = 12) -> Generator[Tuple[np.ndarray, int, dict], None, None]:
-        self._require_type("custom_voice", "Loaded model does not support custom voice generation")
-        self._validate(language, speaker, check_speaker=True)
-        instruct = self._drop_instruct_for_small_model(instruct)
-        m, talker, config, tie, tam, tth, tpe = self._simple(text, speaker, instruct, language, True,
-                                                              non_streaming_mode, None)
-        yield from self.stream_from_embeds(tie, tam, tth, tpe, ref_codes=None, chunk_size=chunk_size,
-                                           max_new_tokens=max_new_tokens, min_new_tokens=min_new_tokens,
-                                           temperature=temperature, top_k=top_k, top_p=top_p, do_sample=do_sample,
-                                           repetition_penalty=repetition_penalty)
+        (instruct,), nsm = self._custom_voice_rules([text], [language], [speaker], [instruct], non_streaming_mode)
+        _, _, _, tie, tam, tth, tpe = self._prepare_generation_custom(text, language, speaker, instruct, nsm)
+        yield from self.stream_from_embeds(tie, tam, tth, tpe, chunk_size=chunk_size, **self._gen_kwargs(
+            max_new_tokens, min_new_tokens, temperature, top_k, top_p, do_sample, repetition_penalty))
 
     @torch.inference_mode()
     def generate_voice_design(self, text: str, instruct: str, language: str,
                               non_streaming_mode: Optional[bool] = None, max_new_tokens: int = 2048,
                               min_new_tokens: int = 2, temperature: float = 0.9, top_k: int = 50, top_p: float = 1.0,
                               do_sample: bool = True, repetition_penalty: float = 1.05) -> Tuple[list, int]:
-        self._require_type("voice_design", "Loaded model does not support voice design generation")
-        self._validate(language)
-        return self._design_impl(text, instruct, language, non_streaming_mode, max_new_tokens, min_new_tokens,
-                                 temperature, top_k, top_p, do_sample, repetition_penalty)
-
-    def _design_impl(self, text, instruct, language, non_streaming_mode, max_new_tokens, min_new_tokens, temperature,
-                     top_k, top_p, do_sample, repetition_penalty):
-        from .generate import fast_generate
-        m, talker, config, tie, tam, tth, tpe = self._simple(text, None, instruct, language, True, non_streaming_mode,
-                                                              None)
-        codec_ids, timing = fast_generate(
-            talker=talker, talker_input_embeds=tie, attention_mask=tam, trailing_text_hiddens=tth, tts_pad_embed=tpe,
-            config=config, **self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p, do_sample,
-                                              repetition_penalty))
-        if codec_ids is None:
-            return [np.zeros(1, dtype=np.float32)], self.sample_rate
-        return self._decode_all(m.speech_tokenizer, codec_ids, None)
+        nsm = self._voice_design_rules(language, non_streaming_mode)
+        prep = self._prepare_generation_custom(text, language, None, instruct, nsm)
+        return self._one_shot(prep, None, self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p,
+                                                           do_sample, repetition_penalty))
 
     @torch.inference_mode()
     def generate_voice_design_streaming(self, text: str, instruct: str, language: str,
@@ -779,14 +754,10 @@ class FasterQwen3TTS:
                                         min_new_tokens: int = 2, temperature: float = 0.9, top_k: int = 50,
                                         top_p: float = 1.0, do_sample: bool = True, repetition_penalty: float = 1.05,
                                         chunk_size: int = 12) -> Generator[Tuple[np.ndarray, int, dict], None, None]:
-        self._require_type("voice_design", "Loaded model does not support voice design generation")
-        self._validate(language)
-        m, talker, config, tie, tam, tth, tpe = self._simple(text, None, instruct, language, True, non_streaming_mode,
-                                                              None)
-        yield from self.stream_from_embeds(tie, tam, tth, tpe, ref_codes=None, chunk_size=chunk_size,
-                                           max_new_tokens=max_new_tokens, min_new_tokens=min_new_tokens,
-                                           temperature=temperature, top_k=top_k, top_p=top_p, do_sample=do_sample,
-                                           repetition_penalty=repetition_penalty)
+        nsm = self._voice_design_rules(language, non_streaming_mode)
+        _, _, _, tie, tam, tth, tpe = self._prepare_generation_custom(text, language, None, instruct, nsm)
+        yield from self.stream_from_embeds(tie, tam, tth, tpe, chunk_size=chunk_size, **self._gen_kwargs(
+            max_new_tokens, min_new_tokens, temperature, top_k, top_p, do_sample, repetition_penalty))
 
     # ------------------------------------------------------------------ several takes of one request
     def _check_takes(self, n_takes, seeds):
@@ -867,15 +838,14 @@ class FasterQwen3TTS:
         holds "logprobs" (float32 [T,16], the log-probability of every code), "eos_logprob", "total_logprob" (their sum,
         EOS term included), "frames" and "seed".  A log-probability says how likely the sampler found its draws, not
         how good the audio is: the calls rank nothing and pick nothing."""
+        voice_clone_prompt, nsm = self._voice_clone_rules(voice_clone_prompt, non_streaming_mode)
         seeds = self._check_takes(n_takes, seeds)
-        nsm = self._resolve_non_streaming_mode(non_streaming_mode, default=False)
-        m, talker, config, tie, tam, tth, tpe, ref_codes = self._prepare_generation(
+        *prep, ref_codes = self._prepare_generation(
             text=text, language=language, ref_audio=ref_audio, ref_text=ref_text, xvec_only=xvec_only,
             non_streaming_mode=nsm, append_silence=append_silence, voice_clone_prompt=voice_clone_prompt,
             instruct=instruct)
-        return self._takes((m, talker, config, tie, tam, tth, tpe), ref_codes, seeds,
-                           self._text_gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p, do_sample,
-                                                 repetition_penalty))
+        return self._takes(prep, ref_codes, seeds, self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k,
+                                                                    top_p, do_sample, repetition_penalty))
 
     @torch.inference_mode()
     def generate_custom_voice_takes(self, text: str, speaker: str, language: str, instruct: Optional[str] = None,
@@ -884,13 +854,11 @@ class FasterQwen3TTS:
                                     top_p: float = 1.0, do_sample: bool = True, repetition_penalty: float = 1.05,
                                     n_takes: int = 4, seeds: Optional[List[int]] = None):
         """``n_takes`` renderings of one ``generate_custom_voice`` request (see ``generate_voice_clone_takes``)."""
-        self._require_type("custom_voice", "Loaded model does not support custom voice generation")
-        self._validate(language, speaker, check_speaker=True)
+        (instruct,), nsm = self._custom_voice_rules([text], [language], [speaker], [instruct], non_streaming_mode)
         seeds = self._check_takes(n_takes, seeds)
-        instruct = self._drop_instruct_for_small_model(instruct)
-        prep = self._simple(text, speaker, instruct, language, True, non_streaming_mode, None)
-        return self._takes(prep, None, seeds, self._text_gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k,
-                                                                     top_p, do_sample, repetition_penalty))
+        prep = self._prepare_generation_custom(text, language, speaker, instruct, nsm)
+        return self._takes(prep, None, seeds, self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k,
+                                                               top_p, do_sample, repetition_penalty))
 
     @torch.inference_mode()
     def generate_voice_design_takes(self, text: str, instruct: str, language: str,
@@ -899,17 +867,17 @@ class FasterQwen3TTS:
                                     top_p: float = 1.0, do_sample: bool = True, repetition_penalty: float = 1.05,
                                     n_takes: int = 4, seeds: Optional[List[int]] = None):
         """``n_takes`` renderings of one ``generate_voice_design`` request (see ``generate_voice_clone_takes``)."""
-        self._require_type("voice_design", "Loaded model does not support voice design generation")
-        self._validate(language)
+        nsm = self._voice_design_rules(language, non_streaming_mode)
         seeds = self._check_takes(n_takes, seeds)
-        prep = self._simple(text, None, instruct, language, True, non_streaming_mode, None)
-        return self._takes(prep, None, seeds, self._text_gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k,
-                                                                     top_p, do_sample, repetition_penalty))
+        prep = self._prepare_generation_custom(text, language, None, instruct, nsm)
+        return self._takes(prep, None, seeds, self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k,
+                                                               top_p, do_sample, repetition_penalty))
 
     # ------------------------------------------------------------------ incremental text input (text_stream.py)
     def _text_streaming(self, text_stream, language, speaker, instruct, voice_clone_prompt, non_streaming_mode,
                         chunk_size, gen):
-        """The one implementation behind the three ``*_text_streaming`` methods."""
+        """The one implementation behind the three ``*_text_streaming`` methods.  Text streaming has one text layout,
+        so the raw ``non_streaming_mode`` is checked here, not the voice kind's default."""
         from .text_stream import _refuse_unsupported, generate_text_streaming
         _refuse_unsupported(voice_clone_prompt, non_streaming_mode)
         instruct_ids = None
@@ -930,12 +898,10 @@ class FasterQwen3TTS:
         ``str`` pieces (an LLM's reply token by token).  The audio equals that of the one-shot streaming request for the
         same text, whatever the split and however fast the pieces come; generation waits where the text has not arrived
         yet.  Timing dicts add ``text_wait_ms``, the time spent blocked on ``text_stream``."""
-        self._require_type("custom_voice", "Loaded model does not support custom voice generation")
-        self._validate(language, speaker, check_speaker=True)
-        instruct = self._drop_instruct_for_small_model(instruct)
+        (instruct,), _ = self._custom_voice_rules([text_stream], [language], [speaker], [instruct], non_streaming_mode)
         yield from self._text_streaming(text_stream, language, speaker, instruct, None, non_streaming_mode, chunk_size,
-                                        self._text_gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p,
-                                                              do_sample, repetition_penalty))
+                                        self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p,
+                                                         do_sample, repetition_penalty))
 
     @torch.inference_mode()
     def generate_voice_design_text_streaming(self, text_stream, instruct: str, language: str,
@@ -946,11 +912,10 @@ class FasterQwen3TTS:
                                              ) -> Generator[Tuple[np.ndarray, int, dict], None, None]:
         """``generate_voice_design_streaming`` with the text fed while it is spoken (see
         ``generate_custom_voice_text_streaming``)."""
-        self._require_type("voice_design", "Loaded model does not support voice design generation")
-        self._validate(language)
+        self._voice_design_rules(language, non_streaming_mode)
         yield from self._text_streaming(text_stream, language, None, instruct, None, non_streaming_mode, chunk_size,
-                                        self._text_gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p,
-                                                              do_sample, repetition_penalty))
+                                        self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p,
+                                                         do_sample, repetition_penalty))
 
     @torch.inference_mode()
     def generate_voice_clone_text_streaming(self, text_stream, language: str, ref_audio=None, ref_text: str = "",
@@ -964,8 +929,8 @@ class FasterQwen3TTS:
         """``generate_voice_clone_streaming`` with the text fed while it is spoken, x-vector cloning only: ICL cloning
         puts the target text under the reference codec frames inside the prompt, so it must be known before prefill
         (ValueError)."""
-        self._reject_ggml_cached_reference_args(ref_spk, ref_rvq, ref_spk_emb, ref_codes)
-        voice_clone_prompt = self._cached_reference_prompt(ref_spk_emb, ref_codes, voice_clone_prompt)
+        voice_clone_prompt, _ = self._voice_clone_rules(voice_clone_prompt, non_streaming_mode, ref_spk, ref_rvq,
+                                                        ref_spk_emb, ref_codes)
         from .text_stream import ICL_REFUSAL, _refuse_unsupported
         _refuse_unsupported(None, non_streaming_mode)
         if voice_clone_prompt is None and not xvec_only:
@@ -974,15 +939,9 @@ class FasterQwen3TTS:
         vcp, _, _ = self._resolve_voice_clone_prompt(
             input_ids=[None], ref_audio=ref_audio, ref_text=ref_text, xvec_only=True, append_silence=append_silence,
             voice_clone_prompt=voice_clone_prompt)
-        _refuse_unsupported(vcp, non_streaming_mode)
         yield from self._text_streaming(text_stream, language, None, None, vcp, non_streaming_mode, chunk_size,
-                                        self._text_gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p,
-                                                              do_sample, repetition_penalty))
-
-    @staticmethod
-    def _text_gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p, do_sample, repetition_penalty):
-        return dict(max_new_tokens=max_new_tokens, min_new_tokens=min_new_tokens, temperature=temperature, top_k=top_k,
-                    top_p=top_p, do_sample=do_sample, repetition_penalty=repetition_penalty)
+                                        self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p,
+                                                         do_sample, repetition_penalty))
 
     def _log_rtf(self, timing):
         n = timing["steps"]

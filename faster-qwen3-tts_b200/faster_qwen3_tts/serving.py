@@ -394,9 +394,7 @@ def custom_voice_text_request(model, speaker: str, language: str, instruct: Opti
     """``prepare`` callable for ``ContinuousBatcher.submit_text``: the prompt of a text-fed custom-voice request, built
     from the feed's first committed id exactly like ``generate_custom_voice_text_streaming`` builds it."""
     from .text_stream import build_prompt
-    model._require_type("custom_voice", "Loaded model does not support custom voice generation")
-    model._validate(language, speaker, check_speaker=True)
-    instruct = model._drop_instruct_for_small_model(instruct)
+    (instruct,), _ = model._custom_voice_rules([None], [language], [speaker], [instruct], None)   # text: from the feed
 
     def prepare(feed):
         ins = model.model._tokenize_texts([model.model._build_instruct_text(instruct)])[0] if instruct else None

@@ -46,7 +46,7 @@ def _streamed(m, prep, ref_codes, seed, gen):
                                                        ("voice_clone_icl", "window", True),
                                                        ("custom_voice", "stateful", True),
                                                        ("voice_clone_icl", "stateful", False)])
-def test_take_equals_the_request_run_alone(kind, codec_mode, fixed_len, monkeypatch):
+def test_each_take_equals_the_request_run_alone(kind, codec_mode, fixed_len, monkeypatch):
     # the ICL prompt crosses 192 cached keys while generating: from there a lone request's single-sequence kernel would
     # switch to its split-key attention, which the batched kernel does not have (as in test_gpu_serving.py)
     monkeypatch.setenv("FQ3_ATTN_SPLIT", "0")
@@ -63,7 +63,7 @@ def test_take_equals_the_request_run_alone(kind, codec_mode, fixed_len, monkeypa
         spk = "ryan"
         audios, sr, scores = m.generate_custom_voice_takes(TEXT, spk, "English", n_takes=4, seeds=seeds, **gen)
         with torch.inference_mode():
-            prep = m._simple(TEXT, spk, None, "English", True, None, None)
+            prep = m._prepare_generation_custom(TEXT, "English", spk)
         ref_codes = None
     else:
         audios, sr, scores = m.generate_voice_clone_takes(TEXT, "English", ref_audio="ref.wav", ref_text="ref words",

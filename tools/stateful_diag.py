@@ -32,6 +32,7 @@ def one(mode):
     sync(); t.append(time.perf_counter())
     chunks = fast_generate_streaming(talker=m.talker, talker_input_embeds=tie, attention_mask=tam, trailing_text_hiddens=tth,
                                      tts_pad_embed=tpe, config=m.config.talker_config, chunk_size=8,
+                                     predictor_graph=model.predictor_graph, talker_graph=model.talker_graph,
                                      **model._gen_kwargs(64, 64, 0.9, 50, 1.0, True, 1.05))
     codes, tm = next(chunks)
     sync(); t.append(time.perf_counter())
