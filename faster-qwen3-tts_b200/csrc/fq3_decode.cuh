@@ -27,6 +27,8 @@
 
 #include <type_traits>
 
+#include "../../include/fq3_engine.h"   // enum fq3_finish: the finish codes the kernels write
+
 namespace fq3 {
 
 constexpr int NCW = 8;               // consumer warps
@@ -90,13 +92,17 @@ __host__ __device__ __forceinline__ uint8_t* kv_row(void* pool, int L, int nKV, 
          ((size_t)(layer * nKV + g) * KV_PAGE + t % KV_PAGE) * 128 * esz;
 }
 
+// a request's loop state: the words of SlotParams::state (and of Smem::bst, the batched kernel's copy).  finished holds
+// an fq3_finish code; emitted counts the frames of the last launch.
+enum StateWord { ST_TOKEN = 0, ST_STEP = 1, ST_GEN = 2, ST_FIN = 3, ST_EMIT = 4, ST_WORDS = 5 };
+
 // one request: its caches, decode state and parameters.  The single-sequence kernel reads it from KParams::req, the
 // batched kernel one per column from KParams::sl.
 struct SlotParams {
   void* kv;             // the engine's talker KV page pool (kv_row)
   const int* kv_pages;  // this slot's page table [ceil(max_seq_len / KV_PAGE)]
   void *pkc, *pvc;      // predictor KV cache of this slot [Lp][nKVp][32][128]
-  int* state;           // [0] token [1] step [2] gen_step [3] finished [4] emitted(last launch)
+  int* state;           // [ST_WORDS] StateWord
   float* past_hidden;   // [HMAX] fp32 holding dtype-rounded values
   uint32_t* seen;       // [VMAX/32] bitmap of cb0 history (sampling.py:22 unique())
   const void* trailing;
@@ -106,7 +112,7 @@ struct SlotParams {
   float* logprob_out;   // [n_frames][16] or nullptr: col k >= 1 = codebook k of the frame, col 0 = the cb0 sampled after it
   int prefill_len, rope_delta, n_left_pad, max_new, min_new, trailing_len;
   int text_open;        // more trailing rows may follow: a frame that would read row >= trailing_len waits (stops the slot)
-  int n_frames;         // batched kernel: frames this slot may emit in the launch (the single-sequence one reads KParams::n_frames)
+  int n_frames;         // frames this request may emit in the launch
   Sampling sp_t, sp_p;
 };
 
@@ -127,7 +133,7 @@ struct KParams {
   const void* mtp_tab;   // [ncb][Vp][Hp] = mtp(embeds[i][code]) precomputed at load time (has_mtp only)
   int has_mtp, ncb, eos, max_seq_len;
   SlotParams req;        // single-sequence kernel: the request of this launch
-  int n_frames;
+  int n_frames;          // MODE_FUSED: the producer's frame bound (no request of the launch runs longer)
   const void* in_embeds;
   void* hidden_out;
   int position;
@@ -247,7 +253,7 @@ struct __align__(128) Smem {
   int stop_flag;            // consumers -> producer
   int prod_done;            // producer -> consumers
   int prod_issued;          // tiles issued by the producer
-  int bst[5][32];           // batched kernel: replicated per-column loop state (token, step, gen_step, finished, emitted)
+  int bst[ST_WORDS][32];    // batched kernel: replicated per-column loop state
   long long prof[12];       // batched kernel, CTA 0 / thread 0: [0] last clock [1] current category [2..] cycles per category
   int runl[36];             // batched kernel: columns running in the current (sub)frame, ascending; [32] = their number
   int kvtab[SEQMAX / KV_PAGE];   // page table of the request being attended to: the single-sequence kernel's, read
@@ -448,29 +454,31 @@ struct Producer {
     __threadfence_block();
     flag_st(&s.prod_done, 1);
   }
-  __device__ __forceinline__ void seg(int sg) {
+  // segment sg, `rep` times over (the batched kernel replays a segment once per column block, see gemv_b)
+  __device__ __forceinline__ void seg(int sg, int rep = 1) {
     if (stopped) return;
     const uint32_t st = s.seg[sg];
     const int gbeg = (int)(st >> 8), gn = (int)(st & 255u);
-    for (int gi = 0; gi < gn; ++gi) {
-      const Grp g = s.grp[gbeg + gi];
-      // fp32 tape: rows x m x 512-byte row chunks; bf16 tape: n_mt x G k-groups x 2048-byte fragment blocks
-      const uint32_t bytes = BF ? (uint32_t)(g.rows & 0xff) * g.m * 2048u : (uint32_t)g.rows * g.m * 512u;
-      const uint8_t* src = P.tape + (size_t)g.off16 * 16;
-      for (int tl = 0; tl < g.ntiles; ++tl) {
-        const int stage = (int)(ctr % NS);
-        const uint32_t par = ((ctr / NS) & 1u) ^ 1u;
-        while (!mbar_try_wait(&s.empty[stage], par)) {
-          if (flag_ld(&s.stop_flag)) {
-            stopped = true;
-            return;
+    for (int r = 0; r < rep; ++r)
+      for (int gi = 0; gi < gn; ++gi) {
+        const Grp g = s.grp[gbeg + gi];
+        // fp32 tape: rows x m x 512-byte row chunks; bf16 tape: n_mt x G k-groups x 2048-byte fragment blocks
+        const uint32_t bytes = BF ? (uint32_t)(g.rows & 0xff) * g.m * 2048u : (uint32_t)g.rows * g.m * 512u;
+        const uint8_t* src = P.tape + (size_t)g.off16 * 16;
+        for (int tl = 0; tl < g.ntiles; ++tl) {
+          const int stage = (int)(ctr % NS);
+          const uint32_t par = ((ctr / NS) & 1u) ^ 1u;
+          while (!mbar_try_wait(&s.empty[stage], par)) {
+            if (flag_ld(&s.stop_flag)) {
+              stopped = true;
+              return;
+            }
           }
+          mbar_expect_tx(&s.full[stage], bytes);
+          bulk_g2s_hint(s.ring[stage], src + (size_t)tl * bytes, bytes, &s.full[stage], pol_first);
+          ++ctr;
         }
-        mbar_expect_tx(&s.full[stage], bytes);
-        bulk_g2s_hint(s.ring[stage], src + (size_t)tl * bytes, bytes, &s.full[stage], pol_first);
-        ++ctr;
       }
-    }
   }
   // K/V rows of this CTA's key slice of layer l -> ring tiles (issued right behind the layer's QKV weights, so they
   // land while the QKV GEMV and its barrier are still in flight).  Must mirror attention_split().
@@ -507,13 +515,29 @@ struct Producer {
     }
   }
   // kv_slot0 >= 0: talker step at cache slot kv_slot0 with split attention
-  __device__ __forceinline__ void stack_layers(const StackDev& S, int kv_slot0 = -1, int kv_start = 0) {
+  __device__ __forceinline__ void stack_layers(const StackDev& S, int rep = 1, int kv_slot0 = -1, int kv_start = 0) {
     for (int l = 0; l < S.L; ++l)
       for (int q = 0; q < 4; ++q) {
-        seg(S.seg_base + 4 * l + q);
+        seg(S.seg_base + 4 * l + q, rep);
         if (BF && q == 0 && kv_slot0 >= 0 && P.attn_split > 0 && kv_slot0 - kv_start >= ATTN_SPLIT_MIN)
           kv_tiles(S, l, kv_slot0, kv_start);
       }
+  }
+  // the code predictor's 15 passes: the MTP projection (pass 0), then per pass its layers and head.  rep0 / rep1: the
+  // replays of pass 0's segments and of the 1-column segments (pass 0 carries two tokens per request)
+  __device__ __forceinline__ void predictor(int rep0, int rep1) {
+    for (int i = 0; i < P.ncb; ++i) {
+      if (P.has_mtp && i == 0) seg(P.seg_mtp, rep0);
+      stack_layers(P.p, i == 0 ? rep0 : rep1);
+      seg(P.p.seg_head + i, rep1);
+    }
+  }
+  // one frame of a fused launch, the order both decode kernels consume it in: the predictor, then the talker step at
+  // cache slot kv_slot0 (-1: no split attention) and its head
+  __device__ __forceinline__ void frame(int rep0, int rep1, int kv_slot0, int kv_start) {
+    predictor(rep0, rep1);
+    stack_layers(P.t, rep1, kv_slot0, kv_start);
+    seg(P.t.seg_head, rep1);
   }
 };
 
@@ -1759,6 +1783,41 @@ __device__ __forceinline__ void head_logits(Ctx& c, int seg, int H) {
   grid_sync(c);
 }
 
+// ------------------------------------------------------------------------------------------------------------
+// Rules of a frame (generate.py:149-199) that both fq3_decode_kernel and fq3_decode_batch_kernel call.  The stop gate,
+// the uniform row, the predictor pass inputs and draws, the talker input and the max_seq_len rule stay written out in
+// each kernel: as calls, they raise the spills of one kernel or the other (DESIGN §4).
+// ------------------------------------------------------------------------------------------------------------
+// the talker's draw (generate.py:46-50): repetition penalty over the seen history; suppress_special: the ids
+// [V - 1024, V) other than eos are never drawn; suppress_eos: nor is eos
+__device__ __forceinline__ SampleArgs talker_draw(const float* logits, int V, const Sampling& sp, float u,
+                                                  bool suppress_special, int eos, bool suppress_eos, float* lp) {
+  SampleArgs a;
+  a.logits = logits; a.V = V; a.sp = sp; a.u = u;
+  a.use_penalty = true; a.sup0 = suppress_special ? (V > 1024 ? V - 1024 : 0) : V;
+  a.suppress_eos = suppress_eos; a.eos = eos;
+  a.lp = lp;
+  return a;
+}
+// ... of frame `step` of request sp: uniform urow[0], eos held back for the first min_new frames; it writes column 0
+// of the frame's log-probability row (the cb0 that follows the frame)
+__device__ __forceinline__ SampleArgs frame_talker_draw(const KParams& P, const SlotParams& sp, const float* logits,
+                                                        const float* urow, int step, float* lp_row) {
+  return talker_draw(logits, P.t.V, sp.sp_t, (sp.sp_t.do_sample && urow) ? __ldg(urow) : 0.f, true, P.eos,
+                     step + 1 < sp.min_new, lp_row);
+}
+
+// after the talker's draw: its cb0 starts the next frame
+__device__ __forceinline__ void frame_advance(int& token, int& step, int& gen_step, int next) {
+  token = next;
+  ++step;
+  ++gen_step;
+}
+
+__device__ __forceinline__ void put_state(int* st, int token, int step, int gen_step, int finished, int emitted) {
+  st[ST_TOKEN] = token; st[ST_STEP] = step; st[ST_GEN] = gen_step; st[ST_FIN] = finished; st[ST_EMIT] = emitted;
+}
+
 // predictor: 15 passes (predictor_graph.py:115-167).  Inputs: s.xin[0] = past_hidden, s.xin[1] = embed(cb0 token).
 // Outputs s.codes[1..15].  u15: 15 uniforms.  lp_row: the frame's log-probability row (pass i -> column i + 1) or nullptr.
 // A real function that works on a private copy of the caller's Ctx and hands the advanced counters back at the end.
@@ -1831,22 +1890,11 @@ __device__ __noinline__ void producer_main(const KParams& P) {
   const int lane = (int)(threadIdx.x & 31u);
   if (lane == 0) {
     Producer<BF> pr(P);
-    if (P.mode == MODE_TALKER_STEP) {
-      pr.stack_layers(P.t, P.position, P.req.n_left_pad);
-    } else {
-      const int iters = P.mode == MODE_FUSED ? P.n_frames : 1;
-      for (int f = 0; f < iters && !pr.stopped; ++f) {
-        for (int i = 0; i < P.ncb; ++i) {
-          if (P.has_mtp && i == 0) pr.seg(P.seg_mtp);
-          pr.stack_layers(P.p);
-          pr.seg(P.p.seg_head + i);
-        }
-        if (P.mode == MODE_FUSED) {
-          pr.stack_layers(P.t, P.req.prefill_len + P.req.state[1] + f, P.req.n_left_pad);
-          pr.seg(P.t.seg_head);
-        }
-      }
-    }
+    if (P.mode == MODE_TALKER_STEP) pr.stack_layers(P.t, 1, P.position, P.req.n_left_pad);
+    else if (P.mode == MODE_PRED_RUN) pr.predictor(1, 1);
+    else
+      for (int f = 0; f < P.n_frames && !pr.stopped; ++f)
+        pr.frame(1, 1, P.req.prefill_len + P.req.state[ST_STEP] + f, P.req.n_left_pad);
     pr.finish();
   }
 }
@@ -1925,14 +1973,14 @@ __global__ void __launch_bounds__(NTHREADS, 1) fq3_decode_kernel(const __grid_co
       if (cta == 0 && tid < P.ncb) rq.codes_out[tid] = (long long)s.codes[tid + 1];
     } else {
       // ---------------- fused frame loop: generate.py:149-199 / streaming.py:106-173 ----------------
-      int token = rq.state[0], step = rq.state[1], gen_step = rq.state[2];
-      int finished = 0, emitted = 0;
+      int token = rq.state[ST_TOKEN], step = rq.state[ST_STEP], gen_step = rq.state[ST_GEN];
+      int finished = FQ3_RUNNING, emitted = 0;
       for (int k = tid; k < Ht; k += NCT) s.hid[k] = rq.past_hidden[k];
       csync();
       while (true) {
-        if (emitted >= P.n_frames) break;
-        if (step >= rq.max_new) { finished = 1; break; }
-        if (token == P.eos) { finished = 2; break; }
+        if (emitted >= rq.n_frames) break;
+        if (step >= rq.max_new) { finished = FQ3_FIN_MAX_NEW; break; }
+        if (token == P.eos) { finished = FQ3_FIN_EOS; break; }
         // open text: this frame's talker step reads trailing row gen_step; stop unfinished before touching any state
         if (rq.text_open && gen_step >= rq.trailing_len) break;
         // predictor input: cat(past_hidden, codec_embedding(token))   generate.py:154-155
@@ -1982,7 +2030,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) fq3_decode_kernel(const __grid_co
           csync();
         }
         const int pos = rq.prefill_len + step;
-        if (pos >= P.max_seq_len - 1) { finished = 3; step++; break; }   // generate.py:175-177 (frame already emitted)
+        // generate.py:175-177 (the frame is already emitted)
+        if (pos >= P.max_seq_len - 1) { finished = FQ3_FIN_MAX_SEQ; step++; break; }
         probe_at(c, pslot + 2);
         run_layers<BF, true>(c, P.t, 1, pos, pos + rq.rope_delta, rq.n_left_pad, true, false);
         probe_at(c, pslot + 3);
@@ -1990,20 +2039,12 @@ __global__ void __launch_bounds__(NTHREADS, 1) fq3_decode_kernel(const __grid_co
         csync();
         head_logits<BF>(c, P.t.seg_head, Ht);
         probe_at(c, pslot + 4);
-        SampleArgs sa;
-        sa.logits = P.LOGITS; sa.V = P.t.V; sa.sp = rq.sp_t; sa.u = rq.sp_t.do_sample ? __ldg(urow) : 0.f;
-        sa.use_penalty = true; sa.sup0 = P.t.V > 1024 ? P.t.V - 1024 : 0;
-        sa.suppress_eos = (step + 1) < rq.min_new; sa.eos = P.eos;
-        sa.lp = lp_row;   // column 0: the cb0 that follows this frame (next frame's, or EOS)
-        token = sample_block<BF>(c, sa);
+        const int next = sample_block<BF>(c, frame_talker_draw(P, rq, P.LOGITS, urow, step, lp_row));
         probe_at(c, pslot + 5);
-        step++;
-        gen_step++;
+        frame_advance(token, step, gen_step, next);
       }
       if (cta == 0) {
-        if (tid == 0) {
-          rq.state[0] = token; rq.state[1] = step; rq.state[2] = gen_step; rq.state[3] = finished; rq.state[4] = emitted;
-        }
+        if (tid == 0) put_state(rq.state, token, step, gen_step, finished, emitted);
         for (int k = tid; k < Ht; k += NCT) rq.past_hidden[k] = s.hid[k];
         for (int i = tid; i < VMAX / 32; i += NCT) rq.seen[i] = s.seen[i];
       }

@@ -5,7 +5,8 @@
 // Same tape, same producer warp / TMA ring, same grid barrier and the same per-element arithmetic (rounding points,
 // accumulation order inside a warp, cross-warp summation order) as the single-sequence kernel in fq3_decode.cuh: row b
 // of a batched launch produces bit-for-bit the codes a single-sequence launch produces for that request (tested).  The
-// attention functions and the fp32 GEMV are the single-sequence kernel's own, called with this slot's pointers.
+// attention functions, the fp32 GEMV, the talker's draw arguments, the step advance, the state record and the
+// producer's frame walk are the single-sequence kernel's own, called with this slot's pointers.
 //
 // What changes with B > 1:
 //   * activations live in global memory (L2-resident) as [column][K] matrices, column = slot (predictor pass 0: column
@@ -25,8 +26,6 @@ namespace fq3 {
 
 constexpr int MAXB = 32;          // slots per launch
 constexpr int MAXCOL = 2 * MAXB;  // activation columns (predictor pass 0 carries 2 tokens per slot)
-
-enum { BS_TOK = 0, BS_STEP = 1, BS_GEN = 2, BS_FIN = 3, BS_EMIT = 4 };
 
 // phase accounting (dbg_on & 2): CTA 0 / thread 0 charges the clock64 cycles since the last mark to the category that
 // was current; dumped to the debug buffer at the end of the launch (tools/batch_bench.py --phases)
@@ -341,7 +340,7 @@ __device__ void stack_b(Ctx& c, const StackDev& S, const BView& v, int nt, uint3
       for (int idx = blockIdx.x; idx < nrun * S.nH; idx += gridDim.x) {
         const int b = SMEM().runl[idx / S.nH], h = idx % S.nH;
         const SlotParams& sp = P.sl[b];
-        const int pos = sp.prefill_len + SMEM().bst[BS_STEP][b];
+        const int pos = sp.prefill_len + SMEM().bst[ST_STEP][b];
         // the column's page table into shared memory for the item's key loops (the previous item's last barrier
         // freed it; this one publishes it)
         for (int i = c.tid; i < (P.max_seq_len + KV_PAGE - 1) / KV_PAGE; i += NCT) SMEM().kvtab[i] = sp.kv_pages[i];
@@ -400,30 +399,18 @@ __device__ void stack_b(Ctx& c, const StackDev& S, const BView& v, int nt, uint3
 }
 
 // ------------------------------------------------------------------------------------------------------------
-// producer warp of the batched kernel: the same tape walk as producer_main(), every segment replayed once per
-// column block (see gemv_b)
+// producer warp of the batched kernel: producer_main()'s frame walk, every segment replayed once per column block
+// (see gemv_b); the talker's attention is never split
 // ------------------------------------------------------------------------------------------------------------
 template <bool BF>
 __device__ __noinline__ void producer_batch_main(const KParams& P) {
   const int lane = (int)(threadIdx.x & 31u);
   if (lane == 0) {
     Producer<BF> pr(P);
-    const int nb1 = col_blocks(BF, P.nslots), nb2 = col_blocks(BF, 2 * P.nslots);
-    auto rep = [&](int sg, int n) {
-      for (int i = 0; i < n; ++i) pr.seg(sg);
-    };
-    if (P.mode == MODE_GEMV_TEST) rep(P.gt_seg, col_blocks(BF, P.gt_ncols));
-    for (int f = 0; P.mode != MODE_GEMV_TEST && f < P.n_frames && !pr.stopped; ++f) {
-      if (P.has_mtp) rep(P.seg_mtp, nb2);
-      for (int i = 0; i < P.ncb; ++i) {
-        for (int l = 0; l < P.p.L; ++l)
-          for (int q = 0; q < 4; ++q) rep(P.p.seg_base + 4 * l + q, i == 0 ? nb2 : nb1);
-        rep(P.p.seg_head + i, nb1);
-      }
-      for (int l = 0; l < P.t.L; ++l)
-        for (int q = 0; q < 4; ++q) rep(P.t.seg_base + 4 * l + q, nb1);
-      rep(P.t.seg_head, nb1);
-    }
+    if (P.mode == MODE_GEMV_TEST) pr.seg(P.gt_seg, col_blocks(BF, P.gt_ncols));
+    else
+      for (int f = 0; f < P.n_frames && !pr.stopped; ++f)
+        pr.frame(col_blocks(BF, 2 * P.nslots), col_blocks(BF, P.nslots), -1, 0);
     pr.finish();
   }
 }
@@ -446,11 +433,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) fq3_decode_batch_kernel(const __g
   cta_prologue(P, P.mode == MODE_GEMV_TEST ? nullptr : me.seen);
   if (tid < B && P.mode != MODE_GEMV_TEST) {
     const int* st = P.sl[tid].state;
-    s.bst[BS_TOK][tid] = st[0];
-    s.bst[BS_STEP][tid] = st[1];
-    s.bst[BS_GEN][tid] = st[2];
-    s.bst[BS_FIN][tid] = 0;
-    s.bst[BS_EMIT][tid] = 0;
+    s.bst[ST_TOKEN][tid] = st[ST_TOKEN]; s.bst[ST_STEP][tid] = st[ST_STEP]; s.bst[ST_GEN][tid] = st[ST_GEN];
+    s.bst[ST_FIN][tid] = FQ3_RUNNING; s.bst[ST_EMIT][tid] = 0;
   }
   __syncthreads();
 
@@ -477,10 +461,10 @@ __global__ void __launch_bounds__(NTHREADS, 1) fq3_decode_batch_kernel(const __g
       // ---- which slots run this frame (identical decision in every CTA)
       if (warp == 0) {
         bool r = false;
-        if (lane < B && s.bst[BS_FIN][lane] == 0 && s.bst[BS_EMIT][lane] < P.sl[lane].n_frames) {   // the slot's own budget
-          if (s.bst[BS_STEP][lane] >= P.sl[lane].max_new) s.bst[BS_FIN][lane] = 1;
-          else if (s.bst[BS_TOK][lane] == P.eos) s.bst[BS_FIN][lane] = 2;
-          else r = !(P.sl[lane].text_open && s.bst[BS_GEN][lane] >= P.sl[lane].trailing_len);   // open text: wait for the row
+        if (lane < B && s.bst[ST_FIN][lane] == FQ3_RUNNING && s.bst[ST_EMIT][lane] < P.sl[lane].n_frames) {   // own budget
+          if (s.bst[ST_STEP][lane] >= P.sl[lane].max_new) s.bst[ST_FIN][lane] = FQ3_FIN_MAX_NEW;
+          else if (s.bst[ST_TOKEN][lane] == P.eos) s.bst[ST_FIN][lane] = FQ3_FIN_EOS;
+          else r = !(P.sl[lane].text_open && s.bst[ST_GEN][lane] >= P.sl[lane].trailing_len);   // open text: wait for the row
         }
         const unsigned m = __ballot_sync(0xffffffffu, r);
         if (lane == 0) s.ibc[0] = (int)m;
@@ -490,7 +474,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) fq3_decode_batch_kernel(const __g
       csync();
       if (run == 0u) break;
       const bool mine = (run >> v.b) & 1u;
-      const int token = s.bst[BS_TOK][v.b], step = s.bst[BS_STEP][v.b], gen_step = s.bst[BS_GEN][v.b];
+      const int token = s.bst[ST_TOKEN][v.b], step = s.bst[ST_STEP][v.b], gen_step = s.bst[ST_GEN][v.b];
       const float* urow = me.uniforms ? me.uniforms + (size_t)(step + 1) * 16 : nullptr;
       if (mine && tid == 0) {
         s.codes[0] = token;
@@ -548,7 +532,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) fq3_decode_batch_kernel(const __g
           sa.u = (me.sp_p.do_sample && urow) ? __ldg(urow + 1 + i) : 0.f;
           sa.use_penalty = false; sa.sup0 = Sp.V; sa.suppress_eos = false; sa.eos = -1;
           // the slot's rank-0 CTA writes the log-probabilities, as it writes the codes
-          if (me.logprob_out && v.rank == 0) sa.lp = me.logprob_out + (size_t)s.bst[BS_EMIT][v.b] * 16 + 1 + i;
+          if (me.logprob_out && v.rank == 0) sa.lp = me.logprob_out + (size_t)s.bst[ST_EMIT][v.b] * 16 + 1 + i;
           const int tok = sample_block<BF>(c, sa);
           if (tid == 0) s.codes[i + 1] = tok;
           csync();
@@ -556,17 +540,17 @@ __global__ void __launch_bounds__(NTHREADS, 1) fq3_decode_batch_kernel(const __g
       }
       pmark(c, PC_OTHER);
       // ---- emit the frame (generate.py:159): cat(cb0, 15 ids)
-      if (mine && v.rank == 0 && tid < 16) me.codes_out[(size_t)s.bst[BS_EMIT][v.b] * 16 + tid] = (long long)s.codes[tid];
+      if (mine && v.rank == 0 && tid < 16) me.codes_out[(size_t)s.bst[ST_EMIT][v.b] * 16 + tid] = (long long)s.codes[tid];
       csync();
       // ---- bookkeeping + max_seq_len rule (generate.py:175-177: the frame is already emitted)
       if (warp == 0) {
         bool r = false;
         if (lane < B && ((run >> lane) & 1u)) {
-          s.bst[BS_EMIT][lane] += 1;
-          const int pos = P.sl[lane].prefill_len + s.bst[BS_STEP][lane];
+          s.bst[ST_EMIT][lane] += 1;
+          const int pos = P.sl[lane].prefill_len + s.bst[ST_STEP][lane];
           if (pos >= P.max_seq_len - 1) {
-            s.bst[BS_FIN][lane] = 3;
-            s.bst[BS_STEP][lane] += 1;
+            s.bst[ST_FIN][lane] = FQ3_FIN_MAX_SEQ;
+            s.bst[ST_STEP][lane] += 1;
           } else {
             r = true;
           }
@@ -589,10 +573,10 @@ __global__ void __launch_bounds__(NTHREADS, 1) fq3_decode_batch_kernel(const __g
       // layer-0 input: sum of 16 embedding rows + trailing text / tts_pad (generate.py:163-171)
       pmark(c, PC_NORM);
       if (mine2 && v.rank < npt) {
-        const void* extra = gen_step < me.trailing_len ? me.trailing : me.tts_pad;
-        const size_t eoff = gen_step < me.trailing_len ? (size_t)gen_step * Ht : 0;
         uint8_t* xn = reinterpret_cast<uint8_t*>(P.XNB) + (size_t)v.b * P.ldX * esz;
         float* xr = P.XB + (size_t)v.b * P.ldX;
+        const void* extra = gen_step < me.trailing_len ? me.trailing : me.tts_pad;
+        const size_t eoff = gen_step < me.trailing_len ? (size_t)gen_step * Ht : 0;
         norm_row_b<BF>(c, [&](int k) {
           float sm = ldw<BF>(P.t_embed, (size_t)token * Ht + k);
           for (int q = 0; q < P.ncb; ++q) sm += ldw<BF>(P.p_embeds, ((size_t)q * P.p.V + s.codes[q + 1]) * Ht + k);
@@ -606,33 +590,23 @@ __global__ void __launch_bounds__(NTHREADS, 1) fq3_decode_batch_kernel(const __g
       }
       grid_sync_p(c, PC_SAMPLE);
       if (mine2) {
-        SampleArgs sa;
-        sa.logits = P.LOGB + (size_t)v.b * VMAX; sa.V = P.t.V; sa.sp = me.sp_t;
-        sa.u = (me.sp_t.do_sample && urow) ? __ldg(urow) : 0.f;
-        sa.use_penalty = true; sa.sup0 = P.t.V > 1024 ? P.t.V - 1024 : 0;
-        sa.suppress_eos = (step + 1) < me.min_new; sa.eos = P.eos;
-        // column 0 of the frame just emitted (the bookkeeping above already counted it)
-        if (me.logprob_out && v.rank == 0) sa.lp = me.logprob_out + (size_t)(s.bst[BS_EMIT][v.b] - 1) * 16;
-        const int tok = sample_block<BF>(c, sa);
+        const int tok = sample_block<BF>(c, frame_talker_draw(P, me, P.LOGB + (size_t)v.b * VMAX, urow, step,
+            // column 0 of the frame just emitted (the bookkeeping above already counted it)
+            (me.logprob_out && v.rank == 0) ? me.logprob_out + (size_t)(s.bst[ST_EMIT][v.b] - 1) * 16 : nullptr));
         if (v.rank == 0 && tid == 0) P.TOKB[v.b] = tok;
       }
       grid_sync_p(c, PC_OTHER);
-      if (tid < B && ((run2 >> tid) & 1u)) {
-        s.bst[BS_TOK][tid] = __ldcg(P.TOKB + tid);
-        s.bst[BS_STEP][tid] += 1;
-        s.bst[BS_GEN][tid] += 1;
-      }
+      if (tid < B && ((run2 >> tid) & 1u))
+        frame_advance(s.bst[ST_TOKEN][tid], s.bst[ST_STEP][tid], s.bst[ST_GEN][tid], __ldcg(P.TOKB + tid));
       csync();
     }
     pmark(c, PC_OTHER);
     if ((P.dbg_on & 2) && cta == 0 && tid == 0 && P.mode != MODE_GEMV_TEST)
       for (int i = 0; i < PC_N; ++i) reinterpret_cast<long long*>(P.dbg)[i] += s.prof[2 + i];   // accumulates over launches
     if (v.rank == 0 && P.mode != MODE_GEMV_TEST) {
-      if (tid == 0) {
-        int* st = me.state;
-        st[0] = s.bst[BS_TOK][v.b]; st[1] = s.bst[BS_STEP][v.b]; st[2] = s.bst[BS_GEN][v.b];
-        st[3] = s.bst[BS_FIN][v.b]; st[4] = s.bst[BS_EMIT][v.b];
-      }
+      if (tid == 0)
+        put_state(me.state, s.bst[ST_TOKEN][v.b], s.bst[ST_STEP][v.b], s.bst[ST_GEN][v.b], s.bst[ST_FIN][v.b],
+                  s.bst[ST_EMIT][v.b]);
       for (int i = tid; i < VMAX / 32; i += NCT) me.seen[i] = s.seen[i];
     }
     drain_producer(c);

@@ -63,7 +63,7 @@ struct SlotHost {
   bool active = false;
   int prefill_len = 0, rope_delta = 0, n_left_pad = 0, max_new = 0, min_new = 0, trailing_len = 0;
   bool text_open = false, text_closed = false;   // fq3_set_text_rows: rows may still follow / the caller closed the text
-  int step = 0;   // frames since fq3_begin_request (state[1] after the slot's last launch): where its next row goes
+  int step = 0;   // frames since fq3_begin_request (state[ST_STEP] after the slot's last launch): where its next row goes
   const void* trailing = nullptr;
   const void* tts_pad = nullptr;
   const float* uniforms = nullptr;
@@ -197,9 +197,7 @@ template <bool BF>
 __global__ void set_state_kernel(int* state, float* past_hidden, uint32_t* seen, const void* ph_src, int Ht,
                                  int token, int gen_step) {
   const int tid = blockIdx.x * blockDim.x + threadIdx.x;
-  if (tid == 0) {
-    state[0] = token; state[1] = 0; state[2] = gen_step; state[3] = 0; state[4] = 0;
-  }
+  if (tid == 0) put_state(state, token, 0, gen_step, FQ3_RUNNING, 0);
   for (int k = tid; k < Ht; k += gridDim.x * blockDim.x) past_hidden[k] = ldw<BF>(ph_src, k);
   for (int k = tid; k < VMAX / 32; k += gridDim.x * blockDim.x) seen[k] = 0u;
 }
@@ -227,14 +225,7 @@ __global__ void __launch_bounds__(NCT, 1)
   __threadfence();
   __syncthreads();
   Ctx c{P, tid, tid >> 5, tid & 31, 0u, 0u};
-  SampleArgs a;
-  a.logits = P.LOGITS; a.V = V; a.sp = sp; a.u = u;
-  a.use_penalty = true;
-  a.sup0 = suppress_special ? (V > 1024 ? V - 1024 : 0) : V;
-  a.suppress_eos = suppress_eos != 0;
-  a.eos = eos;
-  a.lp = lp_out;
-  const int tok = sample_block<BF>(c, a);
+  const int tok = sample_block<BF>(c, talker_draw(P.LOGITS, V, sp, u, suppress_special != 0, eos, suppress_eos != 0, lp_out));
   if (tid == 0) out[0] = tok;
 }
 
@@ -884,10 +875,10 @@ static SlotParams slot_params(fq3_engine* e, int s, int n_frames, long long* cod
   return p;
 }
 
-// kernel parameters of a single-sequence launch on slot s
-static KParams kp_for_slot(fq3_engine* e, int s, long long* codes_out, float* logprob_out = nullptr) {
+// kernel parameters of a step-wise single-sequence launch on slot s
+static KParams kp_for_slot(fq3_engine* e, int s, long long* codes_out) {
   KParams kp = e->kp;
-  kp.req = slot_params(e, s, 0, codes_out, logprob_out);   // the single-sequence kernel's budget is KParams::n_frames
+  kp.req = slot_params(e, s, 0, codes_out, nullptr);
   kp.nslots = 0;
   return kp;
 }
@@ -1051,22 +1042,27 @@ extern "C" int fq3_set_text_rows(fq3_engine* e, int32_t slot, int32_t trailing_l
   return 0;
 }
 
-// batched launch: slots[0..n) become the columns of one pass over the weight tape
-// (column j emits up to n_frames[j] frames into row j of the [n][max_frames][16] outputs)
-static int launch_decode_batch(fq3_engine* e, const int32_t* slots, int n, const int32_t* n_frames, int max_frames,
-                               long long* codes_out_dev, float* logprob_out_dev, cudaStream_t stream) {
-  if (!e->sl_dev) return fail(FQ3_ERR_STATE, "engine was created with max_batch = 1");
-  if (n > e->ncta) return fail(FQ3_ERR_INVALID, "%d slots need at least as many CTAs (engine has %d)", n, e->ncta);
-  for (int j = 0; j < n; ++j)
-    e->sl_host[j] = slot_params(e, slots[j], n_frames[j], codes_out_dev + (size_t)j * max_frames * 16,
-                                logprob_out_dev ? logprob_out_dev + (size_t)j * max_frames * 16 : nullptr);
-  CK(cudaMemcpyAsync(e->sl_dev, e->sl_host, (size_t)n * sizeof(SlotParams), cudaMemcpyHostToDevice, stream));
+// fused launch of slots[0..n): column j emits up to n_frames[j] frames into row j of the [n][max_frames][16] outputs.
+// One slot runs on the single-sequence kernel, more become the columns of one batched pass over the weight tape.
+static int launch_fused(fq3_engine* e, const int32_t* slots, int n, const int32_t* n_frames, int max_frames,
+                        long long* codes_out_dev, float* logprob_out_dev, cudaStream_t stream) {
   KParams kp = e->kp;
   kp.mode = MODE_FUSED;
-  kp.nslots = n;
-  kp.sl = e->sl_dev;
   kp.n_frames = max_frames;   // the producer warp's bound: no slot runs longer
-  kp.dbg_on = e->dbg_on & 2;
+  kp.dbg_on = e->dbg_on & 2;  // timing probes only; layer dumps belong to the step-wise entry points
+  if (n == 1) {
+    kp.req = slot_params(e, slots[0], n_frames[0], codes_out_dev, logprob_out_dev);
+    kp.nslots = 0;
+  } else {
+    if (!e->sl_dev) return fail(FQ3_ERR_STATE, "engine was created with max_batch = 1");
+    if (n > e->ncta) return fail(FQ3_ERR_INVALID, "%d slots need at least as many CTAs (engine has %d)", n, e->ncta);
+    for (int j = 0; j < n; ++j)
+      e->sl_host[j] = slot_params(e, slots[j], n_frames[j], codes_out_dev + (size_t)j * max_frames * 16,
+                                  logprob_out_dev ? logprob_out_dev + (size_t)j * max_frames * 16 : nullptr);
+    CK(cudaMemcpyAsync(e->sl_dev, e->sl_host, (size_t)n * sizeof(SlotParams), cudaMemcpyHostToDevice, stream));
+    kp.nslots = n;
+    kp.sl = e->sl_dev;
+  }
   return launch_decode(e, kp, stream);
 }
 
@@ -1121,25 +1117,17 @@ extern "C" int fq3_decode_chunk_n(fq3_engine* e, const int32_t* slots, int32_t n
   }
   DevGuard dev_guard(e->dev);
   cudaStream_t stream = (cudaStream_t)stream_;
-  if (n_slots == 1) {
-    KParams kp = kp_for_slot(e, slots[0], (long long*)codes_out_dev, logprob_out_dev);
-    kp.mode = MODE_FUSED;
-    kp.n_frames = n_frames[0];
-    kp.dbg_on = e->dbg_on & 2;   // timing probes only; layer dumps belong to the step-wise entry points
-    if ((rc = launch_decode(e, kp, stream))) return rc;
-  } else {
-    if ((rc = launch_decode_batch(e, slots, n_slots, n_frames, max_frames, (long long*)codes_out_dev, logprob_out_dev, stream))) return rc;
-  }
+  if ((rc = launch_fused(e, slots, n_slots, n_frames, max_frames, (long long*)codes_out_dev, logprob_out_dev, stream))) return rc;
   for (int j = 0; j < n_slots; ++j)
     CK(cudaMemcpyAsync(e->state_host + 8 * j, e->state + 8 * slots[j], 32, cudaMemcpyDeviceToHost, stream));
   CK(cudaStreamSynchronize(stream));
   for (int j = 0; j < n_slots; ++j) {
     const int* st = e->state_host + 8 * j;
-    res[j].next_token = st[0];
-    res[j].total_frames = st[1];
-    res[j].finished = st[3];
-    res[j].frames_emitted = st[4];
-    e->slots[slots[j]].step = st[1];
+    res[j].next_token = st[ST_TOKEN];
+    res[j].total_frames = st[ST_STEP];
+    res[j].finished = st[ST_FIN];
+    res[j].frames_emitted = st[ST_EMIT];
+    e->slots[slots[j]].step = st[ST_STEP];
   }
   return 0;
 }

@@ -19,7 +19,7 @@ from typing import Dict, Generator, List, Optional, Tuple
 
 import torch
 
-from .engine import KV_PAGE
+from .engine import FQ3_FIN_MAX_SEQ, KV_PAGE
 from .generate import _sync, begin_fused, begin_fused_batch, shared_engine
 from .logprobs import FrameLogprobs
 
@@ -426,7 +426,7 @@ def _chunks(sched: BatchScheduler, chunk_size: int, t_prefill: float, before_ste
             # leaves its loop before the "buffer full" check (streaming.py:130-132 vs :158-173)
             tm = {"chunk_index": idx, "chunk_steps": n, "prefill_ms": t_prefill * 1000 if idx == 0 else 0,
                   "decode_ms": dt * 1000, "total_steps_so_far": rq.frames,
-                  "is_final": n < chunk_size or rq.finished == 3}
+                  "is_final": n < chunk_size or rq.finished == FQ3_FIN_MAX_SEQ}
             if engine.time_kernels:
                 tm["kernel_ms"] = engine.last_kernel_ms
             if rq.lp is not None:

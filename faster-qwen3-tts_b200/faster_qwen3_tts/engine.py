@@ -22,7 +22,9 @@ LIB_PATH = os.path.join(CSRC, "libfq3_engine.so")
 INCLUDE = os.path.normpath(os.path.join(_HERE, "..", "..", "include"))
 
 FQ3_F32, FQ3_BF16 = 0, 1
-FINISH_NAMES = {0: "running", 1: "max_new_tokens", 2: "eos", 3: "max_seq_len"}
+FQ3_RUNNING, FQ3_FIN_MAX_NEW, FQ3_FIN_EOS, FQ3_FIN_MAX_SEQ = 0, 1, 2, 3   # enum fq3_finish
+FINISH_NAMES = {FQ3_RUNNING: "running", FQ3_FIN_MAX_NEW: "max_new_tokens", FQ3_FIN_EOS: "eos",
+                FQ3_FIN_MAX_SEQ: "max_seq_len"}
 
 
 class StackConfig(C.Structure):
