@@ -123,8 +123,9 @@ struct KParams {
   const Grp* grps;
   const uint32_t* segtab;       // [cta][nseg] : (begin << 8) | n   (begin relative to this CTA's first group)
   const uint32_t* cta_grp_off;  // [ncta + 1]
-  float *X, *X1, *QKV, *ACT, *LOGITS;
+  float *X, *X1, *QKV, *LOGITS;
   void* ATT;                    // model dtype: the talker attention output that feeds o_proj
+  void* ACT;                    // model dtype [2][ldACT]: SiLU(gate) * up, the down projection's input
   int ldX, ldQKV, ldATT, ldACT;
   unsigned* bar;
   const void* t_embed;
@@ -1124,10 +1125,12 @@ __device__ int sample_block(Ctx& c, const SampleArgs& a) {
 
 // ------------------------------------------------------------------------------------------------------------
 // Tensor-core GEMV (bf16): the tape holds mma.sync m16n8k16 A-fragments in register order, so one LDS.128 per lane
-// feeds one mma (16 rows x 16 k).  The activation vector(s) sit in shared memory as bf16 and enter as the B operand
+// feeds one mma (16 rows x 16 k).  The activation vector(s) x (bf16, token t at x + t * ldx) enter as the B operand
 // (column n = token; for 8-row "HALF" tiles columns 2n / 2n+1 carry the two K halves, rows 0-7 / 8-15 of the tile
 // hold the matching halves of the weight rows, and c0 + c3 is the full dot product).  Warps split the k-groups of a
-// tile; partial accumulators are combined in shared memory in a fixed order.
+// tile; partial accumulators are combined in shared memory in a fixed order.  x is the staging vector in shared memory
+// or (XG) an L2-resident vector in global memory; XG loads a warp's B fragments one ring tile ahead, so that the L2
+// round trip overlaps the previous tile's MMAs (a tile holds at most 16 k-groups, two per warp).
 //   pre(row, tok) -> float   value fetched BEFORE streaming starts (residual), handed back to epi
 //   epi(row, tok, v, vup, aux)   GU tiles: row = pair index, v = gate, vup = up
 // ------------------------------------------------------------------------------------------------------------
@@ -1138,9 +1141,8 @@ __device__ __forceinline__ void mma_bf16(float* d, const uint4& a, uint32_t b0, 
       : "r"(a.x), "r"(a.y), "r"(a.z), "r"(a.w), "r"(b0), "r"(b1));
 }
 
-template <int NT, class Pre, class Epi>
-__device__ __forceinline__ void gemv_mma(Ctx& c, int seg, int K, Pre pre, Epi epi) {
-  const __nv_bfloat16* xh = reinterpret_cast<const __nv_bfloat16*>(SMEM().xs);
+template <int NT, bool XG, class Pre, class Epi>
+__device__ __forceinline__ void gemv_mma(Ctx& c, int seg, int K, const __nv_bfloat16* x, int ldx, Pre pre, Epi epi) {
   float* red = SMEM().xs + XS_FLOATS / 2;  // [NCW][2][4][32] partial accumulators
   const uint32_t st = SMEM().seg[seg];
   const int gbeg = (int)(st >> 8), gn = (int)(st & 255u);
@@ -1152,7 +1154,20 @@ __device__ __forceinline__ void gemv_mma(Ctx& c, int seg, int K, Pre pre, Epi ep
     bool bvalid;
     if (kind == 1) { tok = gq >> 1; koff = (gq & 1) * (K >> 1); bvalid = gq < 2 * NT; }
     else { tok = gq; koff = 0; bvalid = gq < NT; }
-    const __nv_bfloat16* xb = xh + (bvalid ? tok * K + koff : 0) + 16 * t;
+    const __nv_bfloat16* xb = x + (bvalid ? tok * ldx + koff : 0) + 16 * t;
+    uint4 bn[2][2];   // XG: B fragments of the next tile, k-groups qq = warp and warp + NCW
+    auto fetch_b = [&](int tl) {
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const int qq = c.warp + NCW * i, kg = tl * G + qq;
+        bn[i][0] = make_uint4(0, 0, 0, 0); bn[i][1] = make_uint4(0, 0, 0, 0);
+        if (bvalid && qq < G) {
+          bn[i][0] = __ldcg(reinterpret_cast<const uint4*>(xb + 64 * kg));
+          bn[i][1] = __ldcg(reinterpret_cast<const uint4*>(xb + 64 * kg + 8));
+        }
+      }
+    };
+    if constexpr (XG) fetch_b(0);
     float aux[4] = {0.f, 0.f, 0.f, 0.f};
     if (c.warp < n_mt) {
       if (kind == 0) {
@@ -1169,14 +1184,26 @@ __device__ __forceinline__ void gemv_mma(Ctx& c, int seg, int K, Pre pre, Epi ep
 #pragma unroll
       for (int r = 0; r < 4; ++r) acc[a][r] = 0.f;
     for (int tl = 0; tl < g.ntiles; ++tl) {
+      uint4 bc[2][2];
+      if constexpr (XG) {
+#pragma unroll
+        for (int i = 0; i < 2; ++i) { bc[i][0] = bn[i][0]; bc[i][1] = bn[i][1]; }
+        if (tl + 1 < g.ntiles) fetch_b(tl + 1);
+      }
       const int stage = (int)(c.tile_ctr % NS);
       const uint32_t par = (c.tile_ctr / NS) & 1u;
       mbar_wait(&SMEM().full[stage], par);
       const uint8_t* tile = SMEM().ring[stage];
-      for (int qq = c.warp; qq < G; qq += NCW) {
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const int qq = c.warp + NCW * i;
+        if (qq >= G) break;
         const int kg = tl * G + qq;
         uint4 blo = make_uint4(0, 0, 0, 0), bhi = make_uint4(0, 0, 0, 0);
-        if (bvalid) {
+        if constexpr (XG) {
+          blo = bc[i][0];
+          bhi = bc[i][1];
+        } else if (bvalid) {
           blo = *reinterpret_cast<const uint4*>(xb + 64 * kg);
           bhi = *reinterpret_cast<const uint4*>(xb + 64 * kg + 8);
         }
@@ -1228,12 +1255,16 @@ __device__ __forceinline__ void gemv_mma(Ctx& c, int seg, int K, Pre pre, Epi ep
   }
 }
 
-// dispatch: bf16 -> tensor-core path on the bf16 staging vector, fp32 -> FMA path on the fp32 staging vector
-template <bool BF, bool GU, class Pre, class Epi>
-__device__ __forceinline__ void gemv_any(Ctx& c, int seg, int nt, int K, Pre pre, Epi epi) {
+// dispatch: bf16 -> tensor-core path, fp32 -> FMA path.  The input is the staging vector (K per token) or, XG, the
+// model-dtype vectors xg [nt][ldx] in global memory, read in place
+template <bool BF, bool GU, bool XG = false, class Pre, class Epi>
+__device__ __forceinline__ void gemv_any(Ctx& c, int seg, int nt, int K, Pre pre, Epi epi, const void* xg = nullptr,
+                                         int ldx = 0) {
   if constexpr (BF) {
-    if (nt == 1) gemv_mma<1>(c, seg, K, pre, epi);
-    else gemv_mma<2>(c, seg, K, pre, epi);
+    const __nv_bfloat16* x = XG ? reinterpret_cast<const __nv_bfloat16*>(xg) : reinterpret_cast<const __nv_bfloat16*>(SMEM().xs);
+    const int ld = XG ? ldx : K;
+    if (nt == 1) gemv_mma<1, XG>(c, seg, K, x, ld, pre, epi);
+    else gemv_mma<2, XG>(c, seg, K, x, ld, pre, epi);
   } else {
     auto epi2 = [&](int row0, const float* v0, const float* v1) {
       for (int t = 0; t < nt; ++t) {
@@ -1245,8 +1276,10 @@ __device__ __forceinline__ void gemv_any(Ctx& c, int seg, int nt, int K, Pre pre
         }
       }
     };
-    if (nt == 1) gemv_seg<1, false>(c, seg, SMEM().xs, K, 1, epi2);
-    else gemv_seg<2, false>(c, seg, SMEM().xs, K, 2, epi2);
+    const float* x = XG ? reinterpret_cast<const float*>(xg) : SMEM().xs;
+    const int ld = XG ? ldx : K;
+    if (nt == 1) gemv_seg<1, XG>(c, seg, x, ld, 1, epi2);
+    else gemv_seg<2, XG>(c, seg, x, ld, 2, epi2);
   }
 }
 
@@ -1320,13 +1353,34 @@ __device__ __forceinline__ void rs34_gather(const float* a, int lane, float* min
 }
 
 template <bool BF>
-struct SmallKV {  // cached K/V rows of this warp's kv group, fetched in the shadow of the QKV barrier
+struct SmallKV {  // what a one-token pass of the attention reads besides its QKV row, fetched in the shadow of the QKV
+                  // barrier: cached K/V rows of this warp's kv group and (bf16) the layer's q/k norm weights and the
+                  // RoPE row.  The fp32 parity kernel loads the latter in the attention: preloading them raised its spills.
   using Raw = typename std::conditional<BF, uint2, float4>::type;
   Raw k[16], v[16];
+  float4 qn, kn, cs, sn;   // dims [4 * lane, 4 * lane + 4)
 };
+// loads of the q/k norm weights and of the RoPE row of position rp (clamped to the table): attention_small_all issues
+// them itself when nothing was preloaded
 template <bool BF>
-__device__ __forceinline__ void small_kv_preload(Ctx& c, const StackDev& S, int layer, int slot0, const void* kc,
-                                                 const void* vc, SmallKV<BF>& pre) {
+__device__ __forceinline__ void small_norm_rope_load(Ctx& c, const StackDev& S, int layer, int rp, float4& qn4,
+                                                     float4& kn4, float4& cs4, float4& sn4) {
+  const int L4 = 4 * c.lane;
+  float qn[4], kn[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    qn[i] = ldw<BF>(S.qnorm, (size_t)layer * 128 + L4 + i);
+    kn[i] = ldw<BF>(S.knorm, (size_t)layer * 128 + L4 + i);
+  }
+  qn4 = make_float4(qn[0], qn[1], qn[2], qn[3]);
+  kn4 = make_float4(kn[0], kn[1], kn[2], kn[3]);
+  rp = rp < 0 ? 0 : (rp >= S.npos ? S.npos - 1 : rp);
+  cs4 = __ldg(reinterpret_cast<const float4*>(S.cos + (size_t)rp * 128) + c.lane);
+  sn4 = __ldg(reinterpret_cast<const float4*>(S.sin + (size_t)rp * 128) + c.lane);
+}
+template <bool BF>
+__device__ __forceinline__ void small_kv_preload(Ctx& c, const StackDev& S, int layer, int slot0, int rpos,
+                                                 const void* kc, const void* vc, SmallKV<BF>& pre) {
   using Raw = typename SmallKV<BF>::Raw;
   const size_t esz = BF ? 2 : 4;
   const int g = c.warp < S.nKV ? c.warp : 0;
@@ -1346,11 +1400,14 @@ __device__ __forceinline__ void small_kv_preload(Ctx& c, const StackDev& S, int 
       else { k[j] = make_float4(0, 0, 0, 0); v[j] = make_float4(0, 0, 0, 0); }
     }
   }
+  float4 qn, kn, cs, sn;
+  if constexpr (BF) small_norm_rope_load<BF>(c, S, layer, rpos, qn, kn, cs, sn);
 #pragma unroll
   for (int j = 0; j < 16; ++j) {
     pre.k[j] = k[j];
     pre.v[j] = v[j];
   }
+  if constexpr (BF) { pre.qn = qn; pre.kn = kn; pre.cs = cs; pre.sn = sn; }
 }
 
 //   qkv0: QKV row of token 0, token t lives qkv_tstride floats further; kc / vc: the request's predictor caches;
@@ -1386,22 +1443,14 @@ __device__ void attention_small_all(Ctx& c, const StackDev& S, int layer, int sl
       else zero_raw(kraw[j]);
     }
     float4 qn4, kn4, cs4[NT], sn4[NT], kr4[NT], vr4[NT], qr4[2][NT];
-    {
-      float qn[4], kn[4];
+    if (BF && pre && NT == 1) {
+      qn4 = pre->qn; kn4 = pre->kn; cs4[0] = pre->cs; sn4[0] = pre->sn;
+    } else {
 #pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        qn[i] = ldw<BF>(S.qnorm, (size_t)layer * 128 + L4 + i);
-        kn[i] = ldw<BF>(S.knorm, (size_t)layer * 128 + L4 + i);
-      }
-      qn4 = make_float4(qn[0], qn[1], qn[2], qn[3]);
-      kn4 = make_float4(kn[0], kn[1], kn[2], kn[3]);
+      for (int t = 0; t < NT; ++t) small_norm_rope_load<BF>(c, S, layer, rpos0 + t, qn4, kn4, cs4[t], sn4[t]);
     }
 #pragma unroll
     for (int t = 0; t < NT; ++t) {
-      int rp = rpos0 + t;
-      rp = rp < 0 ? 0 : (rp >= S.npos ? S.npos - 1 : rp);
-      cs4[t] = __ldg(reinterpret_cast<const float4*>(S.cos + (size_t)rp * 128) + c.lane);
-      sn4[t] = __ldg(reinterpret_cast<const float4*>(S.sin + (size_t)rp * 128) + c.lane);
       const float* row = qkv0 + (size_t)t * qkv_tstride;
       kr4[t] = __ldcg(reinterpret_cast<const float4*>(row + S.qd + g * 128) + c.lane);
       vr4[t] = __ldcg(reinterpret_cast<const float4*>(row + S.qd + S.kd + g * 128) + c.lane);
@@ -1642,7 +1691,8 @@ __device__ void run_layers(Ctx& c, const StackDev& S, int nt, int slot0, int rpo
     const bool kv_pre = small_attn && nt == 1;
     SmallKV<BF> skv;
     grid_arrive(c);
-    if (kv_pre) small_kv_preload<BF>(c, S, l, slot0, kc, vc, skv);  // cached keys/values do not depend on this layer's QKV
+    // cached keys/values, norm weights and RoPE rows do not depend on this layer's QKV
+    if (kv_pre) small_kv_preload<BF>(c, S, l, slot0, rpos0, kc, vc, skv);
     grid_wait(c);
     probe(c, pi);  // 3: after B1
     if (dbg && cta0) {
@@ -1727,37 +1777,25 @@ __device__ void run_layers(Ctx& c, const StackDev& S, int nt, int slot0, int rpo
     gemv_any<BF, true>(c, S.seg_base + 4 * l + 2, nt, S.H, nopre, [&](int pair, int t, float gv, float uv, float) {
       const float gte = rnd<BF>(gv), up = rnd<BF>(uv);
       const float sl = rnd<BF>(gte / (1.0f + expf(-gte)));
-      P.ACT[(size_t)t * P.ldACT + pair] = rnd<BF>(sl * up);
+      stw<BF>(P.ACT, (size_t)t * P.ldACT + pair, rnd<BF>(sl * up));   // exact: the value is model-dtype rounded
     });
     probe(c, pi);  // 8: after GU gemv
     grid_sync(c);
     probe(c, pi);  // 9: after B4
-    // ---- P5: down rows + residual.  ACT -> staging vector with all of a thread's loads in flight before its first
-    //      store (one L2 round trip instead of one per element)
-    for (int t = 0; t < nt; ++t) {
-      constexpr int U = 12;
-      for (int k0 = 0; k0 < S.I; k0 += U * NCT) {
-        float v[U];
-#pragma unroll
-        for (int u = 0; u < U; ++u) {
-          const int k = k0 + u * NCT + c.tid;
-          v[u] = k < S.I ? __ldcg(P.ACT + (size_t)t * P.ldACT + k) : 0.f;
-        }
-#pragma unroll
-        for (int u = 0; u < U; ++u) {
-          const int k = k0 + u * NCT + c.tid;
-          if (k < S.I) xs_put<BF>(c, t * S.I + k, v[u]);
-        }
-      }
-    }
-    csync();
+    // ---- P5: down rows + residual, reading ACT in place (model dtype, L2-resident; no copy into the staging vector)
     if (dbg && cta0) {
       float* d = P.dbg + (size_t)l * P.dbg_stride_layer + (size_t)2 * (S.qd + 2 * S.kd) + 2 * S.qd + 2 * S.H;
-      for (int k = c.tid; k < nt * S.I; k += NCT) d[k] = xs_get<BF>(c, k);
+      for (int t = 0; t < nt; ++t)
+        for (int k = c.tid; k < S.I; k += NCT) {
+          const size_t i = (size_t)t * P.ldACT + k;
+          if constexpr (BF) d[(size_t)t * S.I + k] = __bfloat162float(__ldcg(reinterpret_cast<const __nv_bfloat16*>(P.ACT) + i));
+          else d[(size_t)t * S.I + k] = __ldcg(reinterpret_cast<const float*>(P.ACT) + i);
+        }
     }
-    gemv_any<BF, false>(
+    gemv_any<BF, false, true>(
         c, S.seg_base + 4 * l + 3, nt, S.I, [&](int row, int t) { return __ldcg(P.X1 + (size_t)t * P.ldX + row); },
-        [&](int row, int t, float v, float, float res) { P.X[(size_t)t * P.ldX + row] = rnd<BF>(res + rnd<BF>(v)); });
+        [&](int row, int t, float v, float, float res) { P.X[(size_t)t * P.ldX + row] = rnd<BF>(res + rnd<BF>(v)); },
+        P.ACT, P.ldACT);
     probe(c, pi);  // 10: after DN gemv
     grid_arrive(c);
     if (l + 1 < S.L) norm_wload<BF>(c, S.ln_in, (size_t)(l + 1) * S.H, S.H, wnext);

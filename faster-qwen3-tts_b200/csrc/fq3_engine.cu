@@ -98,8 +98,8 @@ struct fq3_engine {
   SlotParams* sl_host = nullptr;  // pinned
   // device buffers (slot-major: slot s starts at s * <per-slot size>)
   void *p_kc = nullptr, *p_vc = nullptr;
-  float *X = nullptr, *X1 = nullptr, *QKV = nullptr, *ACT = nullptr, *LOGITS = nullptr, *PART = nullptr;
-  void* ATT = nullptr;  // model dtype
+  float *X = nullptr, *X1 = nullptr, *QKV = nullptr, *LOGITS = nullptr, *PART = nullptr;
+  void *ATT = nullptr, *ACT = nullptr;  // model dtype
   unsigned* bar = nullptr;
   int* state = nullptr;
   int* state_host = nullptr;  // pinned
@@ -376,7 +376,7 @@ static int engine_alloc(fq3_engine* e, const cudaDeviceProp& prop) {
   const int ldACT = std::max(T.intermediate_size, Pc.intermediate_size);
   CK(cudaMalloc(&e->X, 2 * ldX * sizeof(float))); CK(cudaMalloc(&e->X1, 2 * ldX * sizeof(float)));
   CK(cudaMalloc(&e->QKV, 2 * ldQKV * sizeof(float))); CK(cudaMalloc(&e->ATT, ldATT * e->esz));
-  CK(cudaMalloc(&e->ACT, 2 * ldACT * sizeof(float))); CK(cudaMalloc(&e->LOGITS, VMAX * sizeof(float)));
+  CK(cudaMalloc(&e->ACT, 2 * ldACT * e->esz)); CK(cudaMalloc(&e->LOGITS, VMAX * sizeof(float)));
   CK(zalloc((void**)&e->bar, 32768));
   CK(cudaMalloc(&e->PART, (size_t)T.num_attention_heads * 16 * PART_STRIDE * sizeof(float)));
   CK(zalloc((void**)&e->state, STATE_BYTES * MS));
