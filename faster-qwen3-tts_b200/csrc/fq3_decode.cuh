@@ -28,6 +28,7 @@
 #include <type_traits>
 
 #include "../../include/fq3_engine.h"   // enum fq3_finish: the finish codes the kernels write
+#include "fq3_tape.cuh"                  // the weight tape: Grp, segment table, STAGE_BYTES
 
 namespace fq3 {
 
@@ -35,12 +36,9 @@ constexpr int NCW = 8;               // consumer warps
 constexpr int NCT = NCW * 32;        // consumer threads
 constexpr int NTHREADS = NCT + 32;   // + producer warp
 constexpr int NS = 5;                // ring stages
-constexpr int STAGE_BYTES = 32768;
 constexpr int XS_FLOATS = 6144;      // activation vector(s) feeding the current GEMV; also attention/sampling scratch
 constexpr int HMAX = 2048;           // max talker hidden (xin / past_hidden buffers)
 constexpr int VMAX = 4096;
-constexpr int MAXGRP = 512;          // row groups per CTA
-constexpr int MAXSEG = 256;          // GEMV segments
 constexpr int SEQMAX = 4096;
 
 enum Mode { MODE_FUSED = 0, MODE_TALKER_STEP = 1, MODE_PRED_RUN = 2, MODE_GEMV_TEST = 3 };
@@ -48,15 +46,6 @@ enum Mode { MODE_FUSED = 0, MODE_TALKER_STEP = 1, MODE_PRED_RUN = 2, MODE_GEMV_T
 // split-key talker attention runs from this many cached keys on (below, one CTA per q-head is faster); run_layers and
 // Producer::stack_layers must take the same decision, so both read this one constant
 constexpr int ATTN_SPLIT_MIN = 192;
-
-struct Grp {           // one row group of one segment, as seen by one CTA (<= 32 rows, full K)
-  uint32_t off16;      // tape offset / 16
-  int32_t row0;        // first row (index inside the segment)
-  uint16_t rows;       // even
-  uint16_t m;          // 512-byte row chunks per tile
-  uint16_t ntiles;     // K-chunks
-  uint16_t pad;
-};
 
 struct Sampling {
   int do_sample, top_k;
@@ -121,7 +110,7 @@ struct KParams {
   int mode, ncta, nseg, seg_mtp;
   const uint8_t* tape;
   const Grp* grps;
-  const uint32_t* segtab;       // [cta][nseg] : (begin << 8) | n   (begin relative to this CTA's first group)
+  const uint32_t* segtab;       // [cta][nseg] seg_begin / seg_count words
   const uint32_t* cta_grp_off;  // [ncta + 1]
   float *X, *X1, *QKV, *LOGITS;
   void* ATT;                    // model dtype: the talker attention output that feeds o_proj
@@ -354,7 +343,7 @@ __device__ __forceinline__ void probe_at(Ctx& c, int idx) {  // fixed slot (fram
 template <int NT, bool XG, class Epi>
 __device__ __forceinline__ void gemv_seg(Ctx& c, int seg, const float* x, int xstride, int ncols, Epi epi) {
   const uint32_t st = SMEM().seg[seg];
-  const int gbeg = (int)(st >> 8), gn = (int)(st & 255u);
+  const int gbeg = seg_begin(st), gn = seg_count(st);
   const float* xr[NT];
 #pragma unroll
   for (int t = 0; t < NT; ++t) xr[t] = x + (size_t)(t < ncols ? t : 0) * xstride + c.lane * 4;
@@ -459,12 +448,11 @@ struct Producer {
   __device__ __forceinline__ void seg(int sg, int rep = 1) {
     if (stopped) return;
     const uint32_t st = s.seg[sg];
-    const int gbeg = (int)(st >> 8), gn = (int)(st & 255u);
+    const int gbeg = seg_begin(st), gn = seg_count(st);
     for (int r = 0; r < rep; ++r)
       for (int gi = 0; gi < gn; ++gi) {
         const Grp g = s.grp[gbeg + gi];
-        // fp32 tape: rows x m x 512-byte row chunks; bf16 tape: n_mt x G k-groups x 2048-byte fragment blocks
-        const uint32_t bytes = BF ? (uint32_t)(g.rows & 0xff) * g.m * 2048u : (uint32_t)g.rows * g.m * 512u;
+        const uint32_t bytes = tile_bytes(BF, g.rows, g.m);
         const uint8_t* src = P.tape + (size_t)g.off16 * 16;
         for (int tl = 0; tl < g.ntiles; ++tl) {
           const int stage = (int)(ctr % NS);
@@ -1145,11 +1133,11 @@ template <int NT, bool XG, class Pre, class Epi>
 __device__ __forceinline__ void gemv_mma(Ctx& c, int seg, int K, const __nv_bfloat16* x, int ldx, Pre pre, Epi epi) {
   float* red = SMEM().xs + XS_FLOATS / 2;  // [NCW][2][4][32] partial accumulators
   const uint32_t st = SMEM().seg[seg];
-  const int gbeg = (int)(st >> 8), gn = (int)(st & 255u);
+  const int gbeg = seg_begin(st), gn = seg_count(st);
   const int gq = c.lane >> 2, t = c.lane & 3;
   for (int gi = 0; gi < gn; ++gi) {
     const Grp g = SMEM().grp[gbeg + gi];
-    const int n_mt = g.rows & 0xff, kind = g.rows >> 8, G = g.m;
+    const int n_mt = grp_nmt(g.rows), kind = grp_kind(g.rows), G = g.m;
     int tok, koff;
     bool bvalid;
     if (kind == 1) { tok = gq >> 1; koff = (gq & 1) * (K >> 1); bvalid = gq < 2 * NT; }

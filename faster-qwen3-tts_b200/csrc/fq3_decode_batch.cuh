@@ -89,13 +89,13 @@ __device__ __noinline__ void gemv_mma_b(Ctx& c, int seg, int K, const __nv_bfloa
   constexpr int NACC = 2 * NG;
   float* red = SMEM().xs;  // [NCW][NACC][4][32] partial accumulators (spills over into xin for NG = 4)
   const uint32_t st = SMEM().seg[seg];
-  const int gbeg = (int)(st >> 8), gn = (int)(st & 255u);
+  const int gbeg = seg_begin(st), gn = seg_count(st);
   const int gq = c.lane >> 2, t = c.lane & 3;
   const int ngr = (ncols + 7) >> 3;   // n-groups in use (FULL / GU tiles)
   const int ngh = (ncols + 3) >> 2;   // token groups of 4 (HALF tiles)
   for (int gi = 0; gi < gn; ++gi) {
     const Grp g = SMEM().grp[gbeg + gi];
-    const int n_mt = g.rows & 0xff, kind = g.rows >> 8, G = g.m;
+    const int n_mt = grp_nmt(g.rows), kind = grp_kind(g.rows), G = g.m;
     const int nacc = kind == 1 ? ngh : n_mt * NG;
     float aux[4] = {0.f, 0.f, 0.f, 0.f};
     if (c.warp < nacc) {

@@ -46,18 +46,6 @@ struct DevGuard {
   }
 };
 
-struct SegHost {
-  int rows, K;
-  uint64_t bytes;  // total tape bytes of this segment (all CTAs)
-};
-
-struct PackGrp {
-  uint64_t tape_off;
-  uint32_t rowsrc_idx;
-  uint16_t rows, m, ntiles, pad;   // fp32 layout: rows, 512-byte chunks per tile; mma layout: n_mt | kind << 8, G
-  int32_t K;
-};
-
 // host-side record of one request slot (fq3_begin_request latches it; slot_params() hands it to the kernels)
 struct SlotHost {
   bool active = false;
@@ -115,7 +103,7 @@ struct fq3_engine {
   uint32_t* segtab = nullptr;
   uint32_t* cta_grp_off = nullptr;
   std::map<std::string, void*> tabs;  // owned small tables (device)
-  std::vector<SegHost> segs;
+  std::vector<TapeSeg> segs;   // tape_segments(cfg), as of the last load
   int64_t talker_step_bytes = 0, predictor_frame_bytes = 0;
   KParams kp;  // template parameters (static part)
   int64_t launches = 0;
@@ -130,69 +118,6 @@ static size_t smem_bytes() { return sizeof(Smem); }
 // ------------------------------------------------------------------------------------------------------------
 // small kernels
 // ------------------------------------------------------------------------------------------------------------
-__global__ void pack_kernel(const PackGrp* __restrict__ pg, int npg, const void* const* __restrict__ rowsrc,
-                            uint8_t* __restrict__ tape) {
-  for (int b = blockIdx.x; b < npg; b += gridDim.x) {
-    const PackGrp g = pg[b];
-    const int rows = g.rows, m = g.m;
-    const long long total = (long long)rows * m * g.ntiles * 32;
-    uint4* dst = reinterpret_cast<uint4*>(tape + g.tape_off);
-    for (long long q = threadIdx.x; q < total; q += blockDim.x) {
-      const int lane = (int)(q & 31);
-      long long rem = q >> 5;
-      const int j = (int)(rem % m);
-      rem /= m;
-      const int r = (int)(rem % rows);
-      const int t = (int)(rem / rows);
-      const int kb = t * m + j;
-      const uint8_t* src = reinterpret_cast<const uint8_t*>(rowsrc[g.rowsrc_idx + r]);
-      dst[q] = *reinterpret_cast<const uint4*>(src + ((size_t)kb * 128 + lane * 4) * 4);
-    }
-  }
-}
-
-// bf16 tensor-core layout: per tile [m-tile][k-group][step 0..3][lane][16 B] holding mma.m16n8k16 A fragments
-// (a0,a1,a2,a3) = rowA[kk,kk+1], rowB[kkB,kkB+1], rowA[kk+2,kk+3], rowB[kkB+2,kkB+3], kk = 64*kgroup + 16*t + 4*step.
-// kind 0 FULL: rowA = r0+16*mt+g, rowB = rowA+8;  kind 1 HALF: rowA = rowB = r0+g, kkB = K/2 + kk;
-// kind 2 GU: rowA = gate row, rowB = up row of pair r0/2 + 8*mt + g (rowsrc holds gate/up interleaved).
-__global__ void pack_mma_kernel(const PackGrp* __restrict__ pg, int npg, const void* const* __restrict__ rowsrc,
-                                uint8_t* __restrict__ tape) {
-  for (int b = blockIdx.x; b < npg; b += gridDim.x) {
-    // header fields read one by one and 32-bit index arithmetic (a group holds ntiles * G <= K / 64 k-groups of at most
-    // 2 m-tiles, far below 2^31 elements): with a struct copy and 64-bit division, ptxas for sm_90a took G from a
-    // uniform register it never wrote, and the tape came out wrong
-    const int n_mt = pg[b].rows & 0xff, kind = pg[b].rows >> 8, G = pg[b].m, ntiles = pg[b].ntiles, K = pg[b].K;
-    const uint32_t rowsrc_idx = pg[b].rowsrc_idx;
-    const int total = ntiles * n_mt * G * 128;
-    uint4* dst = reinterpret_cast<uint4*>(tape + pg[b].tape_off);
-    for (int q = threadIdx.x; q < total; q += blockDim.x) {
-      const int lane = q & 31, st = (q >> 5) & 3;
-      int rem = q >> 7;
-      const int qq = rem % G;
-      rem /= G;
-      const int mt = rem % n_mt;
-      const int tl = rem / n_mt;
-      const int gq = lane >> 2, t = lane & 3;
-      const int kk = 64 * (tl * G + qq) + 16 * t + 4 * st;
-      const uint8_t *ra, *rb;
-      int kb = kk;
-      if (kind == 0) {
-        ra = reinterpret_cast<const uint8_t*>(rowsrc[rowsrc_idx + mt * 16 + gq]);
-        rb = reinterpret_cast<const uint8_t*>(rowsrc[rowsrc_idx + mt * 16 + gq + 8]);
-      } else if (kind == 1) {
-        ra = rb = reinterpret_cast<const uint8_t*>(rowsrc[rowsrc_idx + gq]);
-        kb = K / 2 + kk;
-      } else {
-        ra = reinterpret_cast<const uint8_t*>(rowsrc[rowsrc_idx + 2 * (mt * 8 + gq)]);
-        rb = reinterpret_cast<const uint8_t*>(rowsrc[rowsrc_idx + 2 * (mt * 8 + gq) + 1]);
-      }
-      const uint2 a = *reinterpret_cast<const uint2*>(ra + (size_t)kk * 2);
-      const uint2 c = *reinterpret_cast<const uint2*>(rb + (size_t)kb * 2);
-      dst[q] = make_uint4(a.x, c.x, a.y, c.y);
-    }
-  }
-}
-
 template <bool BF>
 __global__ void set_state_kernel(int* state, float* past_hidden, uint32_t* seen, const void* ph_src, int Ht,
                                  int token, int gen_step) {
@@ -572,245 +497,57 @@ extern "C" int fq3_engine_load_weights(fq3_engine* e, const fq3_tensor* tensors,
       k.mtp_b = nullptr;
     }
   }
-  // ---- segments and their row sources
-  std::vector<SegHost>& segs = e->segs;
-  segs.clear();
-  std::vector<const void*> rowsrc;          // concatenated row pointers
-  std::vector<uint32_t> seg_rowsrc0;        // first index into rowsrc per segment
-  auto add_seg = [&](int rows, int K) {
-    segs.push_back(SegHost{rows, K, 0});
-    seg_rowsrc0.push_back((uint32_t)rowsrc.size());
+  // ---- segments: their tensors resolved by name into the row-source table, then planned over the CTAs
+  TapeSegments T = tape_segments(cfg);
+  std::vector<const void*> rowsrc;
+  for (const TapeSeg& s : T.segs) {
+    const void* w[3];
+    for (size_t i = 0; i < s.runs.size(); ++i)
+      if ((rc = need(s.runs[i].tensor, s.runs[i].tensor_rows * s.K, &w[i]))) return rc;
+    tape_rows(s, w, esz, rowsrc);
+  }
+  TapePlan plan;
+  const std::string err = plan_tape(T.segs, e->ncta, e->bf16, plan);
+  if (!err.empty()) return fail(FQ3_ERR_INVALID, "%s", err.c_str());
+  k.t.seg_base = T.seg_base[0]; k.t.seg_head = T.seg_head[0];
+  k.p.seg_base = T.seg_base[1]; k.p.seg_head = T.seg_head[1];
+  k.seg_mtp = T.seg_mtp;
+  k.nseg = (int)T.segs.size();
+  e->segs = std::move(T.segs);
+  // ---- upload tables, pack.  A reload frees what the previous load allocated.
+  auto upload = [&](auto** dst, const auto& v) -> int {
+    if (*dst) cudaFree((void*)*dst);
+    *dst = nullptr;
+    CK(cudaMalloc(dst, v.size() * sizeof(v[0])));
+    CK(cudaMemcpyAsync((void*)*dst, v.data(), v.size() * sizeof(v[0]), cudaMemcpyHostToDevice, stream));
+    return 0;
   };
-  auto push_rows = [&](const void* base, int64_t row0, int rows, int K) {
-    for (int r = 0; r < rows; ++r) rowsrc.push_back((const uint8_t*)base + (size_t)(row0 + r) * K * esz);
-  };
-  int seg_id = 0;
-  for (int si = 0; si < 2; ++si) {
-    const std::string p = sn[si].pre;
-    const fq3_stack_config& c = *sn[si].c;
-    const int L = c.num_hidden_layers, H = c.hidden_size, I = c.intermediate_size;
-    const int qd = c.num_attention_heads * 128, kd = c.num_key_value_heads * 128;
-    const void *wq, *wk, *wv, *wo, *wg, *wu, *wd;
-    if ((rc = need(p + "q", (int64_t)L * qd * H, &wq))) return rc;
-    if ((rc = need(p + "k", (int64_t)L * kd * H, &wk))) return rc;
-    if ((rc = need(p + "v", (int64_t)L * kd * H, &wv))) return rc;
-    if ((rc = need(p + "o", (int64_t)L * H * qd, &wo))) return rc;
-    if ((rc = need(p + "gate", (int64_t)L * I * H, &wg))) return rc;
-    if ((rc = need(p + "up", (int64_t)L * I * H, &wu))) return rc;
-    if ((rc = need(p + "down", (int64_t)L * H * I, &wd))) return rc;
-    sn[si].s->seg_base = seg_id;
-    for (int l = 0; l < L; ++l) {
-      add_seg(qd + 2 * kd, H);
-      push_rows(wq, (int64_t)l * qd, qd, H);
-      push_rows(wk, (int64_t)l * kd, kd, H);
-      push_rows(wv, (int64_t)l * kd, kd, H);
-      add_seg(H, qd);
-      push_rows(wo, (int64_t)l * H, H, qd);
-      add_seg(2 * I, H);
-      for (int r = 0; r < I; ++r) {
-        rowsrc.push_back((const uint8_t*)wg + ((size_t)l * I + r) * H * esz);
-        rowsrc.push_back((const uint8_t*)wu + ((size_t)l * I + r) * H * esz);
-      }
-      add_seg(H, I);
-      push_rows(wd, (int64_t)l * H, H, I);
-      seg_id += 4;
-    }
-    if (si == 0) {
-      const void* wh;
-      if ((rc = need("t.head", (int64_t)c.vocab_size * H, &wh))) return rc;
-      sn[si].s->seg_head = seg_id;
-      add_seg(c.vocab_size, H);
-      push_rows(wh, 0, c.vocab_size, H);
-      seg_id += 1;
-    } else {
-      const void* wh;
-      if ((rc = need("p.heads", (int64_t)k.ncb * c.vocab_size * H, &wh))) return rc;
-      sn[si].s->seg_head = seg_id;
-      for (int i = 0; i < k.ncb; ++i) {
-        add_seg(c.vocab_size, H);
-        push_rows(wh, (int64_t)i * c.vocab_size, c.vocab_size, H);
-        seg_id += 1;
-      }
-      if (cfg.has_mtp_projection) {
-        const void* wm;
-        const int Ht = cfg.talker.hidden_size;
-        if ((rc = need("p.mtp_w", (int64_t)H * Ht, &wm))) return rc;
-        k.seg_mtp = seg_id;
-        add_seg(H, Ht);
-        push_rows(wm, 0, H, Ht);
-        seg_id += 1;
-      } else {
-        k.seg_mtp = -1;
-      }
-    }
-  }
-  const int nseg = (int)segs.size();
-  if (nseg > MAXSEG) return fail(FQ3_ERR_INVALID, "too many segments (%d > %d)", nseg, MAXSEG);
-  k.nseg = nseg;
-  // ---- distribute row pairs over CTAs, split into groups, lay out the tape
-  const int ncta = e->ncta;
-  const int EPW = e->bf16 ? 256 : 128;  // elements per 512-byte warp read
-  std::vector<std::vector<Grp>> cta_grps(ncta);
-  std::vector<uint32_t> segtab((size_t)ncta * nseg, 0);
-  std::vector<PackGrp> pack;
-  // per-CTA byte totals to place groups: first pass collects sizes
-  struct Tmp { int cta, seg, row0, rows, m, ntiles; uint64_t bytes; uint32_t rsrc; };
-  std::vector<Tmp> tmp;
-  int rot = 0;
-  // which segments are gate/up (interleaved) segments
-  std::vector<char> seg_is_gu(nseg, 0);
-  for (int si = 0; si < 2; ++si)
-    for (int l = 0; l < sn[si].c->num_hidden_layers; ++l) seg_is_gu[sn[si].s->seg_base + 4 * l + 2] = 1;
-  for (int sg = 0; sg < nseg; ++sg) {
-    const int rows = segs[sg].rows, K = segs[sg].K;
-    segs[sg].bytes = (uint64_t)rows * K * esz;
-    if (e->bf16) {
-      // ---- tensor-core layout: units of 8 rows (plain) or 8 gate/up pairs (GU)
-      const bool gu = seg_is_gu[sg];
-      const int unit_rows = gu ? 16 : 8;
-      if (rows % unit_rows || K % 128) return fail(FQ3_ERR_INVALID, "segment %d: rows %d / K %d not tileable for the bf16 tensor-core tape", sg, rows, K);
-      const int units = rows / unit_rows, base = units / ncta, extra = units % ncta;
-      int unit0 = 0;
-      for (int c = 0; c < ncta; ++c) {
-        const int uc = base + ((((c - rot) % ncta + ncta) % ncta) < extra ? 1 : 0);
-        const int begin = (int)cta_grps[c].size();
-        int ng = 0;
-        auto emit = [&](int kind, int n_mt, int row0, uint32_t rsrc) {
-          const int Keff = kind == 1 ? K / 2 : K;
-          const int KG = Keff / 64;
-          int G = 1;
-          for (int d = 1; d <= KG; ++d)
-            if (KG % d == 0 && n_mt * d <= 16) G = d;
-          Tmp t{c, sg, row0, n_mt | (kind << 8), G, KG / G, (uint64_t)n_mt * KG * 2048, rsrc};
-          tmp.push_back(t);
-          Grp g; g.off16 = 0; g.row0 = row0; g.rows = (uint16_t)(n_mt | (kind << 8)); g.m = (uint16_t)G;
-          g.ntiles = (uint16_t)(KG / G); g.pad = 0;
-          cta_grps[c].push_back(g);
-          ++ng;
-        };
-        if (gu) {
-          for (int u = 0; u < uc; u += 2) {
-            const int n_mt = std::min(2, uc - u);
-            const int pair0 = (unit0 + u) * 8;
-            emit(2, n_mt, pair0, seg_rowsrc0[sg] + 2u * pair0);
-          }
-        } else {
-          const int nfull = uc / 2;
-          for (int f = 0; f < nfull; f += 2) {
-            const int n_mt = std::min(2, nfull - f);
-            const int r0 = (unit0 + 2 * f) * 8;
-            emit(0, n_mt, r0, seg_rowsrc0[sg] + (uint32_t)r0);
-          }
-          if (uc % 2) {
-            const int r0 = (unit0 + uc - 1) * 8;
-            emit(1, 1, r0, seg_rowsrc0[sg] + (uint32_t)r0);
-          }
-        }
-        if (ng > 255) return fail(FQ3_ERR_INVALID, "segment %d: too many groups per CTA", sg);
-        segtab[(size_t)c * nseg + sg] = ((uint32_t)begin << 8) | (uint32_t)ng;
-        unit0 += uc;
-      }
-      rot = (rot + extra) % ncta;
-      continue;
-    }
-    if (rows % 2 || K % EPW) return fail(FQ3_ERR_INVALID, "segment %d: rows %d must be even and K %d a multiple of %d", sg, rows, K, EPW);
-    const int KB = K / EPW;
-    const int pairs = rows / 2, base = pairs / ncta, extra = pairs % ncta;
-    int row = 0;
-    for (int c = 0; c < ncta; ++c) {
-      const int pc = base + ((((c - rot) % ncta + ncta) % ncta) < extra ? 1 : 0);
-      const int rows_c = 2 * pc;
-      const int ng = (rows_c + 31) / 32;
-      int begin = (int)cta_grps[c].size();
-      int r0 = row;
-      for (int gi = 0; gi < ng; ++gi) {
-        const int gp = pc / ng + (gi < pc % ng ? 1 : 0);
-        const int gr = 2 * gp;
-        int m = 1;
-        for (int d = 1; d <= KB; ++d)
-          if (KB % d == 0 && (size_t)gr * 512 * d <= (size_t)STAGE_BYTES) m = d;
-        const int ntiles = KB / m;
-        Tmp t{c, sg, r0, gr, m, ntiles, (uint64_t)gr * K * esz, seg_rowsrc0[sg] + (uint32_t)r0};
-        tmp.push_back(t);
-        Grp g; g.off16 = 0; g.row0 = r0; g.rows = (uint16_t)gr; g.m = (uint16_t)m; g.ntiles = (uint16_t)ntiles; g.pad = 0;
-        cta_grps[c].push_back(g);
-        r0 += gr;
-      }
-      if (ng > 255) return fail(FQ3_ERR_INVALID, "segment %d: too many groups per CTA", sg);
-      segtab[(size_t)c * nseg + sg] = ((uint32_t)begin << 8) | (uint32_t)ng;
-      row += rows_c;
-    }
-    rot = (rot + extra) % ncta;
-  }
-  // tape offsets: CTA-major, segment order
-  std::vector<uint64_t> cta_base(ncta + 1, 0);
-  {
-    std::vector<uint64_t> sz(ncta, 0);
-    for (auto& t : tmp) sz[t.cta] += t.bytes;
-    for (int c = 0; c < ncta; ++c) cta_base[c + 1] = cta_base[c] + ((sz[c] + 1023) / 1024) * 1024;
-  }
-  const uint64_t tape_bytes = cta_base[ncta];
-  if (tape_bytes / 16 > 0xffffffffull) return fail(FQ3_ERR_INVALID, "tape too large");
-  {
-    std::vector<uint64_t> cur(cta_base.begin(), cta_base.end() - 1);
-    std::vector<int> gidx(ncta, 0);
-    for (auto& t : tmp) {
-      Grp& g = cta_grps[t.cta][gidx[t.cta]++];
-      g.off16 = (uint32_t)(cur[t.cta] / 16);
-      PackGrp pg; pg.tape_off = cur[t.cta]; pg.rowsrc_idx = t.rsrc;
-      pg.rows = (uint16_t)t.rows; pg.m = (uint16_t)t.m; pg.ntiles = (uint16_t)t.ntiles; pg.pad = 0; pg.K = segs[t.seg].K;
-      pack.push_back(pg);
-      cur[t.cta] += t.bytes;
-    }
-  }
-  std::vector<uint32_t> goff(ncta + 1, 0);
-  std::vector<Grp> allg;
-  for (int c = 0; c < ncta; ++c) {
-    if ((int)cta_grps[c].size() > MAXGRP) return fail(FQ3_ERR_INVALID, "CTA %d has %zu row groups (> %d)", c, cta_grps[c].size(), MAXGRP);
-    goff[c + 1] = goff[c] + (uint32_t)cta_grps[c].size();
-    allg.insert(allg.end(), cta_grps[c].begin(), cta_grps[c].end());
-  }
-  // ---- upload tables, pack
   if (e->tape) { cudaFree(e->tape); e->tape = nullptr; }
-  if (e->grps) { cudaFree(e->grps); e->grps = nullptr; }
-  if (e->segtab) { cudaFree(e->segtab); e->segtab = nullptr; }
-  if (e->cta_grp_off) { cudaFree(e->cta_grp_off); e->cta_grp_off = nullptr; }
-  CK(cudaMalloc(&e->tape, tape_bytes));
-  e->tape_bytes = tape_bytes;
-  CK(cudaMalloc(&e->grps, allg.size() * sizeof(Grp)));
-  CK(cudaMalloc(&e->segtab, segtab.size() * sizeof(uint32_t)));
-  CK(cudaMalloc(&e->cta_grp_off, goff.size() * sizeof(uint32_t)));
-  CK(cudaMemcpyAsync(e->grps, allg.data(), allg.size() * sizeof(Grp), cudaMemcpyHostToDevice, stream));
-  CK(cudaMemcpyAsync(e->segtab, segtab.data(), segtab.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, stream));
-  CK(cudaMemcpyAsync(e->cta_grp_off, goff.data(), goff.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, stream));
-  void** d_rowsrc = nullptr;
+  CK(cudaMalloc(&e->tape, plan.tape_bytes));
+  e->tape_bytes = plan.tape_bytes;
+  const void** d_rowsrc = nullptr;
   PackGrp* d_pack = nullptr;
-  CK(cudaMalloc(&d_rowsrc, rowsrc.size() * sizeof(void*)));
-  CK(cudaMalloc(&d_pack, pack.size() * sizeof(PackGrp)));
-  CK(cudaMemcpyAsync(d_rowsrc, rowsrc.data(), rowsrc.size() * sizeof(void*), cudaMemcpyHostToDevice, stream));
-  CK(cudaMemcpyAsync(d_pack, pack.data(), pack.size() * sizeof(PackGrp), cudaMemcpyHostToDevice, stream));
-  {
-    const int grid = (int)std::min<size_t>(pack.size(), 132 * 16);
-    if (e->bf16) pack_mma_kernel<<<grid, 256, 0, stream>>>(d_pack, (int)pack.size(), (const void* const*)d_rowsrc, e->tape);
-    else pack_kernel<<<grid, 256, 0, stream>>>(d_pack, (int)pack.size(), (const void* const*)d_rowsrc, e->tape);
-    e->launches++;
-    CK(cudaGetLastError());
-  }
+  if ((rc = upload(&e->grps, plan.grps)) || (rc = upload(&e->segtab, plan.segtab)) ||
+      (rc = upload(&e->cta_grp_off, plan.cta_grp_off)) || (rc = upload(&d_rowsrc, rowsrc)) ||
+      (rc = upload(&d_pack, plan.pack)))
+    return rc;
+  const int npack = (int)plan.pack.size(), grid = std::min(npack, 132 * 16);
+  if (e->bf16) pack_mma_kernel<<<grid, 256, 0, stream>>>(d_pack, npack, d_rowsrc, e->tape);
+  else pack_kernel<<<grid, 256, 0, stream>>>(d_pack, npack, d_rowsrc, e->tape);
+  e->launches++;
+  CK(cudaGetLastError());
   CK(cudaStreamSynchronize(stream));
   cudaFree(d_rowsrc);
   cudaFree(d_pack);
   k.tape = e->tape; k.grps = e->grps; k.segtab = e->segtab; k.cta_grp_off = e->cta_grp_off;
-  // ---- byte accounting (algorithmic bytes)
-  {
-    uint64_t tl = 0, pl = 0, ph = 0, pm = 0;
-    for (int l = 0; l < k.t.L * 4; ++l) tl += segs[k.t.seg_base + l].bytes;
-    tl += segs[k.t.seg_head].bytes;
-    for (int l = 0; l < k.p.L * 4; ++l) pl += segs[k.p.seg_base + l].bytes;
-    for (int i = 0; i < k.ncb; ++i) ph += segs[k.p.seg_head + i].bytes;
-    if (k.seg_mtp >= 0) pm = segs[k.seg_mtp].bytes;
-    e->talker_step_bytes = (int64_t)tl;
-    e->predictor_frame_bytes = (int64_t)(k.ncb * pl + pm + ph);
-  }
+  // ---- byte accounting (algorithmic bytes): a stack's layers, its heads and the MTP projection are consecutive segments
+  auto bytes = [&](int sg0, int n) {
+    uint64_t b = 0;
+    for (int sg = sg0; sg < sg0 + n; ++sg) b += (uint64_t)e->segs[sg].rows * e->segs[sg].K * esz;
+    return b;
+  };
+  e->talker_step_bytes = (int64_t)bytes(k.t.seg_base, 4 * k.t.L + 1);
+  e->predictor_frame_bytes = (int64_t)(k.ncb * bytes(k.p.seg_base, 4 * k.p.L) + bytes(k.p.seg_head, k.ncb + (k.seg_mtp >= 0)));
   e->loaded = true;
   return 0;
 }
