@@ -117,6 +117,7 @@ struct KParams {
   void* ACT;                    // model dtype [2][ldACT]: SiLU(gate) * up, the down projection's input
   int ldX, ldQKV, ldATT, ldACT;
   unsigned* bar;
+  int* xerr;                    // sticky: set when a tagged exchange wait gave up (never cleared by a launch)
   const void* t_embed;
   const void* p_embeds;
   const void* mtp_b;
@@ -196,6 +197,66 @@ __device__ __forceinline__ unsigned ld_acquire_u32(const unsigned* p) {
 }
 __device__ __forceinline__ void csync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }  // consumers only
 
+// ---- tagged activation exchange (bf16 single-sequence kernel, DESIGN §4).  Every word of QKV, X1, X and LOGITS is an
+// fp32 word holding a bf16-rounded value, so its low 16 bits are zero; a producer stores bits(v) | tag and a consumer
+// polls the words it needs until their low half equals the exchange's tag, then masks it off.  No counter, no release
+// fence and no second load of the vector.  Tags count exchanges from 1 in every launch (the engine clears the four
+// buffers with the barrier words before each launch) and skip 0 when they wrap.
+constexpr uint32_t XTAG = 0xffffu;
+constexpr uint32_t XWAIT_CAP = 1u << 24;   // polls of one word before the launch gives up on it (seconds, not microseconds)
+__device__ __forceinline__ uint32_t xtag_next(uint32_t t) { return t == XTAG ? 1u : t + 1u; }
+__device__ __forceinline__ float untag(uint32_t w) { return __uint_as_float(w & ~XTAG); }
+__device__ __forceinline__ void st_tagged(float* p, float v, uint32_t tag) {   // v: bf16-rounded
+  asm volatile("st.relaxed.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(__float_as_uint(v) | tag) : "memory");
+}
+__device__ __forceinline__ uint32_t ld_relaxed_u32(const void* p) {
+  uint32_t v;
+  asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ uint4 ld_relaxed_v4(const void* p) {
+  uint4 v;
+  asm volatile("ld.relaxed.gpu.global.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p) : "memory");
+  return v;
+}
+// a wait that passes XWAIT_CAP polls is a protocol bug: it sets *err (the engine turns it into an error return) and
+// gives up, so the launch runs to its end instead of hanging the GPU; once *err is set, every other wait gives up too
+__device__ __noinline__ bool xwait_give_up(int* err, uint32_t n) {
+  if (n >= XWAIT_CAP) {
+    atomicOr(err, 1);
+    return true;
+  }
+  return ld_relaxed_u32(err) != 0;
+}
+__device__ __forceinline__ bool xtag_ok(uint32_t w, uint32_t tag) { return (w & XTAG) == tag; }
+__device__ __forceinline__ bool xtag_ok(const uint4& w, uint32_t tag) {
+  return xtag_ok(w.x, tag) & xtag_ok(w.y, tag) & xtag_ok(w.z, tag) & xtag_ok(w.w, tag);
+}
+// w: a word (or 16-byte vector) already loaded from p; re-polls p alone, with a growing back-off, until it carries tag
+template <class W>
+__device__ __forceinline__ W xwait(int* err, const void* p, W w, uint32_t tag) {
+  uint32_t ns = 32, n = 0;
+  while (!xtag_ok(w, tag)) {
+    if ((++n & 1023u) == 0u && xwait_give_up(err, n)) break;
+    __nanosleep(ns);
+    ns = ns < 256 ? 2 * ns : ns;
+    if constexpr (sizeof(W) == 16) w = ld_relaxed_v4(p);
+    else w = ld_relaxed_u32(p);
+  }
+  return w;
+}
+// one polled word / 16-byte vector of an exchanged buffer, tag masked off
+__device__ __forceinline__ float xload(int* err, const float* p, uint32_t tag) {
+  uint32_t w = ld_relaxed_u32(p);
+  if (!xtag_ok(w, tag)) w = xwait(err, p, w, tag);
+  return untag(w);
+}
+__device__ __forceinline__ float4 xload4(int* err, const float* p, uint32_t tag) {
+  uint4 w = ld_relaxed_v4(p);
+  if (!xtag_ok(w, tag)) w = xwait(err, p, w, tag);
+  return make_float4(untag(w.x), untag(w.y), untag(w.z), untag(w.w));
+}
+
 template <bool BF>
 __device__ __forceinline__ float rnd(float x) {
   if constexpr (BF)
@@ -216,6 +277,18 @@ __device__ __forceinline__ void stw(void* p, size_t i, float v) {
     reinterpret_cast<__nv_bfloat16*>(p)[i] = __float2bfloat16_rn(v);
   else
     reinterpret_cast<float*>(p)[i] = v;
+}
+// an exchanged fp32 activation word: bf16 stores it tagged, fp32 (all 32 bits in use) plainly behind a grid barrier;
+// xget reads one that this CTA has already polled, so it only masks the tag
+template <bool BF>
+__device__ __forceinline__ void xput(float* p, float v, uint32_t tag) {
+  if constexpr (BF) st_tagged(p, v, tag);
+  else *p = v;
+}
+template <bool BF>
+__device__ __forceinline__ float xget(const float* p) {
+  if constexpr (BF) return untag(__float_as_uint(__ldcg(p)));
+  else return __ldcg(p);
 }
 __device__ __forceinline__ float bf_lo(uint32_t u) { return __uint_as_float(u << 16); }
 __device__ __forceinline__ float bf_hi(uint32_t u) { return __uint_as_float(u & 0xffff0000u); }
@@ -264,6 +337,7 @@ struct Ctx {
   int tid, warp, lane;
   uint32_t tile_ctr;   // tiles consumed (identical in every consumer thread)
   unsigned bar_target; // thread 0 only
+  uint32_t xtag;       // tag of the latest tagged exchange (identical in every consumer thread of every CTA)
 };
 
 // ------------------------------------------------------------------------------------------------------------
@@ -537,10 +611,11 @@ struct Producer {
 // attention (attention_split) reads cached rows through the async proxy (TMA), in this launch or a later one, so every
 // append is followed by a proxy fence.
 // ------------------------------------------------------------------------------------------------------------
-template <bool BF>
+// XT: the QKV row is a tagged exchange (tag `tag`): the three rows are polled, not read after a grid barrier
+template <bool BF, bool XT = false>
 __device__ __forceinline__ void head_qkv(Ctx& c, const StackDev& S, int layer, int h, const float* qkv, int rpos,
                                          float* qs, float* ks, float* vs, void* kv, const int* pages, int slot,
-                                         bool append) {
+                                         bool append, uint32_t tag = 0) {
   if (c.warp < 3) {
     const int what = c.warp, g = h / S.rep;
     const float* src = qkv + (what == 0 ? h * 128 : (what == 1 ? S.qd + g * 128 : S.qd + S.kd + g * 128));
@@ -553,10 +628,18 @@ __device__ __forceinline__ void head_qkv(Ctx& c, const StackDev& S, int layer, i
 #pragma unroll
       for (int i = 0; i < 4; ++i) {  // all global loads of this step issued back to back
         const int e = c.lane + 32 * i;
-        v[i] = __ldcg(src + e);
+        v[i] = XT ? __uint_as_float(ld_relaxed_u32(src + e)) : __ldcg(src + e);
         nwv[i] = what < 2 ? ldw<BF>(nw, (size_t)layer * 128 + e) : 0.f;
         cc[i] = what < 2 ? __ldg(cs + e) : 0.f;
         sv[i] = what < 2 ? __ldg(sn + e) : 0.f;
+      }
+      if constexpr (XT) {  // the loads above were the first poll: re-poll only the words still stale, then untag
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          uint32_t w = __float_as_uint(v[i]);
+          if (!xtag_ok(w, tag)) w = xwait(c.P.xerr, src + c.lane + 32 * i, w, tag);
+          v[i] = untag(w);
+        }
       }
     }
     if (what < 2) {
@@ -594,9 +677,9 @@ __device__ __forceinline__ void head_qkv(Ctx& c, const StackDev& S, int layer, i
 // pages: the page pool and the request's page table; the head's output goes to att[h*128 .. h*128+128) in model dtype.
 // Both kernels run it.
 // ------------------------------------------------------------------------------------------------------------
-template <bool BF>
+template <bool BF, bool XT = false>
 __device__ void attention_head(Ctx& c, const StackDev& S, int layer, int h, const float* __restrict__ qkv, void* pool,
-                               const int* pages, void* att, int slot0, int rpos0, int kv_start) {
+                               const int* pages, void* att, int slot0, int rpos0, int kv_start, uint32_t tag = 0) {
   float* sc = SMEM().xs;            // scores [SEQMAX]
   float* qs = SMEM().xs + SEQMAX;   // [128]
   float* ks = qs + 128;             // [128]
@@ -605,7 +688,7 @@ __device__ void attention_head(Ctx& c, const StackDev& S, int layer, int h, cons
   const int g = h / S.rep;
   const size_t esz = BF ? 2 : 4;
   // --- a. q/k norm + rope, v copy; the first q-head of each kv group appends the new row
-  head_qkv<BF>(c, S, layer, h, qkv, rpos0, qs, ks, vs, pool, pages, slot0, (h % S.rep) == 0);
+  head_qkv<BF, XT>(c, S, layer, h, qkv, rpos0, qs, ks, vs, pool, pages, slot0, (h % S.rep) == 0, tag);
   const float scale = 0.08838834764831845f;  // 128^-0.5
   const int nk = slot0 + 1 - kv_start;       // visible keys
   const int nold = slot0 - kv_start;         // keys that live in the global cache
@@ -753,7 +836,8 @@ __device__ void attention_split(Ctx& c, const StackDev& S, int layer, int slot0,
   float* vs = ks + 128;            // [128]
   float* opart = vs + 128;         // [8][128]
   // --- a. q/k norm + rope, v copy; one CTA per kv group appends the new row
-  head_qkv<BF>(c, S, layer, h, P.QKV, rpos0, qs, ks, vs, P.req.kv, SMEM().kvtab, slot0, sp == 0 && (h % S.rep) == 0);
+  head_qkv<BF, BF>(c, S, layer, h, P.QKV, rpos0, qs, ks, vs, P.req.kv, SMEM().kvtab, slot0, sp == 0 && (h % S.rep) == 0,
+                   c.xtag);
   const KvSlice sl = kv_slice(slot0 - kv_start, Sx, sp);
   const bool has_new = sp == Sx - 1;
   const int nloc = sl.n + (has_new ? 1 : 0);
@@ -891,6 +975,7 @@ struct SampleArgs {
   bool suppress_eos;
   int eos;
   float* lp = nullptr;  // when set, thread 0 writes the log-probability of the drawn id here (DESIGN.md §4)
+  uint32_t xtag = 0;    // nonzero (bf16): logits is a tagged exchange with this tag, polled instead of read after a barrier
 };
 
 __device__ __forceinline__ uint32_t fkey(float f) {  // order-preserving float -> uint
@@ -906,8 +991,19 @@ __device__ int sample_block(Ctx& c, const SampleArgs& a) {
   float* lg = SMEM().xs;  // [V]
   const int V = a.V;
   const int sup0 = a.sup0;
+  if (BF && a.xtag) {  // every word of the thread's share in flight at once, then only the stale ones re-polled
+    constexpr int VPT = VMAX / NCT;
+    uint32_t w[VPT];
+#pragma unroll
+    for (int i = 0; i < VPT; ++i) w[i] = c.tid + i * NCT < V ? ld_relaxed_u32(a.logits + c.tid + i * NCT) : a.xtag;
+#pragma unroll
+    for (int i = 0; i < VPT; ++i) {
+      if (!xtag_ok(w[i], a.xtag)) w[i] = xwait(c.P.xerr, a.logits + c.tid + i * NCT, w[i], a.xtag);
+      if (c.tid + i * NCT < V) lg[c.tid + i * NCT] = untag(w[i]);
+    }
+  }
   for (int v = c.tid; v < V; v += NCT) {
-    float l = __ldcg(a.logits + v);
+    float l = (BF && a.xtag) ? lg[v] : __ldcg(a.logits + v);
     if (a.use_penalty && a.sp.penalty != 1.0f && ((SMEM().seen[v >> 5] >> (v & 31)) & 1u))
       l = l > 0.f ? rnd<BF>(l / a.sp.penalty) : rnd<BF>(l * a.sp.penalty);
     if ((v >= sup0 && v != a.eos) || (a.suppress_eos && v == a.eos)) l = -INFINITY;
@@ -1401,9 +1497,11 @@ __device__ __forceinline__ void small_kv_preload(Ctx& c, const StackDev& S, int 
 //   qkv0: QKV row of token 0, token t lives qkv_tstride floats further; kc / vc: the request's predictor caches;
 //   append: this CTA writes the new K/V rows; pre: cached rows already in registers (or nullptr);
 //   out(t, i, v): stores element i of token t's attention output (model-dtype rounded)
-template <bool BF, int NT, class Out>
+//   XT: the QKV rows are the tagged exchange `tag`, polled (everything else of round trip 1 is issued first)
+template <bool BF, int NT, bool XT = false, class Out>
 __device__ void attention_small_all(Ctx& c, const StackDev& S, int layer, int slot0_, int rpos0, const float* __restrict__ qkv0,
-                                    size_t qkv_tstride, void* kc, void* vc, bool append, const SmallKV<BF>* pre, Out out) {
+                                    size_t qkv_tstride, void* kc, void* vc, bool append, const SmallKV<BF>* pre, Out out,
+                                    uint32_t tag = 0) {
   constexpr int NOLD = NT == 2 ? 1 : 16;  // cached keys that can exist
   constexpr int MAXK = NT == 2 ? 2 : 17;
   const int slot0 = NT == 2 ? 0 : slot0_;
@@ -1437,14 +1535,35 @@ __device__ void attention_small_all(Ctx& c, const StackDev& S, int layer, int sl
 #pragma unroll
       for (int t = 0; t < NT; ++t) small_norm_rope_load<BF>(c, S, layer, rpos0 + t, qn4, kn4, cs4[t], sn4[t]);
     }
-#pragma unroll
-    for (int t = 0; t < NT; ++t) {
+    auto qkv_at = [&](int t, int which) {   // which: 0, 1 = q of the group's heads, 2 = k, 3 = v
       const float* row = qkv0 + (size_t)t * qkv_tstride;
-      kr4[t] = __ldcg(reinterpret_cast<const float4*>(row + S.qd + g * 128) + c.lane);
-      vr4[t] = __ldcg(reinterpret_cast<const float4*>(row + S.qd + S.kd + g * 128) + c.lane);
+      return row + (which == 2 ? S.qd + g * 128 : which == 3 ? S.qd + S.kd + g * 128
+                                                 : (g * S.rep + (which < S.rep ? which : 0)) * 128) + L4;
+    };
+    if constexpr (XT) {
+      uint4 w[NT][4];
 #pragma unroll
-      for (int hh = 0; hh < 2; ++hh)
-        qr4[hh][t] = __ldcg(reinterpret_cast<const float4*>(row + (g * S.rep + (hh < S.rep ? hh : 0)) * 128) + c.lane);
+      for (int t = 0; t < NT; ++t)
+#pragma unroll
+        for (int q = 0; q < 4; ++q) w[t][q] = ld_relaxed_v4(qkv_at(t, q));
+      auto un = [](const uint4& u) { return make_float4(untag(u.x), untag(u.y), untag(u.z), untag(u.w)); };
+#pragma unroll
+      for (int t = 0; t < NT; ++t) {
+#pragma unroll
+        for (int q = 0; q < 4; ++q)
+          if (!xtag_ok(w[t][q], tag)) w[t][q] = xwait(c.P.xerr, qkv_at(t, q), w[t][q], tag);
+        qr4[0][t] = un(w[t][0]); qr4[1][t] = un(w[t][1]); kr4[t] = un(w[t][2]); vr4[t] = un(w[t][3]);
+      }
+    } else {
+#pragma unroll
+      for (int t = 0; t < NT; ++t) {
+        const float* row = qkv0 + (size_t)t * qkv_tstride;
+        kr4[t] = __ldcg(reinterpret_cast<const float4*>(row + S.qd + g * 128) + c.lane);
+        vr4[t] = __ldcg(reinterpret_cast<const float4*>(row + S.qd + S.kd + g * 128) + c.lane);
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh)
+          qr4[hh][t] = __ldcg(reinterpret_cast<const float4*>(row + (g * S.rep + (hh < S.rep ? hh : 0)) * 128) + c.lane);
+      }
     }
     auto norm_rope = [&](float* v, const float4& w4, const float4& c4, const float4& s4) {
       const float w[4] = {w4.x, w4.y, w4.z, w4.w}, cc[4] = {c4.x, c4.y, c4.z, c4.w}, sv[4] = {s4.x, s4.y, s4.z, s4.w};
@@ -1614,6 +1733,7 @@ __device__ __forceinline__ void norm_wload(Ctx& c, const void* w, size_t woff, i
     wv[i] = k < H ? ldw<BF>(w, woff + k) : 0.f;
   }
 }
+// bf16: a global src is the tagged exchange c.xtag (X or X1), polled
 template <bool BF>
 __device__ __forceinline__ void norm_stage(Ctx& c, const float* src, bool src_smem, const void* w, size_t woff, int H,
                                            float eps, int off, const float* wpre = nullptr) {
@@ -1625,8 +1745,17 @@ __device__ __forceinline__ void norm_stage(Ctx& c, const float* src, bool src_sm
     v[i] = 0.f;
     wv[i] = 0.f;
     if (k < H) {
-      v[i] = src_smem ? src[k] : __ldcg(src + k);
+      v[i] = src_smem ? src[k] : (BF ? __uint_as_float(ld_relaxed_u32(src + k)) : __ldcg(src + k));
       wv[i] = wpre ? wpre[i] : ldw<BF>(w, woff + k);
+    }
+  }
+  if (BF && !src_smem) {
+#pragma unroll
+    for (int i = 0; i < MAXE; ++i) {
+      const int k = c.tid + i * NCT;
+      uint32_t u = __float_as_uint(v[i]);
+      if (k < H && !xtag_ok(u, c.xtag)) u = xwait(c.P.xerr, src + k, u, c.xtag);
+      v[i] = untag(u);
     }
   }
   float ss = 0.f;
@@ -1671,30 +1800,37 @@ __device__ void run_layers(Ctx& c, const StackDev& S, int nt, int slot0, int rpo
       else norm_stage<BF>(c, P.X + (size_t)t * P.ldX, false, S.ln_in, (size_t)l * S.H, S.H, S.eps, t * S.H, wp);
     }
     probe(c, pi);  // 1: after input norm
-    gemv_any<BF, false>(c, S.seg_base + 4 * l + 0, nt, S.H, nopre,
-                        [&](int row, int t, float v, float, float) { P.QKV[(size_t)t * P.ldQKV + row] = rnd<BF>(v); });
+    // bf16: QKV, X1 and X are tagged exchanges (B1, B3, B5 are polls, not grid barriers); every CTA advances the tag
+    if constexpr (BF) c.xtag = xtag_next(c.xtag);
+    const uint32_t xt_qkv = c.xtag;
+    gemv_any<BF, false>(c, S.seg_base + 4 * l + 0, nt, S.H, nopre, [&](int row, int t, float v, float, float) {
+      xput<BF>(P.QKV + (size_t)t * P.ldQKV + row, rnd<BF>(v), xt_qkv);
+    });
     probe(c, pi);  // 2: after QKV gemv
     const bool small_attn = !TALKER;   // geometry checked by fq3_engine_create (cache <= 32 slots, <= 2 q-heads per kv head)
     // a warp preloads its own kv group (warp < nKV); attention_small_all reads further groups (nKV > NCW) itself
     const bool kv_pre = small_attn && nt == 1;
     SmallKV<BF> skv;
-    grid_arrive(c);
+    if constexpr (!BF) grid_arrive(c);
     // cached keys/values, norm weights and RoPE rows do not depend on this layer's QKV
     if (kv_pre) small_kv_preload<BF>(c, S, l, slot0, rpos0, kc, vc, skv);
-    grid_wait(c);
+    if constexpr (!BF) grid_wait(c);
     probe(c, pi);  // 3: after B1
     if (dbg && cta0) {
       float* d = P.dbg + (size_t)l * P.dbg_stride_layer;
       for (int t = 0; t < nt; ++t)
-        for (int k = c.tid; k < S.qd + 2 * S.kd; k += NCT) d[(size_t)t * (S.qd + 2 * S.kd) + k] = __ldcg(P.QKV + (size_t)t * P.ldQKV + k);
+        for (int k = c.tid; k < S.qd + 2 * S.kd; k += NCT) {
+          const float* q = P.QKV + (size_t)t * P.ldQKV + k;
+          d[(size_t)t * (S.qd + 2 * S.kd) + k] = BF ? xload(P.xerr, q, c.xtag) : __ldcg(q);
+        }
     }
     if constexpr (!TALKER) {
       // ---- P2+P3 fused: redundant small attention straight into the staging vector (no exchange, no barrier)
       auto to_xs = [&](int t, int i, float v) { xs_put<BF>(c, t * S.qd + i, v); };
       // &skv unconditionally (nt == 1 always preloads): a pointer chosen at run time between skv and nullptr would
       // keep skv in local memory, so that every preloaded row took an STL and an LDL
-      if (nt == 1) attention_small_all<BF, 1>(c, S, l, slot0, rpos0, P.QKV, P.ldQKV, kc, vc, cta0, &skv, to_xs);
-      else attention_small_all<BF, 2>(c, S, l, slot0, rpos0, P.QKV, P.ldQKV, kc, vc, cta0, nullptr, to_xs);
+      if (nt == 1) attention_small_all<BF, 1, BF>(c, S, l, slot0, rpos0, P.QKV, P.ldQKV, kc, vc, cta0, &skv, to_xs, c.xtag);
+      else attention_small_all<BF, 2, BF>(c, S, l, slot0, rpos0, P.QKV, P.ldQKV, kc, vc, cta0, nullptr, to_xs, c.xtag);
       probe(c, pi);  // 4
       probe(c, pi);  // 5
     } else {
@@ -1704,7 +1840,7 @@ __device__ void run_layers(Ctx& c, const StackDev& S, int nt, int slot0, int rpo
       if (split) attention_split<BF>(c, S, l, slot0, rpos0, kv_start);
       else
         for (int h = blockIdx.x; h < S.nH; h += gridDim.x)
-          attention_head<BF>(c, S, l, h, P.QKV, P.req.kv, SMEM().kvtab, P.ATT, slot0, rpos0, kv_start);
+          attention_head<BF, BF>(c, S, l, h, P.QKV, P.req.kv, SMEM().kvtab, P.ATT, slot0, rpos0, kv_start, c.xtag);
       if (!split && is_talker && (int)blockIdx.x >= S.nH && slot0 - kv_start > 64) {
         // idle CTAs pull the NEXT layer's keys/values into L2 (evict_last) so the attention CTAs see L2 latency
         const int ln = (l + 1) % S.L;
@@ -1743,16 +1879,20 @@ __device__ void run_layers(Ctx& c, const StackDev& S, int nt, int slot0, int rpo
     }
     {
       const bool loc = (l == 0 && x0_local);
+      if constexpr (BF) c.xtag = xtag_next(c.xtag);
+      const uint32_t xt_x1 = c.xtag;
       gemv_any<BF, false>(
           c, S.seg_base + 4 * l + 1, nt, S.qd,
-          [&](int row, int t) { return loc ? SMEM().xin[t][row] : __ldcg(P.X + (size_t)t * P.ldX + row); },
-          [&](int row, int t, float v, float, float res) { P.X1[(size_t)t * P.ldX + row] = rnd<BF>(res + rnd<BF>(v)); });
+          [&](int row, int t) { return loc ? SMEM().xin[t][row] : xget<BF>(P.X + (size_t)t * P.ldX + row); },
+          [&](int row, int t, float v, float, float res) {
+            xput<BF>(P.X1 + (size_t)t * P.ldX + row, rnd<BF>(res + rnd<BF>(v)), xt_x1);
+          });
     }
     probe(c, pi);  // 6: after O gemv
     float wpost[NORM_E];
-    grid_arrive(c);
+    if constexpr (!BF) grid_arrive(c);
     norm_wload<BF>(c, S.ln_post, (size_t)l * S.H, S.H, wpost);
-    grid_wait(c);
+    if constexpr (!BF) grid_wait(c);
     probe(c, pi);  // 7: after B3
     // ---- P4: post-attention norm + gate/up rows + SiLU*up
     for (int t = 0; t < nt; ++t)
@@ -1760,7 +1900,7 @@ __device__ void run_layers(Ctx& c, const StackDev& S, int nt, int slot0, int rpo
     if (dbg && cta0) {
       float* d = P.dbg + (size_t)l * P.dbg_stride_layer + (size_t)2 * (S.qd + 2 * S.kd) + 2 * S.qd;
       for (int t = 0; t < nt; ++t)
-        for (int k = c.tid; k < S.H; k += NCT) d[(size_t)t * S.H + k] = __ldcg(P.X1 + (size_t)t * P.ldX + k);
+        for (int k = c.tid; k < S.H; k += NCT) d[(size_t)t * S.H + k] = xget<BF>(P.X1 + (size_t)t * P.ldX + k);
     }
     gemv_any<BF, true>(c, S.seg_base + 4 * l + 2, nt, S.H, nopre, [&](int pair, int t, float gv, float uv, float) {
       const float gte = rnd<BF>(gv), up = rnd<BF>(uv);
@@ -1780,33 +1920,47 @@ __device__ void run_layers(Ctx& c, const StackDev& S, int nt, int slot0, int rpo
           else d[(size_t)t * S.I + k] = __ldcg(reinterpret_cast<const float*>(P.ACT) + i);
         }
     }
+    if constexpr (BF) c.xtag = xtag_next(c.xtag);
+    const uint32_t xt_x = c.xtag;
     gemv_any<BF, false, true>(
-        c, S.seg_base + 4 * l + 3, nt, S.I, [&](int row, int t) { return __ldcg(P.X1 + (size_t)t * P.ldX + row); },
-        [&](int row, int t, float v, float, float res) { P.X[(size_t)t * P.ldX + row] = rnd<BF>(res + rnd<BF>(v)); },
+        c, S.seg_base + 4 * l + 3, nt, S.I, [&](int row, int t) { return xget<BF>(P.X1 + (size_t)t * P.ldX + row); },
+        [&](int row, int t, float v, float, float res) {
+          xput<BF>(P.X + (size_t)t * P.ldX + row, rnd<BF>(res + rnd<BF>(v)), xt_x);
+        },
         P.ACT, P.ldACT);
     probe(c, pi);  // 10: after DN gemv
-    grid_arrive(c);
+    if constexpr (!BF) grid_arrive(c);
     if (l + 1 < S.L) norm_wload<BF>(c, S.ln_in, (size_t)(l + 1) * S.H, S.H, wnext);
     else norm_wload<BF>(c, S.ln_f, 0, S.H, wnext);
-    grid_wait(c);
+    if constexpr (!BF) grid_wait(c);
     probe(c, pi);  // 11: after B5
     if (dbg && cta0) {
       float* d = P.dbg + (size_t)l * P.dbg_stride_layer + (size_t)2 * (S.qd + 2 * S.kd) + 2 * S.qd + 2 * S.H + 2 * S.I;
       for (int t = 0; t < nt; ++t)
-        for (int k = c.tid; k < S.H; k += NCT) d[(size_t)t * S.H + k] = __ldcg(P.X + (size_t)t * P.ldX + k);
+        for (int k = c.tid; k < S.H; k += NCT) {
+          const float* x = P.X + (size_t)t * P.ldX + k;
+          d[(size_t)t * S.H + k] = BF ? xload(P.xerr, x, c.xtag) : __ldcg(x);
+        }
     }
   }
   // final norm of the last token -> staging vector [0..H)
   norm_stage<BF>(c, P.X + (size_t)(nt - 1) * P.ldX, false, S.ln_f, 0, S.H, S.eps, 0, wnext);
 }
 
-// head GEMV (rows of a [V,H] matrix) on the staging vector -> LOGITS, then grid barrier
+// head GEMV (rows of a [V,H] matrix) on the staging vector -> LOGITS.  tagged (bf16 predictor): LOGITS is the tagged
+// exchange c.xtag, which the sampler polls; otherwise a grid barrier follows.  The talker's head keeps its barrier: the
+// next frame's MTP projection writes X with no other barrier in between, and a CTA that owns no head rows may still
+// be reading X in the talker's final norm
 template <bool BF>
-__device__ __forceinline__ void head_logits(Ctx& c, int seg, int H) {
+__device__ __forceinline__ void head_logits(Ctx& c, int seg, int H, bool tagged) {
   const KParams& P = c.P;
-  gemv_any<BF, false>(c, seg, 1, H, [](int, int) { return 0.f; },
-                      [&](int row, int, float v, float, float) { P.LOGITS[row] = rnd<BF>(v); });
-  grid_sync(c);
+  if (tagged) c.xtag = xtag_next(c.xtag);
+  const uint32_t xt = c.xtag;
+  gemv_any<BF, false>(c, seg, 1, H, [](int, int) { return 0.f; }, [&](int row, int, float v, float, float) {
+    if (tagged) st_tagged(P.LOGITS + row, rnd<BF>(v), xt);
+    else P.LOGITS[row] = rnd<BF>(v);
+  });
+  if (!tagged) grid_sync(c);
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -1866,20 +2020,25 @@ __device__ void predictor_frame(Ctx& cio, const float* u15, bool dbg, float* lp_
       for (int t = 0; t < nt; ++t)
         for (int k = c.tid; k < Ht; k += NCT) xs_put<BF>(c, t * Ht + k, SMEM().xin[t][k]);
       csync();
+      if constexpr (BF) c.xtag = xtag_next(c.xtag);   // bf16: X is a tagged exchange, polled by layer 0's input norm
+      const uint32_t xt = c.xtag;
       gemv_any<BF, false>(c, P.seg_mtp, nt, Ht, [&](int row, int) { return P.mtp_b ? ldw<BF>(P.mtp_b, row) : 0.f; },
-                          [&](int row, int t, float v, float, float b) { P.X[(size_t)t * P.ldX + row] = rnd<BF>(v + b); });
-      grid_sync(c);
+                          [&](int row, int t, float v, float, float b) {
+                            xput<BF>(P.X + (size_t)t * P.ldX + row, rnd<BF>(v + b), xt);
+                          });
+      if constexpr (!BF) grid_sync(c);
     }
     const int slot0 = (i == 0) ? 0 : i + 1;
     probe_at(c, 1024 + 8 * i + 1);
     run_layers<BF, false>(c, S, nt, slot0, slot0, 0, !project, dbg && i == 0);
     probe_at(c, 1024 + 8 * i + 2);
-    head_logits<BF>(c, S.seg_head + i, S.H);
+    head_logits<BF>(c, S.seg_head + i, S.H, BF);
     probe_at(c, 1024 + 8 * i + 3);
     SampleArgs sa;
     sa.logits = P.LOGITS; sa.V = S.V; sa.sp = P.req.sp_p; sa.u = u15 ? __ldg(u15 + i) : 0.f;
     sa.use_penalty = false; sa.sup0 = S.V; sa.suppress_eos = false; sa.eos = -1;
     sa.lp = lp_row ? lp_row + 1 + i : nullptr;
+    sa.xtag = BF ? c.xtag : 0u;
     const int tok = sample_block<BF>(c, sa);
     if (c.tid == 0) SMEM().codes[i + 1] = tok;
     if (i + 1 < P.ncb) {
@@ -1905,6 +2064,7 @@ __device__ void predictor_frame(Ctx& cio, const float* u15, bool dbg, float* lp_
   }
   cio.tile_ctr = c.tile_ctr;
   cio.bar_target = c.bar_target;
+  cio.xtag = c.xtag;
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -2063,7 +2223,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) fq3_decode_kernel(const __grid_co
         probe_at(c, pslot + 3);
         for (int k = tid; k < Ht; k += NCT) s.hid[k] = xs_get<BF>(c, k);   // past_hidden = post-norm hidden (generate.py:198)
         csync();
-        head_logits<BF>(c, P.t.seg_head, Ht);
+        head_logits<BF>(c, P.t.seg_head, Ht, false);
         probe_at(c, pslot + 4);
         const int next = sample_block<BF>(c, frame_talker_draw(P, rq, P.LOGITS, urow, step, lp_row));
         probe_at(c, pslot + 5);

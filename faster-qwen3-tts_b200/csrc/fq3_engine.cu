@@ -88,7 +88,10 @@ struct fq3_engine {
   void *p_kc = nullptr, *p_vc = nullptr;
   float *X = nullptr, *X1 = nullptr, *QKV = nullptr, *LOGITS = nullptr, *PART = nullptr;
   void *ATT = nullptr, *ACT = nullptr;  // model dtype
-  unsigned* bar = nullptr;
+  unsigned* bar = nullptr;   // one allocation: grid-barrier and split counters, then X, X1, QKV and LOGITS (xch_bytes)
+  size_t xch_bytes = 0;      // cleared before every decode launch
+  int* xerr = nullptr;       // sticky exchange-timeout word (KParams::xerr)
+  int* xerr_host = nullptr;  // pinned
   int* state = nullptr;
   int* state_host = nullptr;  // pinned
   float* past_hidden = nullptr;
@@ -299,10 +302,18 @@ static int engine_alloc(fq3_engine* e, const cudaDeviceProp& prop) {
                              (Pc.num_attention_heads + 2 * Pc.num_key_value_heads) * 128);
   const int ldATT = std::max(T.num_attention_heads, Pc.num_attention_heads) * 128;
   const int ldACT = std::max(T.intermediate_size, Pc.intermediate_size);
-  CK(cudaMalloc(&e->X, 2 * ldX * sizeof(float))); CK(cudaMalloc(&e->X1, 2 * ldX * sizeof(float)));
-  CK(cudaMalloc(&e->QKV, 2 * ldQKV * sizeof(float))); CK(cudaMalloc(&e->ATT, ldATT * e->esz));
-  CK(cudaMalloc(&e->ACT, 2 * ldACT * e->esz)); CK(cudaMalloc(&e->LOGITS, VMAX * sizeof(float)));
-  CK(zalloc((void**)&e->bar, 32768));
+  // the barrier words and the four tagged-exchange buffers (fq3_decode.cuh xput) share one allocation, so that the one
+  // memset before a launch clears the counters and every exchange tag: tags restart at 1 in each launch
+  e->xch_bytes = 32768 + (4 * (size_t)ldX + 2 * (size_t)ldQKV + VMAX) * sizeof(float);
+  CK(zalloc((void**)&e->bar, e->xch_bytes));
+  e->X = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(e->bar) + 32768);
+  e->X1 = e->X + 2 * ldX;
+  e->QKV = e->X1 + 2 * ldX;
+  e->LOGITS = e->QKV + 2 * ldQKV;
+  CK(zalloc((void**)&e->xerr, sizeof(int)));
+  CK(cudaMallocHost(&e->xerr_host, sizeof(int)));
+  CK(cudaMalloc(&e->ATT, ldATT * e->esz));
+  CK(cudaMalloc(&e->ACT, 2 * ldACT * e->esz));
   CK(cudaMalloc(&e->PART, (size_t)T.num_attention_heads * 16 * PART_STRIDE * sizeof(float)));
   CK(zalloc((void**)&e->state, STATE_BYTES * MS));
   CK(cudaMallocHost(&e->state_host, STATE_BYTES * e->max_batch));   // results of one launch: a row per column
@@ -346,6 +357,7 @@ static int engine_alloc(fq3_engine* e, const cudaDeviceProp& prop) {
   k.X = e->X; k.X1 = e->X1; k.QKV = e->QKV; k.ATT = e->ATT; k.ACT = e->ACT; k.LOGITS = e->LOGITS;
   k.ldX = ldX; k.ldQKV = ldQKV; k.ldATT = ldATT; k.ldACT = ldACT;
   k.bar = e->bar;
+  k.xerr = e->xerr;
   k.XB = e->XB; k.X1B = e->X1B; k.QKVB = e->QKVB; k.LOGB = e->LOGB;
   k.XNB = e->XNB; k.ATTB = e->ATTB; k.ACTB = e->ACTB; k.PINB = e->PINB; k.TOKB = e->TOKB;
   k.nslots = 0; k.sl = e->sl_dev;
@@ -367,7 +379,7 @@ static int engine_alloc(fq3_engine* e, const cudaDeviceProp& prop) {
 extern "C" void fq3_engine_destroy(fq3_engine* e) {
   if (!e) return;
   cudaSetDevice(e->dev);
-  void* ptrs[] = {e->kv, e->kv_tab, e->p_kc, e->p_vc, e->X, e->X1, e->QKV, e->ATT, e->ACT, e->LOGITS, e->PART, e->bar,
+  void* ptrs[] = {e->kv, e->kv_tab, e->p_kc, e->p_vc, e->ATT, e->ACT, e->PART, e->bar, e->xerr,
                   e->state, e->past_hidden, e->seen, e->dbg, e->tape, e->grps, e->segtab, e->cta_grp_off,
                   e->XB, e->X1B, e->QKVB, e->LOGB, e->XNB, e->ATTB, e->ACTB, e->PINB, e->TOKB, e->sl_dev};
   for (void* p : ptrs)
@@ -377,6 +389,7 @@ extern "C" void fq3_engine_destroy(fq3_engine* e) {
   for (void* p : e->pf_buf)
     if (p) cudaFree(p);
   if (e->state_host) cudaFreeHost(e->state_host);
+  if (e->xerr_host) cudaFreeHost(e->xerr_host);
   if (e->sl_host) cudaFreeHost(e->sl_host);
   if (e->kv_stage) cudaFreeHost(e->kv_stage);
   if (e->kv_stream) cudaStreamDestroy(e->kv_stream);
@@ -556,11 +569,11 @@ extern "C" int fq3_engine_load_weights(fq3_engine* e, const fq3_tensor* tensors,
 // launches
 // ------------------------------------------------------------------------------------------------------------
 // one cooperative launch of a persistent decode kernel: the single-sequence kernel (kp.nslots == 0) or the batched
-// one, in the engine's dtype, with the grid-barrier and attention-split counters cleared first
+// one, in the engine's dtype, with the grid-barrier and attention-split counters and the exchange tags cleared first
 static int launch_decode(fq3_engine* e, const KParams& kp, cudaStream_t stream) {
   const void* fn = kp.nslots == 0 ? (e->bf16 ? (const void*)fq3_decode_kernel<true> : (const void*)fq3_decode_kernel<false>)
                                   : (e->bf16 ? (const void*)fq3_decode_batch_kernel<true> : (const void*)fq3_decode_batch_kernel<false>);
-  CK(cudaMemsetAsync(e->bar, 0, 32768, stream));
+  CK(cudaMemsetAsync(e->bar, 0, e->xch_bytes, stream));
   void* args[] = {(void*)&kp};
   CK(cudaLaunchCooperativeKernel(fn, dim3(e->ncta), dim3(NTHREADS), args, smem_bytes(), stream));
   e->launches++;
@@ -857,7 +870,11 @@ extern "C" int fq3_decode_chunk_n(fq3_engine* e, const int32_t* slots, int32_t n
   if ((rc = launch_fused(e, slots, n_slots, n_frames, max_frames, (long long*)codes_out_dev, logprob_out_dev, stream))) return rc;
   for (int j = 0; j < n_slots; ++j)
     CK(cudaMemcpyAsync(e->state_host + 8 * j, e->state + 8 * slots[j], 32, cudaMemcpyDeviceToHost, stream));
+  CK(cudaMemcpyAsync(e->xerr_host, e->xerr, sizeof(int), cudaMemcpyDeviceToHost, stream));
   CK(cudaStreamSynchronize(stream));
+  // a tagged exchange gave up waiting in this launch or an earlier one (a protocol error, never expected): the
+  // activations of that launch are undefined, and so is every result since
+  if (*e->xerr_host) return fail(FQ3_ERR_CUDA, "decode kernel: an activation exchange timed out; results are undefined");
   for (int j = 0; j < n_slots; ++j) {
     const int* st = e->state_host + 8 * j;
     res[j].next_token = st[ST_TOKEN];
