@@ -7,7 +7,8 @@ not serialised behind a lock (:71,181): up to --max-batch requests share every p
 requests join between chunks (faster_qwen3_tts/serving.py).  A streamed response is a listener: it is paced at real time
 by default, so the engine, which makes audio several times faster than it is played, serves the clients closest to running
 dry first and holds up to --max-slots requests (each costs its KV cache) on --max-batch launch columns.  The request field
-"pace" overrides that: a number = playback speed relative to real time, null = as fast as possible.
+"pace" overrides that: a number = playback speed relative to real time, null = as fast as possible.  "speed" (0.25 - 4.0)
+is the speaking rate: the audio is time-stretched on the GPU after the codec, at the same pitch.
 
     python examples/openai_server.py --model synthetic:1.7B --max-batch 16 --port 8000
     curl -s localhost:8000/v1/audio/speech -H 'Content-Type: application/json' \\
@@ -37,7 +38,7 @@ def build_app(model, batcher, voices, default_voice):
         input: str
         voice: str = "alloy"
         response_format: str = "wav"   # wav | pcm
-        speed: float = 1.0             # accepted, not applied (as in the reference)
+        speed: float = 1.0             # speaking rate in [0.25, 4.0], same pitch
         pace: Optional[float] = 1.0    # the client plays at pace x real time; null: everything as fast as possible
 
     @app.get("/health")
@@ -56,8 +57,10 @@ def build_app(model, batcher, voices, default_voice):
             raise HTTPException(status_code=400, detail=f"response_format {fmt!r} not supported. Use: wav, pcm")
         if req.pace is not None and not req.pace > 0:
             raise HTTPException(status_code=400, detail=f"'pace' must be a positive number or null, got {req.pace}")
+        if not 0.25 <= req.speed <= 4.0:
+            raise HTTPException(status_code=400, detail=f"'speed' must be in [0.25, 4.0], got {req.speed}")
         ticket = batcher.submit(voice_clone_request(model, req.input, v.get("language", "Auto"), v["ref_audio"],
-                                                    v.get("ref_text", "")), pace=req.pace,
+                                                    v.get("ref_text", "")), pace=req.pace, speed=req.speed,
                                 max_new_tokens=v.get("max_new_tokens", 2048))
         loop = asyncio.get_event_loop()
         it = iter(ticket)

@@ -81,6 +81,8 @@ EXPORTS = [
     "fq3_codec_stream_create", "fq3_codec_stream_reset", "fq3_codec_stream_destroy", "fq3_codec_stream_frames",
     "fq3_codec_stream_decode", "fq3_codec_stream_copy", "fq3_codec_launch_count",
     "fq3_codec_destroy", "fq3_codec_last_error",
+    "fq3_tempo_create", "fq3_tempo_reset", "fq3_tempo_destroy", "fq3_tempo_released", "fq3_tempo_process",
+    "fq3_tempo_last_error",
 ]
 
 
@@ -184,6 +186,15 @@ def load_library() -> C.CDLL:
     lib.fq3_codec_launch_count.argtypes = [C.c_void_p]
     lib.fq3_codec_launch_count.restype = C.c_int64
     lib.fq3_codec_last_error.restype = C.c_char_p
+    lib.fq3_tempo_create.argtypes = [C.c_int32, C.c_double, C.POINTER(C.c_void_p)]
+    lib.fq3_tempo_reset.argtypes = [C.c_void_p]
+    lib.fq3_tempo_destroy.argtypes = [C.c_void_p]
+    lib.fq3_tempo_destroy.restype = None
+    lib.fq3_tempo_released.argtypes = [C.c_int32, C.c_int64, C.c_int64, C.c_int32]
+    lib.fq3_tempo_released.restype = C.c_int64
+    lib.fq3_tempo_process.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int32),
+                                      C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p]
+    lib.fq3_tempo_last_error.restype = C.c_char_p
     _lib = lib
     return lib
 

@@ -36,6 +36,23 @@ def take_uniforms(seed: int, max_new_tokens: int, device="cuda") -> torch.Tensor
     return torch.rand(int(max_new_tokens) + 1, 16, generator=g).to(device)
 
 
+def _check_speed(speed):
+    """a speaking rate outside [0.25, 4.0] is refused (ValueError) before anything is tokenized"""
+    from .tempo import quantize
+    quantize(speed)
+
+
+def _speed_kw(speed):
+    """``speed=`` for the delivery calls, only when it is not 1: at speed 1 every call is made exactly as without it"""
+    return {} if speed == 1.0 else {"speed": speed}
+
+
+def _pcm_device(speech_tokenizer):
+    """the device the codec leaves its PCM on"""
+    dev = getattr(speech_tokenizer, "_dev", None)
+    return dev if dev is not None else next(speech_tokenizer.decoder.parameters()).device
+
+
 class _StreamWindow:
     """Per-request state of the streaming codec-window policy (model.py:1052-1135), push-style so that several
     requests of a batch can each keep their own window while their code chunks arrive interleaved.
@@ -47,10 +64,11 @@ class _StreamWindow:
     reference's warmed template stream (``SpeechTokenizer.reference_stream``): same samples, one chunk's worth of work,
     and the reference itself is decoded once per voice instead of four times per request.  Phase 2 (25-frame context
     windows without the reference) is the reference's approximation and is decoded exactly as the reference does.
-    ``FQ3_PHASE1_STREAM=0`` keeps the literal re-decode."""
+    ``FQ3_PHASE1_STREAM=0`` keeps the literal re-decode.  ``tempo``: the request's speaking rate (``tempo.Tempo``),
+    applied to the new samples on the device before they are converted (``decode_windows_batched``)."""
 
-    def __init__(self, owner, speech_tokenizer, ref_codes, chunk_size, to_host=True):
-        self.st, self.ref_codes = speech_tokenizer, ref_codes
+    def __init__(self, owner, speech_tokenizer, ref_codes, chunk_size, to_host=True, tempo=None):
+        self.st, self.ref_codes, self.tempo = speech_tokenizer, ref_codes, tempo
         self.min_cal = max(CONTEXT_FRAMES, chunk_size)
         self.all_codes, self.prev_len, self.spf = [], 0, None
         self.conv = owner._to_numpy if to_host else (lambda a: a.flatten())
@@ -84,8 +102,9 @@ class _StreamWindow:
         return window, ("phase2", window.shape[0] - n_new, 0)
 
     def finish(self, audio, meta):
-        """decoded window -> the new samples of this chunk (trim of the reference / of the 25-frame context)"""
-        audio = self.conv(audio)
+        """decoded window -> the new samples of this chunk (trim of the reference / of the 25-frame context), still where
+        the codec left them"""
+        audio = audio.flatten()
         kind, a, b = meta
         if kind == "phase1_stream":   # the stream produced exactly gen_audio[prev_len:] of the reference's Phase 1
             self.prev_len += len(audio)
@@ -109,8 +128,8 @@ class _StreamWindow:
         n_ctx = a
         return audio[int(round(n_ctx * self.spf)):] if n_ctx > 0 else audio
 
-    def push(self, codec_chunk):
-        return decode_windows_batched(self.st, [self], [codec_chunk])[0]
+    def push(self, codec_chunk, final=False):
+        return decode_windows_batched(self.st, [self], [codec_chunk], [final])[0]
 
 
 class _StatefulWindow:
@@ -122,46 +141,66 @@ class _StatefulWindow:
 
     any_chunking = True   # the PCM of a stream does not depend on how its frames are split into chunks
 
-    def __init__(self, owner, speech_tokenizer, ref_codes, chunk_size, to_host=True):
-        self.st = speech_tokenizer
+    def __init__(self, owner, speech_tokenizer, ref_codes, chunk_size, to_host=True, tempo=None):
+        self.st, self.tempo = speech_tokenizer, tempo
         self.stream = speech_tokenizer.open_stream()
         self.conv = owner._to_numpy if to_host else (lambda a: a.flatten())
         if ref_codes is not None and ref_codes.shape[0] > 0:
             self.stream.warm(ref_codes)   # 174 reference frames: ~3 ms once, instead of re-decoding them for four chunks
 
-    def push(self, codec_chunk):
-        return decode_windows_batched(self.st, [self], [codec_chunk])[0]
+    def push(self, codec_chunk, final=False):
+        return decode_windows_batched(self.st, [self], [codec_chunk], [final])[0]
 
 
-def decode_windows_batched(speech_tokenizer, wins, chunks):
+def decode_windows_batched(speech_tokenizer, wins, chunks, finals=None):
     """One chunk of several requests: windows of equal length are decoded as ONE batch (every codec launch covers all of
-    them); returns [(new_audio, sample_rate)] in the order of `wins`."""
-    if wins and isinstance(wins[0], _StatefulWindow):
+    them), then the new samples of every window with a tempo are time-stretched in ONE launch, still on the device;
+    returns [(new_audio, sample_rate)] in the order of `wins`.  ``finals[i]`` ends request i: its tempo flushes.  A chunk
+    of no frames decodes nothing (a flush after the last frames)."""
+    raw = [None] * len(wins)
+    sr = speech_tokenizer.sample_rate if hasattr(speech_tokenizer, "sample_rate") else 24000
+    live = [i for i, c in enumerate(chunks) if int(c.shape[0])]
+    if live and isinstance(wins[0], _StatefulWindow):
         # stateful streams: rows with the same number of new frames advance together in one set of launches
         groups = {}
-        for i, c in enumerate(chunks):
-            groups.setdefault(int(c.shape[0]), []).append(i)
-        out = [None] * len(wins)
+        for i in live:
+            groups.setdefault(int(chunks[i].shape[0]), []).append(i)
         for n, idxs in groups.items():
             pcm = speech_tokenizer.push_streams([wins[i].stream for i in idxs], torch.stack([chunks[i] for i in idxs]))
             for i, a in zip(idxs, pcm):
-                out[i] = (wins[i].conv(a), speech_tokenizer.sample_rate)
-        return out
-    prepared = [w.window(c) for w, c in zip(wins, chunks)]
-    groups, sgroups = {}, {}
-    for i, (codes, meta) in enumerate(prepared):
-        (sgroups if meta[0] == "phase1_stream" else groups).setdefault(int(codes.shape[0]), []).append(i)
-    out = [None] * len(wins)
-    sr = speech_tokenizer.sample_rate if hasattr(speech_tokenizer, "sample_rate") else 24000
-    for T, idxs in groups.items():
-        audio_list, sr = speech_tokenizer.decode({"audio_codes": torch.stack([prepared[i][0] for i in idxs])})
-        for i, a in zip(idxs, audio_list):
-            out[i] = (wins[i].finish(a, prepared[i][1]), sr)
-    for n, idxs in sgroups.items():   # Phase-1 rows riding on reference-warmed streams: one call for all of them
-        pcm = speech_tokenizer.push_streams([wins[i].p1 for i in idxs], torch.stack([prepared[i][0] for i in idxs]))
-        for i, a in zip(idxs, pcm):
-            out[i] = (wins[i].finish(a, prepared[i][1]), sr)
-    return out
+                raw[i] = a
+    elif live:
+        prepared = {i: wins[i].window(chunks[i]) for i in live}
+        groups, sgroups = {}, {}
+        for i, (codes, meta) in prepared.items():
+            (sgroups if meta[0] == "phase1_stream" else groups).setdefault(int(codes.shape[0]), []).append(i)
+        for T, idxs in groups.items():
+            audio_list, sr = speech_tokenizer.decode({"audio_codes": torch.stack([prepared[i][0] for i in idxs])})
+            for i, a in zip(idxs, audio_list):
+                raw[i] = wins[i].finish(a, prepared[i][1])
+        for n, idxs in sgroups.items():   # Phase-1 rows riding on reference-warmed streams: one call for all of them
+            pcm = speech_tokenizer.push_streams([wins[i].p1 for i in idxs], torch.stack([prepared[i][0] for i in idxs]))
+            for i, a in zip(idxs, pcm):
+                raw[i] = wins[i].finish(a, prepared[i][1])
+    stretched = [i for i, w in enumerate(wins) if getattr(w, "tempo", None) is not None]
+    if stretched:
+        from . import tempo
+        finals = finals or [False] * len(wins)
+        for i in stretched:
+            if raw[i] is None:
+                raw[i] = torch.zeros(0, dtype=torch.float32, device=wins[i].tempo.device)
+        pcm = tempo.process([wins[i].tempo for i in stretched], [raw[i] for i in stretched], [finals[i] for i in stretched])
+        for i, a in zip(stretched, pcm):
+            raw[i] = a
+    return [(w.conv(a if a is not None else torch.zeros(0)), sr) for w, a in zip(wins, raw)]
+
+
+def flush_windows(speech_tokenizer, wins):
+    """The end of several requests: every window with a tempo flushes, in one launch -> [(last samples, sample_rate)]
+    of those windows, in order (the tempo's lookahead; windows without a tempo have nothing left)"""
+    wins = [w for w in wins if getattr(w, "tempo", None) is not None and not w.tempo.final]
+    empty = torch.zeros(0, 16, dtype=torch.long)
+    return wins, decode_windows_batched(speech_tokenizer, wins, [empty] * len(wins), [True] * len(wins))
 
 
 class FasterQwen3TTS:
@@ -507,25 +546,32 @@ class FasterQwen3TTS:
             return a.flatten().float().cpu().numpy()
         return a.flatten() if hasattr(a, "flatten") else a
 
-    def _decode_all(self, speech_tokenizer, codec_ids, ref_codes):
+    def _decode_all(self, speech_tokenizer, codec_ids, ref_codes, speed=1.0):
         """Non-streaming decode + proportional reference trim (model.py:918-938)."""
-        return self._decode_takes(speech_tokenizer, [codec_ids], ref_codes)
+        return self._decode_takes(speech_tokenizer, [codec_ids], ref_codes, **_speed_kw(speed))
 
-    def _stream_audio(self, chunks, speech_tokenizer, ref_codes, chunk_size, to_host=True):
+    def _stream_audio(self, chunks, speech_tokenizer, ref_codes, chunk_size, to_host=True, speed=1.0):
         """The reference's hybrid streaming decode (model.py:1052-1135): Phase 1 re-decodes everything so far
         (reference codes prepended in ICL mode) until max(25, chunk_size) frames exist and calibrates
-        samples_per_frame; Phase 2 decodes a 25-frame left-context window and trims the context."""
-        win = self._make_window(speech_tokenizer, ref_codes, chunk_size, to_host)
+        samples_per_frame; Phase 2 decodes a 25-frame left-context window and trims the context.  At a speed other than
+        1 the stream ends with one more item: the tempo's last samples (``chunk_steps`` 0)."""
+        win = self._make_window(speech_tokenizer, ref_codes, chunk_size, to_host, **_speed_kw(speed))
+        timing = {}
         for codec_chunk, timing in chunks:
             new_audio, sr = win.push(codec_chunk)
             yield new_audio, sr, timing
+        for _, (tail, sr) in zip(*flush_windows(speech_tokenizer, [win])):
+            yield tail, sr, dict(timing, chunk_steps=0, is_final=True)
 
-    def _make_window(self, speech_tokenizer, ref_codes, chunk_size, to_host=True):
-        if self.streaming_codec == "stateful" and getattr(speech_tokenizer, "supports_streams", False):
-            return _StatefulWindow(self, speech_tokenizer, ref_codes, chunk_size, to_host)
+    def _make_window(self, speech_tokenizer, ref_codes, chunk_size, to_host=True, speed=1.0):
+        """the codec window of one request; at a speed other than 1 it carries the request's ``tempo.Tempo``"""
+        from .tempo import tempo_for
         if self.streaming_codec not in ("window", "stateful"):
             raise ValueError("streaming_codec must be 'window' or 'stateful'")
-        return _StreamWindow(self, speech_tokenizer, ref_codes, chunk_size, to_host)
+        tempo = tempo_for(speed, _pcm_device(speech_tokenizer)) if speed != 1.0 else None
+        if self.streaming_codec == "stateful" and getattr(speech_tokenizer, "supports_streams", False):
+            return _StatefulWindow(self, speech_tokenizer, ref_codes, chunk_size, to_host, tempo=tempo)
+        return _StreamWindow(self, speech_tokenizer, ref_codes, chunk_size, to_host, tempo=tempo)
 
     @staticmethod
     def _gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p, do_sample, repetition_penalty):
@@ -537,9 +583,11 @@ class FasterQwen3TTS:
     def stream_from_embeds(self, tie, tam, tth, tpe, ref_codes=None, chunk_size: int = 8, to_host: bool = True,
                            max_new_tokens: int = 2048, min_new_tokens: int = 2, temperature: float = 0.9,
                            top_k: int = 50, top_p: float = 1.0, do_sample: bool = True,
-                           repetition_penalty: float = 1.05, uniforms=None):
-        """generate_voice_clone_streaming from the point where the prompt embeddings exist (model.py:1079-1137)."""
+                           repetition_penalty: float = 1.05, uniforms=None, speed: float = 1.0):
+        """generate_voice_clone_streaming from the point where the prompt embeddings exist (model.py:1079-1137).
+        ``speed``: speaking rate in [0.25, 4.0] (see ``_stream_audio``)."""
         from .streaming import fast_generate_streaming
+        _check_speed(speed)
         m = self.model.model
         m.talker.rope_deltas = None
         chunks = fast_generate_streaming(
@@ -552,25 +600,29 @@ class FasterQwen3TTS:
             for codes, timing in chunks:
                 yield (codes.cpu().numpy() if to_host else codes), self.sample_rate, timing
             return
-        yield from self._stream_audio(chunks, st, ref_codes, chunk_size, to_host=to_host)
+        yield from self._stream_audio(chunks, st, ref_codes, chunk_size, to_host=to_host, **_speed_kw(speed))
 
     @torch.inference_mode()
     def stream_batch_from_embeds(self, tie, tam, tth, tpe, ref_codes=None, chunk_size: int = 8, to_host: bool = True,
                                  max_new_tokens: int = 2048, min_new_tokens: int = 2, temperature: float = 0.9,
                                  top_k: int = 50, top_p: float = 1.0, do_sample: bool = True,
-                                 repetition_penalty: float = 1.05, uniforms=None, decode_audio: bool = True):
+                                 repetition_penalty: float = 1.05, uniforms=None, decode_audio: bool = True,
+                                 speed: float = 1.0):
         """Batched streaming from the point where the (left-padded) prompt batch exists (the tuple
         ``_build_talker_inputs_local`` returns for a list of requests, model.py:774-805): all rows advance together, one
         persistent-kernel launch per chunk; yields [(row, pcm_or_codes, sr, timing)] per chunk.  ``ref_codes``: None or
-        a list with one entry per row (ICL reference frames / None)."""
+        a list with one entry per row (ICL reference frames / None).  ``speed``: speaking rate of every row, in [0.25,
+        4.0]; other than 1, a last item holds every row's final samples (``chunk_steps`` 0)."""
         from .batching import fast_generate_streaming_batch
+        _check_speed(speed)
         m = self.model.model
         m.talker.rope_deltas = None
         B = tie.shape[0]
         st = m.speech_tokenizer if decode_audio else None
         wins = None
         if st is not None:
-            wins = [self._make_window(st, None if ref_codes is None else ref_codes[b], chunk_size, to_host) for b in range(B)]
+            wins = [self._make_window(st, None if ref_codes is None else ref_codes[b], chunk_size, to_host, **_speed_kw(speed))
+                    for b in range(B)]
         kw = self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p, do_sample, repetition_penalty)
         for items in fast_generate_streaming_batch(
                 talker=m.talker, talker_input_embeds=tie, attention_mask=tam, trailing_text_hiddens=tth,
@@ -581,22 +633,29 @@ class FasterQwen3TTS:
                 continue
             dec = decode_windows_batched(st, [wins[b] for b, _, _ in items], [codes for _, codes, _ in items])
             yield [(b, audio, sr, timing) for (b, _, timing), (audio, sr) in zip(items, dec)]
+        if wins is not None:
+            ended, tails = flush_windows(st, wins)
+            if ended:
+                yield [(wins.index(w), audio, sr, {"chunk_steps": 0, "is_final": True}) for w, (audio, sr) in zip(ended, tails)]
 
     @torch.inference_mode()
     def generate_custom_voice_batch(self, texts: List[str], speakers: List[str], languages: List[str],
                                     instructs: Optional[List[Optional[str]]] = None, max_new_tokens: int = 2048,
                                     min_new_tokens: int = 2, temperature: float = 0.9, top_k: int = 50,
                                     top_p: float = 1.0, do_sample: bool = True, repetition_penalty: float = 1.05,
-                                    non_streaming_mode: Optional[bool] = None, chunk_size: int = 8):
+                                    non_streaming_mode: Optional[bool] = None, chunk_size: int = 8,
+                                    speed: float = 1.0):
         """Concurrent custom-voice requests (BASELINE config 4) sharing every pass over the weights: the prompts are
         batched and left-padded exactly like the reference's builder does for a list of requests (model.py:583-805),
-        then decoded together.  Returns ([audio per request], sample_rate)."""
+        then decoded together.  ``speed`` (one for all requests): speaking rate in [0.25, 4.0], applied on the device.
+        Returns ([audio per request], sample_rate)."""
+        _check_speed(speed)
         instructs, nsm = self._custom_voice_rules(texts, languages, speakers, instructs or [None] * len(texts),
                                                   non_streaming_mode)
         _, _, _, tie, tam, tth, tpe = self._prepare_generation_custom_batch(texts, languages, speakers, instructs, nsm)
         parts = [[] for _ in texts]
         sr = self.sample_rate
-        for items in self.stream_batch_from_embeds(tie, tam, tth, tpe, chunk_size=chunk_size, **self._gen_kwargs(
+        for items in self.stream_batch_from_embeds(tie, tam, tth, tpe, chunk_size=chunk_size, **_speed_kw(speed), **self._gen_kwargs(
                 max_new_tokens, min_new_tokens, temperature, top_k, top_p, do_sample, repetition_penalty)):
             for b, audio, sr, _ in items:
                 parts[b].append(audio)
@@ -610,7 +669,8 @@ class FasterQwen3TTS:
                              repetition_penalty: float = 1.05, xvec_only: bool = False,
                              non_streaming_mode: Optional[bool] = None, append_silence: bool = True,
                              instruct: Optional[str] = None, ref_spk=None, ref_rvq=None, ref_spk_emb=None,
-                             ref_codes=None, voice_clone_prompt=None) -> Tuple[list, int]:
+                             ref_codes=None, voice_clone_prompt=None, speed: float = 1.0) -> Tuple[list, int]:
+        _check_speed(speed)
         voice_clone_prompt, nsm = self._voice_clone_rules(voice_clone_prompt, non_streaming_mode, ref_spk, ref_rvq,
                                                           ref_spk_emb, ref_codes)
         *prep, ref_codes = self._prepare_generation(
@@ -618,7 +678,7 @@ class FasterQwen3TTS:
             non_streaming_mode=nsm, append_silence=append_silence, voice_clone_prompt=voice_clone_prompt,
             instruct=instruct)
         return self._one_shot(prep, ref_codes, self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k,
-                                                                top_p, do_sample, repetition_penalty))
+                                                                top_p, do_sample, repetition_penalty), speed)
 
     @torch.inference_mode()
     def generate_voice_clone_streaming(self, text: str, language: str, ref_audio=None, ref_text: str = "",
@@ -628,8 +688,9 @@ class FasterQwen3TTS:
                                        xvec_only: bool = False, non_streaming_mode: Optional[bool] = None,
                                        append_silence: bool = True, parity_mode: bool = False,
                                        instruct: Optional[str] = None, ref_spk=None, ref_rvq=None, ref_spk_emb=None,
-                                       ref_codes=None, voice_clone_prompt=None
+                                       ref_codes=None, voice_clone_prompt=None, speed: float = 1.0
                                        ) -> Generator[Tuple[np.ndarray, int, dict], None, None]:
+        _check_speed(speed)
         voice_clone_prompt, nsm = self._voice_clone_rules(voice_clone_prompt, non_streaming_mode, ref_spk, ref_rvq,
                                                           ref_spk_emb, ref_codes)
         m, talker, config, tie, tam, tth, tpe, ref_codes = self._prepare_generation(
@@ -642,9 +703,10 @@ class FasterQwen3TTS:
             chunks = parity_generate_streaming(
                 talker=talker, talker_input_embeds=tie, attention_mask=tam, trailing_text_hiddens=tth, tts_pad_embed=tpe,
                 config=config, chunk_size=chunk_size, **gen)
-            yield from self._stream_audio(chunks, m.speech_tokenizer, ref_codes, chunk_size)
+            yield from self._stream_audio(chunks, m.speech_tokenizer, ref_codes, chunk_size, **_speed_kw(speed))
             return
-        yield from self.stream_from_embeds(tie, tam, tth, tpe, ref_codes=ref_codes, chunk_size=chunk_size, **gen)
+        yield from self.stream_from_embeds(tie, tam, tth, tpe, ref_codes=ref_codes, chunk_size=chunk_size,
+                                           **_speed_kw(speed), **gen)
 
     def _voice_clone_rules(self, voice_clone_prompt, non_streaming_mode, ref_spk=None, ref_rvq=None, ref_spk_emb=None,
                            ref_codes=None):
@@ -703,8 +765,9 @@ class FasterQwen3TTS:
         self._validate(language)
         return self._resolve_non_streaming_mode(non_streaming_mode, default=True)
 
-    def _one_shot(self, prep, ref_codes, gen):
-        """The delivery of the three one-shot methods: generate, then decode every frame at once (model.py:893-947)."""
+    def _one_shot(self, prep, ref_codes, gen, speed=1.0):
+        """The delivery of the three one-shot methods: generate, then decode every frame at once (model.py:893-947),
+        time-stretched on the device at a speed other than 1."""
         from .generate import fast_generate
         m, talker, config, tie, tam, tth, tpe = prep
         codec_ids, timing = fast_generate(
@@ -713,7 +776,7 @@ class FasterQwen3TTS:
         if codec_ids is None:
             logger.warning("Generation returned no tokens")
             return [np.zeros(1, dtype=np.float32)], self.sample_rate
-        audio, sr = self._decode_all(m.speech_tokenizer, codec_ids, ref_codes)
+        audio, sr = self._decode_all(m.speech_tokenizer, codec_ids, ref_codes, **_speed_kw(speed))
         self._log_rtf(timing)
         return audio, sr
 
@@ -721,42 +784,50 @@ class FasterQwen3TTS:
     def generate_custom_voice(self, text: str, speaker: str, language: str, instruct: Optional[str] = None,
                               non_streaming_mode: Optional[bool] = None, max_new_tokens: int = 2048,
                               min_new_tokens: int = 2, temperature: float = 0.9, top_k: int = 50, top_p: float = 1.0,
-                              do_sample: bool = True, repetition_penalty: float = 1.05) -> Tuple[list, int]:
+                              do_sample: bool = True, repetition_penalty: float = 1.05, speed: float = 1.0
+                              ) -> Tuple[list, int]:
+        _check_speed(speed)
         (instruct,), nsm = self._custom_voice_rules([text], [language], [speaker], [instruct], non_streaming_mode)
         prep = self._prepare_generation_custom(text, language, speaker, instruct, nsm)
         return self._one_shot(prep, None, self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p,
-                                                           do_sample, repetition_penalty))
+                                                           do_sample, repetition_penalty), speed)
 
     @torch.inference_mode()
     def generate_custom_voice_streaming(self, text: str, speaker: str, language: str, instruct: Optional[str] = None,
                                         non_streaming_mode: Optional[bool] = None, max_new_tokens: int = 2048,
                                         min_new_tokens: int = 2, temperature: float = 0.9, top_k: int = 50,
                                         top_p: float = 1.0, do_sample: bool = True, repetition_penalty: float = 1.05,
-                                        chunk_size: int = 12) -> Generator[Tuple[np.ndarray, int, dict], None, None]:
+                                        chunk_size: int = 12, speed: float = 1.0
+                                        ) -> Generator[Tuple[np.ndarray, int, dict], None, None]:
+        _check_speed(speed)
         (instruct,), nsm = self._custom_voice_rules([text], [language], [speaker], [instruct], non_streaming_mode)
         _, _, _, tie, tam, tth, tpe = self._prepare_generation_custom(text, language, speaker, instruct, nsm)
-        yield from self.stream_from_embeds(tie, tam, tth, tpe, chunk_size=chunk_size, **self._gen_kwargs(
+        yield from self.stream_from_embeds(tie, tam, tth, tpe, chunk_size=chunk_size, **_speed_kw(speed), **self._gen_kwargs(
             max_new_tokens, min_new_tokens, temperature, top_k, top_p, do_sample, repetition_penalty))
 
     @torch.inference_mode()
     def generate_voice_design(self, text: str, instruct: str, language: str,
                               non_streaming_mode: Optional[bool] = None, max_new_tokens: int = 2048,
                               min_new_tokens: int = 2, temperature: float = 0.9, top_k: int = 50, top_p: float = 1.0,
-                              do_sample: bool = True, repetition_penalty: float = 1.05) -> Tuple[list, int]:
+                              do_sample: bool = True, repetition_penalty: float = 1.05, speed: float = 1.0
+                              ) -> Tuple[list, int]:
+        _check_speed(speed)
         nsm = self._voice_design_rules(language, non_streaming_mode)
         prep = self._prepare_generation_custom(text, language, None, instruct, nsm)
         return self._one_shot(prep, None, self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p,
-                                                           do_sample, repetition_penalty))
+                                                           do_sample, repetition_penalty), speed)
 
     @torch.inference_mode()
     def generate_voice_design_streaming(self, text: str, instruct: str, language: str,
                                         non_streaming_mode: Optional[bool] = None, max_new_tokens: int = 2048,
                                         min_new_tokens: int = 2, temperature: float = 0.9, top_k: int = 50,
                                         top_p: float = 1.0, do_sample: bool = True, repetition_penalty: float = 1.05,
-                                        chunk_size: int = 12) -> Generator[Tuple[np.ndarray, int, dict], None, None]:
+                                        chunk_size: int = 12, speed: float = 1.0
+                                        ) -> Generator[Tuple[np.ndarray, int, dict], None, None]:
+        _check_speed(speed)
         nsm = self._voice_design_rules(language, non_streaming_mode)
         _, _, _, tie, tam, tth, tpe = self._prepare_generation_custom(text, language, None, instruct, nsm)
-        yield from self.stream_from_embeds(tie, tam, tth, tpe, chunk_size=chunk_size, **self._gen_kwargs(
+        yield from self.stream_from_embeds(tie, tam, tth, tpe, chunk_size=chunk_size, **_speed_kw(speed), **self._gen_kwargs(
             max_new_tokens, min_new_tokens, temperature, top_k, top_p, do_sample, repetition_penalty))
 
     # ------------------------------------------------------------------ several takes of one request
@@ -774,7 +845,7 @@ class FasterQwen3TTS:
             raise ValueError(f"{len(seeds)} seeds for {n_takes} takes")
         return seeds
 
-    def _takes(self, prep, ref_codes, seeds, gen, chunk_size=64):
+    def _takes(self, prep, ref_codes, seeds, gen, chunk_size=64, speed=1.0):
         """The one implementation behind the three ``*_takes`` methods: the prompt ``prep`` latched into one slot per take
         with ONE batched prefill (``BatchScheduler.submit_many``), all takes decoded together (one launch per chunk),
         their PCM decoded with one codec call per length.  Take i draws its uniforms from ``take_uniforms(seeds[i])``."""
@@ -799,13 +870,16 @@ class FasterQwen3TTS:
             sc = score(rq.lp.frames(), rq.eos_logprob)
             sc["seed"] = seeds[i]
             scores.append(sc)
-        audio, _ = self._decode_takes(m.speech_tokenizer, codes, ref_codes)
+        audio, _ = self._decode_takes(m.speech_tokenizer, codes, ref_codes, **_speed_kw(speed))
         return audio, self.sample_rate, scores
 
-    def _decode_takes(self, st, codes, ref_codes):
+    def _decode_takes(self, st, codes, ref_codes, speed=1.0):
         """Non-streaming decode + proportional reference trim of every take, takes of equal length in ONE codec call (the
-        decoder's rows are independent).  Returns (audio per take, the sample rate the codec returned)."""
+        decoder's rows are independent); at a speed other than 1 every take is time-stretched on the device, all in ONE
+        launch, as one push with flush.  Returns (audio per take, the sample rate the codec returned)."""
+        from . import tempo
         out = [np.zeros(1, dtype=np.float32)] * len(codes)
+        tempos, pcms, at = [], [], []
         sr = self.sample_rate
         groups = {}
         for i, c in enumerate(codes):
@@ -817,10 +891,21 @@ class FasterQwen3TTS:
                                  for i in idxs])
             audio_list, sr = st.decode({"audio_codes": batch})
             for i, a in zip(idxs, audio_list):
-                a = self._to_numpy(a)
+                a = a.flatten()
                 if ref_len > 0:
                     a = a[int(ref_len / max(batch.shape[1], 1) * len(a)):]
-                out[i] = a
+                t = tempo.tempo_for(speed, a.device) if speed != 1.0 else None
+                if t is None:
+                    out[i] = self._to_numpy(a)
+                else:
+                    tempos.append(t)
+                    pcms.append(a)
+                    at.append(i)
+        if tempos:
+            for i, a in zip(at, tempo.process(tempos, pcms, True)):
+                out[i] = self._to_numpy(a)
+            for t in tempos:
+                t.close()
         return out, sr
 
     @torch.inference_mode()
@@ -829,8 +914,8 @@ class FasterQwen3TTS:
                                    top_k: int = 50, top_p: float = 1.0, do_sample: bool = True,
                                    repetition_penalty: float = 1.05, xvec_only: bool = False,
                                    non_streaming_mode: Optional[bool] = None, append_silence: bool = True,
-                                   instruct: Optional[str] = None, voice_clone_prompt=None, n_takes: int = 4,
-                                   seeds: Optional[List[int]] = None):
+                                   instruct: Optional[str] = None, voice_clone_prompt=None, speed: float = 1.0,
+                                   n_takes: int = 4, seeds: Optional[List[int]] = None):
         """``n_takes`` renderings of one ``generate_voice_clone`` request for the price of one batched decode: one prompt,
         one batched prefill, one launch per chunk for all takes.  Take i is the request run alone with the uniforms of
         ``take_uniforms(seeds[i], max_new_tokens)`` -- bit for bit while both run the per-head talker attention (a lone
@@ -838,6 +923,7 @@ class FasterQwen3TTS:
         holds "logprobs" (float32 [T,16], the log-probability of every code), "eos_logprob", "total_logprob" (their sum,
         EOS term included), "frames" and "seed".  A log-probability says how likely the sampler found its draws, not
         how good the audio is: the calls rank nothing and pick nothing."""
+        _check_speed(speed)
         voice_clone_prompt, nsm = self._voice_clone_rules(voice_clone_prompt, non_streaming_mode)
         seeds = self._check_takes(n_takes, seeds)
         *prep, ref_codes = self._prepare_generation(
@@ -845,37 +931,39 @@ class FasterQwen3TTS:
             non_streaming_mode=nsm, append_silence=append_silence, voice_clone_prompt=voice_clone_prompt,
             instruct=instruct)
         return self._takes(prep, ref_codes, seeds, self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k,
-                                                                    top_p, do_sample, repetition_penalty))
+                                                                    top_p, do_sample, repetition_penalty), speed=speed)
 
     @torch.inference_mode()
     def generate_custom_voice_takes(self, text: str, speaker: str, language: str, instruct: Optional[str] = None,
                                     non_streaming_mode: Optional[bool] = None, max_new_tokens: int = 2048,
                                     min_new_tokens: int = 2, temperature: float = 0.9, top_k: int = 50,
                                     top_p: float = 1.0, do_sample: bool = True, repetition_penalty: float = 1.05,
-                                    n_takes: int = 4, seeds: Optional[List[int]] = None):
+                                    speed: float = 1.0, n_takes: int = 4, seeds: Optional[List[int]] = None):
         """``n_takes`` renderings of one ``generate_custom_voice`` request (see ``generate_voice_clone_takes``)."""
+        _check_speed(speed)
         (instruct,), nsm = self._custom_voice_rules([text], [language], [speaker], [instruct], non_streaming_mode)
         seeds = self._check_takes(n_takes, seeds)
         prep = self._prepare_generation_custom(text, language, speaker, instruct, nsm)
         return self._takes(prep, None, seeds, self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k,
-                                                               top_p, do_sample, repetition_penalty))
+                                                               top_p, do_sample, repetition_penalty), speed=speed)
 
     @torch.inference_mode()
     def generate_voice_design_takes(self, text: str, instruct: str, language: str,
                                     non_streaming_mode: Optional[bool] = None, max_new_tokens: int = 2048,
                                     min_new_tokens: int = 2, temperature: float = 0.9, top_k: int = 50,
                                     top_p: float = 1.0, do_sample: bool = True, repetition_penalty: float = 1.05,
-                                    n_takes: int = 4, seeds: Optional[List[int]] = None):
+                                    speed: float = 1.0, n_takes: int = 4, seeds: Optional[List[int]] = None):
         """``n_takes`` renderings of one ``generate_voice_design`` request (see ``generate_voice_clone_takes``)."""
+        _check_speed(speed)
         nsm = self._voice_design_rules(language, non_streaming_mode)
         seeds = self._check_takes(n_takes, seeds)
         prep = self._prepare_generation_custom(text, language, None, instruct, nsm)
         return self._takes(prep, None, seeds, self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k,
-                                                               top_p, do_sample, repetition_penalty))
+                                                               top_p, do_sample, repetition_penalty), speed=speed)
 
     # ------------------------------------------------------------------ incremental text input (text_stream.py)
     def _text_streaming(self, text_stream, language, speaker, instruct, voice_clone_prompt, non_streaming_mode,
-                        chunk_size, gen):
+                        chunk_size, gen, speed=1.0):
         """The one implementation behind the three ``*_text_streaming`` methods.  Text streaming has one text layout,
         so the raw ``non_streaming_mode`` is checked here, not the voice kind's default."""
         from .text_stream import _refuse_unsupported, generate_text_streaming
@@ -885,7 +973,7 @@ class FasterQwen3TTS:
             instruct_ids = self.model._tokenize_texts([self.model._build_instruct_text(instruct)])[0]
         yield from generate_text_streaming(self, text_stream, language=language, speaker=speaker,
                                            instruct_ids=instruct_ids, voice_clone_prompt=voice_clone_prompt,
-                                           chunk_size=chunk_size, **gen)
+                                           chunk_size=chunk_size, **_speed_kw(speed), **gen)
 
     @torch.inference_mode()
     def generate_custom_voice_text_streaming(self, text_stream, speaker: str, language: str,
@@ -893,29 +981,32 @@ class FasterQwen3TTS:
                                              max_new_tokens: int = 2048, min_new_tokens: int = 2,
                                              temperature: float = 0.9, top_k: int = 50, top_p: float = 1.0,
                                              do_sample: bool = True, repetition_penalty: float = 1.05,
-                                             chunk_size: int = 12) -> Generator[Tuple[np.ndarray, int, dict], None, None]:
+                                             chunk_size: int = 12, speed: float = 1.0
+                                             ) -> Generator[Tuple[np.ndarray, int, dict], None, None]:
         """``generate_custom_voice_streaming`` with the text fed while it is spoken: ``text_stream`` is any iterable of
         ``str`` pieces (an LLM's reply token by token).  The audio equals that of the one-shot streaming request for the
         same text, whatever the split and however fast the pieces come; generation waits where the text has not arrived
         yet.  Timing dicts add ``text_wait_ms``, the time spent blocked on ``text_stream``."""
+        _check_speed(speed)
         (instruct,), _ = self._custom_voice_rules([text_stream], [language], [speaker], [instruct], non_streaming_mode)
         yield from self._text_streaming(text_stream, language, speaker, instruct, None, non_streaming_mode, chunk_size,
                                         self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p,
-                                                         do_sample, repetition_penalty))
+                                                         do_sample, repetition_penalty), speed)
 
     @torch.inference_mode()
     def generate_voice_design_text_streaming(self, text_stream, instruct: str, language: str,
                                              non_streaming_mode: Optional[bool] = None, max_new_tokens: int = 2048,
                                              min_new_tokens: int = 2, temperature: float = 0.9, top_k: int = 50,
                                              top_p: float = 1.0, do_sample: bool = True,
-                                             repetition_penalty: float = 1.05, chunk_size: int = 12
+                                             repetition_penalty: float = 1.05, chunk_size: int = 12, speed: float = 1.0
                                              ) -> Generator[Tuple[np.ndarray, int, dict], None, None]:
         """``generate_voice_design_streaming`` with the text fed while it is spoken (see
         ``generate_custom_voice_text_streaming``)."""
+        _check_speed(speed)
         self._voice_design_rules(language, non_streaming_mode)
         yield from self._text_streaming(text_stream, language, None, instruct, None, non_streaming_mode, chunk_size,
                                         self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p,
-                                                         do_sample, repetition_penalty))
+                                                         do_sample, repetition_penalty), speed)
 
     @torch.inference_mode()
     def generate_voice_clone_text_streaming(self, text_stream, language: str, ref_audio=None, ref_text: str = "",
@@ -925,10 +1016,12 @@ class FasterQwen3TTS:
                                             chunk_size: int = 12, xvec_only: bool = True,
                                             non_streaming_mode: Optional[bool] = None, append_silence: bool = True,
                                             ref_spk=None, ref_rvq=None, ref_spk_emb=None, ref_codes=None,
-                                            voice_clone_prompt=None) -> Generator[Tuple[np.ndarray, int, dict], None, None]:
+                                            voice_clone_prompt=None, speed: float = 1.0
+                                            ) -> Generator[Tuple[np.ndarray, int, dict], None, None]:
         """``generate_voice_clone_streaming`` with the text fed while it is spoken, x-vector cloning only: ICL cloning
         puts the target text under the reference codec frames inside the prompt, so it must be known before prefill
         (ValueError)."""
+        _check_speed(speed)
         voice_clone_prompt, _ = self._voice_clone_rules(voice_clone_prompt, non_streaming_mode, ref_spk, ref_rvq,
                                                         ref_spk_emb, ref_codes)
         from .text_stream import ICL_REFUSAL, _refuse_unsupported
@@ -941,7 +1034,7 @@ class FasterQwen3TTS:
             voice_clone_prompt=voice_clone_prompt)
         yield from self._text_streaming(text_stream, language, None, None, vcp, non_streaming_mode, chunk_size,
                                         self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p,
-                                                         do_sample, repetition_penalty))
+                                                         do_sample, repetition_penalty), speed)
 
     def _log_rtf(self, timing):
         n = timing["steps"]

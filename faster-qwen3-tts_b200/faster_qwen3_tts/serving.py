@@ -65,6 +65,7 @@ class Ticket:
     lead_s: float = 0.0                   # paced: audio seconds handed over minus seconds played, as of the last step
     underruns: int = 0                    # paced: chunks delivered after the listener had run dry (lead < 0)
     prepared: Optional[tuple] = None      # (submit arguments, window) of a ticket waiting for KV pages
+    speed: float = 1.0                    # speaking rate: the listener consumes model audio `speed` times as fast
 
     def cancel(self) -> None:
         """End the request: the worker frees its slot (or drops it from the queue) and closes the ticket."""
@@ -134,7 +135,10 @@ class ContinuousBatcher:
     lead is counted in ``Ticket.underruns``.
     The worker launches as soon as one listener is below the watermark; at low load its launches therefore carry few
     slots, each costing a whole pass over the weights (no low watermark or minimum launch width is implemented).
-    ``window_factory`` is called with the ticket's own ``chunk_size`` as a second argument when it has one.
+    ``window_factory`` is called with the ticket's own ``chunk_size`` as a second argument when it has one, and with
+    ``speed=`` when the ticket's speaking rate is not 1 (``submit(..., speed=)``): the window then time-stretches its
+    PCM on the device, ``batch_decode`` gets a third argument (whether each request ends with this chunk: its tempo
+    flushes), and the lead counts audio seconds at that rate, ``frames x frame_s / speed``.
     ``clock`` / ``sleep`` are the worker's time source, replaceable in tests."""
 
     def __init__(self, scheduler, window_factory: Callable, chunk_size: int = 8, idle_sleep: float = 0.002,
@@ -160,12 +164,15 @@ class ContinuousBatcher:
         self._thread.start()
 
     # ---- client side ------------------------------------------------------------------------------------
-    def submit(self, prepare: Callable[[], tuple], pace: Optional[float] = None, **gen_kwargs) -> Ticket:
-        """``pace``: the client plays at ``pace`` x real time (class docstring).  ``gen_kwargs`` are the scheduler's
-        ``submit`` keywords, among them ``chunk_size`` / ``first_chunk`` for this request alone."""
+    def submit(self, prepare: Callable[[], tuple], pace: Optional[float] = None, speed: float = 1.0,
+               **gen_kwargs) -> Ticket:
+        """``pace``: the client plays at ``pace`` x real time (class docstring); ``speed``: speaking rate in [0.25,
+        4.0].  ``gen_kwargs`` are the scheduler's ``submit`` keywords, among them ``chunk_size`` / ``first_chunk`` for
+        this request alone."""
+        speed = self._speed(speed)
         with self._lock:
             self._rid += 1
-            t = Ticket(self._rid, prepare, gen_kwargs, pace=self._pace(pace), submitted_at=self.clock())
+            t = Ticket(self._rid, prepare, gen_kwargs, pace=self._pace(pace), submitted_at=self.clock(), speed=speed)
         self.pending.put(t)
         return t
 
@@ -175,14 +182,22 @@ class ContinuousBatcher:
             raise ValueError(f"pace must be positive (or None for an unpaced client), got {pace}")
         return None if pace is None else float(pace)
 
-    def submit_text(self, prepare: Callable, pace: Optional[float] = None, **gen_kwargs) -> TextTicket:
+    @staticmethod
+    def _speed(speed):
+        from .tempo import quantize
+        quantize(speed)
+        return float(speed)
+
+    def submit_text(self, prepare: Callable, pace: Optional[float] = None, speed: float = 1.0,
+                    **gen_kwargs) -> TextTicket:
         """A text-fed request.  ``prepare(feed)`` -> (tie, tam, tpe, ref_codes) builds the prompt once the feed holds its
         first committed id (``text_stream.TextFeed.prompt_ids``); it runs on the worker thread."""
         if self.feed_factory is None:
             raise RuntimeError("this batcher has no text feed factory")
+        speed = self._speed(speed)
         with self._lock:
             self._rid += 1
-            t = TextTicket(self._rid, prepare, gen_kwargs, pace=self._pace(pace), submitted_at=self.clock())
+            t = TextTicket(self._rid, prepare, gen_kwargs, pace=self._pace(pace), submitted_at=self.clock(), speed=speed)
         t.feed = self.feed_factory(int(gen_kwargs.get("max_new_tokens", 2048)))
         self.pending.put(t)
         return t
@@ -214,10 +229,11 @@ class ContinuousBatcher:
         for t in [t for t in self.waiting if t.cancelled.is_set()]:
             self.waiting.remove(t)
             t.out.put(_DONE)
-        for rid, (t, _) in list(self.live.items()):
+        for rid, (t, win) in list(self.live.items()):
             if t.cancelled.is_set():
                 self.sched.cancel(self.requests.pop(rid))
                 del self.live[rid]
+                self._drop_tempo(win)
                 t.out.put(_DONE)
 
     def _prepare(self, t: Ticket):
@@ -243,11 +259,18 @@ class ContinuousBatcher:
                                "Use shorter text or shorter reference audio.")
         return req, win
 
+    @staticmethod
+    def _drop_tempo(win):
+        tempo = getattr(win, "tempo", None)
+        if tempo is not None:
+            tempo.close()
+
     def _window(self, t: Ticket, ref_codes):
         """the request's codec window, built for the request's own chunk size where it has one (the window policy's
         calibration point depends on it); a short first chunk is for windows whose audio does not depend on the chunking"""
         own = t.gen_kwargs.get("chunk_size")
-        win = self.window_factory(ref_codes) if own is None else self.window_factory(ref_codes, own)
+        kw = {} if t.speed == 1.0 else {"speed": t.speed}
+        win = self.window_factory(ref_codes, **kw) if own is None else self.window_factory(ref_codes, own, **kw)
         if t.gen_kwargs.get("first_chunk") and not getattr(win, "any_chunking", False):
             raise ValueError("first_chunk needs a codec window whose audio does not depend on the chunking (the stateful "
                              "codec stream); under the window policy the audio of a request is defined by one chunk_size")
@@ -317,7 +340,7 @@ class ContinuousBatcher:
             if t.first_chunk_at is None:
                 rq.due, rq.hold = float("-inf"), False
             else:
-                t.lead_s = t.frames * self.frame_s - t.pace * (now - t.first_chunk_at)
+                t.lead_s = t.frames * self.frame_s / t.speed - t.pace * (now - t.first_chunk_at)
                 rq.due, rq.hold = t.lead_s, t.lead_s >= self.lead_high_s
 
     def _run(self):
@@ -340,32 +363,41 @@ class ContinuousBatcher:
                 self.sleep(self.idle_sleep)
                 continue
             self.steps += 1
-            live = [(rq, codes) for rq, codes in results if int(codes.shape[0])]
+            # a stretched request's last step flushes its tempo, even when that step made no frames
+            live = [(rq, codes) for rq, codes in results
+                    if int(codes.shape[0]) or (rq.finished and self.live[rq.tag][0].speed != 1.0)]
+            stretched = any(self.live[rq.tag][0].speed != 1.0 for rq, _ in live)
             # windows of equal length of all requests are decoded as one batch when the window objects support it
             pcm_of = {}
             if live and self.batch_decode is not None:
-                for (rq, _), (pcm, sr) in zip(live, self.batch_decode([self.live[rq.tag][1] for rq, _ in live],
-                                                                      [codes for _, codes in live])):
+                args = ([self.live[rq.tag][1] for rq, _ in live], [codes for _, codes in live])
+                if stretched:
+                    args += ([bool(rq.finished) for rq, _ in live],)
+                for (rq, _), (pcm, sr) in zip(live, self.batch_decode(*args)):
                     pcm_of[rq.tag] = (pcm, sr)
             for rq, codes in results:
                 t, win = self.live[rq.tag]
                 n = int(codes.shape[0])
-                if n:
-                    pcm, sr = pcm_of[rq.tag] if rq.tag in pcm_of else win.push(codes)
+                if n or rq.tag in pcm_of:
+                    if rq.tag in pcm_of:
+                        pcm, sr = pcm_of[rq.tag]
+                    else:
+                        pcm, sr = win.push(codes) if t.speed == 1.0 else win.push(codes, final=bool(rq.finished))
                     now = self.clock()
                     if t.first_chunk_at is None:
                         t.first_chunk_at = now
-                    elif t.pace is not None and t.frames * self.frame_s - t.pace * (now - t.first_chunk_at) < 0:
+                    elif t.pace is not None and t.frames * self.frame_s / t.speed - t.pace * (now - t.first_chunk_at) < 0:
                         t.underruns += 1      # what it had was played out before this chunk arrived
                     t.frames += n
                     if t.pace is not None:
-                        t.lead_s = t.frames * self.frame_s - t.pace * (now - t.first_chunk_at)
+                        t.lead_s = t.frames * self.frame_s / t.speed - t.pace * (now - t.first_chunk_at)
                     t.out.put((pcm, sr, {"chunk_steps": n, "total_steps_so_far": t.frames,
                                          "is_final": bool(rq.finished)}))
                 if rq.finished:
                     t.out.put(_DONE)
                     del self.live[rq.tag]
                     self.requests.pop(rq.tag, None)
+                    self._drop_tempo(win)
 
 
 def batcher_for_model(model, chunk_size: int = 8, to_host: bool = True, **kw) -> ContinuousBatcher:
@@ -381,10 +413,14 @@ def batcher_for_model(model, chunk_size: int = 8, to_host: bool = True, **kw) ->
         def push(self, codes):
             return codes.cpu().numpy(), model.sample_rate
 
-    def window(ref_codes, chunk=chunk_size):
-        return model._make_window(st, ref_codes, chunk, to_host) if st is not None else _CodesOnly()
+    def window(ref_codes, chunk=chunk_size, speed=1.0):
+        if st is None:
+            if speed != 1.0:
+                raise ValueError("a speaking rate other than 1 needs the codec (PCM)")
+            return _CodesOnly()
+        return model._make_window(st, ref_codes, chunk, to_host, **({} if speed == 1.0 else {"speed": speed}))
 
-    bd = (lambda wins, chunks: decode_windows_batched(st, wins, chunks)) if st is not None else None
+    bd = (lambda wins, chunks, finals=None: decode_windows_batched(st, wins, chunks, finals)) if st is not None else None
     from .text_stream import TextFeed
     return ContinuousBatcher(sched, window, chunk_size=chunk_size, batch_decode=bd,
                              feed_factory=lambda max_rows: TextFeed(model, max_rows), **kw)

@@ -185,8 +185,8 @@ def _refuse_unsupported(voice_clone_prompt, non_streaming_mode):
 def generate_text_streaming(model, text_stream: Iterable[str], *, language: str, speaker=None, instruct_ids=None,
                             voice_clone_prompt=None, chunk_size: int = 12, max_new_tokens: int = 2048,
                             min_new_tokens: int = 2, temperature: float = 0.9, top_k: int = 50, top_p: float = 1.0,
-                            do_sample: bool = True, repetition_penalty: float = 1.05, uniforms=None, to_host: bool = True
-                            ) -> Iterator:
+                            do_sample: bool = True, repetition_penalty: float = 1.05, uniforms=None, to_host: bool = True,
+                            speed: float = 1.0) -> Iterator:
     """Yields (pcm, sample_rate, timing) like the ``*_streaming`` methods.  Prefills once the first text id is
     committed, then per launch: pull text until the next chunk's rows exist (window codec policy) or one more row
     exists (stateful codec), or the text closes; announce the rows; decode one chunk.  The request is the one request of
@@ -225,7 +225,9 @@ def generate_text_streaming(model, text_stream: Iterable[str], *, language: str,
         feed.close()   # raises: no text at all
     tie, tam, tpe = build_prompt(model, feed, language=language, speaker=speaker, instruct_ids=instruct_ids,
                                  voice_clone_prompt=voice_clone_prompt)
-    win = model._make_window(st, None, chunk_size, to_host) if st is not None else None
+    win = None
+    if st is not None:
+        win = model._make_window(st, None, chunk_size, to_host, **({} if speed == 1.0 else {"speed": speed}))
     # the window policy's PCM depends on the chunking: launch only when a full chunk of rows exists, so that every launch
     # emits a full chunk or ends the request.  A stateful stream (or codes only) is the same in any chunking.
     ahead = 1 if win is None or getattr(win, "any_chunking", False) else chunk_size
@@ -247,6 +249,13 @@ def generate_text_streaming(model, text_stream: Iterable[str], *, language: str,
         wait[0] = wait_before = 0.0
         if win is None:
             yield (codes.cpu().numpy() if to_host else codes), model.sample_rate, tm
-        else:
+        elif getattr(win, "tempo", None) is None:
             pcm, sr = win.push(codes)
             yield pcm, sr, tm
+        else:   # the last chunk flushes the tempo
+            pcm, sr = win.push(codes, final=bool(rq.finished))
+            yield pcm, sr, tm
+    if win is not None:
+        from .model import flush_windows
+        for _, (pcm, sr) in zip(*flush_windows(st, [win])):   # a request that ended on a step without frames
+            yield pcm, sr, {"chunk_steps": 0, "is_final": True}

@@ -365,6 +365,36 @@ int64_t fq3_codec_launch_count(fq3_codec* c);
 void fq3_codec_destroy(fq3_codec* c);
 const char* fq3_codec_last_error(void);
 
+/* ---- Speaking-rate control: pitch-preserving time-stretch of 24 kHz PCM on the device (csrc/fq3_tempo.cu)
+ * WSOLA (waveform-similarity overlap-add) with a FQ3_TEMPO_WINDOW-sample periodic Hann window, synthesis hop
+ * FQ3_TEMPO_WINDOW / 2 and a search of +-FQ3_TEMPO_SEARCH samples around each frame's nominal position; the score of a
+ * candidate is its correlation with the previous frame's natural continuation over sqrt(FQ3_TEMPO_EPS + its energy).
+ * The speed is quantised to q = round(speed * 1024) in [FQ3_TEMPO_Q_MIN, FQ3_TEMPO_Q_MAX]; q = 1024 is the identity and
+ * has no tempo state (create refuses it: callers pass the PCM through).  The algorithm, bit for bit, is in DESIGN.md
+ * ("Speaking rate") and faster_qwen3_tts/tempo.py.  A push releases exactly fq3_tempo_released(q, samples pushed before,
+ * samples pushed now, flush) samples -- a function of the totals alone, so buffers are sized on the host and nothing is
+ * read back.  The output of a stream depends on its samples and its flush point only, not on how they were pushed. */
+#define FQ3_TEMPO_WINDOW 480
+#define FQ3_TEMPO_SEARCH 240
+#define FQ3_TEMPO_EPS 1e-6f
+#define FQ3_TEMPO_Q_MIN 256
+#define FQ3_TEMPO_Q_MAX 4096
+typedef struct fq3_tempo fq3_tempo;
+int fq3_tempo_create(int32_t device, double speed, fq3_tempo** out);
+int fq3_tempo_reset(fq3_tempo* t);   /* a new stream at the same speed; host-side, nothing is launched */
+void fq3_tempo_destroy(fq3_tempo* t);
+/* samples released by a push of n samples after total_in (-1 for an invalid q or a negative count) */
+int64_t fq3_tempo_released(int32_t q, int64_t total_in, int64_t n, int32_t flush);
+/* One launch for n_streams distinct tempos.  in_dev float32: the streams' new samples packed in order (in_lens[i] of
+ * stream i, host array); flush[i] (host) != 0 ends stream i (zeros after its end; it must be reset before more input).
+ * out_dev float32 [out_cap]: the released samples packed in order; pk_dev int32 [pk_cap] or NULL: p_k of every frame run,
+ * packed in order.  A null, misaligned or too small buffer, a tempo listed twice or a flushed tempo is refused before
+ * anything is launched. */
+int fq3_tempo_process(fq3_tempo* const* tempos, int32_t n_streams, const float* in_dev, const int64_t* in_lens,
+                      const int32_t* flush, float* out_dev, int64_t out_cap, int32_t* pk_dev, int64_t pk_cap,
+                      void* stream);
+const char* fq3_tempo_last_error(void);
+
 const char* fq3_last_error(void);
 const char* fq3_version(void);
 
