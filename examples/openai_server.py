@@ -1,14 +1,17 @@
 #!/usr/bin/env python3
 """OpenAI-compatible TTS server over the H100 engine with CONTINUOUS BATCHING.
 
-Same endpoint and wire format as the reference's example server (POST /v1/audio/speech, response_format wav | pcm,
-streaming WAV with an unknown-length header; the reference's examples/openai_server.py:91-118,215-263), but requests are
-not serialised behind a lock (:71,181): up to --max-batch requests share every pass over the model weights and new
-requests join between chunks (faster_qwen3_tts/serving.py).  A streamed response is a listener: it is paced at real time
-by default, so the engine, which makes audio several times faster than it is played, serves the clients closest to running
-dry first and holds up to --max-slots requests (each costs its KV cache) on --max-batch launch columns.  The request field
-"pace" overrides that: a number = playback speed relative to real time, null = as fast as possible.  "speed" (0.25 - 4.0)
-is the speaking rate: the audio is time-stretched on the GPU after the codec, at the same pitch.
+Same endpoint and wire format as the reference's example server (POST /v1/audio/speech, response_format wav | pcm, plus
+ulaw | alaw: raw 8-bit G.711; streaming WAV with an unknown-length header; the reference's
+examples/openai_server.py:91-118,215-263), but requests are not serialised behind a lock (:71,181): up to --max-batch
+requests share every pass over the model weights and new requests join between chunks (faster_qwen3_tts/serving.py).  A
+streamed response is a listener: it is paced at real time by default, so the engine, which makes audio several times
+faster than it is played, serves the clients closest to running dry first and holds up to --max-slots requests (each
+costs its KV cache) on --max-batch launch columns.  The request field "pace" overrides that: a number = playback speed
+relative to real time, null = as fast as possible.  "speed" (0.25 - 4.0) is the speaking rate: the audio is
+time-stretched on the GPU after the codec, at the same pitch.  "sample_rate" (8000, 16000, 22050, 24000, 32000, 44100 or
+48000; default 24000) is the rate of the response: the audio is resampled and encoded (s16 for wav / pcm, G.711 for ulaw
+/ alaw) on the GPU, so only the encoded bytes leave it.
 
     python examples/openai_server.py --model synthetic:1.7B --max-batch 16 --port 8000
     curl -s localhost:8000/v1/audio/speech -H 'Content-Type: application/json' \\
@@ -29,7 +32,8 @@ def build_app(model, batcher, voices, default_voice):
     from fastapi.responses import StreamingResponse
     from typing import Optional
     from pydantic import BaseModel
-    from faster_qwen3_tts.serving import to_pcm16, voice_clone_request, wav_header
+    from faster_qwen3_tts.resample import RATES
+    from faster_qwen3_tts.serving import voice_clone_request, wav_header
 
     app = FastAPI(title="faster-qwen3-tts (H100 engine) OpenAI-compatible API")
 
@@ -37,7 +41,8 @@ def build_app(model, batcher, voices, default_voice):
         model: str = "tts-1"
         input: str
         voice: str = "alloy"
-        response_format: str = "wav"   # wav | pcm
+        response_format: str = "wav"   # wav | pcm (16-bit) | ulaw | alaw (8-bit G.711)
+        sample_rate: int = 24000        # one of 8000, 16000, 22050, 24000, 32000, 44100, 48000
         speed: float = 1.0             # speaking rate in [0.25, 4.0], same pitch
         pace: Optional[float] = 1.0    # the client plays at pace x real time; null: everything as fast as possible
 
@@ -53,28 +58,32 @@ def build_app(model, batcher, voices, default_voice):
         if v is None:
             raise HTTPException(status_code=400, detail=f"Voice {req.voice!r} is not configured. Available voices: {list(voices)}")
         fmt = req.response_format.lower()
-        if fmt not in ("wav", "pcm"):
-            raise HTTPException(status_code=400, detail=f"response_format {fmt!r} not supported. Use: wav, pcm")
+        encoding = {"wav": "s16", "pcm": "s16", "ulaw": "ulaw", "alaw": "alaw"}.get(fmt)
+        if encoding is None:
+            raise HTTPException(status_code=400, detail=f"response_format {fmt!r} not supported. Use: wav, pcm, ulaw, alaw")
+        if req.sample_rate not in RATES:
+            raise HTTPException(status_code=400, detail=f"'sample_rate' must be one of {list(RATES)}, got {req.sample_rate}")
         if req.pace is not None and not req.pace > 0:
             raise HTTPException(status_code=400, detail=f"'pace' must be a positive number or null, got {req.pace}")
         if not 0.25 <= req.speed <= 4.0:
             raise HTTPException(status_code=400, detail=f"'speed' must be in [0.25, 4.0], got {req.speed}")
         ticket = batcher.submit(voice_clone_request(model, req.input, v.get("language", "Auto"), v["ref_audio"],
                                                     v.get("ref_text", "")), pace=req.pace, speed=req.speed,
-                                max_new_tokens=v.get("max_new_tokens", 2048))
+                                sample_rate=req.sample_rate, encoding=encoding, max_new_tokens=v.get("max_new_tokens", 2048))
         loop = asyncio.get_event_loop()
         it = iter(ticket)
 
         async def audio_stream():
             if fmt == "wav":
-                yield wav_header(model.sample_rate)
+                yield wav_header(req.sample_rate)
             while True:
                 item = await loop.run_in_executor(None, lambda: next(it, None))
                 if item is None:
                     return
-                yield to_pcm16(item[0])
+                yield item[0].tobytes()   # encoded on the device
 
-        return StreamingResponse(audio_stream(), media_type="audio/wav" if fmt == "wav" else "audio/pcm")
+        media = {"wav": "audio/wav", "pcm": "audio/pcm", "ulaw": "audio/basic", "alaw": "audio/x-alaw-basic"}[fmt]
+        return StreamingResponse(audio_stream(), media_type=media)
 
     return app
 

@@ -83,6 +83,8 @@ EXPORTS = [
     "fq3_codec_destroy", "fq3_codec_last_error",
     "fq3_tempo_create", "fq3_tempo_reset", "fq3_tempo_destroy", "fq3_tempo_released", "fq3_tempo_process",
     "fq3_tempo_last_error",
+    "fq3_resample_create", "fq3_resample_reset", "fq3_resample_destroy", "fq3_resample_released", "fq3_resample_taps",
+    "fq3_resample_process", "fq3_resample_last_error",
 ]
 
 
@@ -195,6 +197,17 @@ def load_library() -> C.CDLL:
     lib.fq3_tempo_process.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int32),
                                       C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p]
     lib.fq3_tempo_last_error.restype = C.c_char_p
+    lib.fq3_resample_create.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_void_p)]
+    lib.fq3_resample_reset.argtypes = [C.c_void_p]
+    lib.fq3_resample_destroy.argtypes = [C.c_void_p]
+    lib.fq3_resample_destroy.restype = None
+    lib.fq3_resample_released.argtypes = [C.c_int32, C.c_int64, C.c_int64, C.c_int32]
+    lib.fq3_resample_released.restype = C.c_int64
+    lib.fq3_resample_taps.argtypes = [C.c_int32, C.POINTER(C.c_double), C.c_int32]
+    lib.fq3_resample_taps.restype = C.c_int32
+    lib.fq3_resample_process.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.POINTER(C.c_int64),
+                                         C.POINTER(C.c_int32), C.c_void_p, C.c_int64, C.c_void_p]
+    lib.fq3_resample_last_error.restype = C.c_char_p
     _lib = lib
     return lib
 

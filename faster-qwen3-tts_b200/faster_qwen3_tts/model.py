@@ -42,9 +42,24 @@ def _check_speed(speed):
     quantize(speed)
 
 
-def _speed_kw(speed):
-    """``speed=`` for the delivery calls, only when it is not 1: at speed 1 every call is made exactly as without it"""
-    return {} if speed == 1.0 else {"speed": speed}
+def _check_rate(sample_rate):
+    """an output rate outside ``resample.RATES`` is refused (ValueError) before anything is tokenized"""
+    from .resample import check_rate
+    check_rate(sample_rate)
+
+
+def _post_kw(speed, sample_rate=None):
+    """``speed=`` / ``sample_rate=`` for the delivery calls, only where they are not the identity (speed 1, 24 kHz): at
+    the defaults every call is made exactly as without them"""
+    kw = {} if speed == 1.0 else {"speed": speed}
+    if sample_rate is not None and int(sample_rate) != 24000:
+        kw["sample_rate"] = sample_rate
+    return kw
+
+
+def _rate_of(sr, sample_rate):
+    """the rate a delivery returns: the requested one, else what the codec gave"""
+    return sr if sample_rate is None else int(sample_rate)
 
 
 def _pcm_device(speech_tokenizer):
@@ -64,11 +79,12 @@ class _StreamWindow:
     reference's warmed template stream (``SpeechTokenizer.reference_stream``): same samples, one chunk's worth of work,
     and the reference itself is decoded once per voice instead of four times per request.  Phase 2 (25-frame context
     windows without the reference) is the reference's approximation and is decoded exactly as the reference does.
-    ``FQ3_PHASE1_STREAM=0`` keeps the literal re-decode.  ``tempo``: the request's speaking rate (``tempo.Tempo``),
-    applied to the new samples on the device before they are converted (``decode_windows_batched``)."""
+    ``FQ3_PHASE1_STREAM=0`` keeps the literal re-decode.  ``tempo``: the request's speaking rate (``tempo.Tempo``), and
+    ``resampler``: its output rate and encoding (``resample.Resampler``), applied in that order to the new samples on the
+    device before they are converted (``decode_windows_batched``)."""
 
-    def __init__(self, owner, speech_tokenizer, ref_codes, chunk_size, to_host=True, tempo=None):
-        self.st, self.ref_codes, self.tempo = speech_tokenizer, ref_codes, tempo
+    def __init__(self, owner, speech_tokenizer, ref_codes, chunk_size, to_host=True, tempo=None, resampler=None):
+        self.st, self.ref_codes, self.tempo, self.resampler = speech_tokenizer, ref_codes, tempo, resampler
         self.min_cal = max(CONTEXT_FRAMES, chunk_size)
         self.all_codes, self.prev_len, self.spf = [], 0, None
         self.conv = owner._to_numpy if to_host else (lambda a: a.flatten())
@@ -141,8 +157,8 @@ class _StatefulWindow:
 
     any_chunking = True   # the PCM of a stream does not depend on how its frames are split into chunks
 
-    def __init__(self, owner, speech_tokenizer, ref_codes, chunk_size, to_host=True, tempo=None):
-        self.st, self.tempo = speech_tokenizer, tempo
+    def __init__(self, owner, speech_tokenizer, ref_codes, chunk_size, to_host=True, tempo=None, resampler=None):
+        self.st, self.tempo, self.resampler = speech_tokenizer, tempo, resampler
         self.stream = speech_tokenizer.open_stream()
         self.conv = owner._to_numpy if to_host else (lambda a: a.flatten())
         if ref_codes is not None and ref_codes.shape[0] > 0:
@@ -154,9 +170,10 @@ class _StatefulWindow:
 
 def decode_windows_batched(speech_tokenizer, wins, chunks, finals=None):
     """One chunk of several requests: windows of equal length are decoded as ONE batch (every codec launch covers all of
-    them), then the new samples of every window with a tempo are time-stretched in ONE launch, still on the device;
-    returns [(new_audio, sample_rate)] in the order of `wins`.  ``finals[i]`` ends request i: its tempo flushes.  A chunk
-    of no frames decodes nothing (a flush after the last frames)."""
+    them), then the new samples of every window with a tempo are time-stretched in ONE launch, and those of every window
+    with a resampler are resampled and encoded in ONE more launch, still on the device; returns [(new_audio,
+    sample_rate)] in the order of `wins`.  ``finals[i]`` ends request i: its tempo and resampler flush.  A chunk of no
+    frames decodes nothing (a flush after the last frames)."""
     raw = [None] * len(wins)
     sr = speech_tokenizer.sample_rate if hasattr(speech_tokenizer, "sample_rate") else 24000
     live = [i for i, c in enumerate(chunks) if int(c.shape[0])]
@@ -192,13 +209,34 @@ def decode_windows_batched(speech_tokenizer, wins, chunks, finals=None):
         pcm = tempo.process([wins[i].tempo for i in stretched], [raw[i] for i in stretched], [finals[i] for i in stretched])
         for i, a in zip(stretched, pcm):
             raw[i] = a
-    return [(w.conv(a if a is not None else torch.zeros(0)), sr) for w, a in zip(wins, raw)]
+    resampled = [i for i, w in enumerate(wins) if getattr(w, "resampler", None) is not None]
+    if resampled:
+        from . import resample
+        finals = finals or [False] * len(wins)
+        for i in resampled:
+            if raw[i] is None:
+                raw[i] = torch.zeros(0, dtype=torch.float32, device=wins[i].resampler.device)
+        out = resample.process([wins[i].resampler for i in resampled], [raw[i] for i in resampled],
+                               [finals[i] for i in resampled])
+        for i, a in zip(resampled, out):
+            raw[i] = a
+    return [(w.conv(a if a is not None else torch.zeros(0)), _window_rate(w, sr)) for w, a in zip(wins, raw)]
+
+
+def _window_rate(win, sr):
+    r = getattr(win, "resampler", None)
+    return sr if r is None else r.rate
+
+
+def _open_stages(win):
+    """whether a window still holds device stages that have not flushed (a tempo or a resampler)"""
+    return any(s is not None and not s.final for s in (getattr(win, "tempo", None), getattr(win, "resampler", None)))
 
 
 def flush_windows(speech_tokenizer, wins):
-    """The end of several requests: every window with a tempo flushes, in one launch -> [(last samples, sample_rate)]
-    of those windows, in order (the tempo's lookahead; windows without a tempo have nothing left)"""
-    wins = [w for w in wins if getattr(w, "tempo", None) is not None and not w.tempo.final]
+    """The end of several requests: every window with a tempo or a resampler flushes, in one launch per stage ->
+    [(last samples, sample_rate)] of those windows, in order (their look-ahead; other windows have nothing left)"""
+    wins = [w for w in wins if _open_stages(w)]
     empty = torch.zeros(0, 16, dtype=torch.long)
     return wins, decode_windows_batched(speech_tokenizer, wins, [empty] * len(wins), [True] * len(wins))
 
@@ -542,20 +580,22 @@ class FasterQwen3TTS:
     # ------------------------------------------------------------------ codec helpers
     @staticmethod
     def _to_numpy(a):
-        if hasattr(a, "cpu"):
-            return a.flatten().float().cpu().numpy()
+        if hasattr(a, "cpu"):   # encoded output (int16 / uint8) leaves the device as it is
+            return (a.flatten().float() if a.is_floating_point() else a.flatten()).cpu().numpy()
         return a.flatten() if hasattr(a, "flatten") else a
 
-    def _decode_all(self, speech_tokenizer, codec_ids, ref_codes, speed=1.0):
+    def _decode_all(self, speech_tokenizer, codec_ids, ref_codes, speed=1.0, sample_rate=None):
         """Non-streaming decode + proportional reference trim (model.py:918-938)."""
-        return self._decode_takes(speech_tokenizer, [codec_ids], ref_codes, **_speed_kw(speed))
+        return self._decode_takes(speech_tokenizer, [codec_ids], ref_codes, **_post_kw(speed, sample_rate))
 
-    def _stream_audio(self, chunks, speech_tokenizer, ref_codes, chunk_size, to_host=True, speed=1.0):
+    def _stream_audio(self, chunks, speech_tokenizer, ref_codes, chunk_size, to_host=True, speed=1.0,
+                      sample_rate=None):
         """The reference's hybrid streaming decode (model.py:1052-1135): Phase 1 re-decodes everything so far
         (reference codes prepended in ICL mode) until max(25, chunk_size) frames exist and calibrates
         samples_per_frame; Phase 2 decodes a 25-frame left-context window and trims the context.  At a speed other than
-        1 the stream ends with one more item: the tempo's last samples (``chunk_steps`` 0)."""
-        win = self._make_window(speech_tokenizer, ref_codes, chunk_size, to_host, **_speed_kw(speed))
+        1, or an output rate other than 24 kHz, the stream ends with one more item: the last samples of the tempo and
+        the resampler (``chunk_steps`` 0)."""
+        win = self._make_window(speech_tokenizer, ref_codes, chunk_size, to_host, **_post_kw(speed, sample_rate))
         timing = {}
         for codec_chunk, timing in chunks:
             new_audio, sr = win.push(codec_chunk)
@@ -563,15 +603,22 @@ class FasterQwen3TTS:
         for _, (tail, sr) in zip(*flush_windows(speech_tokenizer, [win])):
             yield tail, sr, dict(timing, chunk_steps=0, is_final=True)
 
-    def _make_window(self, speech_tokenizer, ref_codes, chunk_size, to_host=True, speed=1.0):
-        """the codec window of one request; at a speed other than 1 it carries the request's ``tempo.Tempo``"""
+    def _make_window(self, speech_tokenizer, ref_codes, chunk_size, to_host=True, speed=1.0, sample_rate=None,
+                     encoding="f32"):
+        """the codec window of one request; at a speed other than 1 it carries the request's ``tempo.Tempo``, at an
+        output rate or encoding other than 24 kHz f32 its ``resample.Resampler``"""
+        from .resample import resampler_for
         from .tempo import tempo_for
         if self.streaming_codec not in ("window", "stateful"):
             raise ValueError("streaming_codec must be 'window' or 'stateful'")
         tempo = tempo_for(speed, _pcm_device(speech_tokenizer)) if speed != 1.0 else None
+        rs = None
+        if sample_rate is not None or encoding != "f32":
+            rs = resampler_for(sample_rate, encoding, _pcm_device(speech_tokenizer))
+        kw = dict(tempo=tempo, resampler=rs)
         if self.streaming_codec == "stateful" and getattr(speech_tokenizer, "supports_streams", False):
-            return _StatefulWindow(self, speech_tokenizer, ref_codes, chunk_size, to_host, tempo=tempo)
-        return _StreamWindow(self, speech_tokenizer, ref_codes, chunk_size, to_host, tempo=tempo)
+            return _StatefulWindow(self, speech_tokenizer, ref_codes, chunk_size, to_host, **kw)
+        return _StreamWindow(self, speech_tokenizer, ref_codes, chunk_size, to_host, **kw)
 
     @staticmethod
     def _gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p, do_sample, repetition_penalty):
@@ -583,11 +630,14 @@ class FasterQwen3TTS:
     def stream_from_embeds(self, tie, tam, tth, tpe, ref_codes=None, chunk_size: int = 8, to_host: bool = True,
                            max_new_tokens: int = 2048, min_new_tokens: int = 2, temperature: float = 0.9,
                            top_k: int = 50, top_p: float = 1.0, do_sample: bool = True,
-                           repetition_penalty: float = 1.05, uniforms=None, speed: float = 1.0):
+                           repetition_penalty: float = 1.05, uniforms=None, speed: float = 1.0,
+                           sample_rate: Optional[int] = None):
         """generate_voice_clone_streaming from the point where the prompt embeddings exist (model.py:1079-1137).
-        ``speed``: speaking rate in [0.25, 4.0] (see ``_stream_audio``)."""
+        ``speed``: speaking rate in [0.25, 4.0]; ``sample_rate``: output rate (None: 24000), one of
+        ``resample.RATES`` (see ``_stream_audio``)."""
         from .streaming import fast_generate_streaming
         _check_speed(speed)
+        _check_rate(sample_rate)
         m = self.model.model
         m.talker.rope_deltas = None
         chunks = fast_generate_streaming(
@@ -600,29 +650,32 @@ class FasterQwen3TTS:
             for codes, timing in chunks:
                 yield (codes.cpu().numpy() if to_host else codes), self.sample_rate, timing
             return
-        yield from self._stream_audio(chunks, st, ref_codes, chunk_size, to_host=to_host, **_speed_kw(speed))
+        yield from self._stream_audio(chunks, st, ref_codes, chunk_size, to_host=to_host,
+                                      **_post_kw(speed, sample_rate))
 
     @torch.inference_mode()
     def stream_batch_from_embeds(self, tie, tam, tth, tpe, ref_codes=None, chunk_size: int = 8, to_host: bool = True,
                                  max_new_tokens: int = 2048, min_new_tokens: int = 2, temperature: float = 0.9,
                                  top_k: int = 50, top_p: float = 1.0, do_sample: bool = True,
                                  repetition_penalty: float = 1.05, uniforms=None, decode_audio: bool = True,
-                                 speed: float = 1.0):
+                                 speed: float = 1.0, sample_rate: Optional[int] = None):
         """Batched streaming from the point where the (left-padded) prompt batch exists (the tuple
         ``_build_talker_inputs_local`` returns for a list of requests, model.py:774-805): all rows advance together, one
         persistent-kernel launch per chunk; yields [(row, pcm_or_codes, sr, timing)] per chunk.  ``ref_codes``: None or
         a list with one entry per row (ICL reference frames / None).  ``speed``: speaking rate of every row, in [0.25,
-        4.0]; other than 1, a last item holds every row's final samples (``chunk_steps`` 0)."""
+        4.0]; ``sample_rate``: output rate of every row (None: 24000); other than the identity, a last item holds every
+        row's final samples (``chunk_steps`` 0)."""
         from .batching import fast_generate_streaming_batch
         _check_speed(speed)
+        _check_rate(sample_rate)
         m = self.model.model
         m.talker.rope_deltas = None
         B = tie.shape[0]
         st = m.speech_tokenizer if decode_audio else None
         wins = None
         if st is not None:
-            wins = [self._make_window(st, None if ref_codes is None else ref_codes[b], chunk_size, to_host, **_speed_kw(speed))
-                    for b in range(B)]
+            wins = [self._make_window(st, None if ref_codes is None else ref_codes[b], chunk_size, to_host,
+                                      **_post_kw(speed, sample_rate)) for b in range(B)]
         kw = self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p, do_sample, repetition_penalty)
         for items in fast_generate_streaming_batch(
                 talker=m.talker, talker_input_embeds=tie, attention_mask=tam, trailing_text_hiddens=tth,
@@ -644,18 +697,19 @@ class FasterQwen3TTS:
                                     min_new_tokens: int = 2, temperature: float = 0.9, top_k: int = 50,
                                     top_p: float = 1.0, do_sample: bool = True, repetition_penalty: float = 1.05,
                                     non_streaming_mode: Optional[bool] = None, chunk_size: int = 8,
-                                    speed: float = 1.0):
+                                    speed: float = 1.0, sample_rate: Optional[int] = None):
         """Concurrent custom-voice requests (BASELINE config 4) sharing every pass over the weights: the prompts are
         batched and left-padded exactly like the reference's builder does for a list of requests (model.py:583-805),
-        then decoded together.  ``speed`` (one for all requests): speaking rate in [0.25, 4.0], applied on the device.
-        Returns ([audio per request], sample_rate)."""
+        then decoded together.  ``speed`` (one for all requests): speaking rate in [0.25, 4.0], and ``sample_rate``: output
+        rate (None: 24000), both applied on the device.  Returns ([audio per request], sample_rate)."""
         _check_speed(speed)
+        _check_rate(sample_rate)
         instructs, nsm = self._custom_voice_rules(texts, languages, speakers, instructs or [None] * len(texts),
                                                   non_streaming_mode)
         _, _, _, tie, tam, tth, tpe = self._prepare_generation_custom_batch(texts, languages, speakers, instructs, nsm)
         parts = [[] for _ in texts]
-        sr = self.sample_rate
-        for items in self.stream_batch_from_embeds(tie, tam, tth, tpe, chunk_size=chunk_size, **_speed_kw(speed), **self._gen_kwargs(
+        sr = _rate_of(self.sample_rate, sample_rate)
+        for items in self.stream_batch_from_embeds(tie, tam, tth, tpe, chunk_size=chunk_size, **_post_kw(speed, sample_rate), **self._gen_kwargs(
                 max_new_tokens, min_new_tokens, temperature, top_k, top_p, do_sample, repetition_penalty)):
             for b, audio, sr, _ in items:
                 parts[b].append(audio)
@@ -669,8 +723,10 @@ class FasterQwen3TTS:
                              repetition_penalty: float = 1.05, xvec_only: bool = False,
                              non_streaming_mode: Optional[bool] = None, append_silence: bool = True,
                              instruct: Optional[str] = None, ref_spk=None, ref_rvq=None, ref_spk_emb=None,
-                             ref_codes=None, voice_clone_prompt=None, speed: float = 1.0) -> Tuple[list, int]:
+                             ref_codes=None, voice_clone_prompt=None, speed: float = 1.0,
+                             sample_rate: Optional[int] = None) -> Tuple[list, int]:
         _check_speed(speed)
+        _check_rate(sample_rate)
         voice_clone_prompt, nsm = self._voice_clone_rules(voice_clone_prompt, non_streaming_mode, ref_spk, ref_rvq,
                                                           ref_spk_emb, ref_codes)
         *prep, ref_codes = self._prepare_generation(
@@ -678,7 +734,7 @@ class FasterQwen3TTS:
             non_streaming_mode=nsm, append_silence=append_silence, voice_clone_prompt=voice_clone_prompt,
             instruct=instruct)
         return self._one_shot(prep, ref_codes, self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k,
-                                                                top_p, do_sample, repetition_penalty), speed)
+                                                                top_p, do_sample, repetition_penalty), speed, sample_rate)
 
     @torch.inference_mode()
     def generate_voice_clone_streaming(self, text: str, language: str, ref_audio=None, ref_text: str = "",
@@ -688,9 +744,11 @@ class FasterQwen3TTS:
                                        xvec_only: bool = False, non_streaming_mode: Optional[bool] = None,
                                        append_silence: bool = True, parity_mode: bool = False,
                                        instruct: Optional[str] = None, ref_spk=None, ref_rvq=None, ref_spk_emb=None,
-                                       ref_codes=None, voice_clone_prompt=None, speed: float = 1.0
+                                       ref_codes=None, voice_clone_prompt=None, speed: float = 1.0,
+                                       sample_rate: Optional[int] = None
                                        ) -> Generator[Tuple[np.ndarray, int, dict], None, None]:
         _check_speed(speed)
+        _check_rate(sample_rate)
         voice_clone_prompt, nsm = self._voice_clone_rules(voice_clone_prompt, non_streaming_mode, ref_spk, ref_rvq,
                                                           ref_spk_emb, ref_codes)
         m, talker, config, tie, tam, tth, tpe, ref_codes = self._prepare_generation(
@@ -703,10 +761,10 @@ class FasterQwen3TTS:
             chunks = parity_generate_streaming(
                 talker=talker, talker_input_embeds=tie, attention_mask=tam, trailing_text_hiddens=tth, tts_pad_embed=tpe,
                 config=config, chunk_size=chunk_size, **gen)
-            yield from self._stream_audio(chunks, m.speech_tokenizer, ref_codes, chunk_size, **_speed_kw(speed))
+            yield from self._stream_audio(chunks, m.speech_tokenizer, ref_codes, chunk_size, **_post_kw(speed, sample_rate))
             return
         yield from self.stream_from_embeds(tie, tam, tth, tpe, ref_codes=ref_codes, chunk_size=chunk_size,
-                                           **_speed_kw(speed), **gen)
+                                           **_post_kw(speed, sample_rate), **gen)
 
     def _voice_clone_rules(self, voice_clone_prompt, non_streaming_mode, ref_spk=None, ref_rvq=None, ref_spk_emb=None,
                            ref_codes=None):
@@ -765,9 +823,9 @@ class FasterQwen3TTS:
         self._validate(language)
         return self._resolve_non_streaming_mode(non_streaming_mode, default=True)
 
-    def _one_shot(self, prep, ref_codes, gen, speed=1.0):
+    def _one_shot(self, prep, ref_codes, gen, speed=1.0, sample_rate=None):
         """The delivery of the three one-shot methods: generate, then decode every frame at once (model.py:893-947),
-        time-stretched on the device at a speed other than 1."""
+        time-stretched on the device at a speed other than 1, resampled at an output rate other than 24 kHz."""
         from .generate import fast_generate
         m, talker, config, tie, tam, tth, tpe = prep
         codec_ids, timing = fast_generate(
@@ -775,8 +833,8 @@ class FasterQwen3TTS:
             config=config, predictor_graph=self.predictor_graph, talker_graph=self.talker_graph, **gen)
         if codec_ids is None:
             logger.warning("Generation returned no tokens")
-            return [np.zeros(1, dtype=np.float32)], self.sample_rate
-        audio, sr = self._decode_all(m.speech_tokenizer, codec_ids, ref_codes, **_speed_kw(speed))
+            return [np.zeros(1, dtype=np.float32)], _rate_of(self.sample_rate, sample_rate)
+        audio, sr = self._decode_all(m.speech_tokenizer, codec_ids, ref_codes, **_post_kw(speed, sample_rate))
         self._log_rtf(timing)
         return audio, sr
 
@@ -784,50 +842,58 @@ class FasterQwen3TTS:
     def generate_custom_voice(self, text: str, speaker: str, language: str, instruct: Optional[str] = None,
                               non_streaming_mode: Optional[bool] = None, max_new_tokens: int = 2048,
                               min_new_tokens: int = 2, temperature: float = 0.9, top_k: int = 50, top_p: float = 1.0,
-                              do_sample: bool = True, repetition_penalty: float = 1.05, speed: float = 1.0
+                              do_sample: bool = True, repetition_penalty: float = 1.05, speed: float = 1.0,
+                              sample_rate: Optional[int] = None
                               ) -> Tuple[list, int]:
         _check_speed(speed)
+        _check_rate(sample_rate)
         (instruct,), nsm = self._custom_voice_rules([text], [language], [speaker], [instruct], non_streaming_mode)
         prep = self._prepare_generation_custom(text, language, speaker, instruct, nsm)
         return self._one_shot(prep, None, self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p,
-                                                           do_sample, repetition_penalty), speed)
+                                                           do_sample, repetition_penalty), speed, sample_rate)
 
     @torch.inference_mode()
     def generate_custom_voice_streaming(self, text: str, speaker: str, language: str, instruct: Optional[str] = None,
                                         non_streaming_mode: Optional[bool] = None, max_new_tokens: int = 2048,
                                         min_new_tokens: int = 2, temperature: float = 0.9, top_k: int = 50,
                                         top_p: float = 1.0, do_sample: bool = True, repetition_penalty: float = 1.05,
-                                        chunk_size: int = 12, speed: float = 1.0
+                                        chunk_size: int = 12, speed: float = 1.0,
+                                        sample_rate: Optional[int] = None
                                         ) -> Generator[Tuple[np.ndarray, int, dict], None, None]:
         _check_speed(speed)
+        _check_rate(sample_rate)
         (instruct,), nsm = self._custom_voice_rules([text], [language], [speaker], [instruct], non_streaming_mode)
         _, _, _, tie, tam, tth, tpe = self._prepare_generation_custom(text, language, speaker, instruct, nsm)
-        yield from self.stream_from_embeds(tie, tam, tth, tpe, chunk_size=chunk_size, **_speed_kw(speed), **self._gen_kwargs(
+        yield from self.stream_from_embeds(tie, tam, tth, tpe, chunk_size=chunk_size, **_post_kw(speed, sample_rate), **self._gen_kwargs(
             max_new_tokens, min_new_tokens, temperature, top_k, top_p, do_sample, repetition_penalty))
 
     @torch.inference_mode()
     def generate_voice_design(self, text: str, instruct: str, language: str,
                               non_streaming_mode: Optional[bool] = None, max_new_tokens: int = 2048,
                               min_new_tokens: int = 2, temperature: float = 0.9, top_k: int = 50, top_p: float = 1.0,
-                              do_sample: bool = True, repetition_penalty: float = 1.05, speed: float = 1.0
+                              do_sample: bool = True, repetition_penalty: float = 1.05, speed: float = 1.0,
+                              sample_rate: Optional[int] = None
                               ) -> Tuple[list, int]:
         _check_speed(speed)
+        _check_rate(sample_rate)
         nsm = self._voice_design_rules(language, non_streaming_mode)
         prep = self._prepare_generation_custom(text, language, None, instruct, nsm)
         return self._one_shot(prep, None, self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p,
-                                                           do_sample, repetition_penalty), speed)
+                                                           do_sample, repetition_penalty), speed, sample_rate)
 
     @torch.inference_mode()
     def generate_voice_design_streaming(self, text: str, instruct: str, language: str,
                                         non_streaming_mode: Optional[bool] = None, max_new_tokens: int = 2048,
                                         min_new_tokens: int = 2, temperature: float = 0.9, top_k: int = 50,
                                         top_p: float = 1.0, do_sample: bool = True, repetition_penalty: float = 1.05,
-                                        chunk_size: int = 12, speed: float = 1.0
+                                        chunk_size: int = 12, speed: float = 1.0,
+                                        sample_rate: Optional[int] = None
                                         ) -> Generator[Tuple[np.ndarray, int, dict], None, None]:
         _check_speed(speed)
+        _check_rate(sample_rate)
         nsm = self._voice_design_rules(language, non_streaming_mode)
         _, _, _, tie, tam, tth, tpe = self._prepare_generation_custom(text, language, None, instruct, nsm)
-        yield from self.stream_from_embeds(tie, tam, tth, tpe, chunk_size=chunk_size, **_speed_kw(speed), **self._gen_kwargs(
+        yield from self.stream_from_embeds(tie, tam, tth, tpe, chunk_size=chunk_size, **_post_kw(speed, sample_rate), **self._gen_kwargs(
             max_new_tokens, min_new_tokens, temperature, top_k, top_p, do_sample, repetition_penalty))
 
     # ------------------------------------------------------------------ several takes of one request
@@ -845,7 +911,7 @@ class FasterQwen3TTS:
             raise ValueError(f"{len(seeds)} seeds for {n_takes} takes")
         return seeds
 
-    def _takes(self, prep, ref_codes, seeds, gen, chunk_size=64, speed=1.0):
+    def _takes(self, prep, ref_codes, seeds, gen, chunk_size=64, speed=1.0, sample_rate=None):
         """The one implementation behind the three ``*_takes`` methods: the prompt ``prep`` latched into one slot per take
         with ONE batched prefill (``BatchScheduler.submit_many``), all takes decoded together (one launch per chunk),
         their PCM decoded with one codec call per length.  Take i draws its uniforms from ``take_uniforms(seeds[i])``."""
@@ -870,16 +936,17 @@ class FasterQwen3TTS:
             sc = score(rq.lp.frames(), rq.eos_logprob)
             sc["seed"] = seeds[i]
             scores.append(sc)
-        audio, _ = self._decode_takes(m.speech_tokenizer, codes, ref_codes, **_speed_kw(speed))
-        return audio, self.sample_rate, scores
+        audio, _ = self._decode_takes(m.speech_tokenizer, codes, ref_codes, **_post_kw(speed, sample_rate))
+        return audio, _rate_of(self.sample_rate, sample_rate), scores
 
-    def _decode_takes(self, st, codes, ref_codes, speed=1.0):
+    def _decode_takes(self, st, codes, ref_codes, speed=1.0, sample_rate=None):
         """Non-streaming decode + proportional reference trim of every take, takes of equal length in ONE codec call (the
         decoder's rows are independent); at a speed other than 1 every take is time-stretched on the device, all in ONE
-        launch, as one push with flush.  Returns (audio per take, the sample rate the codec returned)."""
-        from . import tempo
+        launch, and at an output rate other than 24 kHz resampled, all in ONE more launch, each as one push with flush.
+        Returns (audio per take, the sample rate the codec returned, or the requested one)."""
+        from . import resample, tempo
         out = [np.zeros(1, dtype=np.float32)] * len(codes)
-        tempos, pcms, at = [], [], []
+        pcms, at = [], []
         sr = self.sample_rate
         groups = {}
         for i, c in enumerate(codes):
@@ -894,19 +961,25 @@ class FasterQwen3TTS:
                 a = a.flatten()
                 if ref_len > 0:
                     a = a[int(ref_len / max(batch.shape[1], 1) * len(a)):]
-                t = tempo.tempo_for(speed, a.device) if speed != 1.0 else None
-                if t is None:
+                if speed == 1.0 and sample_rate is None:
                     out[i] = self._to_numpy(a)
                 else:
-                    tempos.append(t)
                     pcms.append(a)
                     at.append(i)
-        if tempos:
-            for i, a in zip(at, tempo.process(tempos, pcms, True)):
+        if at:
+            tempos = [tempo.tempo_for(speed, a.device) for a in pcms]   # None where speed quantises to 1
+            if tempos[0] is not None:
+                pcms = tempo.process(tempos, pcms, True)
+                for t in tempos:
+                    t.close()
+            rss = [resample.resampler_for(sample_rate, "f32", a.device) for a in pcms]
+            if rss and rss[0] is not None:
+                pcms = resample.process(rss, pcms, True)
+                for r in rss:
+                    r.close()
+            for i, a in zip(at, pcms):
                 out[i] = self._to_numpy(a)
-            for t in tempos:
-                t.close()
-        return out, sr
+        return out, _rate_of(sr, sample_rate)
 
     @torch.inference_mode()
     def generate_voice_clone_takes(self, text: str, language: str, ref_audio=None, ref_text: str = "",
@@ -915,7 +988,7 @@ class FasterQwen3TTS:
                                    repetition_penalty: float = 1.05, xvec_only: bool = False,
                                    non_streaming_mode: Optional[bool] = None, append_silence: bool = True,
                                    instruct: Optional[str] = None, voice_clone_prompt=None, speed: float = 1.0,
-                                   n_takes: int = 4, seeds: Optional[List[int]] = None):
+                                   sample_rate: Optional[int] = None, n_takes: int = 4, seeds: Optional[List[int]] = None):
         """``n_takes`` renderings of one ``generate_voice_clone`` request for the price of one batched decode: one prompt,
         one batched prefill, one launch per chunk for all takes.  Take i is the request run alone with the uniforms of
         ``take_uniforms(seeds[i], max_new_tokens)`` -- bit for bit while both run the per-head talker attention (a lone
@@ -924,6 +997,7 @@ class FasterQwen3TTS:
         EOS term included), "frames" and "seed".  A log-probability says how likely the sampler found its draws, not
         how good the audio is: the calls rank nothing and pick nothing."""
         _check_speed(speed)
+        _check_rate(sample_rate)
         voice_clone_prompt, nsm = self._voice_clone_rules(voice_clone_prompt, non_streaming_mode)
         seeds = self._check_takes(n_takes, seeds)
         *prep, ref_codes = self._prepare_generation(
@@ -931,39 +1005,46 @@ class FasterQwen3TTS:
             non_streaming_mode=nsm, append_silence=append_silence, voice_clone_prompt=voice_clone_prompt,
             instruct=instruct)
         return self._takes(prep, ref_codes, seeds, self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k,
-                                                                    top_p, do_sample, repetition_penalty), speed=speed)
+                                                                    top_p, do_sample, repetition_penalty), speed=speed,
+                           sample_rate=sample_rate)
 
     @torch.inference_mode()
     def generate_custom_voice_takes(self, text: str, speaker: str, language: str, instruct: Optional[str] = None,
                                     non_streaming_mode: Optional[bool] = None, max_new_tokens: int = 2048,
                                     min_new_tokens: int = 2, temperature: float = 0.9, top_k: int = 50,
                                     top_p: float = 1.0, do_sample: bool = True, repetition_penalty: float = 1.05,
-                                    speed: float = 1.0, n_takes: int = 4, seeds: Optional[List[int]] = None):
+                                    speed: float = 1.0, sample_rate: Optional[int] = None, n_takes: int = 4,
+                                    seeds: Optional[List[int]] = None):
         """``n_takes`` renderings of one ``generate_custom_voice`` request (see ``generate_voice_clone_takes``)."""
         _check_speed(speed)
+        _check_rate(sample_rate)
         (instruct,), nsm = self._custom_voice_rules([text], [language], [speaker], [instruct], non_streaming_mode)
         seeds = self._check_takes(n_takes, seeds)
         prep = self._prepare_generation_custom(text, language, speaker, instruct, nsm)
         return self._takes(prep, None, seeds, self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k,
-                                                               top_p, do_sample, repetition_penalty), speed=speed)
+                                                               top_p, do_sample, repetition_penalty), speed=speed,
+                           sample_rate=sample_rate)
 
     @torch.inference_mode()
     def generate_voice_design_takes(self, text: str, instruct: str, language: str,
                                     non_streaming_mode: Optional[bool] = None, max_new_tokens: int = 2048,
                                     min_new_tokens: int = 2, temperature: float = 0.9, top_k: int = 50,
                                     top_p: float = 1.0, do_sample: bool = True, repetition_penalty: float = 1.05,
-                                    speed: float = 1.0, n_takes: int = 4, seeds: Optional[List[int]] = None):
+                                    speed: float = 1.0, sample_rate: Optional[int] = None, n_takes: int = 4,
+                                    seeds: Optional[List[int]] = None):
         """``n_takes`` renderings of one ``generate_voice_design`` request (see ``generate_voice_clone_takes``)."""
         _check_speed(speed)
+        _check_rate(sample_rate)
         nsm = self._voice_design_rules(language, non_streaming_mode)
         seeds = self._check_takes(n_takes, seeds)
         prep = self._prepare_generation_custom(text, language, None, instruct, nsm)
         return self._takes(prep, None, seeds, self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k,
-                                                               top_p, do_sample, repetition_penalty), speed=speed)
+                                                               top_p, do_sample, repetition_penalty), speed=speed,
+                           sample_rate=sample_rate)
 
     # ------------------------------------------------------------------ incremental text input (text_stream.py)
     def _text_streaming(self, text_stream, language, speaker, instruct, voice_clone_prompt, non_streaming_mode,
-                        chunk_size, gen, speed=1.0):
+                        chunk_size, gen, speed=1.0, sample_rate=None):
         """The one implementation behind the three ``*_text_streaming`` methods.  Text streaming has one text layout,
         so the raw ``non_streaming_mode`` is checked here, not the voice kind's default."""
         from .text_stream import _refuse_unsupported, generate_text_streaming
@@ -973,7 +1054,7 @@ class FasterQwen3TTS:
             instruct_ids = self.model._tokenize_texts([self.model._build_instruct_text(instruct)])[0]
         yield from generate_text_streaming(self, text_stream, language=language, speaker=speaker,
                                            instruct_ids=instruct_ids, voice_clone_prompt=voice_clone_prompt,
-                                           chunk_size=chunk_size, **_speed_kw(speed), **gen)
+                                           chunk_size=chunk_size, **_post_kw(speed, sample_rate), **gen)
 
     @torch.inference_mode()
     def generate_custom_voice_text_streaming(self, text_stream, speaker: str, language: str,
@@ -981,32 +1062,36 @@ class FasterQwen3TTS:
                                              max_new_tokens: int = 2048, min_new_tokens: int = 2,
                                              temperature: float = 0.9, top_k: int = 50, top_p: float = 1.0,
                                              do_sample: bool = True, repetition_penalty: float = 1.05,
-                                             chunk_size: int = 12, speed: float = 1.0
+                                             chunk_size: int = 12, speed: float = 1.0,
+                                             sample_rate: Optional[int] = None
                                              ) -> Generator[Tuple[np.ndarray, int, dict], None, None]:
         """``generate_custom_voice_streaming`` with the text fed while it is spoken: ``text_stream`` is any iterable of
         ``str`` pieces (an LLM's reply token by token).  The audio equals that of the one-shot streaming request for the
         same text, whatever the split and however fast the pieces come; generation waits where the text has not arrived
         yet.  Timing dicts add ``text_wait_ms``, the time spent blocked on ``text_stream``."""
         _check_speed(speed)
+        _check_rate(sample_rate)
         (instruct,), _ = self._custom_voice_rules([text_stream], [language], [speaker], [instruct], non_streaming_mode)
         yield from self._text_streaming(text_stream, language, speaker, instruct, None, non_streaming_mode, chunk_size,
                                         self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p,
-                                                         do_sample, repetition_penalty), speed)
+                                                         do_sample, repetition_penalty), speed, sample_rate)
 
     @torch.inference_mode()
     def generate_voice_design_text_streaming(self, text_stream, instruct: str, language: str,
                                              non_streaming_mode: Optional[bool] = None, max_new_tokens: int = 2048,
                                              min_new_tokens: int = 2, temperature: float = 0.9, top_k: int = 50,
                                              top_p: float = 1.0, do_sample: bool = True,
-                                             repetition_penalty: float = 1.05, chunk_size: int = 12, speed: float = 1.0
+                                             repetition_penalty: float = 1.05, chunk_size: int = 12, speed: float = 1.0,
+                                             sample_rate: Optional[int] = None
                                              ) -> Generator[Tuple[np.ndarray, int, dict], None, None]:
         """``generate_voice_design_streaming`` with the text fed while it is spoken (see
         ``generate_custom_voice_text_streaming``)."""
         _check_speed(speed)
+        _check_rate(sample_rate)
         self._voice_design_rules(language, non_streaming_mode)
         yield from self._text_streaming(text_stream, language, None, instruct, None, non_streaming_mode, chunk_size,
                                         self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p,
-                                                         do_sample, repetition_penalty), speed)
+                                                         do_sample, repetition_penalty), speed, sample_rate)
 
     @torch.inference_mode()
     def generate_voice_clone_text_streaming(self, text_stream, language: str, ref_audio=None, ref_text: str = "",
@@ -1016,12 +1101,14 @@ class FasterQwen3TTS:
                                             chunk_size: int = 12, xvec_only: bool = True,
                                             non_streaming_mode: Optional[bool] = None, append_silence: bool = True,
                                             ref_spk=None, ref_rvq=None, ref_spk_emb=None, ref_codes=None,
-                                            voice_clone_prompt=None, speed: float = 1.0
+                                            voice_clone_prompt=None, speed: float = 1.0,
+                                            sample_rate: Optional[int] = None
                                             ) -> Generator[Tuple[np.ndarray, int, dict], None, None]:
         """``generate_voice_clone_streaming`` with the text fed while it is spoken, x-vector cloning only: ICL cloning
         puts the target text under the reference codec frames inside the prompt, so it must be known before prefill
         (ValueError)."""
         _check_speed(speed)
+        _check_rate(sample_rate)
         voice_clone_prompt, _ = self._voice_clone_rules(voice_clone_prompt, non_streaming_mode, ref_spk, ref_rvq,
                                                         ref_spk_emb, ref_codes)
         from .text_stream import ICL_REFUSAL, _refuse_unsupported
@@ -1034,7 +1121,7 @@ class FasterQwen3TTS:
             voice_clone_prompt=voice_clone_prompt)
         yield from self._text_streaming(text_stream, language, None, None, vcp, non_streaming_mode, chunk_size,
                                         self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p,
-                                                         do_sample, repetition_penalty), speed)
+                                                         do_sample, repetition_penalty), speed, sample_rate)
 
     def _log_rtf(self, timing):
         n = timing["steps"]

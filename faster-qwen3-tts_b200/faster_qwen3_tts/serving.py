@@ -52,7 +52,8 @@ def to_wav_bytes(pcm: np.ndarray, sample_rate: int) -> bytes:
 
 @dataclass
 class Ticket:
-    """Handle of one submitted request: iterate it for (pcm float32, sample_rate, timing) chunks."""
+    """Handle of one submitted request: iterate it for (audio, sample_rate, timing) chunks; the audio is float32, or
+    int16 / uint8 in the encodings ``s16`` / ``ulaw`` / ``alaw``."""
     rid: int
     prepare: Callable[[], tuple]          # -> (tie, tam, tth, tpe, ref_codes); runs on the worker thread
     gen_kwargs: dict
@@ -66,6 +67,13 @@ class Ticket:
     underruns: int = 0                    # paced: chunks delivered after the listener had run dry (lead < 0)
     prepared: Optional[tuple] = None      # (submit arguments, window) of a ticket waiting for KV pages
     speed: float = 1.0                    # speaking rate: the listener consumes model audio `speed` times as fast
+    sample_rate: int = 24000              # output rate and encoding of the audio (resample.py)
+    encoding: str = "f32"
+
+    @property
+    def flushes(self) -> bool:
+        """whether the request's window holds device stages (a tempo, a resampler) that flush with its last chunk"""
+        return self.speed != 1.0 or (self.sample_rate, self.encoding) != (24000, "f32")
 
     def cancel(self) -> None:
         """End the request: the worker frees its slot (or drops it from the queue) and closes the ticket."""
@@ -82,7 +90,8 @@ class Ticket:
 
     def audio(self) -> np.ndarray:
         parts = [c[0] for c in self]
-        return np.concatenate(parts) if parts else np.zeros(0, dtype=np.float32)
+        empty = {"f32": np.float32, "s16": np.int16}.get(self.encoding, np.uint8)
+        return np.concatenate(parts) if parts else np.zeros(0, dtype=empty)
 
 
 @dataclass
@@ -138,7 +147,10 @@ class ContinuousBatcher:
     ``window_factory`` is called with the ticket's own ``chunk_size`` as a second argument when it has one, and with
     ``speed=`` when the ticket's speaking rate is not 1 (``submit(..., speed=)``): the window then time-stretches its
     PCM on the device, ``batch_decode`` gets a third argument (whether each request ends with this chunk: its tempo
-    flushes), and the lead counts audio seconds at that rate, ``frames x frame_s / speed``.
+    flushes), and the lead counts audio seconds at that rate, ``frames x frame_s / speed``.  Likewise with
+    ``sample_rate=`` / ``encoding=`` when the ticket asks for other than 24 kHz f32 (``submit(..., sample_rate=,
+    encoding=)``): the window resamples and encodes on the device, its resampler flushes with the last chunk, and the
+    lead, which counts audio seconds, is the same at every rate.
     ``clock`` / ``sleep`` are the worker's time source, replaceable in tests."""
 
     def __init__(self, scheduler, window_factory: Callable, chunk_size: int = 8, idle_sleep: float = 0.002,
@@ -165,14 +177,17 @@ class ContinuousBatcher:
 
     # ---- client side ------------------------------------------------------------------------------------
     def submit(self, prepare: Callable[[], tuple], pace: Optional[float] = None, speed: float = 1.0,
-               **gen_kwargs) -> Ticket:
+               sample_rate: Optional[int] = None, encoding: str = "f32", **gen_kwargs) -> Ticket:
         """``pace``: the client plays at ``pace`` x real time (class docstring); ``speed``: speaking rate in [0.25,
-        4.0].  ``gen_kwargs`` are the scheduler's ``submit`` keywords, among them ``chunk_size`` / ``first_chunk`` for
-        this request alone."""
+        4.0]; ``sample_rate`` (None: 24000) and ``encoding`` (``f32 | s16 | ulaw | alaw``): the audio the ticket carries.
+        ``gen_kwargs`` are the scheduler's ``submit`` keywords, among them ``chunk_size`` / ``first_chunk`` for this
+        request alone."""
         speed = self._speed(speed)
+        out = self._output(sample_rate, encoding)
         with self._lock:
             self._rid += 1
-            t = Ticket(self._rid, prepare, gen_kwargs, pace=self._pace(pace), submitted_at=self.clock(), speed=speed)
+            t = Ticket(self._rid, prepare, gen_kwargs, pace=self._pace(pace), submitted_at=self.clock(), speed=speed,
+                       **out)
         self.pending.put(t)
         return t
 
@@ -188,16 +203,23 @@ class ContinuousBatcher:
         quantize(speed)
         return float(speed)
 
+    @staticmethod
+    def _output(sample_rate, encoding):
+        from .resample import check_encoding, check_rate
+        return dict(sample_rate=check_rate(sample_rate), encoding=check_encoding(encoding))
+
     def submit_text(self, prepare: Callable, pace: Optional[float] = None, speed: float = 1.0,
-                    **gen_kwargs) -> TextTicket:
+                    sample_rate: Optional[int] = None, encoding: str = "f32", **gen_kwargs) -> TextTicket:
         """A text-fed request.  ``prepare(feed)`` -> (tie, tam, tpe, ref_codes) builds the prompt once the feed holds its
         first committed id (``text_stream.TextFeed.prompt_ids``); it runs on the worker thread."""
         if self.feed_factory is None:
             raise RuntimeError("this batcher has no text feed factory")
         speed = self._speed(speed)
+        out = self._output(sample_rate, encoding)
         with self._lock:
             self._rid += 1
-            t = TextTicket(self._rid, prepare, gen_kwargs, pace=self._pace(pace), submitted_at=self.clock(), speed=speed)
+            t = TextTicket(self._rid, prepare, gen_kwargs, pace=self._pace(pace), submitted_at=self.clock(), speed=speed,
+                           **out)
         t.feed = self.feed_factory(int(gen_kwargs.get("max_new_tokens", 2048)))
         self.pending.put(t)
         return t
@@ -233,7 +255,7 @@ class ContinuousBatcher:
             if t.cancelled.is_set():
                 self.sched.cancel(self.requests.pop(rid))
                 del self.live[rid]
-                self._drop_tempo(win)
+                self._drop_stages(win)
                 t.out.put(_DONE)
 
     def _prepare(self, t: Ticket):
@@ -260,16 +282,19 @@ class ContinuousBatcher:
         return req, win
 
     @staticmethod
-    def _drop_tempo(win):
-        tempo = getattr(win, "tempo", None)
-        if tempo is not None:
-            tempo.close()
+    def _drop_stages(win):
+        """hand the window's tempo and resampler state back to their pools"""
+        for stage in (getattr(win, "tempo", None), getattr(win, "resampler", None)):
+            if stage is not None:
+                stage.close()
 
     def _window(self, t: Ticket, ref_codes):
         """the request's codec window, built for the request's own chunk size where it has one (the window policy's
         calibration point depends on it); a short first chunk is for windows whose audio does not depend on the chunking"""
         own = t.gen_kwargs.get("chunk_size")
         kw = {} if t.speed == 1.0 else {"speed": t.speed}
+        if (t.sample_rate, t.encoding) != (24000, "f32"):
+            kw.update(sample_rate=t.sample_rate, encoding=t.encoding)
         win = self.window_factory(ref_codes, **kw) if own is None else self.window_factory(ref_codes, own, **kw)
         if t.gen_kwargs.get("first_chunk") and not getattr(win, "any_chunking", False):
             raise ValueError("first_chunk needs a codec window whose audio does not depend on the chunking (the stateful "
@@ -363,10 +388,10 @@ class ContinuousBatcher:
                 self.sleep(self.idle_sleep)
                 continue
             self.steps += 1
-            # a stretched request's last step flushes its tempo, even when that step made no frames
+            # the last step of a request with device stages flushes them, even when that step made no frames
             live = [(rq, codes) for rq, codes in results
-                    if int(codes.shape[0]) or (rq.finished and self.live[rq.tag][0].speed != 1.0)]
-            stretched = any(self.live[rq.tag][0].speed != 1.0 for rq, _ in live)
+                    if int(codes.shape[0]) or (rq.finished and self.live[rq.tag][0].flushes)]
+            stretched = any(self.live[rq.tag][0].flushes for rq, _ in live)
             # windows of equal length of all requests are decoded as one batch when the window objects support it
             pcm_of = {}
             if live and self.batch_decode is not None:
@@ -382,7 +407,7 @@ class ContinuousBatcher:
                     if rq.tag in pcm_of:
                         pcm, sr = pcm_of[rq.tag]
                     else:
-                        pcm, sr = win.push(codes) if t.speed == 1.0 else win.push(codes, final=bool(rq.finished))
+                        pcm, sr = win.push(codes, final=bool(rq.finished)) if t.flushes else win.push(codes)
                     now = self.clock()
                     if t.first_chunk_at is None:
                         t.first_chunk_at = now
@@ -397,7 +422,7 @@ class ContinuousBatcher:
                     t.out.put(_DONE)
                     del self.live[rq.tag]
                     self.requests.pop(rq.tag, None)
-                    self._drop_tempo(win)
+                    self._drop_stages(win)
 
 
 def batcher_for_model(model, chunk_size: int = 8, to_host: bool = True, **kw) -> ContinuousBatcher:
@@ -413,12 +438,14 @@ def batcher_for_model(model, chunk_size: int = 8, to_host: bool = True, **kw) ->
         def push(self, codes):
             return codes.cpu().numpy(), model.sample_rate
 
-    def window(ref_codes, chunk=chunk_size, speed=1.0):
+    def window(ref_codes, chunk=chunk_size, speed=1.0, **out):
         if st is None:
             if speed != 1.0:
                 raise ValueError("a speaking rate other than 1 needs the codec (PCM)")
+            if out:
+                raise ValueError("an output rate or encoding other than 24 kHz f32 needs the codec (PCM)")
             return _CodesOnly()
-        return model._make_window(st, ref_codes, chunk, to_host, **({} if speed == 1.0 else {"speed": speed}))
+        return model._make_window(st, ref_codes, chunk, to_host, **({} if speed == 1.0 else {"speed": speed}), **out)
 
     bd = (lambda wins, chunks, finals=None: decode_windows_batched(st, wins, chunks, finals)) if st is not None else None
     from .text_stream import TextFeed

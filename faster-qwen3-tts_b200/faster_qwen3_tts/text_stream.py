@@ -186,7 +186,7 @@ def generate_text_streaming(model, text_stream: Iterable[str], *, language: str,
                             voice_clone_prompt=None, chunk_size: int = 12, max_new_tokens: int = 2048,
                             min_new_tokens: int = 2, temperature: float = 0.9, top_k: int = 50, top_p: float = 1.0,
                             do_sample: bool = True, repetition_penalty: float = 1.05, uniforms=None, to_host: bool = True,
-                            speed: float = 1.0) -> Iterator:
+                            speed: float = 1.0, sample_rate=None) -> Iterator:
     """Yields (pcm, sample_rate, timing) like the ``*_streaming`` methods.  Prefills once the first text id is
     committed, then per launch: pull text until the next chunk's rows exist (window codec policy) or one more row
     exists (stateful codec), or the text closes; announce the rows; decode one chunk.  The request is the one request of
@@ -227,7 +227,8 @@ def generate_text_streaming(model, text_stream: Iterable[str], *, language: str,
                                  voice_clone_prompt=voice_clone_prompt)
     win = None
     if st is not None:
-        win = model._make_window(st, None, chunk_size, to_host, **({} if speed == 1.0 else {"speed": speed}))
+        from .model import _post_kw
+        win = model._make_window(st, None, chunk_size, to_host, **_post_kw(speed, sample_rate))
     # the window policy's PCM depends on the chunking: launch only when a full chunk of rows exists, so that every launch
     # emits a full chunk or ends the request.  A stateful stream (or codes only) is the same in any chunking.
     ahead = 1 if win is None or getattr(win, "any_chunking", False) else chunk_size
@@ -249,10 +250,10 @@ def generate_text_streaming(model, text_stream: Iterable[str], *, language: str,
         wait[0] = wait_before = 0.0
         if win is None:
             yield (codes.cpu().numpy() if to_host else codes), model.sample_rate, tm
-        elif getattr(win, "tempo", None) is None:
+        elif getattr(win, "tempo", None) is None and getattr(win, "resampler", None) is None:
             pcm, sr = win.push(codes)
             yield pcm, sr, tm
-        else:   # the last chunk flushes the tempo
+        else:   # the last chunk flushes the tempo and the resampler
             pcm, sr = win.push(codes, final=bool(rq.finished))
             yield pcm, sr, tm
     if win is not None:

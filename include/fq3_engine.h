@@ -395,6 +395,46 @@ int fq3_tempo_process(fq3_tempo* const* tempos, int32_t n_streams, const float* 
                       void* stream);
 const char* fq3_tempo_last_error(void);
 
+/* ---- Output sample rate and encoding: polyphase resampling of 24 kHz PCM on the device (csrc/fq3_resample.cu)
+ * Output rates R in {8000, 16000, 22050, 24000, 32000, 44100, 48000}; g = gcd(R, FQ3_RESAMPLE_IN_RATE), L = R / g,
+ * M = FQ3_RESAMPLE_IN_RATE / g, m = max(L, M), half = FQ3_RESAMPLE_HALF_PER_M * m.  The filter is
+ * firwin(2 half + 1, FQ3_RESAMPLE_CUTOFF / m, Kaiser window beta FQ3_RESAMPLE_BETA), scaled to unit DC gain, and
+ * y[n] = L * sum_j h[j] x[(n M + half - j) / L] over the j where n M + half - j is a non-negative multiple of L (x is
+ * zero outside the stream).  R = 24000 with a non-f32 encoding is the encode-only case (h = {1}, half = 0); R = 24000
+ * with FQ3_ENC_F32 is the identity and has no resampler state (create refuses it: callers pass the PCM through).
+ * The encoding is applied in the kernel's store: f32; s16 = clip(x * 32768, -32768, 32767) truncated toward zero;
+ * G.711 mu-law / A-law of that s16.  A push releases exactly fq3_resample_released(R, samples pushed before, samples
+ * pushed now, flush) samples -- a function of the totals alone, so buffers are sized on the host and nothing is read
+ * back; a flushed stream of N samples has ceil(N L / M).  The output does not depend on how the input was pushed.
+ * The algorithm, bit for bit, is in DESIGN.md ("Output rate and encoding") and faster_qwen3_tts/resample.py. */
+#define FQ3_RESAMPLE_IN_RATE 24000
+#define FQ3_RESAMPLE_HALF_PER_M 32
+#define FQ3_RESAMPLE_CUTOFF 0.9
+#define FQ3_RESAMPLE_BETA 8.6
+#define FQ3_RESAMPLE_ALIGN 16
+#define FQ3_ENC_F32 0
+#define FQ3_ENC_S16 1
+#define FQ3_ENC_ULAW 2
+#define FQ3_ENC_ALAW 3
+typedef struct fq3_resample fq3_resample;
+/* designs the rate's filter on the host in double precision; the polyphase table is uploaded once per (device, rate)
+ * and shared by every resampler at that rate */
+int fq3_resample_create(int32_t device, int32_t out_rate, int32_t encoding, fq3_resample** out);
+int fq3_resample_reset(fq3_resample* r);   /* a new stream at the same rate; host-side, nothing is launched */
+void fq3_resample_destroy(fq3_resample* r);
+/* samples released by a push of n samples after total_in (-1 for an unknown rate or a negative count) */
+int64_t fq3_resample_released(int32_t out_rate, int64_t total_in, int64_t n, int32_t flush);
+/* the rate's filter h (double, 2 half + 1 taps) into out[0, cap); returns the number of taps (-1 for an unknown rate) */
+int32_t fq3_resample_taps(int32_t out_rate, double* out, int32_t cap);
+/* One launch for n_streams distinct resamplers.  in_dev float32: the streams' new samples packed in order (in_lens[i]
+ * of stream i, host array); flush[i] (host) != 0 ends stream i (it must be reset before more input).  out_dev
+ * [out_cap bytes]: the released samples of every stream in its encoding, packed in order, each stream's slice starting
+ * at the next FQ3_RESAMPLE_ALIGN-byte boundary.  A null, misaligned or too small buffer, a resampler listed twice or a
+ * flushed resampler is refused before anything is launched. */
+int fq3_resample_process(fq3_resample* const* rs, int32_t n_streams, const float* in_dev, const int64_t* in_lens,
+                         const int32_t* flush, void* out_dev, int64_t out_cap, void* stream);
+const char* fq3_resample_last_error(void);
+
 const char* fq3_last_error(void);
 const char* fq3_version(void);
 

@@ -11,7 +11,8 @@ JSON record per run, each with the card's name, power limit and SM clock read in
 N = 32 unpaced requests (pace = None: the engine calls of a build without paced listeners) give the reference point.
 ``--kv-pages N`` serves the listeners from a pool of N 64-row talker KV pages instead of max_seq_len rows per slot: the
 records then also hold the parks and the most pages in use at once.  ``--speed S`` gives every request the speaking rate S
-(time-stretched on the GPU after the codec): a listener then consumes model audio S times as fast.
+(time-stretched on the GPU after the codec): a listener then consumes model audio S times as fast.  ``--sample-rate R``
+/ ``--encoding E`` give every request that output rate and encoding (resampled and encoded on the GPU after the codec).
 
     python tools/paced_serving_bench.py --listeners 32,64,96,128,160,192 --codec window,stateful --repeats 2 \\
         --out profiles/h100_paced_serving.jsonl
@@ -60,7 +61,7 @@ class Timed:
         return out
 
 
-def run(model, n, codec, first_chunk, seed, stagger_s, chunk, pace=1.0, speed=1.0):
+def run(model, n, codec, first_chunk, seed, stagger_s, chunk, pace=1.0, speed=1.0, sample_rate=24000, encoding="f32"):
     from faster_qwen3_tts.serving import batcher_for_model, voice_clone_request
     model.streaming_codec = codec
     rng = np.random.default_rng(seed)
@@ -74,6 +75,8 @@ def run(model, n, codec, first_chunk, seed, stagger_s, chunk, pace=1.0, speed=1.
     extra = {"first_chunk": first_chunk} if first_chunk else {}
     if speed != 1.0:
         extra["speed"] = speed
+    out = {} if (sample_rate, encoding) == (24000, "f32") else {"sample_rate": sample_rate, "encoding": encoding}
+    extra.update(out)
     tickets, ttfa, t_start = [None] * n, [None] * n, time.monotonic()
 
     def listener(i):
@@ -94,7 +97,7 @@ def run(model, n, codec, first_chunk, seed, stagger_s, chunk, pace=1.0, speed=1.
     b.close()
     under = [t.underruns for t in tickets]
     assert all(t.frames == f for t, f in zip(tickets, frames)), "a listener did not get all its audio"
-    return {"listeners": n, "pace": pace, **({"speed": speed} if speed != 1.0 else {}), "codec": codec, "first_chunk": first_chunk, "chunk": chunk, "seed": seed,
+    return {"listeners": n, "pace": pace, **({"speed": speed} if speed != 1.0 else {}), **out, "codec": codec, "first_chunk": first_chunk, "chunk": chunk, "seed": seed,
             "audio_s": round(sum(frames) * 0.08, 1), "wall_s": round(wall, 2),
             "underruns_total": int(sum(under)), "listeners_with_underruns": int(sum(u > 0 for u in under)),
             "underruns_per_listener": round(float(np.mean(under)), 3), "underruns_max": int(max(under)),
@@ -119,6 +122,8 @@ def main():
     ap.add_argument("--size", default="1.7B")
     ap.add_argument("--kv-pages", type=int, default=0, help="talker KV page pool (0: max_seq_len rows per slot)")
     ap.add_argument("--speed", type=float, default=1.0, help="speaking rate of every request, in [0.25, 4.0]")
+    ap.add_argument("--sample-rate", type=int, default=24000, help="output rate of every request")
+    ap.add_argument("--encoding", default="f32", choices=["f32", "s16", "ulaw", "alaw"])
     ap.add_argument("--out", default=os.path.join(ROOT, "profiles", "h100_paced_serving.jsonl"))
     args = ap.parse_args()
     if not torch.cuda.is_available():
@@ -143,7 +148,8 @@ def main():
     os.makedirs(os.path.dirname(args.out), exist_ok=True)
     with open(args.out, "a") as f:
         def record(*a, **k):
-            rec = dict(base, **card(), **run(model, *a, speed=args.speed, **k))
+            rec = dict(base, **card(), **run(model, *a, speed=args.speed, sample_rate=args.sample_rate,
+                                                  encoding=args.encoding, **k))
             print(json.dumps(rec), flush=True)
             f.write(json.dumps(rec) + "\n")
             f.flush()
