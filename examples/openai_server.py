@@ -2,7 +2,7 @@
 """OpenAI-compatible TTS server over the H100 engine with CONTINUOUS BATCHING.
 
 Same endpoint and wire format as the reference's example server (POST /v1/audio/speech, response_format wav | pcm, plus
-ulaw | alaw: raw 8-bit G.711; streaming WAV with an unknown-length header; the reference's
+ulaw | alaw: raw 8-bit G.711, and flac: lossless FLAC; streaming WAV with an unknown-length header; the reference's
 examples/openai_server.py:91-118,215-263), but requests are not serialised behind a lock (:71,181): up to --max-batch
 requests share every pass over the model weights and new requests join between chunks (faster_qwen3_tts/serving.py).  A
 streamed response is a listener: it is paced at real time by default, so the engine, which makes audio several times
@@ -11,7 +11,7 @@ costs its KV cache) on --max-batch launch columns.  The request field "pace" ove
 relative to real time, null = as fast as possible.  "speed" (0.25 - 4.0) is the speaking rate: the audio is
 time-stretched on the GPU after the codec, at the same pitch.  "sample_rate" (8000, 16000, 22050, 24000, 32000, 44100 or
 48000; default 24000) is the rate of the response: the audio is resampled and encoded (s16 for wav / pcm, G.711 for ulaw
-/ alaw) on the GPU, so only the encoded bytes leave it.
+/ alaw, s16 compressed to a FLAC stream for flac) on the GPU, so only the encoded bytes leave it.
 
     python examples/openai_server.py --model synthetic:1.7B --max-batch 16 --port 8000
     curl -s localhost:8000/v1/audio/speech -H 'Content-Type: application/json' \\
@@ -41,7 +41,7 @@ def build_app(model, batcher, voices, default_voice):
         model: str = "tts-1"
         input: str
         voice: str = "alloy"
-        response_format: str = "wav"   # wav | pcm (16-bit) | ulaw | alaw (8-bit G.711)
+        response_format: str = "wav"   # wav | pcm (16-bit) | ulaw | alaw (8-bit G.711) | flac (lossless, 16-bit)
         sample_rate: int = 24000        # one of 8000, 16000, 22050, 24000, 32000, 44100, 48000
         speed: float = 1.0             # speaking rate in [0.25, 4.0], same pitch
         pace: Optional[float] = 1.0    # the client plays at pace x real time; null: everything as fast as possible
@@ -58,9 +58,10 @@ def build_app(model, batcher, voices, default_voice):
         if v is None:
             raise HTTPException(status_code=400, detail=f"Voice {req.voice!r} is not configured. Available voices: {list(voices)}")
         fmt = req.response_format.lower()
-        encoding = {"wav": "s16", "pcm": "s16", "ulaw": "ulaw", "alaw": "alaw"}.get(fmt)
+        encoding = {"wav": "s16", "pcm": "s16", "ulaw": "ulaw", "alaw": "alaw", "flac": "flac"}.get(fmt)
         if encoding is None:
-            raise HTTPException(status_code=400, detail=f"response_format {fmt!r} not supported. Use: wav, pcm, ulaw, alaw")
+            raise HTTPException(status_code=400,
+                                detail=f"response_format {fmt!r} not supported. Use: wav, pcm, ulaw, alaw, flac")
         if req.sample_rate not in RATES:
             raise HTTPException(status_code=400, detail=f"'sample_rate' must be one of {list(RATES)}, got {req.sample_rate}")
         if req.pace is not None and not req.pace > 0:
@@ -82,7 +83,8 @@ def build_app(model, batcher, voices, default_voice):
                     return
                 yield item[0].tobytes()   # encoded on the device
 
-        media = {"wav": "audio/wav", "pcm": "audio/pcm", "ulaw": "audio/basic", "alaw": "audio/x-alaw-basic"}[fmt]
+        media = {"wav": "audio/wav", "pcm": "audio/pcm", "ulaw": "audio/basic", "alaw": "audio/x-alaw-basic",
+                 "flac": "audio/flac"}[fmt]
         return StreamingResponse(audio_stream(), media_type=media)
 
     return app

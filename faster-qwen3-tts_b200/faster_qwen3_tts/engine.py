@@ -85,6 +85,8 @@ EXPORTS = [
     "fq3_tempo_last_error",
     "fq3_resample_create", "fq3_resample_reset", "fq3_resample_destroy", "fq3_resample_released", "fq3_resample_taps",
     "fq3_resample_process", "fq3_resample_last_error",
+    "fq3_flac_create", "fq3_flac_reset", "fq3_flac_destroy", "fq3_flac_max_bytes", "fq3_flac_process",
+    "fq3_flac_last_error",
 ]
 
 
@@ -208,6 +210,15 @@ def load_library() -> C.CDLL:
     lib.fq3_resample_process.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.POINTER(C.c_int64),
                                          C.POINTER(C.c_int32), C.c_void_p, C.c_int64, C.c_void_p]
     lib.fq3_resample_last_error.restype = C.c_char_p
+    lib.fq3_flac_create.argtypes = [C.c_int32, C.c_int32, C.POINTER(C.c_void_p)]
+    lib.fq3_flac_reset.argtypes = [C.c_void_p]
+    lib.fq3_flac_destroy.argtypes = [C.c_void_p]
+    lib.fq3_flac_destroy.restype = None
+    lib.fq3_flac_max_bytes.argtypes = [C.c_int64, C.c_int64, C.c_int32]
+    lib.fq3_flac_max_bytes.restype = C.c_int64
+    lib.fq3_flac_process.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int32),
+                                     C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
+    lib.fq3_flac_last_error.restype = C.c_char_p
     _lib = lib
     return lib
 

@@ -79,12 +79,15 @@ class _StreamWindow:
     reference's warmed template stream (``SpeechTokenizer.reference_stream``): same samples, one chunk's worth of work,
     and the reference itself is decoded once per voice instead of four times per request.  Phase 2 (25-frame context
     windows without the reference) is the reference's approximation and is decoded exactly as the reference does.
-    ``FQ3_PHASE1_STREAM=0`` keeps the literal re-decode.  ``tempo``: the request's speaking rate (``tempo.Tempo``), and
-    ``resampler``: its output rate and encoding (``resample.Resampler``), applied in that order to the new samples on the
-    device before they are converted (``decode_windows_batched``)."""
+    ``FQ3_PHASE1_STREAM=0`` keeps the literal re-decode.  ``tempo``: the request's speaking rate (``tempo.Tempo``),
+    ``resampler``: its output rate and encoding (``resample.Resampler``), and ``flac``: its FLAC encoder
+    (``flac.Encoder``, after an s16 resampler), applied in that order to the new samples on the device before they are
+    converted (``decode_windows_batched``)."""
 
-    def __init__(self, owner, speech_tokenizer, ref_codes, chunk_size, to_host=True, tempo=None, resampler=None):
-        self.st, self.ref_codes, self.tempo, self.resampler = speech_tokenizer, ref_codes, tempo, resampler
+    def __init__(self, owner, speech_tokenizer, ref_codes, chunk_size, to_host=True, tempo=None, resampler=None,
+                 flac=None):
+        self.st, self.ref_codes, self.tempo, self.resampler, self.flac = (speech_tokenizer, ref_codes, tempo, resampler,
+                                                                          flac)
         self.min_cal = max(CONTEXT_FRAMES, chunk_size)
         self.all_codes, self.prev_len, self.spf = [], 0, None
         self.conv = owner._to_numpy if to_host else (lambda a: a.flatten())
@@ -157,8 +160,9 @@ class _StatefulWindow:
 
     any_chunking = True   # the PCM of a stream does not depend on how its frames are split into chunks
 
-    def __init__(self, owner, speech_tokenizer, ref_codes, chunk_size, to_host=True, tempo=None, resampler=None):
-        self.st, self.tempo, self.resampler = speech_tokenizer, tempo, resampler
+    def __init__(self, owner, speech_tokenizer, ref_codes, chunk_size, to_host=True, tempo=None, resampler=None,
+                 flac=None):
+        self.st, self.tempo, self.resampler, self.flac = speech_tokenizer, tempo, resampler, flac
         self.stream = speech_tokenizer.open_stream()
         self.conv = owner._to_numpy if to_host else (lambda a: a.flatten())
         if ref_codes is not None and ref_codes.shape[0] > 0:
@@ -171,9 +175,10 @@ class _StatefulWindow:
 def decode_windows_batched(speech_tokenizer, wins, chunks, finals=None):
     """One chunk of several requests: windows of equal length are decoded as ONE batch (every codec launch covers all of
     them), then the new samples of every window with a tempo are time-stretched in ONE launch, and those of every window
-    with a resampler are resampled and encoded in ONE more launch, still on the device; returns [(new_audio,
-    sample_rate)] in the order of `wins`.  ``finals[i]`` ends request i: its tempo and resampler flush.  A chunk of no
-    frames decodes nothing (a flush after the last frames)."""
+    with a resampler are resampled and encoded in ONE more launch, and those of every window with a FLAC encoder are
+    compressed in one more encoding launch (and its packing launch), still on the device; returns [(new_audio,
+    sample_rate)] in the order of `wins`.  ``finals[i]`` ends request i: its tempo, resampler and FLAC encoder flush.  A
+    chunk of no frames decodes nothing (a flush after the last frames)."""
     raw = [None] * len(wins)
     sr = speech_tokenizer.sample_rate if hasattr(speech_tokenizer, "sample_rate") else 24000
     live = [i for i, c in enumerate(chunks) if int(c.shape[0])]
@@ -220,6 +225,14 @@ def decode_windows_batched(speech_tokenizer, wins, chunks, finals=None):
                                [finals[i] for i in resampled])
         for i, a in zip(resampled, out):
             raw[i] = a
+    compressed = [i for i, w in enumerate(wins) if getattr(w, "flac", None) is not None]
+    if compressed:
+        from . import flac
+        finals = finals or [False] * len(wins)
+        out = flac.process([wins[i].flac for i in compressed], [raw[i] for i in compressed],
+                           [finals[i] for i in compressed])
+        for i, a in zip(compressed, out):
+            raw[i] = a
     return [(w.conv(a if a is not None else torch.zeros(0)), _window_rate(w, sr)) for w, a in zip(wins, raw)]
 
 
@@ -229,12 +242,13 @@ def _window_rate(win, sr):
 
 
 def _open_stages(win):
-    """whether a window still holds device stages that have not flushed (a tempo or a resampler)"""
-    return any(s is not None and not s.final for s in (getattr(win, "tempo", None), getattr(win, "resampler", None)))
+    """whether a window still holds device stages that have not flushed (a tempo, a resampler or a FLAC encoder)"""
+    return any(s is not None and not s.final
+               for s in (getattr(win, "tempo", None), getattr(win, "resampler", None), getattr(win, "flac", None)))
 
 
 def flush_windows(speech_tokenizer, wins):
-    """The end of several requests: every window with a tempo or a resampler flushes, in one launch per stage ->
+    """The end of several requests: every window with device stages flushes, in one launch per stage ->
     [(last samples, sample_rate)] of those windows, in order (their look-ahead; other windows have nothing left)"""
     wins = [w for w in wins if _open_stages(w)]
     empty = torch.zeros(0, 16, dtype=torch.long)
@@ -606,16 +620,21 @@ class FasterQwen3TTS:
     def _make_window(self, speech_tokenizer, ref_codes, chunk_size, to_host=True, speed=1.0, sample_rate=None,
                      encoding="f32"):
         """the codec window of one request; at a speed other than 1 it carries the request's ``tempo.Tempo``, at an
-        output rate or encoding other than 24 kHz f32 its ``resample.Resampler``"""
+        output rate or encoding other than 24 kHz f32 its ``resample.Resampler``; ``encoding="flac"`` is an s16
+        resampler followed by a ``flac.Encoder``"""
         from .resample import resampler_for
         from .tempo import tempo_for
         if self.streaming_codec not in ("window", "stateful"):
             raise ValueError("streaming_codec must be 'window' or 'stateful'")
         tempo = tempo_for(speed, _pcm_device(speech_tokenizer)) if speed != 1.0 else None
-        rs = None
-        if sample_rate is not None or encoding != "f32":
+        rs = enc = None
+        if encoding == "flac":
+            from .flac import Encoder
+            rs = resampler_for(sample_rate, "s16", _pcm_device(speech_tokenizer))
+            enc = Encoder(rs.rate, _pcm_device(speech_tokenizer))
+        elif sample_rate is not None or encoding != "f32":
             rs = resampler_for(sample_rate, encoding, _pcm_device(speech_tokenizer))
-        kw = dict(tempo=tempo, resampler=rs)
+        kw = dict(tempo=tempo, resampler=rs, flac=enc)
         if self.streaming_codec == "stateful" and getattr(speech_tokenizer, "supports_streams", False):
             return _StatefulWindow(self, speech_tokenizer, ref_codes, chunk_size, to_host, **kw)
         return _StreamWindow(self, speech_tokenizer, ref_codes, chunk_size, to_host, **kw)

@@ -53,7 +53,8 @@ def to_wav_bytes(pcm: np.ndarray, sample_rate: int) -> bytes:
 @dataclass
 class Ticket:
     """Handle of one submitted request: iterate it for (audio, sample_rate, timing) chunks; the audio is float32, or
-    int16 / uint8 in the encodings ``s16`` / ``ulaw`` / ``alaw``."""
+    int16 / uint8 in the encodings ``s16`` / ``ulaw`` / ``alaw``, or uint8 FLAC bytes in ``flac`` (the chunks of a
+    finished ticket concatenate to one complete .flac file)."""
     rid: int
     prepare: Callable[[], tuple]          # -> (tie, tam, tth, tpe, ref_codes); runs on the worker thread
     gen_kwargs: dict
@@ -72,7 +73,8 @@ class Ticket:
 
     @property
     def flushes(self) -> bool:
-        """whether the request's window holds device stages (a tempo, a resampler) that flush with its last chunk"""
+        """whether the request's window holds device stages (a tempo, a resampler, a FLAC encoder) that flush with its
+        last chunk"""
         return self.speed != 1.0 or (self.sample_rate, self.encoding) != (24000, "f32")
 
     def cancel(self) -> None:
@@ -150,7 +152,8 @@ class ContinuousBatcher:
     flushes), and the lead counts audio seconds at that rate, ``frames x frame_s / speed``.  Likewise with
     ``sample_rate=`` / ``encoding=`` when the ticket asks for other than 24 kHz f32 (``submit(..., sample_rate=,
     encoding=)``): the window resamples and encodes on the device, its resampler flushes with the last chunk, and the
-    lead, which counts audio seconds, is the same at every rate.
+    lead, which counts audio seconds, is the same at every rate.  ``encoding="flac"`` adds a FLAC encoder after an s16
+    resampler: the ticket's chunks are FLAC bytes, and its lead still counts audio seconds.
     ``clock`` / ``sleep`` are the worker's time source, replaceable in tests."""
 
     def __init__(self, scheduler, window_factory: Callable, chunk_size: int = 8, idle_sleep: float = 0.002,
@@ -179,7 +182,8 @@ class ContinuousBatcher:
     def submit(self, prepare: Callable[[], tuple], pace: Optional[float] = None, speed: float = 1.0,
                sample_rate: Optional[int] = None, encoding: str = "f32", **gen_kwargs) -> Ticket:
         """``pace``: the client plays at ``pace`` x real time (class docstring); ``speed``: speaking rate in [0.25,
-        4.0]; ``sample_rate`` (None: 24000) and ``encoding`` (``f32 | s16 | ulaw | alaw``): the audio the ticket carries.
+        4.0]; ``sample_rate`` (None: 24000) and ``encoding`` (``f32 | s16 | ulaw | alaw | flac``): the audio the ticket
+        carries.
         ``gen_kwargs`` are the scheduler's ``submit`` keywords, among them ``chunk_size`` / ``first_chunk`` for this
         request alone."""
         speed = self._speed(speed)
@@ -205,7 +209,8 @@ class ContinuousBatcher:
 
     @staticmethod
     def _output(sample_rate, encoding):
-        from .resample import check_encoding, check_rate
+        from .flac import check_encoding
+        from .resample import check_rate
         return dict(sample_rate=check_rate(sample_rate), encoding=check_encoding(encoding))
 
     def submit_text(self, prepare: Callable, pace: Optional[float] = None, speed: float = 1.0,
@@ -283,8 +288,8 @@ class ContinuousBatcher:
 
     @staticmethod
     def _drop_stages(win):
-        """hand the window's tempo and resampler state back to their pools"""
-        for stage in (getattr(win, "tempo", None), getattr(win, "resampler", None)):
+        """hand the window's tempo, resampler and FLAC encoder state back to their pools"""
+        for stage in (getattr(win, "tempo", None), getattr(win, "resampler", None), getattr(win, "flac", None)):
             if stage is not None:
                 stage.close()
 

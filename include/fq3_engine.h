@@ -435,6 +435,43 @@ int fq3_resample_process(fq3_resample* const* rs, int32_t n_streams, const float
                          const int32_t* flush, void* out_dev, int64_t out_cap, void* stream);
 const char* fq3_resample_last_error(void);
 
+/* ---- FLAC output: lossless compression of s16 PCM on the device (csrc/fq3_flac.cu)
+ * A FLAC stream (RFC 9639), mono, 16 bits, at any rate the resampler offers.  The stream starts with "fLaC" and one
+ * STREAMINFO block (FQ3_FLAC_HEAD_BYTES in all: block sizes FQ3_FLAC_GRAIN .. FQ3_FLAC_BLOCK, frame sizes 0, MD5 0,
+ * total samples 0 unless the push that releases the header also flushes).  Variable blocking: a push of m samples after
+ * c carried ones encodes FQ3_FLAC_GRAIN * floor((c + m) / FQ3_FLAC_GRAIN) of them (all at flush) as blocks of
+ * FQ3_FLAC_BLOCK and one block of the remainder, and carries the rest (< FQ3_FLAC_GRAIN).  Each block is a CONSTANT
+ * subframe when its samples are equal, else the fewest-bit FIXED subframe over orders 0 .. min(FQ3_FLAC_MAX_ORDER, n-1),
+ * partition orders 0 .. FQ3_FLAC_MAX_PARTITION_ORDER (n divisible by 2^p, more than `order` samples per partition) and
+ * per partition the Rice parameter 0 .. FQ3_FLAC_MAX_K with the fewest bits, ties to the lowest order, then p, then k;
+ * VERBATIM when that is not smaller.  The algorithm, bit for bit, is in DESIGN.md ("FLAC output") and
+ * faster_qwen3_tts/flac.py.  The bytes are a function of the samples, the push sizes and the flush point. */
+#define FQ3_FLAC_BLOCK 4096
+#define FQ3_FLAC_GRAIN 16
+#define FQ3_FLAC_MAX_ORDER 4
+#define FQ3_FLAC_MAX_PARTITION_ORDER 8
+#define FQ3_FLAC_MAX_K 30
+#define FQ3_FLAC_HEAD_BYTES 42
+#define FQ3_FLAC_ALIGN 16
+typedef struct fq3_flac fq3_flac;
+int fq3_flac_create(int32_t device, int32_t rate, fq3_flac** out);
+int fq3_flac_reset(fq3_flac* f);   /* a new stream at the same rate; host-side, nothing is launched */
+void fq3_flac_destroy(fq3_flac* f);
+/* a bound on the bytes a push of n samples after `carried` (0 .. FQ3_FLAC_GRAIN - 1) releases: the stream header and,
+ * per block of b samples, 2 b + 19 bytes (16 of frame header, the subframe header, the samples verbatim, the CRC-16);
+ * -1 for a negative count or a carry out of range */
+int64_t fq3_flac_max_bytes(int64_t carried, int64_t n, int32_t flush);
+/* One encoding launch for every block of n_streams distinct encoders, then one launch that packs each stream's
+ * output.  in_dev int16: the streams' new samples packed in order (in_lens[i] of stream i, host array); flush[i]
+ * (host) != 0 ends stream i.  Stream i's output region in out_dev starts at the next FQ3_FLAC_ALIGN-byte boundary after
+ * the previous region and is fq3_flac_max_bytes(carried_i, in_lens[i], flush[i]) bytes long; the stream's bytes are
+ * packed at its start and out_lens_dev[i] (int32, device) receives their count, so reading the counts back is the
+ * stage's one host synchronisation.  A null, misaligned or too small buffer, an encoder listed twice or a flushed
+ * encoder is refused before anything is launched. */
+int fq3_flac_process(fq3_flac* const* encs, int32_t n_streams, const int16_t* in_dev, const int64_t* in_lens,
+                     const int32_t* flush, void* out_dev, int64_t out_cap, int32_t* out_lens_dev, void* stream);
+const char* fq3_flac_last_error(void);
+
 const char* fq3_last_error(void);
 const char* fq3_version(void);
 

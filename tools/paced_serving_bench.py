@@ -12,7 +12,8 @@ N = 32 unpaced requests (pace = None: the engine calls of a build without paced 
 ``--kv-pages N`` serves the listeners from a pool of N 64-row talker KV pages instead of max_seq_len rows per slot: the
 records then also hold the parks and the most pages in use at once.  ``--speed S`` gives every request the speaking rate S
 (time-stretched on the GPU after the codec): a listener then consumes model audio S times as fast.  ``--sample-rate R``
-/ ``--encoding E`` give every request that output rate and encoding (resampled and encoded on the GPU after the codec).
+/ ``--encoding E`` give every request that output rate and encoding (resampled and encoded on the GPU after the codec;
+``flac`` compresses the s16 on the GPU as well).
 
     python tools/paced_serving_bench.py --listeners 32,64,96,128,160,192 --codec window,stateful --repeats 2 \\
         --out profiles/h100_paced_serving.jsonl
@@ -123,7 +124,7 @@ def main():
     ap.add_argument("--kv-pages", type=int, default=0, help="talker KV page pool (0: max_seq_len rows per slot)")
     ap.add_argument("--speed", type=float, default=1.0, help="speaking rate of every request, in [0.25, 4.0]")
     ap.add_argument("--sample-rate", type=int, default=24000, help="output rate of every request")
-    ap.add_argument("--encoding", default="f32", choices=["f32", "s16", "ulaw", "alaw"])
+    ap.add_argument("--encoding", default="f32", choices=["f32", "s16", "ulaw", "alaw", "flac"])
     ap.add_argument("--out", default=os.path.join(ROOT, "profiles", "h100_paced_serving.jsonl"))
     args = ap.parse_args()
     if not torch.cuda.is_available():
