@@ -11,7 +11,9 @@ costs its KV cache) on --max-batch launch columns.  The request field "pace" ove
 relative to real time, null = as fast as possible.  "speed" (0.25 - 4.0) is the speaking rate: the audio is
 time-stretched on the GPU after the codec, at the same pitch.  "sample_rate" (8000, 16000, 22050, 24000, 32000, 44100 or
 48000; default 24000) is the rate of the response: the audio is resampled and encoded (s16 for wav / pcm, G.711 for ulaw
-/ alaw, s16 compressed to a FLAC stream for flac) on the GPU, so only the encoded bytes leave it.
+/ alaw, s16 compressed to a FLAC stream for flac) on the GPU, so only the encoded bytes leave it.  "pitch" (semitones,
+-12 - 12) shifts the voice up or down (formants move with it) and "gain_db" (-96 - 16) scales the level before the
+encoding clips; both are applied on the GPU by the same time-stretch and resampler.
 
     python examples/openai_server.py --model synthetic:1.7B --max-batch 16 --port 8000
     curl -s localhost:8000/v1/audio/speech -H 'Content-Type: application/json' \\
@@ -32,7 +34,7 @@ def build_app(model, batcher, voices, default_voice):
     from fastapi.responses import StreamingResponse
     from typing import Optional
     from pydantic import BaseModel
-    from faster_qwen3_tts.resample import RATES
+    from faster_qwen3_tts.resample import RATES, check_prosody
     from faster_qwen3_tts.serving import voice_clone_request, wav_header
 
     app = FastAPI(title="faster-qwen3-tts (H100 engine) OpenAI-compatible API")
@@ -44,6 +46,8 @@ def build_app(model, batcher, voices, default_voice):
         response_format: str = "wav"   # wav | pcm (16-bit) | ulaw | alaw (8-bit G.711) | flac (lossless, 16-bit)
         sample_rate: int = 24000        # one of 8000, 16000, 22050, 24000, 32000, 44100, 48000
         speed: float = 1.0             # speaking rate in [0.25, 4.0], same pitch
+        pitch: float = 0.0             # semitones in [-12, 12]
+        gain_db: float = 0.0           # level in [-96, 16] dB
         pace: Optional[float] = 1.0    # the client plays at pace x real time; null: everything as fast as possible
 
     @app.get("/health")
@@ -68,9 +72,14 @@ def build_app(model, batcher, voices, default_voice):
             raise HTTPException(status_code=400, detail=f"'pace' must be a positive number or null, got {req.pace}")
         if not 0.25 <= req.speed <= 4.0:
             raise HTTPException(status_code=400, detail=f"'speed' must be in [0.25, 4.0], got {req.speed}")
+        try:
+            check_prosody(req.speed, req.pitch, req.gain_db)
+        except ValueError as ex:
+            raise HTTPException(status_code=400, detail=str(ex))
         ticket = batcher.submit(voice_clone_request(model, req.input, v.get("language", "Auto"), v["ref_audio"],
                                                     v.get("ref_text", "")), pace=req.pace, speed=req.speed,
-                                sample_rate=req.sample_rate, encoding=encoding, max_new_tokens=v.get("max_new_tokens", 2048))
+                                sample_rate=req.sample_rate, encoding=encoding, pitch=req.pitch, gain_db=req.gain_db,
+                                max_new_tokens=v.get("max_new_tokens", 2048))
         loop = asyncio.get_event_loop()
         it = iter(ticket)
 

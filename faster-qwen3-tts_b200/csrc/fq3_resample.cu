@@ -1,25 +1,32 @@
-// fq3_resample.cu -- output sample rate and encoding: a rational polyphase resampler of 24 kHz PCM that is already on
-// the device, with the encoding (f32, s16, G.711 mu-law / A-law) applied in the store, for any number of streams in one
-// launch.  The algorithm is fixed exactly (DESIGN.md, "Output rate and encoding"; faster_qwen3_tts/resample.py restates
-// the counts, oracle/resample_oracle.py the arithmetic in float64):
+// fq3_resample.cu -- output sample rate, pitch, gain and encoding: a rational polyphase resampler of 24 kHz PCM that is
+// already on the device, with the gain and the encoding (f32, s16, G.711 mu-law / A-law) applied in the store, for any
+// number of streams in one launch.  The algorithm is fixed exactly (DESIGN.md, "Output rate and encoding" and "Pitch and
+// gain"; faster_qwen3_tts/resample.py restates the counts; oracle/resample_oracle.py restates the arithmetic in float64
+// at rho 256, tests/pitch_oracle.py at every rho):
 //
-//   R in {8000, 16000, 22050, 24000, 32000, 44100, 48000}; g = gcd(R, 24000), L = R / g, M = 24000 / g, m = max(L, M),
-//   half = 32 m.  h = firwin(2 half + 1, 0.9 / m, Kaiser beta 8.6), scaled to unit DC gain, designed here in double.
-//   y[n] = L * sum_j h[j] x[(n M + half - j) / L] over the j with (n M + half - j) a non-negative multiple of L and the
-//   index in [0, N); x is zero outside [0, N).  A flushed stream of N samples has ceil(N L / M) outputs.
-//   R = 24000 with a non-f32 encoding is the encode-only case: h = {1}, half = 0.  R = 24000 with f32 is the identity
-//   and has no state (create refuses it: callers pass the PCM through).
+//   R in {8000, 16000, 22050, 24000, 32000, 44100, 48000}; rho in [128, 512] (the pitch ratio is rho / 256; 256 is no
+//   pitch shift).  (L, M) = (256 R, 24000 rho) reduced by their gcd, m = max(L, M), half = 32 m.
+//   h = firwin(2 half + 1, 0.9 / m, Kaiser beta 8.6), scaled to unit DC gain, designed here in double.
+//   y[n] = g * (L * sum_j h[j] x[(n M + half - j) / L]) over the j with (n M + half - j) a non-negative multiple of L
+//   and the index in [0, N); x is zero outside [0, N); g is the stream's float32 gain, one fp32 multiply (g = 1 leaves
+//   the sum's bits).  A flushed stream of N samples has ceil(N L / M) outputs.
+//   L == M (R = 24000 at rho 256, 48000 at rho 512) is the encode-only case: h = {1}, half = 0.  R = 24000 at rho 256
+//   with f32 and g = 1 is the identity: callers pass the PCM through (fq3_resample_create refuses it).
 //
 // Output n is released once input floor((n M + half) / L) exists, so the counts of a push are a function of the stream's
 // totals alone: the host sizes every buffer before the launch and nothing is read back.  Output n is a dot product over
 // fixed input indices in a fixed order (phase p = (n M + half) mod L, taps k = 0 .. K_p - 1 with input top - k, top =
-// floor((n M + half) / L)), so the bits do not depend on how the input was split into pushes.
+// floor((n M + half) / L)), so the bits do not depend on how the input was split into pushes, nor on which streams share
+// the launch.
 //
 // Outputs are independent: the grid is one CTA per (stream, tile of TILE outputs), one thread per output.  A CTA stages
-// the rate's phase table (shared by every stream at that rate) and the input span its tile reads into shared memory.
-// New samples are read in place from the caller's packed buffer; the per-stream device state is the last
-// TC = ceil(2 half / L) input samples, in two alternating buffers, so the CTA that writes the next tail never overwrites
-// the one the other CTAs of the same launch read.
+// the input span its tile reads in shared memory.  Where the whole phase table fits beside that span in 48 KB (every
+// plain rate, up to 41 KB at 22.05 kHz, and the small pitched tables) the CTA stages the table too; otherwise (most
+// pitched tables, up to 0.65 MB) each thread reads its output's phase row from the L2-resident table in global memory.
+// The choice is a function of (L, M, half) alone, so host and kernel make it alike, and both paths sum the same fp32
+// values in the same order: the bits do not depend on the path.  New samples are read in place from the caller's
+// packed buffer; the per-stream device state is the last TC = ceil(2 half / L) input samples, in two alternating
+// buffers, so the CTA that writes the next tail never overwrites the one the other CTAs of the same launch read.
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdint.h>
@@ -27,7 +34,9 @@
 
 #include <algorithm>
 #include <cstring>
+#include <list>
 #include <map>
+#include <tuple>
 #include <mutex>
 #include <utility>
 #include <vector>
@@ -37,8 +46,8 @@
 namespace {
 
 constexpr int TILE = 256;               // outputs per CTA, one per thread
-constexpr int TCAP = 256;               // tail buffer capacity (the largest tail is 192 samples, at 8 kHz)
-constexpr size_t SMEM_MAX = 48 * 1024;  // no opt-in needed: the largest need is ~42.5 KB (22.05 kHz)
+constexpr int TCAP = 384;               // tail buffer capacity: the largest tail is 384 samples (8 kHz, rho 512)
+constexpr int SMEM_MAX = 48 * 1024;     // no opt-in needed: a table is staged only where it fits beside its span
 
 thread_local char g_rerr[256] = "";
 int rfail(int code, const char* msg) {
@@ -75,17 +84,31 @@ bool valid_rate(int rate) {
 
 int sample_bytes(int enc) { return enc == FQ3_ENC_F32 ? 4 : enc == FQ3_ENC_S16 ? 2 : 1; }
 
+// floats of input a tile of TILE outputs reads, at most
+__host__ __device__ inline long long span_floats(int L, int M, int half) {
+  return ((TILE - 1) * (long long)M + 2 * half) / L + 2;
+}
+
+// whether a CTA stages the L x kmax phase table in shared memory (beside its input span) or reads rows from global
+__host__ __device__ inline bool stages_table(int L, int M, int half, int kmax) {
+  return ((long long)L * kmax + span_floats(L, M, half)) * (long long)sizeof(float) <= (long long)SMEM_MAX;
+}
+
 struct Ratio {
   int L, M, half;
   int kmax() const { return 2 * half / L + 1; }        // taps of phase 0, the most of any phase
   int tail() const { return (2 * half + L - 1) / L; }  // ceil(2 half / L)
 };
 
-// rate 24000 is the encode-only identity filter: one tap, no look-ahead
-Ratio ratio_of(int rate) {
-  if (rate == FQ3_RESAMPLE_IN_RATE) return Ratio{1, 1, 0};
-  const int g = (int)gcd64(rate, FQ3_RESAMPLE_IN_RATE);
-  const int L = rate / g, M = FQ3_RESAMPLE_IN_RATE / g;
+bool valid_pitch(int rho) { return rho >= FQ3_RESAMPLE_PITCH_MIN && rho <= FQ3_RESAMPLE_PITCH_MAX; }
+
+// (L, M) = (256 R, 24000 rho) / gcd; L == M is the encode-only identity filter: one tap, no look-ahead.  At rho 256
+// this is (R, 24000) / gcd, with 24000 the encode-only rate.
+Ratio ratio_of(int rate, int rho) {
+  const int64_t a = (int64_t)rate * FQ3_RESAMPLE_PITCH_ONE, b = (int64_t)FQ3_RESAMPLE_IN_RATE * rho;
+  const int64_t g = gcd64(a, b);
+  const int L = (int)(a / g), M = (int)(b / g);
+  if (L == M) return Ratio{1, 1, 0};
   return Ratio{L, M, FQ3_RESAMPLE_HALF_PER_M * (L > M ? L : M)};
 }
 
@@ -102,8 +125,8 @@ double bessel_i0(double x) {
 }
 
 // firwin(2 half + 1, 0.9 / m, window=("kaiser", 8.6)), scaled to unit DC gain
-std::vector<double> design(int rate) {
-  const Ratio r = ratio_of(rate);
+std::vector<double> design(int rate, int rho) {
+  const Ratio r = ratio_of(rate, rho);
   if (r.half == 0) return {1.0};
   const int n = 2 * r.half + 1;
   const double m = r.L > r.M ? r.L : r.M;
@@ -123,34 +146,64 @@ std::vector<double> design(int rate) {
   return h;
 }
 
-// one device phase table per (device, rate), shared by every stream at that rate and kept for the process's lifetime:
-// row p holds L * h[p + L k] for k < K_p, zero-padded to kmax
-std::mutex g_tab_mu;
-std::map<std::pair<int, int>, float*> g_tabs;
-
-int table_for(int dev, int rate, float** out) {
-  std::lock_guard<std::mutex> lk(g_tab_mu);
-  auto it = g_tabs.find({dev, rate});
-  if (it != g_tabs.end()) {
-    *out = it->second;
-    return 0;
-  }
-  const Ratio r = ratio_of(rate);
-  const std::vector<double> h = design(rate);
-  const int kmax = r.kmax();
-  std::vector<float> tab((size_t)r.L * kmax, 0.f);
-  for (int p = 0; p < r.L; ++p)
-    for (int k = 0; p + r.L * k <= 2 * r.half; ++k) tab[(size_t)p * kmax + k] = (float)(r.L * h[p + r.L * k]);
+// one device phase table per (device, rate, rho), shared by every stream at that rate and pitch: row p holds
+// L * h[p + L k] for k < K_p, zero-padded to kmax.  Plain tables (rho 256, seven at most) are kept for the process's
+// lifetime.  Pitched tables are counted by the handles that use them; once unreferenced they stay cached, and beyond
+// FQ3_RESAMPLE_TABLE_CACHE unreferenced ones the least recently released is freed.
+struct Table {
   float* d = nullptr;
-  if (cudaMalloc(&d, tab.size() * sizeof(float)) != cudaSuccess)
-    return rfail(FQ3_ERR_CUDA, "cudaMalloc of a phase table failed");
-  if (cudaMemcpy(d, tab.data(), tab.size() * sizeof(float), cudaMemcpyHostToDevice) != cudaSuccess) {
-    cudaFree(d);
-    return rfail(FQ3_ERR_CUDA, "upload of a phase table failed");
+  int64_t bytes = 0;
+  int refs = 0;
+};
+using TabKey = std::tuple<int, int, int>;   // (device, rate, rho)
+std::mutex g_tab_mu;
+std::map<TabKey, Table> g_tabs;
+std::list<TabKey> g_idle;                   // unreferenced pitched tables, least recently released first
+
+int table_for(int dev, int rate, int rho, float** out) {
+  std::lock_guard<std::mutex> lk(g_tab_mu);
+  const TabKey key{dev, rate, rho};
+  auto it = g_tabs.find(key);
+  if (it == g_tabs.end()) {
+    const Ratio r = ratio_of(rate, rho);
+    const std::vector<double> h = design(rate, rho);
+    const int kmax = r.kmax();
+    std::vector<float> tab((size_t)r.L * kmax, 0.f);
+    for (int p = 0; p < r.L; ++p)
+      for (int k = 0; p + r.L * k <= 2 * r.half; ++k) tab[(size_t)p * kmax + k] = (float)(r.L * h[p + r.L * k]);
+    float* d = nullptr;
+    if (cudaMalloc(&d, tab.size() * sizeof(float)) != cudaSuccess)
+      return rfail(FQ3_ERR_CUDA, "cudaMalloc of a phase table failed");
+    if (cudaMemcpy(d, tab.data(), tab.size() * sizeof(float), cudaMemcpyHostToDevice) != cudaSuccess) {
+      cudaFree(d);
+      return rfail(FQ3_ERR_CUDA, "upload of a phase table failed");
+    }
+    it = g_tabs.emplace(key, Table{d, (int64_t)(tab.size() * sizeof(float)), 0}).first;
   }
-  g_tabs[{dev, rate}] = d;
-  *out = d;
+  if (rho != FQ3_RESAMPLE_PITCH_ONE && it->second.refs++ == 0) g_idle.remove(key);
+  *out = it->second.d;
   return 0;
+}
+
+// a handle of a pitched table is gone: an unreferenced table joins the idle list, whose oldest entries beyond
+// FQ3_RESAMPLE_TABLE_CACHE are freed
+void table_release(int dev, int rate, int rho) {
+  if (rho == FQ3_RESAMPLE_PITCH_ONE) return;
+  std::lock_guard<std::mutex> lk(g_tab_mu);
+  const TabKey key{dev, rate, rho};
+  auto it = g_tabs.find(key);
+  if (it == g_tabs.end() || --it->second.refs > 0) return;
+  g_idle.push_back(key);
+  while ((int)g_idle.size() > FQ3_RESAMPLE_TABLE_CACHE) {
+    const TabKey old = g_idle.front();
+    g_idle.pop_front();
+    auto o = g_tabs.find(old);
+    {
+      DevGuard g(std::get<0>(old));
+      cudaFree(o->second.d);
+    }
+    g_tabs.erase(o);
+  }
 }
 
 int64_t ceil_div(int64_t a, int64_t b) { return a >= 0 ? (a + b - 1) / b : -((-a) / b); }
@@ -168,9 +221,10 @@ struct Job {
   float* tail_next;        // <- x[L1 - tc, L1), written by the job's first tile unless the stream flushes
   const float* in;         // new samples x[L0, L1)
   const float* tab;        // L x kmax phase table
-  unsigned char* out;      // encoded y[E0, E1)
+  unsigned char* out;      // encoded g * y[E0, E1)
   long long L0, L1, E0, E1;
   int L, M, half, kmax, tc, enc, write_tail;
+  float gain;
 };
 
 struct Tile {
@@ -225,12 +279,13 @@ __global__ void __launch_bounds__(TILE) resample_kernel(const Job* __restrict__ 
   if (J.write_tail && T.n0 == 0)
     for (int j = tid; j < J.tc; j += TILE) J.tail_next[j] = xin(J, J.L1 - J.tc + j);
   if (cnt <= 0) return;
-  float* tab = smem;
-  float* xs = smem + J.L * J.kmax;
+  const bool staged = stages_table(J.L, J.M, J.half, J.kmax);
+  float* xs = smem + (staged ? J.L * J.kmax : 0);
   const long long top0 = (n0 * J.M + J.half) / J.L;
   const long long lo = top0 - (J.kmax - 1);
   const int span = (int)(((n0 + cnt - 1) * J.M + J.half) / J.L - lo + 1);
-  for (int i = tid; i < J.L * J.kmax; i += TILE) tab[i] = J.tab[i];
+  if (staged)
+    for (int i = tid; i < J.L * J.kmax; i += TILE) smem[i] = J.tab[i];
   for (int i = tid; i < span; i += TILE) xs[i] = xin(J, lo + i);
   __syncthreads();
   if (tid >= cnt) return;
@@ -238,10 +293,17 @@ __global__ void __launch_bounds__(TILE) resample_kernel(const Job* __restrict__ 
   const long long t = n * J.M + J.half;
   const int p = (int)(t % J.L);
   const int K = (2 * J.half - p) / J.L + 1;
-  const float* g = tab + p * J.kmax;
   const float* x = xs + (t / J.L - lo);
   float acc = 0.f;
-  for (int k = 0; k < K; ++k) acc = fmaf(g[k], x[-k], acc);
+  if (staged) {
+    const float* g = smem + p * J.kmax;
+    for (int k = 0; k < K; ++k) acc = fmaf(g[k], x[-k], acc);
+  } else {
+    const float* __restrict__ g = J.tab + (size_t)p * J.kmax;
+#pragma unroll 4
+    for (int k = 0; k < K; ++k) acc = fmaf(__ldg(g + k), x[-k], acc);
+  }
+  acc *= J.gain;
   const long long o = n - J.E0;
   switch (J.enc) {
     case FQ3_ENC_F32: reinterpret_cast<float*>(J.out)[o] = acc; break;
@@ -254,37 +316,51 @@ __global__ void __launch_bounds__(TILE) resample_kernel(const Job* __restrict__ 
 }  // namespace
 
 struct fq3_resample {
-  int dev = 0, rate = 0, enc = 0, cur = 0;
+  int dev = 0, rate = 0, rho = FQ3_RESAMPLE_PITCH_ONE, enc = 0, cur = 0;
   Ratio r{1, 1, 0};
+  float gain = 1.f;
   int64_t total_in = 0, emitted = 0;
   bool flushed = false;
   float* state = nullptr;   // two TCAP tail buffers
   const float* tab = nullptr;
 };
 
-extern "C" int fq3_resample_create(int32_t device, int32_t out_rate, int32_t encoding, fq3_resample** out) {
+extern "C" int fq3_resample_create_pitch(int32_t device, int32_t out_rate, int32_t pitch_rho, int32_t encoding,
+                                         fq3_resample** out) {
   if (!out) return rfail(FQ3_ERR_INVALID, "null argument");
   if (!valid_rate(out_rate))
     return rfail(FQ3_ERR_INVALID, "output rate must be one of 8000, 16000, 22050, 24000, 32000, 44100, 48000");
+  if (!valid_pitch(pitch_rho)) return rfail(FQ3_ERR_INVALID, "pitch rho must be in [128, 512]");
   if (encoding < FQ3_ENC_F32 || encoding > FQ3_ENC_ALAW) return rfail(FQ3_ERR_INVALID, "unknown encoding");
-  if (out_rate == FQ3_RESAMPLE_IN_RATE && encoding == FQ3_ENC_F32)
-    return rfail(FQ3_ERR_INVALID, "24000 Hz f32 is the identity: no resampler state exists for it");
   DevGuard g(device);
-  const float* tab = nullptr;
-  float* t = nullptr;
-  if (int rc = table_for(device, out_rate, &t)) return rc;
-  tab = t;
+  float* tab = nullptr;
+  if (int rc = table_for(device, out_rate, pitch_rho, &tab)) return rc;
   fq3_resample* s = new fq3_resample();
   s->dev = device;
   s->rate = out_rate;
+  s->rho = pitch_rho;
   s->enc = encoding;
-  s->r = ratio_of(out_rate);
+  s->r = ratio_of(out_rate, pitch_rho);
   s->tab = tab;
   if (cudaMalloc(&s->state, 2 * TCAP * sizeof(float)) != cudaSuccess) {
+    table_release(device, out_rate, pitch_rho);
     delete s;
     return rfail(FQ3_ERR_CUDA, "cudaMalloc of the resampler state failed");
   }
   *out = s;
+  return 0;
+}
+
+extern "C" int fq3_resample_create(int32_t device, int32_t out_rate, int32_t encoding, fq3_resample** out) {
+  if (out_rate == FQ3_RESAMPLE_IN_RATE && encoding == FQ3_ENC_F32)
+    return rfail(FQ3_ERR_INVALID, "24000 Hz f32 is the identity: no resampler state exists for it");
+  return fq3_resample_create_pitch(device, out_rate, FQ3_RESAMPLE_PITCH_ONE, encoding, out);
+}
+
+extern "C" int fq3_resample_set_gain(fq3_resample* s, float gain) {
+  if (!s) return rfail(FQ3_ERR_INVALID, "null argument");
+  if (!(gain >= 0.f && gain <= 1e6f)) return rfail(FQ3_ERR_INVALID, "gain must be a finite non-negative number");
+  s->gain = gain;
   return 0;
 }
 
@@ -301,21 +377,39 @@ extern "C" void fq3_resample_destroy(fq3_resample* s) {
   if (!s) return;
   DevGuard g(s->dev);
   cudaFree(s->state);
+  table_release(s->dev, s->rate, s->rho);
   delete s;
 }
 
-extern "C" int64_t fq3_resample_released(int32_t out_rate, int64_t total_in, int64_t n, int32_t flush) {
-  if (!valid_rate(out_rate) || total_in < 0 || n < 0) return -1;
-  const Ratio r = ratio_of(out_rate);
+extern "C" int64_t fq3_resample_released_pitch(int32_t out_rate, int32_t pitch_rho, int64_t total_in, int64_t n,
+                                               int32_t flush) {
+  if (!valid_rate(out_rate) || !valid_pitch(pitch_rho) || total_in < 0 || n < 0) return -1;
+  const Ratio r = ratio_of(out_rate, pitch_rho);
   return emitted(r, total_in + n, flush != 0) - emitted(r, total_in, false);
 }
 
-extern "C" int32_t fq3_resample_taps(int32_t out_rate, double* out, int32_t cap) {
-  if (!valid_rate(out_rate)) return -1;
-  const std::vector<double> h = design(out_rate);
+extern "C" int64_t fq3_resample_released(int32_t out_rate, int64_t total_in, int64_t n, int32_t flush) {
+  return fq3_resample_released_pitch(out_rate, FQ3_RESAMPLE_PITCH_ONE, total_in, n, flush);
+}
+
+extern "C" int32_t fq3_resample_taps_pitch(int32_t out_rate, int32_t pitch_rho, double* out, int32_t cap) {
+  if (!valid_rate(out_rate) || !valid_pitch(pitch_rho)) return -1;
+  const std::vector<double> h = design(out_rate, pitch_rho);
   if (out)
     for (int i = 0; i < (int)h.size() && i < cap; ++i) out[i] = h[i];
   return (int32_t)h.size();
+}
+
+extern "C" int32_t fq3_resample_taps(int32_t out_rate, double* out, int32_t cap) {
+  return fq3_resample_taps_pitch(out_rate, FQ3_RESAMPLE_PITCH_ONE, out, cap);
+}
+
+extern "C" int64_t fq3_resample_table_bytes(int32_t device) {
+  std::lock_guard<std::mutex> lk(g_tab_mu);
+  int64_t total = 0;
+  for (const auto& kv : g_tabs)
+    if (std::get<0>(kv.first) == device) total += kv.second.bytes;
+  return total;
 }
 
 extern "C" int fq3_resample_process(fq3_resample* const* rs, int32_t n_streams, const float* in_dev,
@@ -346,6 +440,7 @@ extern "C" int fq3_resample_process(fq3_resample* const* rs, int32_t n_streams, 
     J.kmax = r.kmax();
     J.tc = r.tail();
     J.enc = s->enc;
+    J.gain = s->gain;
     J.tab = s->tab;
     J.tail = s->state + (size_t)s->cur * TCAP;
     J.tail_next = s->state + (size_t)(s->cur ^ 1) * TCAP;
@@ -364,14 +459,14 @@ extern "C" int fq3_resample_process(fq3_resample* const* rs, int32_t n_streams, 
     for (int64_t n0 = 0; n0 < n_out; n0 += TILE) tiles.push_back(Tile{b, (int)n0});
     if (n_out == 0 && J.write_tail) tiles.push_back(Tile{b, 0});
     if (n_out > 0) {
-      const size_t span = (size_t)(((TILE - 1) * (int64_t)r.M + 2 * r.half) / r.L + 2);
-      smem = std::max(smem, ((size_t)r.L * J.kmax + span) * sizeof(float));
+      const size_t tab = stages_table(r.L, r.M, r.half, J.kmax) ? (size_t)r.L * J.kmax : 0;
+      smem = std::max(smem, (tab + (size_t)span_floats(r.L, r.M, r.half)) * sizeof(float));
     }
   }
   if (in_off > 0 && !in_dev) return rfail(FQ3_ERR_INVALID, "null input buffer");
   if (out_off > 0 && !out_dev) return rfail(FQ3_ERR_INVALID, "null output buffer");
   if (out_off > out_cap) return rfail(FQ3_ERR_INVALID, "output buffer smaller than the released samples");
-  if (smem > SMEM_MAX) return rfail(FQ3_ERR_INVALID, "internal: resampler tile exceeds shared memory");
+  if (smem > (size_t)SMEM_MAX) return rfail(FQ3_ERR_INVALID, "internal: resampler tile exceeds shared memory");
   if (!tiles.empty()) {
     DevGuard g(dev);
     cudaStream_t stream = (cudaStream_t)stream_;

@@ -84,7 +84,8 @@ EXPORTS = [
     "fq3_tempo_create", "fq3_tempo_reset", "fq3_tempo_destroy", "fq3_tempo_released", "fq3_tempo_process",
     "fq3_tempo_last_error",
     "fq3_resample_create", "fq3_resample_reset", "fq3_resample_destroy", "fq3_resample_released", "fq3_resample_taps",
-    "fq3_resample_process", "fq3_resample_last_error",
+    "fq3_resample_process", "fq3_resample_last_error", "fq3_resample_create_pitch", "fq3_resample_set_gain",
+    "fq3_resample_released_pitch", "fq3_resample_taps_pitch", "fq3_resample_table_bytes",
     "fq3_flac_create", "fq3_flac_reset", "fq3_flac_destroy", "fq3_flac_max_bytes", "fq3_flac_process",
     "fq3_flac_last_error",
 ]
@@ -210,6 +211,14 @@ def load_library() -> C.CDLL:
     lib.fq3_resample_process.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.POINTER(C.c_int64),
                                          C.POINTER(C.c_int32), C.c_void_p, C.c_int64, C.c_void_p]
     lib.fq3_resample_last_error.restype = C.c_char_p
+    lib.fq3_resample_create_pitch.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_void_p)]
+    lib.fq3_resample_set_gain.argtypes = [C.c_void_p, C.c_float]
+    lib.fq3_resample_released_pitch.argtypes = [C.c_int32, C.c_int32, C.c_int64, C.c_int64, C.c_int32]
+    lib.fq3_resample_released_pitch.restype = C.c_int64
+    lib.fq3_resample_taps_pitch.argtypes = [C.c_int32, C.c_int32, C.POINTER(C.c_double), C.c_int32]
+    lib.fq3_resample_taps_pitch.restype = C.c_int32
+    lib.fq3_resample_table_bytes.argtypes = [C.c_int32]
+    lib.fq3_resample_table_bytes.restype = C.c_int64
     lib.fq3_flac_create.argtypes = [C.c_int32, C.c_int32, C.POINTER(C.c_void_p)]
     lib.fq3_flac_reset.argtypes = [C.c_void_p]
     lib.fq3_flac_destroy.argtypes = [C.c_void_p]

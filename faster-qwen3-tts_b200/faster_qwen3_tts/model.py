@@ -36,10 +36,11 @@ def take_uniforms(seed: int, max_new_tokens: int, device="cuda") -> torch.Tensor
     return torch.rand(int(max_new_tokens) + 1, 16, generator=g).to(device)
 
 
-def _check_speed(speed):
-    """a speaking rate outside [0.25, 4.0] is refused (ValueError) before anything is tokenized"""
-    from .tempo import quantize
-    quantize(speed)
+def _check_speed(speed, pitch=0.0, gain_db=0.0):
+    """a speaking rate outside [0.25, 4.0], a pitch outside [-12, 12] semitones, a gain outside [-96, 16] dB or a speed
+    and pitch whose tempo falls outside [0.25, 4.0] are refused (ValueError) before anything is tokenized"""
+    from .resample import check_prosody
+    check_prosody(speed, pitch, gain_db)
 
 
 def _check_rate(sample_rate):
@@ -48,12 +49,16 @@ def _check_rate(sample_rate):
     check_rate(sample_rate)
 
 
-def _post_kw(speed, sample_rate=None):
-    """``speed=`` / ``sample_rate=`` for the delivery calls, only where they are not the identity (speed 1, 24 kHz): at
-    the defaults every call is made exactly as without them"""
+def _post_kw(speed, sample_rate=None, pitch=0.0, gain_db=0.0):
+    """``speed=`` / ``sample_rate=`` / ``pitch=`` / ``gain_db=`` for the delivery calls, only where they are not the
+    identity (speed 1, 24 kHz, pitch 0, 0 dB): at the defaults every call is made exactly as without them"""
     kw = {} if speed == 1.0 else {"speed": speed}
     if sample_rate is not None and int(sample_rate) != 24000:
         kw["sample_rate"] = sample_rate
+    if pitch != 0:
+        kw["pitch"] = pitch
+    if gain_db != 0:
+        kw["gain_db"] = gain_db
     return kw
 
 
@@ -598,18 +603,18 @@ class FasterQwen3TTS:
             return (a.flatten().float() if a.is_floating_point() else a.flatten()).cpu().numpy()
         return a.flatten() if hasattr(a, "flatten") else a
 
-    def _decode_all(self, speech_tokenizer, codec_ids, ref_codes, speed=1.0, sample_rate=None):
+    def _decode_all(self, speech_tokenizer, codec_ids, ref_codes, speed=1.0, sample_rate=None, pitch=0.0, gain_db=0.0):
         """Non-streaming decode + proportional reference trim (model.py:918-938)."""
-        return self._decode_takes(speech_tokenizer, [codec_ids], ref_codes, **_post_kw(speed, sample_rate))
+        return self._decode_takes(speech_tokenizer, [codec_ids], ref_codes, **_post_kw(speed, sample_rate, pitch, gain_db))
 
     def _stream_audio(self, chunks, speech_tokenizer, ref_codes, chunk_size, to_host=True, speed=1.0,
-                      sample_rate=None):
+                      sample_rate=None, pitch=0.0, gain_db=0.0):
         """The reference's hybrid streaming decode (model.py:1052-1135): Phase 1 re-decodes everything so far
         (reference codes prepended in ICL mode) until max(25, chunk_size) frames exist and calibrates
         samples_per_frame; Phase 2 decodes a 25-frame left-context window and trims the context.  At a speed other than
         1, or an output rate other than 24 kHz, the stream ends with one more item: the last samples of the tempo and
         the resampler (``chunk_steps`` 0)."""
-        win = self._make_window(speech_tokenizer, ref_codes, chunk_size, to_host, **_post_kw(speed, sample_rate))
+        win = self._make_window(speech_tokenizer, ref_codes, chunk_size, to_host, **_post_kw(speed, sample_rate, pitch, gain_db))
         timing = {}
         for codec_chunk, timing in chunks:
             new_audio, sr = win.push(codec_chunk)
@@ -618,22 +623,23 @@ class FasterQwen3TTS:
             yield tail, sr, dict(timing, chunk_steps=0, is_final=True)
 
     def _make_window(self, speech_tokenizer, ref_codes, chunk_size, to_host=True, speed=1.0, sample_rate=None,
-                     encoding="f32"):
-        """the codec window of one request; at a speed other than 1 it carries the request's ``tempo.Tempo``, at an
-        output rate or encoding other than 24 kHz f32 its ``resample.Resampler``; ``encoding="flac"`` is an s16
-        resampler followed by a ``flac.Encoder``"""
-        from .resample import resampler_for
+                     encoding="f32", pitch=0.0, gain_db=0.0):
+        """the codec window of one request; at a speed or pitch other than 1 / 0 it carries the request's
+        ``tempo.Tempo`` (at ``resample.tempo_speed``), at an output rate or encoding other than 24 kHz f32, a pitch or a
+        gain its ``resample.Resampler``; ``encoding="flac"`` is an s16 resampler followed by a ``flac.Encoder``"""
+        from .resample import resampler_for, tempo_speed
         from .tempo import tempo_for
         if self.streaming_codec not in ("window", "stateful"):
             raise ValueError("streaming_codec must be 'window' or 'stateful'")
-        tempo = tempo_for(speed, _pcm_device(speech_tokenizer)) if speed != 1.0 else None
+        tempo = (tempo_for(tempo_speed(speed, pitch), _pcm_device(speech_tokenizer))
+                 if speed != 1.0 or pitch != 0 else None)
         rs = enc = None
         if encoding == "flac":
             from .flac import Encoder
-            rs = resampler_for(sample_rate, "s16", _pcm_device(speech_tokenizer))
+            rs = resampler_for(sample_rate, "s16", _pcm_device(speech_tokenizer), pitch, gain_db)
             enc = Encoder(rs.rate, _pcm_device(speech_tokenizer))
-        elif sample_rate is not None or encoding != "f32":
-            rs = resampler_for(sample_rate, encoding, _pcm_device(speech_tokenizer))
+        elif sample_rate is not None or encoding != "f32" or pitch != 0 or gain_db != 0:
+            rs = resampler_for(sample_rate, encoding, _pcm_device(speech_tokenizer), pitch, gain_db)
         kw = dict(tempo=tempo, resampler=rs, flac=enc)
         if self.streaming_codec == "stateful" and getattr(speech_tokenizer, "supports_streams", False):
             return _StatefulWindow(self, speech_tokenizer, ref_codes, chunk_size, to_host, **kw)
@@ -650,12 +656,12 @@ class FasterQwen3TTS:
                            max_new_tokens: int = 2048, min_new_tokens: int = 2, temperature: float = 0.9,
                            top_k: int = 50, top_p: float = 1.0, do_sample: bool = True,
                            repetition_penalty: float = 1.05, uniforms=None, speed: float = 1.0,
-                           sample_rate: Optional[int] = None):
+                           sample_rate: Optional[int] = None, pitch: float = 0.0, gain_db: float = 0.0):
         """generate_voice_clone_streaming from the point where the prompt embeddings exist (model.py:1079-1137).
         ``speed``: speaking rate in [0.25, 4.0]; ``sample_rate``: output rate (None: 24000), one of
         ``resample.RATES`` (see ``_stream_audio``)."""
         from .streaming import fast_generate_streaming
-        _check_speed(speed)
+        _check_speed(speed, pitch, gain_db)
         _check_rate(sample_rate)
         m = self.model.model
         m.talker.rope_deltas = None
@@ -670,14 +676,14 @@ class FasterQwen3TTS:
                 yield (codes.cpu().numpy() if to_host else codes), self.sample_rate, timing
             return
         yield from self._stream_audio(chunks, st, ref_codes, chunk_size, to_host=to_host,
-                                      **_post_kw(speed, sample_rate))
+                                      **_post_kw(speed, sample_rate, pitch, gain_db))
 
     @torch.inference_mode()
     def stream_batch_from_embeds(self, tie, tam, tth, tpe, ref_codes=None, chunk_size: int = 8, to_host: bool = True,
                                  max_new_tokens: int = 2048, min_new_tokens: int = 2, temperature: float = 0.9,
                                  top_k: int = 50, top_p: float = 1.0, do_sample: bool = True,
                                  repetition_penalty: float = 1.05, uniforms=None, decode_audio: bool = True,
-                                 speed: float = 1.0, sample_rate: Optional[int] = None):
+                                 speed: float = 1.0, sample_rate: Optional[int] = None, pitch: float = 0.0, gain_db: float = 0.0):
         """Batched streaming from the point where the (left-padded) prompt batch exists (the tuple
         ``_build_talker_inputs_local`` returns for a list of requests, model.py:774-805): all rows advance together, one
         persistent-kernel launch per chunk; yields [(row, pcm_or_codes, sr, timing)] per chunk.  ``ref_codes``: None or
@@ -685,7 +691,7 @@ class FasterQwen3TTS:
         4.0]; ``sample_rate``: output rate of every row (None: 24000); other than the identity, a last item holds every
         row's final samples (``chunk_steps`` 0)."""
         from .batching import fast_generate_streaming_batch
-        _check_speed(speed)
+        _check_speed(speed, pitch, gain_db)
         _check_rate(sample_rate)
         m = self.model.model
         m.talker.rope_deltas = None
@@ -694,7 +700,7 @@ class FasterQwen3TTS:
         wins = None
         if st is not None:
             wins = [self._make_window(st, None if ref_codes is None else ref_codes[b], chunk_size, to_host,
-                                      **_post_kw(speed, sample_rate)) for b in range(B)]
+                                      **_post_kw(speed, sample_rate, pitch, gain_db)) for b in range(B)]
         kw = self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p, do_sample, repetition_penalty)
         for items in fast_generate_streaming_batch(
                 talker=m.talker, talker_input_embeds=tie, attention_mask=tam, trailing_text_hiddens=tth,
@@ -716,19 +722,19 @@ class FasterQwen3TTS:
                                     min_new_tokens: int = 2, temperature: float = 0.9, top_k: int = 50,
                                     top_p: float = 1.0, do_sample: bool = True, repetition_penalty: float = 1.05,
                                     non_streaming_mode: Optional[bool] = None, chunk_size: int = 8,
-                                    speed: float = 1.0, sample_rate: Optional[int] = None):
+                                    speed: float = 1.0, sample_rate: Optional[int] = None, pitch: float = 0.0, gain_db: float = 0.0):
         """Concurrent custom-voice requests (BASELINE config 4) sharing every pass over the weights: the prompts are
         batched and left-padded exactly like the reference's builder does for a list of requests (model.py:583-805),
         then decoded together.  ``speed`` (one for all requests): speaking rate in [0.25, 4.0], and ``sample_rate``: output
         rate (None: 24000), both applied on the device.  Returns ([audio per request], sample_rate)."""
-        _check_speed(speed)
+        _check_speed(speed, pitch, gain_db)
         _check_rate(sample_rate)
         instructs, nsm = self._custom_voice_rules(texts, languages, speakers, instructs or [None] * len(texts),
                                                   non_streaming_mode)
         _, _, _, tie, tam, tth, tpe = self._prepare_generation_custom_batch(texts, languages, speakers, instructs, nsm)
         parts = [[] for _ in texts]
         sr = _rate_of(self.sample_rate, sample_rate)
-        for items in self.stream_batch_from_embeds(tie, tam, tth, tpe, chunk_size=chunk_size, **_post_kw(speed, sample_rate), **self._gen_kwargs(
+        for items in self.stream_batch_from_embeds(tie, tam, tth, tpe, chunk_size=chunk_size, **_post_kw(speed, sample_rate, pitch, gain_db), **self._gen_kwargs(
                 max_new_tokens, min_new_tokens, temperature, top_k, top_p, do_sample, repetition_penalty)):
             for b, audio, sr, _ in items:
                 parts[b].append(audio)
@@ -743,8 +749,8 @@ class FasterQwen3TTS:
                              non_streaming_mode: Optional[bool] = None, append_silence: bool = True,
                              instruct: Optional[str] = None, ref_spk=None, ref_rvq=None, ref_spk_emb=None,
                              ref_codes=None, voice_clone_prompt=None, speed: float = 1.0,
-                             sample_rate: Optional[int] = None) -> Tuple[list, int]:
-        _check_speed(speed)
+                             sample_rate: Optional[int] = None, pitch: float = 0.0, gain_db: float = 0.0) -> Tuple[list, int]:
+        _check_speed(speed, pitch, gain_db)
         _check_rate(sample_rate)
         voice_clone_prompt, nsm = self._voice_clone_rules(voice_clone_prompt, non_streaming_mode, ref_spk, ref_rvq,
                                                           ref_spk_emb, ref_codes)
@@ -753,7 +759,7 @@ class FasterQwen3TTS:
             non_streaming_mode=nsm, append_silence=append_silence, voice_clone_prompt=voice_clone_prompt,
             instruct=instruct)
         return self._one_shot(prep, ref_codes, self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k,
-                                                                top_p, do_sample, repetition_penalty), speed, sample_rate)
+                                                                top_p, do_sample, repetition_penalty), speed, sample_rate, pitch, gain_db)
 
     @torch.inference_mode()
     def generate_voice_clone_streaming(self, text: str, language: str, ref_audio=None, ref_text: str = "",
@@ -764,9 +770,9 @@ class FasterQwen3TTS:
                                        append_silence: bool = True, parity_mode: bool = False,
                                        instruct: Optional[str] = None, ref_spk=None, ref_rvq=None, ref_spk_emb=None,
                                        ref_codes=None, voice_clone_prompt=None, speed: float = 1.0,
-                                       sample_rate: Optional[int] = None
+                                       sample_rate: Optional[int] = None, pitch: float = 0.0, gain_db: float = 0.0
                                        ) -> Generator[Tuple[np.ndarray, int, dict], None, None]:
-        _check_speed(speed)
+        _check_speed(speed, pitch, gain_db)
         _check_rate(sample_rate)
         voice_clone_prompt, nsm = self._voice_clone_rules(voice_clone_prompt, non_streaming_mode, ref_spk, ref_rvq,
                                                           ref_spk_emb, ref_codes)
@@ -780,10 +786,10 @@ class FasterQwen3TTS:
             chunks = parity_generate_streaming(
                 talker=talker, talker_input_embeds=tie, attention_mask=tam, trailing_text_hiddens=tth, tts_pad_embed=tpe,
                 config=config, chunk_size=chunk_size, **gen)
-            yield from self._stream_audio(chunks, m.speech_tokenizer, ref_codes, chunk_size, **_post_kw(speed, sample_rate))
+            yield from self._stream_audio(chunks, m.speech_tokenizer, ref_codes, chunk_size, **_post_kw(speed, sample_rate, pitch, gain_db))
             return
         yield from self.stream_from_embeds(tie, tam, tth, tpe, ref_codes=ref_codes, chunk_size=chunk_size,
-                                           **_post_kw(speed, sample_rate), **gen)
+                                           **_post_kw(speed, sample_rate, pitch, gain_db), **gen)
 
     def _voice_clone_rules(self, voice_clone_prompt, non_streaming_mode, ref_spk=None, ref_rvq=None, ref_spk_emb=None,
                            ref_codes=None):
@@ -842,7 +848,7 @@ class FasterQwen3TTS:
         self._validate(language)
         return self._resolve_non_streaming_mode(non_streaming_mode, default=True)
 
-    def _one_shot(self, prep, ref_codes, gen, speed=1.0, sample_rate=None):
+    def _one_shot(self, prep, ref_codes, gen, speed=1.0, sample_rate=None, pitch=0.0, gain_db=0.0):
         """The delivery of the three one-shot methods: generate, then decode every frame at once (model.py:893-947),
         time-stretched on the device at a speed other than 1, resampled at an output rate other than 24 kHz."""
         from .generate import fast_generate
@@ -853,7 +859,7 @@ class FasterQwen3TTS:
         if codec_ids is None:
             logger.warning("Generation returned no tokens")
             return [np.zeros(1, dtype=np.float32)], _rate_of(self.sample_rate, sample_rate)
-        audio, sr = self._decode_all(m.speech_tokenizer, codec_ids, ref_codes, **_post_kw(speed, sample_rate))
+        audio, sr = self._decode_all(m.speech_tokenizer, codec_ids, ref_codes, **_post_kw(speed, sample_rate, pitch, gain_db))
         self._log_rtf(timing)
         return audio, sr
 
@@ -862,14 +868,14 @@ class FasterQwen3TTS:
                               non_streaming_mode: Optional[bool] = None, max_new_tokens: int = 2048,
                               min_new_tokens: int = 2, temperature: float = 0.9, top_k: int = 50, top_p: float = 1.0,
                               do_sample: bool = True, repetition_penalty: float = 1.05, speed: float = 1.0,
-                              sample_rate: Optional[int] = None
+                              sample_rate: Optional[int] = None, pitch: float = 0.0, gain_db: float = 0.0
                               ) -> Tuple[list, int]:
-        _check_speed(speed)
+        _check_speed(speed, pitch, gain_db)
         _check_rate(sample_rate)
         (instruct,), nsm = self._custom_voice_rules([text], [language], [speaker], [instruct], non_streaming_mode)
         prep = self._prepare_generation_custom(text, language, speaker, instruct, nsm)
         return self._one_shot(prep, None, self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p,
-                                                           do_sample, repetition_penalty), speed, sample_rate)
+                                                           do_sample, repetition_penalty), speed, sample_rate, pitch, gain_db)
 
     @torch.inference_mode()
     def generate_custom_voice_streaming(self, text: str, speaker: str, language: str, instruct: Optional[str] = None,
@@ -877,13 +883,13 @@ class FasterQwen3TTS:
                                         min_new_tokens: int = 2, temperature: float = 0.9, top_k: int = 50,
                                         top_p: float = 1.0, do_sample: bool = True, repetition_penalty: float = 1.05,
                                         chunk_size: int = 12, speed: float = 1.0,
-                                        sample_rate: Optional[int] = None
+                                        sample_rate: Optional[int] = None, pitch: float = 0.0, gain_db: float = 0.0
                                         ) -> Generator[Tuple[np.ndarray, int, dict], None, None]:
-        _check_speed(speed)
+        _check_speed(speed, pitch, gain_db)
         _check_rate(sample_rate)
         (instruct,), nsm = self._custom_voice_rules([text], [language], [speaker], [instruct], non_streaming_mode)
         _, _, _, tie, tam, tth, tpe = self._prepare_generation_custom(text, language, speaker, instruct, nsm)
-        yield from self.stream_from_embeds(tie, tam, tth, tpe, chunk_size=chunk_size, **_post_kw(speed, sample_rate), **self._gen_kwargs(
+        yield from self.stream_from_embeds(tie, tam, tth, tpe, chunk_size=chunk_size, **_post_kw(speed, sample_rate, pitch, gain_db), **self._gen_kwargs(
             max_new_tokens, min_new_tokens, temperature, top_k, top_p, do_sample, repetition_penalty))
 
     @torch.inference_mode()
@@ -891,14 +897,14 @@ class FasterQwen3TTS:
                               non_streaming_mode: Optional[bool] = None, max_new_tokens: int = 2048,
                               min_new_tokens: int = 2, temperature: float = 0.9, top_k: int = 50, top_p: float = 1.0,
                               do_sample: bool = True, repetition_penalty: float = 1.05, speed: float = 1.0,
-                              sample_rate: Optional[int] = None
+                              sample_rate: Optional[int] = None, pitch: float = 0.0, gain_db: float = 0.0
                               ) -> Tuple[list, int]:
-        _check_speed(speed)
+        _check_speed(speed, pitch, gain_db)
         _check_rate(sample_rate)
         nsm = self._voice_design_rules(language, non_streaming_mode)
         prep = self._prepare_generation_custom(text, language, None, instruct, nsm)
         return self._one_shot(prep, None, self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p,
-                                                           do_sample, repetition_penalty), speed, sample_rate)
+                                                           do_sample, repetition_penalty), speed, sample_rate, pitch, gain_db)
 
     @torch.inference_mode()
     def generate_voice_design_streaming(self, text: str, instruct: str, language: str,
@@ -906,13 +912,13 @@ class FasterQwen3TTS:
                                         min_new_tokens: int = 2, temperature: float = 0.9, top_k: int = 50,
                                         top_p: float = 1.0, do_sample: bool = True, repetition_penalty: float = 1.05,
                                         chunk_size: int = 12, speed: float = 1.0,
-                                        sample_rate: Optional[int] = None
+                                        sample_rate: Optional[int] = None, pitch: float = 0.0, gain_db: float = 0.0
                                         ) -> Generator[Tuple[np.ndarray, int, dict], None, None]:
-        _check_speed(speed)
+        _check_speed(speed, pitch, gain_db)
         _check_rate(sample_rate)
         nsm = self._voice_design_rules(language, non_streaming_mode)
         _, _, _, tie, tam, tth, tpe = self._prepare_generation_custom(text, language, None, instruct, nsm)
-        yield from self.stream_from_embeds(tie, tam, tth, tpe, chunk_size=chunk_size, **_post_kw(speed, sample_rate), **self._gen_kwargs(
+        yield from self.stream_from_embeds(tie, tam, tth, tpe, chunk_size=chunk_size, **_post_kw(speed, sample_rate, pitch, gain_db), **self._gen_kwargs(
             max_new_tokens, min_new_tokens, temperature, top_k, top_p, do_sample, repetition_penalty))
 
     # ------------------------------------------------------------------ several takes of one request
@@ -930,7 +936,7 @@ class FasterQwen3TTS:
             raise ValueError(f"{len(seeds)} seeds for {n_takes} takes")
         return seeds
 
-    def _takes(self, prep, ref_codes, seeds, gen, chunk_size=64, speed=1.0, sample_rate=None):
+    def _takes(self, prep, ref_codes, seeds, gen, chunk_size=64, speed=1.0, sample_rate=None, pitch=0.0, gain_db=0.0):
         """The one implementation behind the three ``*_takes`` methods: the prompt ``prep`` latched into one slot per take
         with ONE batched prefill (``BatchScheduler.submit_many``), all takes decoded together (one launch per chunk),
         their PCM decoded with one codec call per length.  Take i draws its uniforms from ``take_uniforms(seeds[i])``."""
@@ -955,10 +961,10 @@ class FasterQwen3TTS:
             sc = score(rq.lp.frames(), rq.eos_logprob)
             sc["seed"] = seeds[i]
             scores.append(sc)
-        audio, _ = self._decode_takes(m.speech_tokenizer, codes, ref_codes, **_post_kw(speed, sample_rate))
+        audio, _ = self._decode_takes(m.speech_tokenizer, codes, ref_codes, **_post_kw(speed, sample_rate, pitch, gain_db))
         return audio, _rate_of(self.sample_rate, sample_rate), scores
 
-    def _decode_takes(self, st, codes, ref_codes, speed=1.0, sample_rate=None):
+    def _decode_takes(self, st, codes, ref_codes, speed=1.0, sample_rate=None, pitch=0.0, gain_db=0.0):
         """Non-streaming decode + proportional reference trim of every take, takes of equal length in ONE codec call (the
         decoder's rows are independent); at a speed other than 1 every take is time-stretched on the device, all in ONE
         launch, and at an output rate other than 24 kHz resampled, all in ONE more launch, each as one push with flush.
@@ -980,18 +986,18 @@ class FasterQwen3TTS:
                 a = a.flatten()
                 if ref_len > 0:
                     a = a[int(ref_len / max(batch.shape[1], 1) * len(a)):]
-                if speed == 1.0 and sample_rate is None:
+                if speed == 1.0 and sample_rate is None and pitch == 0 and gain_db == 0:
                     out[i] = self._to_numpy(a)
                 else:
                     pcms.append(a)
                     at.append(i)
         if at:
-            tempos = [tempo.tempo_for(speed, a.device) for a in pcms]   # None where speed quantises to 1
+            tempos = [tempo.tempo_for(resample.tempo_speed(speed, pitch), a.device) for a in pcms]   # None at q 1024
             if tempos[0] is not None:
                 pcms = tempo.process(tempos, pcms, True)
                 for t in tempos:
                     t.close()
-            rss = [resample.resampler_for(sample_rate, "f32", a.device) for a in pcms]
+            rss = [resample.resampler_for(sample_rate, "f32", a.device, pitch, gain_db) for a in pcms]
             if rss and rss[0] is not None:
                 pcms = resample.process(rss, pcms, True)
                 for r in rss:
@@ -1007,7 +1013,8 @@ class FasterQwen3TTS:
                                    repetition_penalty: float = 1.05, xvec_only: bool = False,
                                    non_streaming_mode: Optional[bool] = None, append_silence: bool = True,
                                    instruct: Optional[str] = None, voice_clone_prompt=None, speed: float = 1.0,
-                                   sample_rate: Optional[int] = None, n_takes: int = 4, seeds: Optional[List[int]] = None):
+                                   sample_rate: Optional[int] = None, pitch: float = 0.0,
+                                   gain_db: float = 0.0, n_takes: int = 4, seeds: Optional[List[int]] = None):
         """``n_takes`` renderings of one ``generate_voice_clone`` request for the price of one batched decode: one prompt,
         one batched prefill, one launch per chunk for all takes.  Take i is the request run alone with the uniforms of
         ``take_uniforms(seeds[i], max_new_tokens)`` -- bit for bit while both run the per-head talker attention (a lone
@@ -1015,7 +1022,7 @@ class FasterQwen3TTS:
         holds "logprobs" (float32 [T,16], the log-probability of every code), "eos_logprob", "total_logprob" (their sum,
         EOS term included), "frames" and "seed".  A log-probability says how likely the sampler found its draws, not
         how good the audio is: the calls rank nothing and pick nothing."""
-        _check_speed(speed)
+        _check_speed(speed, pitch, gain_db)
         _check_rate(sample_rate)
         voice_clone_prompt, nsm = self._voice_clone_rules(voice_clone_prompt, non_streaming_mode)
         seeds = self._check_takes(n_takes, seeds)
@@ -1025,45 +1032,47 @@ class FasterQwen3TTS:
             instruct=instruct)
         return self._takes(prep, ref_codes, seeds, self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k,
                                                                     top_p, do_sample, repetition_penalty), speed=speed,
-                           sample_rate=sample_rate)
+                           sample_rate=sample_rate, pitch=pitch, gain_db=gain_db)
 
     @torch.inference_mode()
     def generate_custom_voice_takes(self, text: str, speaker: str, language: str, instruct: Optional[str] = None,
                                     non_streaming_mode: Optional[bool] = None, max_new_tokens: int = 2048,
                                     min_new_tokens: int = 2, temperature: float = 0.9, top_k: int = 50,
                                     top_p: float = 1.0, do_sample: bool = True, repetition_penalty: float = 1.05,
-                                    speed: float = 1.0, sample_rate: Optional[int] = None, n_takes: int = 4,
+                                    speed: float = 1.0, sample_rate: Optional[int] = None, pitch: float = 0.0,
+                                    gain_db: float = 0.0, n_takes: int = 4,
                                     seeds: Optional[List[int]] = None):
         """``n_takes`` renderings of one ``generate_custom_voice`` request (see ``generate_voice_clone_takes``)."""
-        _check_speed(speed)
+        _check_speed(speed, pitch, gain_db)
         _check_rate(sample_rate)
         (instruct,), nsm = self._custom_voice_rules([text], [language], [speaker], [instruct], non_streaming_mode)
         seeds = self._check_takes(n_takes, seeds)
         prep = self._prepare_generation_custom(text, language, speaker, instruct, nsm)
         return self._takes(prep, None, seeds, self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k,
                                                                top_p, do_sample, repetition_penalty), speed=speed,
-                           sample_rate=sample_rate)
+                           sample_rate=sample_rate, pitch=pitch, gain_db=gain_db)
 
     @torch.inference_mode()
     def generate_voice_design_takes(self, text: str, instruct: str, language: str,
                                     non_streaming_mode: Optional[bool] = None, max_new_tokens: int = 2048,
                                     min_new_tokens: int = 2, temperature: float = 0.9, top_k: int = 50,
                                     top_p: float = 1.0, do_sample: bool = True, repetition_penalty: float = 1.05,
-                                    speed: float = 1.0, sample_rate: Optional[int] = None, n_takes: int = 4,
+                                    speed: float = 1.0, sample_rate: Optional[int] = None, pitch: float = 0.0,
+                                    gain_db: float = 0.0, n_takes: int = 4,
                                     seeds: Optional[List[int]] = None):
         """``n_takes`` renderings of one ``generate_voice_design`` request (see ``generate_voice_clone_takes``)."""
-        _check_speed(speed)
+        _check_speed(speed, pitch, gain_db)
         _check_rate(sample_rate)
         nsm = self._voice_design_rules(language, non_streaming_mode)
         seeds = self._check_takes(n_takes, seeds)
         prep = self._prepare_generation_custom(text, language, None, instruct, nsm)
         return self._takes(prep, None, seeds, self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k,
                                                                top_p, do_sample, repetition_penalty), speed=speed,
-                           sample_rate=sample_rate)
+                           sample_rate=sample_rate, pitch=pitch, gain_db=gain_db)
 
     # ------------------------------------------------------------------ incremental text input (text_stream.py)
     def _text_streaming(self, text_stream, language, speaker, instruct, voice_clone_prompt, non_streaming_mode,
-                        chunk_size, gen, speed=1.0, sample_rate=None):
+                        chunk_size, gen, speed=1.0, sample_rate=None, pitch=0.0, gain_db=0.0):
         """The one implementation behind the three ``*_text_streaming`` methods.  Text streaming has one text layout,
         so the raw ``non_streaming_mode`` is checked here, not the voice kind's default."""
         from .text_stream import _refuse_unsupported, generate_text_streaming
@@ -1073,7 +1082,7 @@ class FasterQwen3TTS:
             instruct_ids = self.model._tokenize_texts([self.model._build_instruct_text(instruct)])[0]
         yield from generate_text_streaming(self, text_stream, language=language, speaker=speaker,
                                            instruct_ids=instruct_ids, voice_clone_prompt=voice_clone_prompt,
-                                           chunk_size=chunk_size, **_post_kw(speed, sample_rate), **gen)
+                                           chunk_size=chunk_size, **_post_kw(speed, sample_rate, pitch, gain_db), **gen)
 
     @torch.inference_mode()
     def generate_custom_voice_text_streaming(self, text_stream, speaker: str, language: str,
@@ -1082,18 +1091,18 @@ class FasterQwen3TTS:
                                              temperature: float = 0.9, top_k: int = 50, top_p: float = 1.0,
                                              do_sample: bool = True, repetition_penalty: float = 1.05,
                                              chunk_size: int = 12, speed: float = 1.0,
-                                             sample_rate: Optional[int] = None
+                                             sample_rate: Optional[int] = None, pitch: float = 0.0, gain_db: float = 0.0
                                              ) -> Generator[Tuple[np.ndarray, int, dict], None, None]:
         """``generate_custom_voice_streaming`` with the text fed while it is spoken: ``text_stream`` is any iterable of
         ``str`` pieces (an LLM's reply token by token).  The audio equals that of the one-shot streaming request for the
         same text, whatever the split and however fast the pieces come; generation waits where the text has not arrived
         yet.  Timing dicts add ``text_wait_ms``, the time spent blocked on ``text_stream``."""
-        _check_speed(speed)
+        _check_speed(speed, pitch, gain_db)
         _check_rate(sample_rate)
         (instruct,), _ = self._custom_voice_rules([text_stream], [language], [speaker], [instruct], non_streaming_mode)
         yield from self._text_streaming(text_stream, language, speaker, instruct, None, non_streaming_mode, chunk_size,
                                         self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p,
-                                                         do_sample, repetition_penalty), speed, sample_rate)
+                                                         do_sample, repetition_penalty), speed, sample_rate, pitch, gain_db)
 
     @torch.inference_mode()
     def generate_voice_design_text_streaming(self, text_stream, instruct: str, language: str,
@@ -1101,16 +1110,16 @@ class FasterQwen3TTS:
                                              min_new_tokens: int = 2, temperature: float = 0.9, top_k: int = 50,
                                              top_p: float = 1.0, do_sample: bool = True,
                                              repetition_penalty: float = 1.05, chunk_size: int = 12, speed: float = 1.0,
-                                             sample_rate: Optional[int] = None
+                                             sample_rate: Optional[int] = None, pitch: float = 0.0, gain_db: float = 0.0
                                              ) -> Generator[Tuple[np.ndarray, int, dict], None, None]:
         """``generate_voice_design_streaming`` with the text fed while it is spoken (see
         ``generate_custom_voice_text_streaming``)."""
-        _check_speed(speed)
+        _check_speed(speed, pitch, gain_db)
         _check_rate(sample_rate)
         self._voice_design_rules(language, non_streaming_mode)
         yield from self._text_streaming(text_stream, language, None, instruct, None, non_streaming_mode, chunk_size,
                                         self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p,
-                                                         do_sample, repetition_penalty), speed, sample_rate)
+                                                         do_sample, repetition_penalty), speed, sample_rate, pitch, gain_db)
 
     @torch.inference_mode()
     def generate_voice_clone_text_streaming(self, text_stream, language: str, ref_audio=None, ref_text: str = "",
@@ -1121,12 +1130,12 @@ class FasterQwen3TTS:
                                             non_streaming_mode: Optional[bool] = None, append_silence: bool = True,
                                             ref_spk=None, ref_rvq=None, ref_spk_emb=None, ref_codes=None,
                                             voice_clone_prompt=None, speed: float = 1.0,
-                                            sample_rate: Optional[int] = None
+                                            sample_rate: Optional[int] = None, pitch: float = 0.0, gain_db: float = 0.0
                                             ) -> Generator[Tuple[np.ndarray, int, dict], None, None]:
         """``generate_voice_clone_streaming`` with the text fed while it is spoken, x-vector cloning only: ICL cloning
         puts the target text under the reference codec frames inside the prompt, so it must be known before prefill
         (ValueError)."""
-        _check_speed(speed)
+        _check_speed(speed, pitch, gain_db)
         _check_rate(sample_rate)
         voice_clone_prompt, _ = self._voice_clone_rules(voice_clone_prompt, non_streaming_mode, ref_spk, ref_rvq,
                                                         ref_spk_emb, ref_codes)
@@ -1140,7 +1149,7 @@ class FasterQwen3TTS:
             voice_clone_prompt=voice_clone_prompt)
         yield from self._text_streaming(text_stream, language, None, None, vcp, non_streaming_mode, chunk_size,
                                         self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p,
-                                                         do_sample, repetition_penalty), speed, sample_rate)
+                                                         do_sample, repetition_penalty), speed, sample_rate, pitch, gain_db)
 
     def _log_rtf(self, timing):
         n = timing["steps"]

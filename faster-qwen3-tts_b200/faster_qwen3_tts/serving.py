@@ -70,12 +70,15 @@ class Ticket:
     speed: float = 1.0                    # speaking rate: the listener consumes model audio `speed` times as fast
     sample_rate: int = 24000              # output rate and encoding of the audio (resample.py)
     encoding: str = "f32"
+    pitch: float = 0.0                    # semitones and dB, applied by the tempo and the resampler (resample.py)
+    gain_db: float = 0.0
 
     @property
     def flushes(self) -> bool:
         """whether the request's window holds device stages (a tempo, a resampler, a FLAC encoder) that flush with its
         last chunk"""
-        return self.speed != 1.0 or (self.sample_rate, self.encoding) != (24000, "f32")
+        return (self.speed != 1.0 or (self.sample_rate, self.encoding) != (24000, "f32") or self.pitch != 0
+                or self.gain_db != 0)
 
     def cancel(self) -> None:
         """End the request: the worker frees its slot (or drops it from the queue) and closes the ticket."""
@@ -153,7 +156,10 @@ class ContinuousBatcher:
     ``sample_rate=`` / ``encoding=`` when the ticket asks for other than 24 kHz f32 (``submit(..., sample_rate=,
     encoding=)``): the window resamples and encodes on the device, its resampler flushes with the last chunk, and the
     lead, which counts audio seconds, is the same at every rate.  ``encoding="flac"`` adds a FLAC encoder after an s16
-    resampler: the ticket's chunks are FLAC bytes, and its lead still counts audio seconds.
+    resampler: the ticket's chunks are FLAC bytes, and its lead still counts audio seconds.  ``pitch=`` / ``gain_db=``
+    (``submit(..., pitch=, gain_db=)``) reach the window likewise when not 0; the lead is still ``frames x frame_s /
+    speed`` (a pitched delivery lasts within 0.2 % of that).  A pitch's filter table is designed and uploaded by
+    ``submit`` on the caller's thread (``window_factory.warm``, when the factory has one), not by the worker.
     ``clock`` / ``sleep`` are the worker's time source, replaceable in tests."""
 
     def __init__(self, scheduler, window_factory: Callable, chunk_size: int = 8, idle_sleep: float = 0.002,
@@ -180,14 +186,15 @@ class ContinuousBatcher:
 
     # ---- client side ------------------------------------------------------------------------------------
     def submit(self, prepare: Callable[[], tuple], pace: Optional[float] = None, speed: float = 1.0,
-               sample_rate: Optional[int] = None, encoding: str = "f32", **gen_kwargs) -> Ticket:
+               sample_rate: Optional[int] = None, encoding: str = "f32", pitch: float = 0.0, gain_db: float = 0.0,
+               **gen_kwargs) -> Ticket:
         """``pace``: the client plays at ``pace`` x real time (class docstring); ``speed``: speaking rate in [0.25,
         4.0]; ``sample_rate`` (None: 24000) and ``encoding`` (``f32 | s16 | ulaw | alaw | flac``): the audio the ticket
-        carries.
+        carries; ``pitch``: semitones in [-12, 12]; ``gain_db``: in [-96, 16].
         ``gen_kwargs`` are the scheduler's ``submit`` keywords, among them ``chunk_size`` / ``first_chunk`` for this
         request alone."""
-        speed = self._speed(speed)
-        out = self._output(sample_rate, encoding)
+        speed = self._speed(speed, pitch, gain_db)
+        out = self._output(sample_rate, encoding, pitch, gain_db)
         with self._lock:
             self._rid += 1
             t = Ticket(self._rid, prepare, gen_kwargs, pace=self._pace(pace), submitted_at=self.clock(), speed=speed,
@@ -202,25 +209,29 @@ class ContinuousBatcher:
         return None if pace is None else float(pace)
 
     @staticmethod
-    def _speed(speed):
-        from .tempo import quantize
-        quantize(speed)
+    def _speed(speed, pitch=0.0, gain_db=0.0):
+        from .resample import check_prosody
+        check_prosody(speed, pitch, gain_db)
         return float(speed)
 
-    @staticmethod
-    def _output(sample_rate, encoding):
+    def _output(self, sample_rate, encoding, pitch=0.0, gain_db=0.0):
         from .flac import check_encoding
         from .resample import check_rate
-        return dict(sample_rate=check_rate(sample_rate), encoding=check_encoding(encoding))
+        out = dict(sample_rate=check_rate(sample_rate), encoding=check_encoding(encoding))
+        warm = getattr(self.window_factory, "warm", None)
+        if pitch != 0 and warm is not None:
+            warm(out["sample_rate"], "s16" if out["encoding"] == "flac" else out["encoding"], pitch)
+        return dict(out, pitch=float(pitch), gain_db=float(gain_db))
 
     def submit_text(self, prepare: Callable, pace: Optional[float] = None, speed: float = 1.0,
-                    sample_rate: Optional[int] = None, encoding: str = "f32", **gen_kwargs) -> TextTicket:
+                    sample_rate: Optional[int] = None, encoding: str = "f32", pitch: float = 0.0, gain_db: float = 0.0,
+                    **gen_kwargs) -> TextTicket:
         """A text-fed request.  ``prepare(feed)`` -> (tie, tam, tpe, ref_codes) builds the prompt once the feed holds its
         first committed id (``text_stream.TextFeed.prompt_ids``); it runs on the worker thread."""
         if self.feed_factory is None:
             raise RuntimeError("this batcher has no text feed factory")
-        speed = self._speed(speed)
-        out = self._output(sample_rate, encoding)
+        speed = self._speed(speed, pitch, gain_db)
+        out = self._output(sample_rate, encoding, pitch, gain_db)
         with self._lock:
             self._rid += 1
             t = TextTicket(self._rid, prepare, gen_kwargs, pace=self._pace(pace), submitted_at=self.clock(), speed=speed,
@@ -300,6 +311,10 @@ class ContinuousBatcher:
         kw = {} if t.speed == 1.0 else {"speed": t.speed}
         if (t.sample_rate, t.encoding) != (24000, "f32"):
             kw.update(sample_rate=t.sample_rate, encoding=t.encoding)
+        if t.pitch != 0:
+            kw["pitch"] = t.pitch
+        if t.gain_db != 0:
+            kw["gain_db"] = t.gain_db
         win = self.window_factory(ref_codes, **kw) if own is None else self.window_factory(ref_codes, own, **kw)
         if t.gen_kwargs.get("first_chunk") and not getattr(win, "any_chunking", False):
             raise ValueError("first_chunk needs a codec window whose audio does not depend on the chunking (the stateful "
@@ -448,9 +463,15 @@ def batcher_for_model(model, chunk_size: int = 8, to_host: bool = True, **kw) ->
             if speed != 1.0:
                 raise ValueError("a speaking rate other than 1 needs the codec (PCM)")
             if out:
-                raise ValueError("an output rate or encoding other than 24 kHz f32 needs the codec (PCM)")
+                raise ValueError("an output rate, encoding, pitch or gain other than 24 kHz f32, 0, 0 dB needs the codec "
+                                 "(PCM)")
             return _CodesOnly()
         return model._make_window(st, ref_codes, chunk, to_host, **({} if speed == 1.0 else {"speed": speed}), **out)
+
+    if st is not None:
+        from .model import _pcm_device
+        from .resample import warm as _warm
+        window.warm = lambda rate, encoding, pitch: _warm(rate, encoding, _pcm_device(st), pitch)
 
     bd = (lambda wins, chunks, finals=None: decode_windows_batched(st, wins, chunks, finals)) if st is not None else None
     from .text_stream import TextFeed

@@ -186,7 +186,8 @@ def generate_text_streaming(model, text_stream: Iterable[str], *, language: str,
                             voice_clone_prompt=None, chunk_size: int = 12, max_new_tokens: int = 2048,
                             min_new_tokens: int = 2, temperature: float = 0.9, top_k: int = 50, top_p: float = 1.0,
                             do_sample: bool = True, repetition_penalty: float = 1.05, uniforms=None, to_host: bool = True,
-                            speed: float = 1.0, sample_rate=None) -> Iterator:
+                            speed: float = 1.0, sample_rate=None, pitch: float = 0.0,
+                            gain_db: float = 0.0) -> Iterator:
     """Yields (pcm, sample_rate, timing) like the ``*_streaming`` methods.  Prefills once the first text id is
     committed, then per launch: pull text until the next chunk's rows exist (window codec policy) or one more row
     exists (stateful codec), or the text closes; announce the rows; decode one chunk.  The request is the one request of
@@ -228,7 +229,7 @@ def generate_text_streaming(model, text_stream: Iterable[str], *, language: str,
     win = None
     if st is not None:
         from .model import _post_kw
-        win = model._make_window(st, None, chunk_size, to_host, **_post_kw(speed, sample_rate))
+        win = model._make_window(st, None, chunk_size, to_host, **_post_kw(speed, sample_rate, pitch, gain_db))
     # the window policy's PCM depends on the chunking: launch only when a full chunk of rows exists, so that every launch
     # emits a full chunk or ends the request.  A stateful stream (or codes only) is the same in any chunking.
     ahead = 1 if win is None or getattr(win, "any_chunking", False) else chunk_size

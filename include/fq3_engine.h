@@ -406,12 +406,27 @@ const char* fq3_tempo_last_error(void);
  * G.711 mu-law / A-law of that s16.  A push releases exactly fq3_resample_released(R, samples pushed before, samples
  * pushed now, flush) samples -- a function of the totals alone, so buffers are sized on the host and nothing is read
  * back; a flushed stream of N samples has ceil(N L / M).  The output does not depend on how the input was pushed.
- * The algorithm, bit for bit, is in DESIGN.md ("Output rate and encoding") and faster_qwen3_tts/resample.py. */
+ * The algorithm, bit for bit, is in DESIGN.md ("Output rate and encoding") and faster_qwen3_tts/resample.py.
+ *
+ * Pitch and gain (DESIGN.md "Pitch and gain").  A pitch of p semitones in [-12, 12] is rho = round(256 * 2^(p / 12)) in
+ * [FQ3_RESAMPLE_PITCH_MIN, FQ3_RESAMPLE_PITCH_MAX]; the pitch ratio is rho / FQ3_RESAMPLE_PITCH_ONE.  The caller
+ * time-stretches first, with a tempo at q = round(speed * 2^18 / rho) (fq3_tempo_create(dev, q / 1024.0); q must lie in
+ * [256, 4096], q = 1024 is no tempo), and the resampler at (R, rho) then maps the input rate 24000 rho / 256 to R:
+ * (L, M) = (256 R, 24000 rho) reduced by their gcd, half = FQ3_RESAMPLE_HALF_PER_M * max(L, M), the same filter and
+ * closed form; L == M is the encode-only case.  At rho 256 every count, table and bit is the plain rate's.  A gain
+ * g = float32(10^(gain_db / 20)), gain_db in [-96, 16], multiplies each output once in fp32 before the encoding (so s16
+ * and G.711 clip by the s16 rule); g = 1 leaves the bits.  Phase tables are shared per (device, rate, rho): those at
+ * rho 256 live for the process, pitched ones as long as a handle uses them, plus at most FQ3_RESAMPLE_TABLE_CACHE
+ * unreferenced ones (least recently released freed first). */
 #define FQ3_RESAMPLE_IN_RATE 24000
 #define FQ3_RESAMPLE_HALF_PER_M 32
 #define FQ3_RESAMPLE_CUTOFF 0.9
 #define FQ3_RESAMPLE_BETA 8.6
 #define FQ3_RESAMPLE_ALIGN 16
+#define FQ3_RESAMPLE_PITCH_ONE 256
+#define FQ3_RESAMPLE_PITCH_MIN 128
+#define FQ3_RESAMPLE_PITCH_MAX 512
+#define FQ3_RESAMPLE_TABLE_CACHE 8
 #define FQ3_ENC_F32 0
 #define FQ3_ENC_S16 1
 #define FQ3_ENC_ULAW 2
@@ -420,12 +435,23 @@ typedef struct fq3_resample fq3_resample;
 /* designs the rate's filter on the host in double precision; the polyphase table is uploaded once per (device, rate)
  * and shared by every resampler at that rate */
 int fq3_resample_create(int32_t device, int32_t out_rate, int32_t encoding, fq3_resample** out);
+/* a resampler at rate R and pitch rho (fq3_resample_create is the rho = 256 case).  Any (R, rho, encoding) is accepted,
+ * 24000 Hz f32 at rho 256 included: the one-tap filter, for a gain alone.  Designs the (R, rho) table on the host in
+ * double (O(taps) Kaiser evaluations, up to 162 881 taps) and uploads it unless the device already holds it. */
+int fq3_resample_create_pitch(int32_t device, int32_t out_rate, int32_t pitch_rho, int32_t encoding,
+                              fq3_resample** out);
+/* the stream's gain g (float32, finite, >= 0; 1 at create, kept by reset); host-side, applies from the next process */
+int fq3_resample_set_gain(fq3_resample* r, float gain);
+/* bytes of phase tables the device holds (plain, pitched in use and cached unreferenced ones) */
+int64_t fq3_resample_table_bytes(int32_t device);
 int fq3_resample_reset(fq3_resample* r);   /* a new stream at the same rate; host-side, nothing is launched */
 void fq3_resample_destroy(fq3_resample* r);
 /* samples released by a push of n samples after total_in (-1 for an unknown rate or a negative count) */
 int64_t fq3_resample_released(int32_t out_rate, int64_t total_in, int64_t n, int32_t flush);
+int64_t fq3_resample_released_pitch(int32_t out_rate, int32_t pitch_rho, int64_t total_in, int64_t n, int32_t flush);
 /* the rate's filter h (double, 2 half + 1 taps) into out[0, cap); returns the number of taps (-1 for an unknown rate) */
 int32_t fq3_resample_taps(int32_t out_rate, double* out, int32_t cap);
+int32_t fq3_resample_taps_pitch(int32_t out_rate, int32_t pitch_rho, double* out, int32_t cap);
 /* One launch for n_streams distinct resamplers.  in_dev float32: the streams' new samples packed in order (in_lens[i]
  * of stream i, host array); flush[i] (host) != 0 ends stream i (it must be reset before more input).  out_dev
  * [out_cap bytes]: the released samples of every stream in its encoding, packed in order, each stream's slice starting

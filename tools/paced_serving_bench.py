@@ -13,7 +13,8 @@ N = 32 unpaced requests (pace = None: the engine calls of a build without paced 
 records then also hold the parks and the most pages in use at once.  ``--speed S`` gives every request the speaking rate S
 (time-stretched on the GPU after the codec): a listener then consumes model audio S times as fast.  ``--sample-rate R``
 / ``--encoding E`` give every request that output rate and encoding (resampled and encoded on the GPU after the codec;
-``flac`` compresses the s16 on the GPU as well).
+``flac`` compresses the s16 on the GPU as well).  ``--pitch P`` gives every request a pitch of P semitones (the tempo
+and the resampler together, on the GPU).
 
     python tools/paced_serving_bench.py --listeners 32,64,96,128,160,192 --codec window,stateful --repeats 2 \\
         --out profiles/h100_paced_serving.jsonl
@@ -62,7 +63,8 @@ class Timed:
         return out
 
 
-def run(model, n, codec, first_chunk, seed, stagger_s, chunk, pace=1.0, speed=1.0, sample_rate=24000, encoding="f32"):
+def run(model, n, codec, first_chunk, seed, stagger_s, chunk, pace=1.0, speed=1.0, sample_rate=24000, encoding="f32",
+        pitch=0.0):
     from faster_qwen3_tts.serving import batcher_for_model, voice_clone_request
     model.streaming_codec = codec
     rng = np.random.default_rng(seed)
@@ -76,6 +78,8 @@ def run(model, n, codec, first_chunk, seed, stagger_s, chunk, pace=1.0, speed=1.
     extra = {"first_chunk": first_chunk} if first_chunk else {}
     if speed != 1.0:
         extra["speed"] = speed
+    if pitch != 0:
+        extra["pitch"] = pitch
     out = {} if (sample_rate, encoding) == (24000, "f32") else {"sample_rate": sample_rate, "encoding": encoding}
     extra.update(out)
     tickets, ttfa, t_start = [None] * n, [None] * n, time.monotonic()
@@ -98,7 +102,8 @@ def run(model, n, codec, first_chunk, seed, stagger_s, chunk, pace=1.0, speed=1.
     b.close()
     under = [t.underruns for t in tickets]
     assert all(t.frames == f for t, f in zip(tickets, frames)), "a listener did not get all its audio"
-    return {"listeners": n, "pace": pace, **({"speed": speed} if speed != 1.0 else {}), **out, "codec": codec, "first_chunk": first_chunk, "chunk": chunk, "seed": seed,
+    return {"listeners": n, "pace": pace, **({"speed": speed} if speed != 1.0 else {}),
+            **({"pitch": pitch} if pitch != 0 else {}), **out, "codec": codec, "first_chunk": first_chunk, "chunk": chunk, "seed": seed,
             "audio_s": round(sum(frames) * 0.08, 1), "wall_s": round(wall, 2),
             "underruns_total": int(sum(under)), "listeners_with_underruns": int(sum(u > 0 for u in under)),
             "underruns_per_listener": round(float(np.mean(under)), 3), "underruns_max": int(max(under)),
@@ -125,6 +130,7 @@ def main():
     ap.add_argument("--speed", type=float, default=1.0, help="speaking rate of every request, in [0.25, 4.0]")
     ap.add_argument("--sample-rate", type=int, default=24000, help="output rate of every request")
     ap.add_argument("--encoding", default="f32", choices=["f32", "s16", "ulaw", "alaw", "flac"])
+    ap.add_argument("--pitch", type=float, default=0.0, help="pitch of every request, in semitones in [-12, 12]")
     ap.add_argument("--out", default=os.path.join(ROOT, "profiles", "h100_paced_serving.jsonl"))
     args = ap.parse_args()
     if not torch.cuda.is_available():
@@ -150,7 +156,7 @@ def main():
     with open(args.out, "a") as f:
         def record(*a, **k):
             rec = dict(base, **card(), **run(model, *a, speed=args.speed, sample_rate=args.sample_rate,
-                                                  encoding=args.encoding, **k))
+                                                  encoding=args.encoding, pitch=args.pitch, **k))
             print(json.dumps(rec), flush=True)
             f.write(json.dumps(rec) + "\n")
             f.flush()
