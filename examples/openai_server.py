@@ -13,7 +13,9 @@ time-stretched on the GPU after the codec, at the same pitch.  "sample_rate" (80
 48000; default 24000) is the rate of the response: the audio is resampled and encoded (s16 for wav / pcm, G.711 for ulaw
 / alaw, s16 compressed to a FLAC stream for flac) on the GPU, so only the encoded bytes leave it.  "pitch" (semitones,
 -12 - 12) shifts the voice up or down (formants move with it) and "gain_db" (-96 - 16) scales the level before the
-encoding clips; both are applied on the GPU by the same time-stretch and resampler.
+encoding clips; both are applied on the GPU by the same time-stretch and resampler.  "split" (default false, true for every
+request with --split) speaks a long input sentence by sentence: the segments are decoded side by side and joined on the
+GPU, "pause_ms" (0 - 2000) of silence between them.
 
     python examples/openai_server.py --model synthetic:1.7B --max-batch 16 --port 8000
     curl -s localhost:8000/v1/audio/speech -H 'Content-Type: application/json' \\
@@ -29,11 +31,12 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "faster-qwen3-tts_b200"))
 
 
-def build_app(model, batcher, voices, default_voice):
+def build_app(model, batcher, voices, default_voice, split_default=False):
     from fastapi import FastAPI, HTTPException
     from fastapi.responses import StreamingResponse
     from typing import Optional
     from pydantic import BaseModel
+    from faster_qwen3_tts.join import check_pause
     from faster_qwen3_tts.resample import RATES, check_prosody
     from faster_qwen3_tts.serving import voice_clone_request, wav_header
 
@@ -49,6 +52,8 @@ def build_app(model, batcher, voices, default_voice):
         pitch: float = 0.0             # semitones in [-12, 12]
         gain_db: float = 0.0           # level in [-96, 16] dB
         pace: Optional[float] = 1.0    # the client plays at pace x real time; null: everything as fast as possible
+        split: Optional[bool] = None   # speak the input segment by segment (null: the server's --split)
+        pause_ms: int = 0              # silence between segments, 0 - 2000 ms
 
     @app.get("/health")
     async def health():
@@ -72,13 +77,16 @@ def build_app(model, batcher, voices, default_voice):
             raise HTTPException(status_code=400, detail=f"'pace' must be a positive number or null, got {req.pace}")
         if not 0.25 <= req.speed <= 4.0:
             raise HTTPException(status_code=400, detail=f"'speed' must be in [0.25, 4.0], got {req.speed}")
+        split = split_default if req.split is None else req.split
         try:
             check_prosody(req.speed, req.pitch, req.gain_db)
+            check_pause(req.pause_ms)
+            prepare = voice_clone_request(model, req.input, v.get("language", "Auto"), v["ref_audio"],
+                                          v.get("ref_text", ""), split=split)
         except ValueError as ex:
             raise HTTPException(status_code=400, detail=str(ex))
-        ticket = batcher.submit(voice_clone_request(model, req.input, v.get("language", "Auto"), v["ref_audio"],
-                                                    v.get("ref_text", "")), pace=req.pace, speed=req.speed,
-                                sample_rate=req.sample_rate, encoding=encoding, pitch=req.pitch, gain_db=req.gain_db,
+        ticket = batcher.submit(prepare, pace=req.pace, speed=req.speed, sample_rate=req.sample_rate, encoding=encoding,
+                                pitch=req.pitch, gain_db=req.gain_db, split=split, pause_ms=req.pause_ms,
                                 max_new_tokens=v.get("max_new_tokens", 2048))
         loop = asyncio.get_event_loop()
         it = iter(ticket)
@@ -113,6 +121,8 @@ def main():
     ap.add_argument("--streaming-codec", default="window", choices=["window", "stateful"],
                     help="window: the reference's two-phase window policy (sample-exact); stateful: one decoder stream per "
                          "request, a third of the codec work under load, audio = the non-streaming decode")
+    ap.add_argument("--split", action="store_true",
+                    help="speak every request's input segment by segment unless the request sets \"split\"")
     ap.add_argument("--host", default="0.0.0.0")
     ap.add_argument("--port", type=int, default=8000)
     ap.add_argument("--device", default="cuda")
@@ -135,7 +145,7 @@ def main():
         voices = {"default": {"ref_audio": args.ref_audio, "ref_text": args.ref_text, "language": args.language}}
         default = "default"
     batcher = batcher_for_model(model, chunk_size=args.chunk_size)
-    uvicorn.run(build_app(model, batcher, voices, default), host=args.host, port=args.port)
+    uvicorn.run(build_app(model, batcher, voices, default, split_default=args.split), host=args.host, port=args.port)
 
 
 if __name__ == "__main__":

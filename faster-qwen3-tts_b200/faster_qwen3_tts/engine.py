@@ -88,6 +88,8 @@ EXPORTS = [
     "fq3_resample_released_pitch", "fq3_resample_taps_pitch", "fq3_resample_table_bytes",
     "fq3_flac_create", "fq3_flac_reset", "fq3_flac_destroy", "fq3_flac_max_bytes", "fq3_flac_process",
     "fq3_flac_last_error",
+    "fq3_join_create", "fq3_join_reset", "fq3_join_destroy", "fq3_join_released", "fq3_join_total", "fq3_join_process",
+    "fq3_join_last_error",
 ]
 
 
@@ -228,6 +230,18 @@ def load_library() -> C.CDLL:
     lib.fq3_flac_process.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int32),
                                      C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
     lib.fq3_flac_last_error.restype = C.c_char_p
+    lib.fq3_join_create.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_void_p)]
+    lib.fq3_join_reset.argtypes = [C.c_void_p, C.c_int32, C.c_int32]
+    lib.fq3_join_destroy.argtypes = [C.c_void_p]
+    lib.fq3_join_destroy.restype = None
+    lib.fq3_join_released.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32),
+                                      C.POINTER(C.c_int64), C.POINTER(C.c_int32), C.POINTER(C.c_int64)]
+    lib.fq3_join_total.argtypes = [C.c_void_p]
+    lib.fq3_join_total.restype = C.c_int64
+    lib.fq3_join_process.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32),
+                                     C.POINTER(C.c_int64), C.POINTER(C.c_int32), C.c_void_p, C.c_void_p, C.c_int64,
+                                     C.c_void_p]
+    lib.fq3_join_last_error.restype = C.c_char_p
     _lib = lib
     return lib
 

@@ -49,6 +49,13 @@ def _check_rate(sample_rate):
     check_rate(sample_rate)
 
 
+def _refuse_split(split):
+    """takes and text fed while it is spoken are not split (ValueError before anything is tokenized)"""
+    if split:
+        raise ValueError("split=True is supported by the one-shot and streaming calls only, not by takes or text fed "
+                         "while it is spoken")
+
+
 def _post_kw(speed, sample_rate=None, pitch=0.0, gain_db=0.0):
     """``speed=`` / ``sample_rate=`` / ``pitch=`` / ``gain_db=`` for the delivery calls, only where they are not the
     identity (speed 1, 24 kHz, pitch 0, 0 dB): at the defaults every call is made exactly as without them"""
@@ -209,6 +216,13 @@ def decode_windows_batched(speech_tokenizer, wins, chunks, finals=None):
             pcm = speech_tokenizer.push_streams([wins[i].p1 for i in idxs], torch.stack([prepared[i][0] for i in idxs]))
             for i, a in zip(idxs, pcm):
                 raw[i] = wins[i].finish(a, prepared[i][1])
+    return run_stages(wins, raw, finals, sr)
+
+
+def run_stages(wins, raw, finals, sr):
+    """The device stages of several windows (or ``_Chain``s) on their new 24 kHz PCM ``raw`` (None: no samples): every
+    tempo in one launch, every resampler in one more, every FLAC encoder in one more; ``finals[i]`` flushes window i's
+    stages.  Returns [(audio, sample_rate)] converted by each window's ``conv``."""
     stretched = [i for i, w in enumerate(wins) if getattr(w, "tempo", None) is not None]
     if stretched:
         from . import tempo
@@ -239,6 +253,33 @@ def decode_windows_batched(speech_tokenizer, wins, chunks, finals=None):
         for i, a in zip(compressed, out):
             raw[i] = a
     return [(w.conv(a if a is not None else torch.zeros(0)), _window_rate(w, sr)) for w, a in zip(wins, raw)]
+
+
+def _stages(speech_tokenizer, speed=1.0, sample_rate=None, encoding="f32", pitch=0.0, gain_db=0.0):
+    """a request's post-codec stages: at a speed or pitch other than 1 / 0 its ``tempo.Tempo`` (at
+    ``resample.tempo_speed``), at an output rate or encoding other than 24 kHz f32, a pitch or a gain its
+    ``resample.Resampler``; ``encoding="flac"`` is an s16 resampler followed by a ``flac.Encoder``"""
+    from .resample import resampler_for, tempo_speed
+    from .tempo import tempo_for
+    tempo = (tempo_for(tempo_speed(speed, pitch), _pcm_device(speech_tokenizer))
+             if speed != 1.0 or pitch != 0 else None)
+    rs = enc = None
+    if encoding == "flac":
+        from .flac import Encoder
+        rs = resampler_for(sample_rate, "s16", _pcm_device(speech_tokenizer), pitch, gain_db)
+        enc = Encoder(rs.rate, _pcm_device(speech_tokenizer))
+    elif sample_rate is not None or encoding != "f32" or pitch != 0 or gain_db != 0:
+        rs = resampler_for(sample_rate, encoding, _pcm_device(speech_tokenizer), pitch, gain_db)
+    return dict(tempo=tempo, resampler=rs, flac=enc)
+
+
+class _Chain:
+    """The post-codec stages of a segmented request, run once on its joined stream (``run_stages``)"""
+
+    def __init__(self, owner, speech_tokenizer, to_host=True, **out):
+        for k, v in _stages(speech_tokenizer, **out).items():
+            setattr(self, k, v)
+        self.conv = owner._to_numpy if to_host else (lambda a: a.flatten())
 
 
 def _window_rate(win, sr):
@@ -627,20 +668,9 @@ class FasterQwen3TTS:
         """the codec window of one request; at a speed or pitch other than 1 / 0 it carries the request's
         ``tempo.Tempo`` (at ``resample.tempo_speed``), at an output rate or encoding other than 24 kHz f32, a pitch or a
         gain its ``resample.Resampler``; ``encoding="flac"`` is an s16 resampler followed by a ``flac.Encoder``"""
-        from .resample import resampler_for, tempo_speed
-        from .tempo import tempo_for
         if self.streaming_codec not in ("window", "stateful"):
             raise ValueError("streaming_codec must be 'window' or 'stateful'")
-        tempo = (tempo_for(tempo_speed(speed, pitch), _pcm_device(speech_tokenizer))
-                 if speed != 1.0 or pitch != 0 else None)
-        rs = enc = None
-        if encoding == "flac":
-            from .flac import Encoder
-            rs = resampler_for(sample_rate, "s16", _pcm_device(speech_tokenizer), pitch, gain_db)
-            enc = Encoder(rs.rate, _pcm_device(speech_tokenizer))
-        elif sample_rate is not None or encoding != "f32" or pitch != 0 or gain_db != 0:
-            rs = resampler_for(sample_rate, encoding, _pcm_device(speech_tokenizer), pitch, gain_db)
-        kw = dict(tempo=tempo, resampler=rs, flac=enc)
+        kw = _stages(speech_tokenizer, speed, sample_rate, encoding, pitch, gain_db)
         if self.streaming_codec == "stateful" and getattr(speech_tokenizer, "supports_streams", False):
             return _StatefulWindow(self, speech_tokenizer, ref_codes, chunk_size, to_host, **kw)
         return _StreamWindow(self, speech_tokenizer, ref_codes, chunk_size, to_host, **kw)
@@ -749,11 +779,18 @@ class FasterQwen3TTS:
                              non_streaming_mode: Optional[bool] = None, append_silence: bool = True,
                              instruct: Optional[str] = None, ref_spk=None, ref_rvq=None, ref_spk_emb=None,
                              ref_codes=None, voice_clone_prompt=None, speed: float = 1.0,
-                             sample_rate: Optional[int] = None, pitch: float = 0.0, gain_db: float = 0.0) -> Tuple[list, int]:
+                             sample_rate: Optional[int] = None, pitch: float = 0.0, gain_db: float = 0.0, split: bool = False,
+                              max_segment_chars: int = 400, pause_ms: int = 0, seed: Optional[int] = None) -> Tuple[list, int]:
         _check_speed(speed, pitch, gain_db)
         _check_rate(sample_rate)
         voice_clone_prompt, nsm = self._voice_clone_rules(voice_clone_prompt, non_streaming_mode, ref_spk, ref_rvq,
                                                           ref_spk_emb, ref_codes)
+        if self._check_split(split, max_segment_chars, pause_ms, seed):
+            return self._split_one_shot(
+                self._clone_make(language, ref_audio, ref_text, xvec_only, nsm, append_silence, voice_clone_prompt,
+                                 instruct), text, max_segment_chars, pause_ms, seed, 12,
+                self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p, do_sample,
+                                 repetition_penalty), **_post_kw(speed, sample_rate, pitch, gain_db))
         *prep, ref_codes = self._prepare_generation(
             text=text, language=language, ref_audio=ref_audio, ref_text=ref_text, xvec_only=xvec_only,
             non_streaming_mode=nsm, append_silence=append_silence, voice_clone_prompt=voice_clone_prompt,
@@ -770,12 +807,22 @@ class FasterQwen3TTS:
                                        append_silence: bool = True, parity_mode: bool = False,
                                        instruct: Optional[str] = None, ref_spk=None, ref_rvq=None, ref_spk_emb=None,
                                        ref_codes=None, voice_clone_prompt=None, speed: float = 1.0,
-                                       sample_rate: Optional[int] = None, pitch: float = 0.0, gain_db: float = 0.0
+                                       sample_rate: Optional[int] = None, pitch: float = 0.0, gain_db: float = 0.0, split: bool = False,
+                              max_segment_chars: int = 400, pause_ms: int = 0, seed: Optional[int] = None
                                        ) -> Generator[Tuple[np.ndarray, int, dict], None, None]:
         _check_speed(speed, pitch, gain_db)
         _check_rate(sample_rate)
         voice_clone_prompt, nsm = self._voice_clone_rules(voice_clone_prompt, non_streaming_mode, ref_spk, ref_rvq,
                                                           ref_spk_emb, ref_codes)
+        if self._check_split(split, max_segment_chars, pause_ms, seed):
+            if parity_mode:
+                raise ValueError("split=True runs on the engine's batched decode, not the parity_mode baseline")
+            yield from self._split_stream(
+                self._clone_make(language, ref_audio, ref_text, xvec_only, nsm, append_silence, voice_clone_prompt,
+                                 instruct), text, max_segment_chars, pause_ms, seed, chunk_size,
+                self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p, do_sample,
+                                 repetition_penalty), **_post_kw(speed, sample_rate, pitch, gain_db))
+            return
         m, talker, config, tie, tam, tth, tpe, ref_codes = self._prepare_generation(
             text=text, language=language, ref_audio=ref_audio, ref_text=ref_text, xvec_only=xvec_only,
             non_streaming_mode=nsm, append_silence=append_silence, voice_clone_prompt=voice_clone_prompt,
@@ -848,6 +895,54 @@ class FasterQwen3TTS:
         self._validate(language)
         return self._resolve_non_streaming_mode(non_streaming_mode, default=True)
 
+    def _split_stream(self, make, text, max_segment_chars, pause_ms, seed, chunk_size, gen, speed=1.0,
+                      sample_rate=None, pitch=0.0, gain_db=0.0):
+        """A ``split=True`` request (DESIGN.md "Long inputs"): ``text`` cut by ``segment.split_text``, one row per
+        segment with the prompt ``make(segment_text)()`` builds, all decoded side by side through a
+        ``serving.ContinuousBatcher`` on this model and joined on the device; yields (audio, sample_rate, timing)."""
+        from .serving import batcher_for_model, segment_requests
+        segs = segment_requests(make, text, max_segment_chars)
+        b = batcher_for_model(self, chunk_size=chunk_size)
+        try:
+            ticket = b.submit(segs, split=True, pause_ms=pause_ms, seed=seed, **_post_kw(speed, sample_rate, pitch, gain_db),
+                              **gen)
+            yield from ticket
+        finally:
+            b.close()
+
+    def _clone_make(self, language, ref_audio, ref_text, xvec_only, nsm, append_silence, voice_clone_prompt, instruct):
+        """segment text -> ``prepare`` of its voice-clone prompt (same voice for every segment)"""
+        def make(text):
+            return lambda: self._prepare_generation(
+                text=text, language=language, ref_audio=ref_audio, ref_text=ref_text, xvec_only=xvec_only,
+                non_streaming_mode=nsm, append_silence=append_silence, voice_clone_prompt=voice_clone_prompt,
+                instruct=instruct)[3:]
+        return make
+
+    def _custom_make(self, language, speaker, instruct, nsm):
+        """segment text -> ``prepare`` of its custom-voice (voice-design: speaker None) prompt"""
+        def make(text):
+            return lambda: self._prepare_generation_custom(text, language, speaker, instruct, nsm)[3:] + (None,)
+        return make
+
+    def _split_one_shot(self, *args, **kw):
+        sr, parts = _rate_of(self.sample_rate, kw.get("sample_rate")), []
+        for audio, sr, _ in self._split_stream(*args, **kw):
+            parts.append(audio)
+        return [np.concatenate(parts) if parts else np.zeros(1, dtype=np.float32)], sr
+
+    @staticmethod
+    def _check_split(split, max_segment_chars, pause_ms, seed=None):
+        """the long-input arguments, refused (ValueError) before anything is tokenized; ``seed`` is the seed of a split
+        request (``segment.segment_seed``) and is refused without ``split``"""
+        from .join import check_pause
+        from .segment import check_max_chars
+        check_max_chars(max_segment_chars)
+        check_pause(pause_ms)
+        if seed is not None and not split:
+            raise ValueError("seed= is the seed of a split request: it needs split=True")
+        return bool(split)
+
     def _one_shot(self, prep, ref_codes, gen, speed=1.0, sample_rate=None, pitch=0.0, gain_db=0.0):
         """The delivery of the three one-shot methods: generate, then decode every frame at once (model.py:893-947),
         time-stretched on the device at a speed other than 1, resampled at an output rate other than 24 kHz."""
@@ -868,11 +963,17 @@ class FasterQwen3TTS:
                               non_streaming_mode: Optional[bool] = None, max_new_tokens: int = 2048,
                               min_new_tokens: int = 2, temperature: float = 0.9, top_k: int = 50, top_p: float = 1.0,
                               do_sample: bool = True, repetition_penalty: float = 1.05, speed: float = 1.0,
-                              sample_rate: Optional[int] = None, pitch: float = 0.0, gain_db: float = 0.0
+                              sample_rate: Optional[int] = None, pitch: float = 0.0, gain_db: float = 0.0, split: bool = False,
+                              max_segment_chars: int = 400, pause_ms: int = 0, seed: Optional[int] = None
                               ) -> Tuple[list, int]:
         _check_speed(speed, pitch, gain_db)
         _check_rate(sample_rate)
         (instruct,), nsm = self._custom_voice_rules([text], [language], [speaker], [instruct], non_streaming_mode)
+        if self._check_split(split, max_segment_chars, pause_ms, seed):
+            return self._split_one_shot(
+                self._custom_make(language, speaker, instruct, nsm), text, max_segment_chars, pause_ms, seed, 12,
+                self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p, do_sample,
+                                 repetition_penalty), **_post_kw(speed, sample_rate, pitch, gain_db))
         prep = self._prepare_generation_custom(text, language, speaker, instruct, nsm)
         return self._one_shot(prep, None, self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p,
                                                            do_sample, repetition_penalty), speed, sample_rate, pitch, gain_db)
@@ -883,11 +984,18 @@ class FasterQwen3TTS:
                                         min_new_tokens: int = 2, temperature: float = 0.9, top_k: int = 50,
                                         top_p: float = 1.0, do_sample: bool = True, repetition_penalty: float = 1.05,
                                         chunk_size: int = 12, speed: float = 1.0,
-                                        sample_rate: Optional[int] = None, pitch: float = 0.0, gain_db: float = 0.0
+                                        sample_rate: Optional[int] = None, pitch: float = 0.0, gain_db: float = 0.0, split: bool = False,
+                              max_segment_chars: int = 400, pause_ms: int = 0, seed: Optional[int] = None
                                         ) -> Generator[Tuple[np.ndarray, int, dict], None, None]:
         _check_speed(speed, pitch, gain_db)
         _check_rate(sample_rate)
         (instruct,), nsm = self._custom_voice_rules([text], [language], [speaker], [instruct], non_streaming_mode)
+        if self._check_split(split, max_segment_chars, pause_ms, seed):
+            yield from self._split_stream(
+                self._custom_make(language, speaker, instruct, nsm), text, max_segment_chars, pause_ms, seed,
+                chunk_size, self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p, do_sample,
+                                             repetition_penalty), **_post_kw(speed, sample_rate, pitch, gain_db))
+            return
         _, _, _, tie, tam, tth, tpe = self._prepare_generation_custom(text, language, speaker, instruct, nsm)
         yield from self.stream_from_embeds(tie, tam, tth, tpe, chunk_size=chunk_size, **_post_kw(speed, sample_rate, pitch, gain_db), **self._gen_kwargs(
             max_new_tokens, min_new_tokens, temperature, top_k, top_p, do_sample, repetition_penalty))
@@ -897,11 +1005,17 @@ class FasterQwen3TTS:
                               non_streaming_mode: Optional[bool] = None, max_new_tokens: int = 2048,
                               min_new_tokens: int = 2, temperature: float = 0.9, top_k: int = 50, top_p: float = 1.0,
                               do_sample: bool = True, repetition_penalty: float = 1.05, speed: float = 1.0,
-                              sample_rate: Optional[int] = None, pitch: float = 0.0, gain_db: float = 0.0
+                              sample_rate: Optional[int] = None, pitch: float = 0.0, gain_db: float = 0.0, split: bool = False,
+                              max_segment_chars: int = 400, pause_ms: int = 0, seed: Optional[int] = None
                               ) -> Tuple[list, int]:
         _check_speed(speed, pitch, gain_db)
         _check_rate(sample_rate)
         nsm = self._voice_design_rules(language, non_streaming_mode)
+        if self._check_split(split, max_segment_chars, pause_ms, seed):
+            return self._split_one_shot(
+                self._custom_make(language, None, instruct, nsm), text, max_segment_chars, pause_ms, seed, 12,
+                self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p, do_sample,
+                                 repetition_penalty), **_post_kw(speed, sample_rate, pitch, gain_db))
         prep = self._prepare_generation_custom(text, language, None, instruct, nsm)
         return self._one_shot(prep, None, self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p,
                                                            do_sample, repetition_penalty), speed, sample_rate, pitch, gain_db)
@@ -912,11 +1026,18 @@ class FasterQwen3TTS:
                                         min_new_tokens: int = 2, temperature: float = 0.9, top_k: int = 50,
                                         top_p: float = 1.0, do_sample: bool = True, repetition_penalty: float = 1.05,
                                         chunk_size: int = 12, speed: float = 1.0,
-                                        sample_rate: Optional[int] = None, pitch: float = 0.0, gain_db: float = 0.0
+                                        sample_rate: Optional[int] = None, pitch: float = 0.0, gain_db: float = 0.0, split: bool = False,
+                              max_segment_chars: int = 400, pause_ms: int = 0, seed: Optional[int] = None
                                         ) -> Generator[Tuple[np.ndarray, int, dict], None, None]:
         _check_speed(speed, pitch, gain_db)
         _check_rate(sample_rate)
         nsm = self._voice_design_rules(language, non_streaming_mode)
+        if self._check_split(split, max_segment_chars, pause_ms, seed):
+            yield from self._split_stream(
+                self._custom_make(language, None, instruct, nsm), text, max_segment_chars, pause_ms, seed,
+                chunk_size, self._gen_kwargs(max_new_tokens, min_new_tokens, temperature, top_k, top_p, do_sample,
+                                             repetition_penalty), **_post_kw(speed, sample_rate, pitch, gain_db))
+            return
         _, _, _, tie, tam, tth, tpe = self._prepare_generation_custom(text, language, None, instruct, nsm)
         yield from self.stream_from_embeds(tie, tam, tth, tpe, chunk_size=chunk_size, **_post_kw(speed, sample_rate, pitch, gain_db), **self._gen_kwargs(
             max_new_tokens, min_new_tokens, temperature, top_k, top_p, do_sample, repetition_penalty))
@@ -1014,7 +1135,8 @@ class FasterQwen3TTS:
                                    non_streaming_mode: Optional[bool] = None, append_silence: bool = True,
                                    instruct: Optional[str] = None, voice_clone_prompt=None, speed: float = 1.0,
                                    sample_rate: Optional[int] = None, pitch: float = 0.0,
-                                   gain_db: float = 0.0, n_takes: int = 4, seeds: Optional[List[int]] = None):
+                                   gain_db: float = 0.0, split: bool = False, max_segment_chars: int = 400,
+                                    pause_ms: int = 0, n_takes: int = 4, seeds: Optional[List[int]] = None):
         """``n_takes`` renderings of one ``generate_voice_clone`` request for the price of one batched decode: one prompt,
         one batched prefill, one launch per chunk for all takes.  Take i is the request run alone with the uniforms of
         ``take_uniforms(seeds[i], max_new_tokens)`` -- bit for bit while both run the per-head talker attention (a lone
@@ -1022,6 +1144,7 @@ class FasterQwen3TTS:
         holds "logprobs" (float32 [T,16], the log-probability of every code), "eos_logprob", "total_logprob" (their sum,
         EOS term included), "frames" and "seed".  A log-probability says how likely the sampler found its draws, not
         how good the audio is: the calls rank nothing and pick nothing."""
+        _refuse_split(split)
         _check_speed(speed, pitch, gain_db)
         _check_rate(sample_rate)
         voice_clone_prompt, nsm = self._voice_clone_rules(voice_clone_prompt, non_streaming_mode)
@@ -1040,9 +1163,11 @@ class FasterQwen3TTS:
                                     min_new_tokens: int = 2, temperature: float = 0.9, top_k: int = 50,
                                     top_p: float = 1.0, do_sample: bool = True, repetition_penalty: float = 1.05,
                                     speed: float = 1.0, sample_rate: Optional[int] = None, pitch: float = 0.0,
-                                    gain_db: float = 0.0, n_takes: int = 4,
+                                    gain_db: float = 0.0, split: bool = False, max_segment_chars: int = 400,
+                                    pause_ms: int = 0, n_takes: int = 4,
                                     seeds: Optional[List[int]] = None):
         """``n_takes`` renderings of one ``generate_custom_voice`` request (see ``generate_voice_clone_takes``)."""
+        _refuse_split(split)
         _check_speed(speed, pitch, gain_db)
         _check_rate(sample_rate)
         (instruct,), nsm = self._custom_voice_rules([text], [language], [speaker], [instruct], non_streaming_mode)
@@ -1058,9 +1183,11 @@ class FasterQwen3TTS:
                                     min_new_tokens: int = 2, temperature: float = 0.9, top_k: int = 50,
                                     top_p: float = 1.0, do_sample: bool = True, repetition_penalty: float = 1.05,
                                     speed: float = 1.0, sample_rate: Optional[int] = None, pitch: float = 0.0,
-                                    gain_db: float = 0.0, n_takes: int = 4,
+                                    gain_db: float = 0.0, split: bool = False, max_segment_chars: int = 400,
+                                    pause_ms: int = 0, n_takes: int = 4,
                                     seeds: Optional[List[int]] = None):
         """``n_takes`` renderings of one ``generate_voice_design`` request (see ``generate_voice_clone_takes``)."""
+        _refuse_split(split)
         _check_speed(speed, pitch, gain_db)
         _check_rate(sample_rate)
         nsm = self._voice_design_rules(language, non_streaming_mode)
@@ -1091,12 +1218,14 @@ class FasterQwen3TTS:
                                              temperature: float = 0.9, top_k: int = 50, top_p: float = 1.0,
                                              do_sample: bool = True, repetition_penalty: float = 1.05,
                                              chunk_size: int = 12, speed: float = 1.0,
-                                             sample_rate: Optional[int] = None, pitch: float = 0.0, gain_db: float = 0.0
+                                             sample_rate: Optional[int] = None, pitch: float = 0.0, gain_db: float = 0.0, split: bool = False,
+                                             max_segment_chars: int = 400, pause_ms: int = 0
                                              ) -> Generator[Tuple[np.ndarray, int, dict], None, None]:
         """``generate_custom_voice_streaming`` with the text fed while it is spoken: ``text_stream`` is any iterable of
         ``str`` pieces (an LLM's reply token by token).  The audio equals that of the one-shot streaming request for the
         same text, whatever the split and however fast the pieces come; generation waits where the text has not arrived
         yet.  Timing dicts add ``text_wait_ms``, the time spent blocked on ``text_stream``."""
+        _refuse_split(split)
         _check_speed(speed, pitch, gain_db)
         _check_rate(sample_rate)
         (instruct,), _ = self._custom_voice_rules([text_stream], [language], [speaker], [instruct], non_streaming_mode)
@@ -1110,10 +1239,12 @@ class FasterQwen3TTS:
                                              min_new_tokens: int = 2, temperature: float = 0.9, top_k: int = 50,
                                              top_p: float = 1.0, do_sample: bool = True,
                                              repetition_penalty: float = 1.05, chunk_size: int = 12, speed: float = 1.0,
-                                             sample_rate: Optional[int] = None, pitch: float = 0.0, gain_db: float = 0.0
+                                             sample_rate: Optional[int] = None, pitch: float = 0.0, gain_db: float = 0.0, split: bool = False,
+                                             max_segment_chars: int = 400, pause_ms: int = 0
                                              ) -> Generator[Tuple[np.ndarray, int, dict], None, None]:
         """``generate_voice_design_streaming`` with the text fed while it is spoken (see
         ``generate_custom_voice_text_streaming``)."""
+        _refuse_split(split)
         _check_speed(speed, pitch, gain_db)
         _check_rate(sample_rate)
         self._voice_design_rules(language, non_streaming_mode)
@@ -1130,11 +1261,13 @@ class FasterQwen3TTS:
                                             non_streaming_mode: Optional[bool] = None, append_silence: bool = True,
                                             ref_spk=None, ref_rvq=None, ref_spk_emb=None, ref_codes=None,
                                             voice_clone_prompt=None, speed: float = 1.0,
-                                            sample_rate: Optional[int] = None, pitch: float = 0.0, gain_db: float = 0.0
+                                            sample_rate: Optional[int] = None, pitch: float = 0.0, gain_db: float = 0.0, split: bool = False,
+                                             max_segment_chars: int = 400, pause_ms: int = 0
                                             ) -> Generator[Tuple[np.ndarray, int, dict], None, None]:
         """``generate_voice_clone_streaming`` with the text fed while it is spoken, x-vector cloning only: ICL cloning
         puts the target text under the reference codec frames inside the prompt, so it must be known before prefill
         (ValueError)."""
+        _refuse_split(split)
         _check_speed(speed, pitch, gain_db)
         _check_rate(sample_rate)
         voice_clone_prompt, _ = self._voice_clone_rules(voice_clone_prompt, non_streaming_mode, ref_spk, ref_rvq,

@@ -72,6 +72,9 @@ class Ticket:
     encoding: str = "f32"
     pitch: float = 0.0                    # semitones and dB, applied by the tempo and the resampler (resample.py)
     gain_db: float = 0.0
+    segments: Optional["Segments"] = None   # a segmented request: its rows, join and post-codec chain (split=True)
+    parent: Optional["Ticket"] = None     # a row of a segmented request: the request, and the row's segment index
+    seg: int = -1
 
     @property
     def flushes(self) -> bool:
@@ -97,6 +100,36 @@ class Ticket:
         parts = [c[0] for c in self]
         empty = {"f32": np.float32, "s16": np.int16}.get(self.encoding, np.uint8)
         return np.concatenate(parts) if parts else np.zeros(0, dtype=empty)
+
+
+class Segments(list):
+    """The per-segment ``prepare`` callables of a segmented request, in order (what the ``*_request`` helpers return
+    with ``split=True``), with the texts they speak; on the worker also the request's state: the next segment to admit,
+    the frames each row has made, which rows have ended, and the join."""
+
+    def __init__(self, prepares, texts):
+        super().__init__(prepares)
+        if not self:
+            raise ValueError("the text has no segment to speak")
+        self.texts = list(texts)
+        self.next = 0                       # rows [0, next) have been admitted
+        self.frames = [0] * len(self)
+        self.ended = [False] * len(self)
+        self.rows = {}                      # segment -> its row ticket, once the worker made it
+        self.joined = 0                     # 24 kHz samples of the joined stream released so far
+        self.seed, self.pause_ms = 0, 0
+        self.state = None                   # the joiner's per-request state
+
+    def current(self) -> int:
+        """the segment being played: the first that has not ended"""
+        return next((k for k, e in enumerate(self.ended) if not e), len(self) - 1)
+
+
+def segment_requests(make, text: str, max_segment_chars: int):
+    """``Segments`` of ``make(segment_text)`` over the segments of ``text`` (``segment.split_text``)"""
+    from .segment import split_text
+    texts = split_text(text, max_segment_chars)
+    return Segments([make(s) for s in texts], texts)
 
 
 @dataclass
@@ -160,14 +193,28 @@ class ContinuousBatcher:
     (``submit(..., pitch=, gain_db=)``) reach the window likewise when not 0; the lead is still ``frames x frame_s /
     speed`` (a pitched delivery lasts within 0.2 % of that).  A pitch's filter table is designed and uploaded by
     ``submit`` on the caller's thread (``window_factory.warm``, when the factory has one), not by the worker.
-    ``clock`` / ``sleep`` are the worker's time source, replaceable in tests."""
+    ``clock`` / ``sleep`` are the worker's time source, replaceable in tests.
+
+    Long inputs (``submit(segments, split=True, pause_ms=)``, DESIGN.md "Long inputs").  A segmented request is one
+    ticket made of N rows, one per segment of its text (``Segments``), each with its own prompt, slot and codec window
+    (``window_factory(ref_codes, [chunk], segment=True)``: codec only, PCM left on the device).  Row k is admitted only
+    after row k-1 (in ``submit_many`` order) and samples with the uniforms of ``segment.segment_seed(seed, k)``
+    (``joiner.uniforms``); ``max_new_tokens`` is per row.  ``joiner`` runs the join (``join.py``): ``open(ticket)`` ->
+    per-request state, ``run(states, pushes)`` with pushes (state, segment, pcm, ended) -> [(audio, sr, joined 24 kHz
+    samples)] per state, after the request's own tempo, resampler and FLAC encoder, and ``close(state)``.  Paced: the
+    segment being played gets the ticket's lead as ``due``; a later one ``lead + `` the seconds before it starts --
+    real seconds for audio already made, ``segment.CHARS_PER_S`` characters per second for text not yet made, plus the
+    pauses -- and is held (not admitted, not launched) while that is at least ``lead_high_s``.  The lead counts the
+    joined audio.  ``cancel`` frees every row."""
 
     def __init__(self, scheduler, window_factory: Callable, chunk_size: int = 8, idle_sleep: float = 0.002,
                  batch_decode: Optional[Callable] = None, feed_factory: Optional[Callable] = None,
                  lead_high_s: float = 2.0, frame_s: float = 0.08, clock: Callable[[], float] = time.monotonic,
-                 sleep: Callable[[float], None] = time.sleep):
+                 sleep: Callable[[float], None] = time.sleep, joiner=None):
         self.sched, self.window_factory, self.chunk_size = scheduler, window_factory, chunk_size
         self.lead_high_s, self.frame_s, self.clock, self.sleep = lead_high_s, frame_s, clock, sleep
+        self.joiner = joiner
+        self.segmented: List[Ticket] = []   # segmented requests on the worker, in arrival order
         self.batch_decode = batch_decode   # (windows, code chunks) -> [(pcm, sr)]: one codec batch per window length
         self.idle_sleep = idle_sleep
         self.pending: "queue.Queue[Ticket]" = queue.Queue()
@@ -187,20 +234,47 @@ class ContinuousBatcher:
     # ---- client side ------------------------------------------------------------------------------------
     def submit(self, prepare: Callable[[], tuple], pace: Optional[float] = None, speed: float = 1.0,
                sample_rate: Optional[int] = None, encoding: str = "f32", pitch: float = 0.0, gain_db: float = 0.0,
-               **gen_kwargs) -> Ticket:
+               split: bool = False, pause_ms: int = 0, seed: Optional[int] = None, **gen_kwargs) -> Ticket:
         """``pace``: the client plays at ``pace`` x real time (class docstring); ``speed``: speaking rate in [0.25,
         4.0]; ``sample_rate`` (None: 24000) and ``encoding`` (``f32 | s16 | ulaw | alaw | flac``): the audio the ticket
         carries; ``pitch``: semitones in [-12, 12]; ``gain_db``: in [-96, 16].
+        ``split``: ``prepare`` is a ``Segments`` (a ``*_request`` helper with ``split=True``) and the request is spoken
+        segment by segment, joined with ``pause_ms`` (integer in [0, 2000]) of silence; ``seed`` (None: drawn) is the
+        request's seed, segment k uses ``segment.segment_seed(seed, k)``.  Streamed chunks then carry ``segment`` and
+        ``n_segments`` in their timing dict.
         ``gen_kwargs`` are the scheduler's ``submit`` keywords, among them ``chunk_size`` / ``first_chunk`` for this
         request alone."""
         speed = self._speed(speed, pitch, gain_db)
         out = self._output(sample_rate, encoding, pitch, gain_db)
+        segs = self._segments(prepare, split, pause_ms, seed, gen_kwargs)
         with self._lock:
             self._rid += 1
             t = Ticket(self._rid, prepare, gen_kwargs, pace=self._pace(pace), submitted_at=self.clock(), speed=speed,
-                       **out)
+                       segments=segs, **out)
         self.pending.put(t)
         return t
+
+    def _segments(self, prepare, split, pause_ms, seed, gen_kwargs):
+        """the checked ``Segments`` of a ``split`` submission (None without split)"""
+        from .join import check_pause
+        check_pause(pause_ms)
+        if not split:
+            if isinstance(prepare, Segments):
+                raise ValueError("segmented prepare callables need split=True")
+            if seed is not None:
+                raise ValueError("seed= is the seed of a split request: it needs split=True")
+            return None
+        if not isinstance(prepare, Segments):
+            raise ValueError("split=True needs the Segments of a *_request helper called with split=True")
+        if self.joiner is None:
+            raise ValueError("this batcher has no joiner: it cannot serve segmented requests")
+        if "uniforms" in gen_kwargs:
+            raise ValueError("a segmented request draws its rows' uniforms from its seed")
+        if seed is None:
+            import random
+            seed = random.getrandbits(62)
+        prepare.seed, prepare.pause_ms = int(seed), pause_ms
+        return prepare
 
     @staticmethod
     def _pace(pace):
@@ -225,9 +299,12 @@ class ContinuousBatcher:
 
     def submit_text(self, prepare: Callable, pace: Optional[float] = None, speed: float = 1.0,
                     sample_rate: Optional[int] = None, encoding: str = "f32", pitch: float = 0.0, gain_db: float = 0.0,
-                    **gen_kwargs) -> TextTicket:
+                    split: bool = False, **gen_kwargs) -> TextTicket:
         """A text-fed request.  ``prepare(feed)`` -> (tie, tam, tpe, ref_codes) builds the prompt once the feed holds its
-        first committed id (``text_stream.TextFeed.prompt_ids``); it runs on the worker thread."""
+        first committed id (``text_stream.TextFeed.prompt_ids``); it runs on the worker thread.  Text that arrives
+        incrementally is not split (``split=True``: ValueError)."""
+        if split:
+            raise ValueError("split=True is not supported for text fed while it is spoken")
         if self.feed_factory is None:
             raise RuntimeError("this batcher has no text feed factory")
         speed = self._speed(speed, pitch, gain_db)
@@ -268,11 +345,74 @@ class ContinuousBatcher:
             self.waiting.remove(t)
             t.out.put(_DONE)
         for rid, (t, win) in list(self.live.items()):
-            if t.cancelled.is_set():
+            if t.cancelled.is_set():   # a row shares its request's event: cancelling the request frees every row
                 self.sched.cancel(self.requests.pop(rid))
                 del self.live[rid]
                 self._drop_stages(win)
                 t.out.put(_DONE)
+        for t in [t for t in self.segmented if t.cancelled.is_set()]:
+            self._end_segmented(t)
+
+    def _end_segmented(self, t: Ticket):
+        self.segmented.remove(t)
+        self.joiner.close(t.segments.state)
+        t.out.put(_DONE)
+
+    def _row(self, t: Ticket, k: int) -> Ticket:
+        """the row of segment k of the segmented request t (made once; it shares t's cancel event)"""
+        segs = t.segments
+        row = segs.rows.get(k)
+        if row is None:
+            from .segment import segment_seed
+            gen = dict(t.gen_kwargs)
+            uniforms = getattr(self.joiner, "uniforms", None)
+            if uniforms is not None:
+                gen["uniforms"] = uniforms(segment_seed(segs.seed, k), int(gen.get("max_new_tokens", 2048)))
+            with self._lock:
+                self._rid += 1
+                row = Ticket(self._rid, segs[k], gen, submitted_at=t.submitted_at, cancelled=t.cancelled, parent=t,
+                             seg=k)
+            segs.rows[k] = row
+        return row
+
+    def _made_s(self, t: Ticket) -> float:
+        """audio seconds handed to the listener: frames, or the joined samples of a segmented request"""
+        if t.segments is not None:
+            from .join import RATE
+            return t.segments.joined / RATE / t.speed
+        return t.frames * self.frame_s / t.speed
+
+    def _segment_due(self, t: Ticket, k: int, now: float) -> float:
+        """``due`` of segment k of a paced segmented request (class docstring)"""
+        from .segment import CHARS_PER_S
+        segs = t.segments
+        cur = segs.current()
+        if t.first_chunk_at is None:
+            lead = float("-inf") if k <= cur else 0.0
+        else:
+            lead = self._made_s(t) - t.pace * (now - t.first_chunk_at)
+        before = 0.0
+        for j in range(cur, k):
+            made = segs.frames[j] * self.frame_s / t.speed
+            est = len(segs.texts[j]) / CHARS_PER_S / t.speed
+            if j == cur:
+                before += 0.0 if segs.ended[j] else max(0.0, est - made)
+            else:
+                before += made if segs.ended[j] else max(made, est)
+            before += segs.pause_ms / 1000.0 / t.speed
+        return lead + before
+
+    def _candidate_rows(self) -> List[Ticket]:
+        """the rows of segmented requests that may be admitted now: in segment order, and for a paced request only
+        while the segment's due is below ``lead_high_s``"""
+        now, rows = self.clock(), []
+        for t in self.segmented:
+            segs = t.segments
+            for k in range(segs.next, len(segs)):
+                if t.pace is not None and k > segs.current() and self._segment_due(t, k, now) >= self.lead_high_s:
+                    break
+                rows.append(self._row(t, k))
+        return rows
 
     def _prepare(self, t: Ticket):
         """-> (the ticket's ``submit`` arguments by name, its codec window); a prompt longer than the scheduler's
@@ -308,6 +448,16 @@ class ContinuousBatcher:
         """the request's codec window, built for the request's own chunk size where it has one (the window policy's
         calibration point depends on it); a short first chunk is for windows whose audio does not depend on the chunking"""
         own = t.gen_kwargs.get("chunk_size")
+        kw = {"segment": True} if t.parent is not None else self._out_kw(t)
+        win = self.window_factory(ref_codes, **kw) if own is None else self.window_factory(ref_codes, own, **kw)
+        if t.gen_kwargs.get("first_chunk") and not getattr(win, "any_chunking", False):
+            raise ValueError("first_chunk needs a codec window whose audio does not depend on the chunking (the stateful "
+                             "codec stream); under the window policy the audio of a request is defined by one chunk_size")
+        return win
+
+    @staticmethod
+    def _out_kw(t: Ticket) -> dict:
+        """the ticket's post-codec stages as window keywords, only where they are not the identity"""
         kw = {} if t.speed == 1.0 else {"speed": t.speed}
         if (t.sample_rate, t.encoding) != (24000, "f32"):
             kw.update(sample_rate=t.sample_rate, encoding=t.encoding)
@@ -315,11 +465,7 @@ class ContinuousBatcher:
             kw["pitch"] = t.pitch
         if t.gain_db != 0:
             kw["gain_db"] = t.gain_db
-        win = self.window_factory(ref_codes, **kw) if own is None else self.window_factory(ref_codes, own, **kw)
-        if t.gen_kwargs.get("first_chunk") and not getattr(win, "any_chunking", False):
-            raise ValueError("first_chunk needs a codec window whose audio does not depend on the chunking (the stateful "
-                             "codec stream); under the window policy the audio of a request is defined by one chunk_size")
-        return win
+        return kw
 
     def _live(self, t: Ticket, rq, win):
         self.requests[t.rid] = rq
@@ -333,6 +479,12 @@ class ContinuousBatcher:
                 break
             if isinstance(t, TextTicket):
                 self.waiting.append(t)
+            elif t.segments is not None:
+                try:
+                    t.segments.state = self.joiner.open(t, self._out_kw(t))
+                    self.segmented.append(t)
+                except BaseException as ex:
+                    self._fail(t, ex)
             else:
                 self._queued.append(t)
         self._reap_cancelled()
@@ -340,28 +492,40 @@ class ContinuousBatcher:
         for t in [t for t in self._queued if t.cancelled.is_set()]:
             self._queued.remove(t)
             t.out.put(_DONE)
-        # text-fed requests enter once their first id is committed (the prompt holds it), in arrival order
-        ready = sorted([t for t in self.waiting if t.feed.n_ids] + self._queued, key=lambda t: t.rid)
+        # text-fed requests enter once their first id is committed (the prompt holds it), in arrival order; the rows of
+        # a segmented request in segment order, at its place in that order
+        ready = sorted([t for t in self.waiting if t.feed.n_ids] + self._queued + self._candidate_rows(),
+                       key=lambda t: (t.parent.rid, t.seg) if t.parent is not None else (t.rid, -1))
         many = hasattr(self.sched, "submit_many")
         admits = getattr(self.sched, "admits", None)   # a paged scheduler: do the prompts' KV pages fit as well
         batch = []   # (ticket, submit arguments, window) admitted together by one submit_many
         for t in ready:
             if (len(batch) >= self.sched.capacity()) if many else not self.sched.has_capacity():
                 break
-            queue_of = self.waiting if isinstance(t, TextTicket) else self._queued
-            queue_of.remove(t)
+            if t.parent is not None and (t.cancelled.is_set() or t.seg != t.parent.segments.next):
+                continue   # its request failed, or an earlier row of it is still waiting
+            queue_of = self.waiting if isinstance(t, TextTicket) else self._queued if t.parent is None else None
+            if queue_of is not None:
+                queue_of.remove(t)
             try:   # a bad request must not take the worker down, nor the requests admitted with it
                 req, win = t.prepared or self._prepare(t)
                 if many and admits is not None and not admits([r for _, r, _ in batch] + [req]):
                     t.prepared = (req, win)   # waits, prompt built, until finished requests free pages
-                    queue_of.append(t)
+                    if queue_of is not None:
+                        queue_of.append(t)
                     break
+                if t.parent is not None:
+                    t.parent.segments.next += 1
                 if many:
                     batch.append((t, req, win))
                 else:
                     self._live(t, self.sched.submit(**req), win)
             except BaseException as ex:
-                self._fail(t, ex)
+                if t.parent is not None:   # a row that cannot be spoken fails its request
+                    t.parent.cancel()
+                    self._fail(t.parent, ex)
+                else:
+                    self._fail(t, ex)
         # one batched prefill takes as many prompts as a launch has columns; free slots may be more
         per_call = getattr(self.sched, "max_prompts", None) or len(batch) or 1
         for i in range(0, len(batch), per_call):
@@ -370,7 +534,9 @@ class ContinuousBatcher:
                 rqs = self.sched.submit_many([req for _, req, _ in part])
             except BaseException as ex:
                 for t, _, _ in part:
-                    self._fail(t, ex)
+                    if t.parent is not None:
+                        t.parent.cancel()
+                    self._fail(t.parent or t, ex)
                 continue
             for (t, _, win), rq in zip(part, rqs):
                 self._live(t, rq, win)
@@ -379,13 +545,19 @@ class ContinuousBatcher:
         """hand every paced request's lead to the scheduler (class docstring)"""
         now = self.clock()
         for rid, (t, _) in self.live.items():
+            if t.parent is not None:
+                if t.parent.pace is not None:
+                    rq = self.requests[rid]
+                    rq.due = self._segment_due(t.parent, t.seg, now)
+                    rq.hold = rq.due >= self.lead_high_s
+                continue
             if t.pace is None:
                 continue
             rq = self.requests[rid]
             if t.first_chunk_at is None:
                 rq.due, rq.hold = float("-inf"), False
             else:
-                t.lead_s = t.frames * self.frame_s / t.speed - t.pace * (now - t.first_chunk_at)
+                t.lead_s = self._made_s(t) - t.pace * (now - t.first_chunk_at)
                 rq.due, rq.hold = t.lead_s, t.lead_s >= self.lead_high_s
 
     def _run(self):
@@ -403,6 +575,9 @@ class ContinuousBatcher:
                     t.out.put(ex)
                     t.out.put(_DONE)
                 self.live.clear()
+                for t in list(self.segmented):
+                    t.out.put(ex)
+                    self._end_segmented(t)
                 continue
             if not results:   # every active request is waiting for text, or is a listener far enough ahead
                 self.sleep(self.idle_sleep)
@@ -420,9 +595,17 @@ class ContinuousBatcher:
                     args += ([bool(rq.finished) for rq, _ in live],)
                 for (rq, _), (pcm, sr) in zip(live, self.batch_decode(*args)):
                     pcm_of[rq.tag] = (pcm, sr)
+            pushes = []   # (row, frames, its new PCM or None, whether it ended) of segmented requests
             for rq, codes in results:
                 t, win = self.live[rq.tag]
                 n = int(codes.shape[0])
+                if t.parent is not None:
+                    pcm = pcm_of[rq.tag][0] if rq.tag in pcm_of else (win.push(codes)[0] if n else None)
+                    pushes.append((t, n, pcm, bool(rq.finished)))
+                    if rq.finished:
+                        del self.live[rq.tag]
+                        self.requests.pop(rq.tag, None)
+                    continue
                 if n or rq.tag in pcm_of:
                     if rq.tag in pcm_of:
                         pcm, sr = pcm_of[rq.tag]
@@ -435,7 +618,7 @@ class ContinuousBatcher:
                         t.underruns += 1      # what it had was played out before this chunk arrived
                     t.frames += n
                     if t.pace is not None:
-                        t.lead_s = t.frames * self.frame_s / t.speed - t.pace * (now - t.first_chunk_at)
+                        t.lead_s = self._made_s(t) - t.pace * (now - t.first_chunk_at)
                     t.out.put((pcm, sr, {"chunk_steps": n, "total_steps_so_far": t.frames,
                                          "is_final": bool(rq.finished)}))
                 if rq.finished:
@@ -443,6 +626,47 @@ class ContinuousBatcher:
                     del self.live[rq.tag]
                     self.requests.pop(rq.tag, None)
                     self._drop_stages(win)
+            if pushes:
+                self._join_step(pushes)
+
+    def _join_step(self, pushes):
+        """the rows' new PCM -> the join of every segmented request they belong to, in one ``joiner.run``; delivers
+        what each request's join released, in order"""
+        parents = []
+        for row, n, _, ended in pushes:
+            segs = row.parent.segments
+            segs.frames[row.seg] += n
+            segs.ended[row.seg] = segs.ended[row.seg] or ended
+            if row.parent not in parents:
+                parents.append(row.parent)
+        try:
+            outs = self.joiner.run([p.segments.state for p in parents],
+                                   [(row.parent.segments.state, row.seg, pcm, ended) for row, _, pcm, ended in pushes])
+        except BaseException as ex:   # the join failed: end these requests (their rows are freed), not the worker
+            for p in parents:
+                p.cancel()
+                p.out.put(ex)
+                self._end_segmented(p)
+            return
+        for p, (audio, sr, n24) in zip(parents, outs):
+            segs, n = p.segments, sum(m for row, m, _, _ in pushes if row.parent is p)
+            final = all(segs.ended)
+            if len(audio) or final:
+                now = self.clock()
+                if p.first_chunk_at is None:
+                    p.first_chunk_at = now
+                elif p.pace is not None and self._made_s(p) - p.pace * (now - p.first_chunk_at) < 0:
+                    p.underruns += 1
+                p.frames += n
+                segs.joined += n24
+                if p.pace is not None:
+                    p.lead_s = self._made_s(p) - p.pace * (now - p.first_chunk_at)
+                p.out.put((audio, sr, {"chunk_steps": n, "total_steps_so_far": p.frames, "is_final": final,
+                                       "segment": segs.current(), "n_segments": len(segs)}))
+            else:
+                p.frames += n
+            if final:
+                self._end_segmented(p)
 
 
 def batcher_for_model(model, chunk_size: int = 8, to_host: bool = True, **kw) -> ContinuousBatcher:
@@ -458,7 +682,11 @@ def batcher_for_model(model, chunk_size: int = 8, to_host: bool = True, **kw) ->
         def push(self, codes):
             return codes.cpu().numpy(), model.sample_rate
 
-    def window(ref_codes, chunk=chunk_size, speed=1.0, **out):
+    def window(ref_codes, chunk=chunk_size, speed=1.0, segment=False, **out):
+        if segment:   # a row of a segmented request: codec only, its PCM stays on the device for the join
+            if st is None:
+                raise ValueError("split=True needs the codec (PCM)")
+            return model._make_window(st, ref_codes, chunk, False)
         if st is None:
             if speed != 1.0:
                 raise ValueError("a speaking rate other than 1 needs the codec (PCM)")
@@ -476,12 +704,51 @@ def batcher_for_model(model, chunk_size: int = 8, to_host: bool = True, **kw) ->
     bd = (lambda wins, chunks, finals=None: decode_windows_batched(st, wins, chunks, finals)) if st is not None else None
     from .text_stream import TextFeed
     return ContinuousBatcher(sched, window, chunk_size=chunk_size, batch_decode=bd,
-                             feed_factory=lambda max_rows: TextFeed(model, max_rows), **kw)
+                             feed_factory=lambda max_rows: TextFeed(model, max_rows),
+                             joiner=_Joiner(model, to_host) if st is not None else None, **kw)
 
 
-def custom_voice_text_request(model, speaker: str, language: str, instruct: Optional[str] = None):
+class _Joiner:
+    """The join of segmented requests on a model's device (``ContinuousBatcher`` class docstring): a ``join.Join`` and
+    a ``model._Chain`` of the request's post-codec stages per request"""
+
+    def __init__(self, model, to_host=True):
+        from .model import _pcm_device
+        self.model, self.to_host = model, to_host
+        self.st = model.model.model.speech_tokenizer
+        self.device = _pcm_device(self.st)
+
+    def uniforms(self, seed, n):
+        from .model import take_uniforms
+        return take_uniforms(seed, n, self.model.engine.device)
+
+    def open(self, t, out_kw):
+        from .join import Join
+        from .model import _Chain
+        return Join(len(t.segments), t.segments.pause_ms, self.device), _Chain(self.model, self.st, self.to_host,
+                                                                               **out_kw)
+
+    def run(self, states, pushes):
+        import torch
+        from . import join
+        from .model import run_stages
+        empty = torch.zeros(0, dtype=torch.float32, device=self.device)
+        pcm = join.process([j for j, _ in states], [(s[0], k, empty if p is None else p, e) for s, k, p, e in pushes])
+        outs = run_stages([c for _, c in states], pcm, [j.done for j, _ in states], 24000)
+        return [(a, sr, int(p.numel())) for (a, sr), p in zip(outs, pcm)]
+
+    def close(self, state):
+        j, chain = state
+        j.close()
+        ContinuousBatcher._drop_stages(chain)
+
+
+def custom_voice_text_request(model, speaker: str, language: str, instruct: Optional[str] = None, split: bool = False):
     """``prepare`` callable for ``ContinuousBatcher.submit_text``: the prompt of a text-fed custom-voice request, built
-    from the feed's first committed id exactly like ``generate_custom_voice_text_streaming`` builds it."""
+    from the feed's first committed id exactly like ``generate_custom_voice_text_streaming`` builds it.  Text that
+    arrives incrementally is not split (``split=True``: ValueError)."""
+    if split:
+        raise ValueError("split=True is not supported for text fed while it is spoken")
     from .text_stream import build_prompt
     (instruct,), _ = model._custom_voice_rules([None], [language], [speaker], [instruct], None)   # text: from the feed
 
@@ -493,12 +760,34 @@ def custom_voice_text_request(model, speaker: str, language: str, instruct: Opti
 
 
 def voice_clone_request(model, text: str, language: str, ref_audio, ref_text: str = "", xvec_only: bool = False,
-                        non_streaming_mode: bool = False, append_silence: bool = True):
+                        non_streaming_mode: bool = False, append_silence: bool = True, split: bool = False,
+                        max_segment_chars: int = 400):
     """``prepare`` callable for ``ContinuousBatcher.submit``: the voice-clone prompt path of the public API
-    (model.py:465-543) up to the embeddings."""
-    def prepare():
-        _, _, _, tie, tam, tth, tpe, ref_codes = model._prepare_generation(
-            text, ref_audio=ref_audio, ref_text=ref_text, language=language, xvec_only=xvec_only,
-            non_streaming_mode=non_streaming_mode, append_silence=append_silence)
-        return tie, tam, tth, tpe, ref_codes
-    return prepare
+    (model.py:465-543) up to the embeddings.  ``split=True``: the ``Segments`` of ``text`` (``segment.split_text`` at
+    ``max_segment_chars``), one prompt per segment in the same voice, for ``submit(..., split=True)``."""
+    def make(text):
+        def prepare():
+            _, _, _, tie, tam, tth, tpe, ref_codes = model._prepare_generation(
+                text, ref_audio=ref_audio, ref_text=ref_text, language=language, xvec_only=xvec_only,
+                non_streaming_mode=non_streaming_mode, append_silence=append_silence)
+            return tie, tam, tth, tpe, ref_codes
+        return prepare
+    return segment_requests(make, text, max_segment_chars) if split else make(text)
+
+
+def custom_voice_request(model, text: str, speaker: Optional[str], language: str, instruct: Optional[str] = None,
+                         non_streaming_mode: Optional[bool] = None, split: bool = False, max_segment_chars: int = 400):
+    """``prepare`` callable for ``ContinuousBatcher.submit``: a custom-voice request (a voice-design one with speaker
+    None and the design as ``instruct``), built like ``generate_custom_voice`` / ``generate_voice_design`` build it.
+    ``split=True``: the ``Segments`` of ``text``, as in ``voice_clone_request``."""
+    if speaker is None:
+        nsm = model._voice_design_rules(language, non_streaming_mode)
+    else:
+        (instruct,), nsm = model._custom_voice_rules([text], [language], [speaker], [instruct], non_streaming_mode)
+
+    def make(text):
+        def prepare():
+            _, _, _, tie, tam, tth, tpe = model._prepare_generation_custom(text, language, speaker, instruct, nsm)
+            return tie, tam, tth, tpe, None
+        return prepare
+    return segment_requests(make, text, max_segment_chars) if split else make(text)

@@ -498,6 +498,42 @@ int fq3_flac_process(fq3_flac* const* encs, int32_t n_streams, const int16_t* in
                      const int32_t* flush, void* out_dev, int64_t out_cap, int32_t* out_lens_dev, void* stream);
 const char* fq3_flac_last_error(void);
 
+/* ---- Long inputs: the join of a segmented request's rows into one stream (csrc/fq3_join.cu)
+ * A segmented request speaks its text as S segments, each decoded as its own row with its own codec window; rows finish
+ * in any order.  The join turns their 24 kHz float32 PCM into the request's one stream, before its tempo, resampler and
+ * FLAC encoder: seg_0, P zeros, seg_1, ..., seg_{S-1}, with P = pause_ms * FQ3_JOIN_RATE / 1000 and pause_ms in
+ * [0, FQ3_JOIN_PAUSE_MAX_MS].  Every inner boundary is faded, also at pause 0: sample n of segment k (length L) becomes
+ * x * a * b in fp32, a = w[n] for k > 0 and n < F, b = w[L - 1 - n] for k < S - 1 and L - 1 - n < F (1 otherwise),
+ * F = FQ3_JOIN_FADE (5 ms), w[i] = float32(0.5 - 0.5 cos(pi (i + 0.5) / F)).  Samples of the segment being played are
+ * released as they arrive, but for its last F while it has not ended (the last segment has no fade-out and holds
+ * nothing back); samples of a later segment stay on the device until every earlier one has ended.  The rule, bit for
+ * bit, is in DESIGN.md ("Long inputs") and faster_qwen3_tts/join.py.  The released counts depend on the lengths and end
+ * flags alone (fq3_join_released), so buffers are sized on the host and nothing is read back; the output does not
+ * depend on how the segments were pushed. */
+#define FQ3_JOIN_RATE 24000
+#define FQ3_JOIN_FADE 120
+#define FQ3_JOIN_PAUSE_MAX_MS 2000
+typedef struct fq3_join fq3_join;
+int fq3_join_create(int32_t device, int32_t n_segments, int32_t pause_ms, fq3_join** out);
+/* a new request of n_segments at pause_ms; frees the samples still held (host-side, nothing is launched) */
+int fq3_join_reset(fq3_join* j, int32_t n_segments, int32_t pause_ms);
+void fq3_join_destroy(fq3_join* j);
+/* A call's pushes: push i gives lens[i] new samples of segment seg[i] of join join_of[i] (index into joins), ends[i] != 0
+ * ends that segment; all host arrays, one push per (join, segment) and call.  released[j] (host, n_joins) receives the
+ * samples the call would release for joins[j], without changing any state.  A push to an ended segment or out of range,
+ * a join listed twice or a segment pushed twice is refused. */
+int fq3_join_released(fq3_join* const* joins, int32_t n_joins, int32_t n_pushes, const int32_t* join_of,
+                      const int32_t* seg, const int64_t* lens, const int32_t* ends, int64_t* released);
+/* samples the join has released so far (-1 for null) */
+int64_t fq3_join_total(const fq3_join* j);
+/* One launch for every join of the call.  in_dev float32: the pushes' samples packed in push order; out_dev float32
+ * [out_cap]: the released samples of every join packed in the order of `joins` (fq3_join_released counts).  Every refusal
+ * of fq3_join_released, and a null, misaligned or too small buffer, is made before anything is launched. */
+int fq3_join_process(fq3_join* const* joins, int32_t n_joins, int32_t n_pushes, const int32_t* join_of,
+                     const int32_t* seg, const int64_t* lens, const int32_t* ends, const float* in_dev, float* out_dev,
+                     int64_t out_cap, void* stream);
+const char* fq3_join_last_error(void);
+
 const char* fq3_last_error(void);
 const char* fq3_version(void);
 
