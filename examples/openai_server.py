@@ -15,7 +15,11 @@ time-stretched on the GPU after the codec, at the same pitch.  "sample_rate" (80
 -12 - 12) shifts the voice up or down (formants move with it) and "gain_db" (-96 - 16) scales the level before the
 encoding clips; both are applied on the GPU by the same time-stretch and resampler.  "split" (default false, true for every
 request with --split) speaks a long input sentence by sentence: the segments are decoded side by side and joined on the
-GPU, "pause_ms" (0 - 2000) of silence between them.
+GPU, "pause_ms" (0 - 2000) of silence between them.  "input_format": "ssml" reads the input as an SSML document
+(faster_qwen3_tts/ssml.py: <voice>, <prosody>, <break>, <p>, <s>, <sub>): "voice" is then the voice spoken outside every
+<voice>, "pause_ms" the pause at a boundary without a <break>, and "split" must be null or true.  A --voices file maps
+names to voice specs: {"ref_audio": ..., "ref_text": ..., "xvec_only": ...} (a clone), {"speaker": ..., "instruct": ...}
+(a custom voice) or {"design": ...} (a voice design), each with an optional "language" and "max_new_tokens".
 
     python examples/openai_server.py --model synthetic:1.7B --max-batch 16 --port 8000
     curl -s localhost:8000/v1/audio/speech -H 'Content-Type: application/json' \\
@@ -38,7 +42,8 @@ def build_app(model, batcher, voices, default_voice, split_default=False):
     from pydantic import BaseModel
     from faster_qwen3_tts.join import check_pause
     from faster_qwen3_tts.resample import RATES, check_prosody
-    from faster_qwen3_tts.serving import voice_clone_request, wav_header
+    from faster_qwen3_tts.serving import ssml_request, wav_header
+    from faster_qwen3_tts.ssml import voice_request
 
     app = FastAPI(title="faster-qwen3-tts (H100 engine) OpenAI-compatible API")
 
@@ -54,6 +59,7 @@ def build_app(model, batcher, voices, default_voice, split_default=False):
         pace: Optional[float] = 1.0    # the client plays at pace x real time; null: everything as fast as possible
         split: Optional[bool] = None   # speak the input segment by segment (null: the server's --split)
         pause_ms: int = 0              # silence between segments, 0 - 2000 ms
+        input_format: str = "text"     # text | ssml
 
     @app.get("/health")
     async def health():
@@ -63,9 +69,16 @@ def build_app(model, batcher, voices, default_voice, split_default=False):
     async def create_speech(req: SpeechRequest):
         if not req.input.strip():
             raise HTTPException(status_code=400, detail="'input' text is empty")
-        v = voices.get(req.voice) or (voices.get(default_voice) if default_voice else None)
+        name = req.voice if req.voice in voices else default_voice
+        v = voices.get(name) if name else None
         if v is None:
             raise HTTPException(status_code=400, detail=f"Voice {req.voice!r} is not configured. Available voices: {list(voices)}")
+        if req.input_format not in ("text", "ssml"):
+            raise HTTPException(status_code=400, detail=f"'input_format' must be text or ssml, got {req.input_format!r}")
+        ssml = req.input_format == "ssml"
+        if ssml and req.split is False:
+            raise HTTPException(status_code=400, detail="an SSML input is spoken segment by segment: 'split' must be "
+                                                        "null or true")
         fmt = req.response_format.lower()
         encoding = {"wav": "s16", "pcm": "s16", "ulaw": "ulaw", "alaw": "alaw", "flac": "flac"}.get(fmt)
         if encoding is None:
@@ -77,12 +90,14 @@ def build_app(model, batcher, voices, default_voice, split_default=False):
             raise HTTPException(status_code=400, detail=f"'pace' must be a positive number or null, got {req.pace}")
         if not 0.25 <= req.speed <= 4.0:
             raise HTTPException(status_code=400, detail=f"'speed' must be in [0.25, 4.0], got {req.speed}")
-        split = split_default if req.split is None else req.split
+        split = ssml or (split_default if req.split is None else req.split)
         try:
             check_prosody(req.speed, req.pitch, req.gain_db)
             check_pause(req.pause_ms)
-            prepare = voice_clone_request(model, req.input, v.get("language", "Auto"), v["ref_audio"],
-                                          v.get("ref_text", ""), split=split)
+            if ssml:
+                prepare = ssml_request(model, req.input, voices, voice=name)
+            else:
+                prepare = voice_request(model, v, req.input, split=split)
         except ValueError as ex:
             raise HTTPException(status_code=400, detail=str(ex))
         ticket = batcher.submit(prepare, pace=req.pace, speed=req.speed, sample_rate=req.sample_rate, encoding=encoding,

@@ -2,7 +2,10 @@
 // tests/join_oracle.py the arithmetic): the 24 kHz float32 PCM of its S segments, which are decoded as separate rows and
 // finish in any order, becomes one stream, in segment order:
 //
-//   out = seg_0 · P zeros · seg_1 · P zeros · ... · seg_{S-1},   P = 24 * pause_ms
+//   out = P_0 zeros · seg_0 · P_1 zeros · seg_1 · ... · P_{S-1} zeros · seg_{S-1} · P_S zeros,   P_k = 24 * pauses_ms[k]
+//
+// fq3_join_create(pause_ms) is the plan [0, P, ..., P, 0].  The leading P_0 zeros are released with segment 0's first
+// push, the trailing P_S zeros in the call that completes the stream.
 //
 // with a raised-cosine fade at every inner boundary: sample n of segment k (length L) is x * a * b in fp32, in that
 // order, with a = w[n] for k > 0 and n < F (else 1) and b = w[L - 1 - n] for k < S - 1 and L - 1 - n < F (else 1), where
@@ -99,7 +102,9 @@ struct Seg {
 }  // namespace
 
 struct fq3_join {
-  int dev = 0, S = 0, P = 0, cur = 0, pp = 0;
+  int dev = 0, S = 0, cur = 0, pp = 0;
+  bool lead_done = false, tail_done = false;   // the leading / trailing zeros have been released
+  std::vector<int64_t> pause;                  // S + 1 zero runs, in samples: before segment 0, between, after the last
   int64_t out_pos = 0, released = 0;   // of segment cur: samples [out_pos, segs[cur].total) are in tail[pp]
   float* tail = nullptr;               // 2 x F
   std::vector<Seg> segs;
@@ -127,6 +132,7 @@ int plan(fq3_join* j, const std::map<int, Push>& pushes, bool run, const float* 
     if (kv.second.n < 0) return jfail(FQ3_ERR_INVALID, "negative input length");
   }
   int64_t emitted = 0;
+  const bool lead = !j->lead_done && pushes.count(0);
   float* tail_old = j->tail + (size_t)j->pp * F;
   float* tail_new = j->tail + (size_t)(j->pp ^ 1) * F;
   auto add = [&](const float* src, float* dst, int64_t n, int64_t pos, int64_t L, bool fin, bool fout) {
@@ -149,9 +155,14 @@ int plan(fq3_join* j, const std::map<int, Push>& pushes, bool run, const float* 
       for (const Chunk& c : s.chunks) span(c.p, c.pos, c.pos + c.n);
     if (it != pushes.end()) span(in_dev + it->second.in_off, in0, in0 + it->second.n);
   };
+  if (lead) {   // the leading zeros, with segment 0's first push
+    if (run) add(nullptr, out, j->pause[0], 0, -1, false, false);
+    emitted += j->pause[0];
+  }
   // the state after this call, applied only when `run`
   int cur = j->cur;
   int64_t out_pos = j->out_pos;
+  bool tail = false;
   for (int k = cur;; ++k) {
     const Seg& s = j->segs[k];
     auto it = pushes.find(k);
@@ -169,9 +180,18 @@ int plan(fq3_join* j, const std::map<int, Push>& pushes, bool run, const float* 
     emitted += upto - from;
     cur = k;
     out_pos = upto;
-    if (!ended || k == j->S - 1) break;
-    emitted += j->P;   // the pause after segment k
-    if (run) add(nullptr, out + emitted - j->P, j->P, 0, -1, false, false);
+    const int64_t P = j->pause[k + 1];   // the zeros after segment k
+    if (k == j->S - 1) {
+      tail = ended && !j->tail_done;
+      if (tail) {
+        if (run) add(nullptr, out + emitted, P, 0, -1, false, false);
+        emitted += P;
+      }
+      break;
+    }
+    if (!ended) break;
+    if (run) add(nullptr, out + emitted, P, 0, -1, false, false);
+    emitted += P;
   }
   if (n_out) *n_out = emitted;
   if (!run) return 0;
@@ -195,6 +215,8 @@ int plan(fq3_join* j, const std::map<int, Push>& pushes, bool run, const float* 
   }
   j->cur = cur;
   j->out_pos = out_pos;
+  j->lead_done = j->lead_done || lead;
+  j->tail_done = j->tail_done || tail;
   j->pp ^= 1;
   j->released += emitted;
   return 0;
@@ -223,38 +245,68 @@ int group(fq3_join* const* joins, int32_t n_joins, int32_t n_pushes, const int32
   return 0;
 }
 
-}  // namespace
-
-extern "C" int fq3_join_create(int32_t device, int32_t n_segments, int32_t pause_ms, fq3_join** out) {
-  if (!out) return jfail(FQ3_ERR_INVALID, "null argument");
+// the uniform plan of fq3_join_create / fq3_join_reset: [0, P, ..., P, 0]
+int uniform(int32_t n_segments, int32_t pause_ms, std::vector<int32_t>* plan) {
   if (n_segments < 1) return jfail(FQ3_ERR_INVALID, "a join needs at least one segment");
   if (pause_ms < 0 || pause_ms > FQ3_JOIN_PAUSE_MAX_MS) return jfail(FQ3_ERR_INVALID, "pause_ms must be in [0, 2000]");
+  plan->assign(n_segments + 1, pause_ms);
+  plan->front() = plan->back() = 0;
+  return 0;
+}
+
+// a new request of n_segments with the plan pauses_ms[0 .. n_segments]; frees what the join still held
+int start(fq3_join* j, int32_t n_segments, const int32_t* pauses_ms) {
+  if (n_segments < 1) return jfail(FQ3_ERR_INVALID, "a join needs at least one segment");
+  if (!pauses_ms) return jfail(FQ3_ERR_INVALID, "null argument");
+  for (int k = 0; k <= n_segments; ++k)
+    if (pauses_ms[k] < 0 || pauses_ms[k] > FQ3_JOIN_BREAK_MAX_MS)
+      return jfail(FQ3_ERR_INVALID, "every pause must be in [0, 10000] ms");
+  free_chunks(j);
+  j->S = n_segments;
+  j->pause.resize(n_segments + 1);
+  for (int k = 0; k <= n_segments; ++k) j->pause[k] = (int64_t)pauses_ms[k] * (FQ3_JOIN_RATE / 1000);
+  j->cur = j->pp = 0;
+  j->out_pos = j->released = 0;
+  j->lead_done = j->tail_done = false;
+  j->segs.assign(n_segments, Seg());
+  return 0;
+}
+
+}  // namespace
+
+extern "C" int fq3_join_create_pauses(int32_t device, int32_t n_segments, const int32_t* pauses_ms, fq3_join** out) {
+  if (!out) return jfail(FQ3_ERR_INVALID, "null argument");
   DevGuard g(device);
   fq3_join* j = new fq3_join();
   j->dev = device;
+  if (int rc = start(j, n_segments, pauses_ms)) {
+    delete j;
+    return rc;
+  }
   if (cudaMalloc(&j->tail, 2 * F * sizeof(float)) != cudaSuccess) {
     delete j;
     return jfail(FQ3_ERR_CUDA, "cudaMalloc of the join tail failed");
   }
-  j->S = n_segments;
-  j->P = pause_ms * (FQ3_JOIN_RATE / 1000);
-  j->segs.assign(n_segments, Seg());
   *out = j;
   return 0;
 }
 
-extern "C" int fq3_join_reset(fq3_join* j, int32_t n_segments, int32_t pause_ms) {
+extern "C" int fq3_join_create(int32_t device, int32_t n_segments, int32_t pause_ms, fq3_join** out) {
+  std::vector<int32_t> plan;
+  if (int rc = uniform(n_segments, pause_ms, &plan)) return rc;
+  return fq3_join_create_pauses(device, n_segments, plan.data(), out);
+}
+
+extern "C" int fq3_join_reset_pauses(fq3_join* j, int32_t n_segments, const int32_t* pauses_ms) {
   if (!j) return jfail(FQ3_ERR_INVALID, "null argument");
-  if (n_segments < 1) return jfail(FQ3_ERR_INVALID, "a join needs at least one segment");
-  if (pause_ms < 0 || pause_ms > FQ3_JOIN_PAUSE_MAX_MS) return jfail(FQ3_ERR_INVALID, "pause_ms must be in [0, 2000]");
   DevGuard g(j->dev);
-  free_chunks(j);
-  j->S = n_segments;
-  j->P = pause_ms * (FQ3_JOIN_RATE / 1000);
-  j->cur = j->pp = 0;
-  j->out_pos = j->released = 0;
-  j->segs.assign(n_segments, Seg());
-  return 0;
+  return start(j, n_segments, pauses_ms);
+}
+
+extern "C" int fq3_join_reset(fq3_join* j, int32_t n_segments, int32_t pause_ms) {
+  std::vector<int32_t> plan;
+  if (int rc = uniform(n_segments, pause_ms, &plan)) return rc;
+  return fq3_join_reset_pauses(j, n_segments, plan.data());
 }
 
 extern "C" void fq3_join_destroy(fq3_join* j) {

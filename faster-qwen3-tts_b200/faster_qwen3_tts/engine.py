@@ -89,7 +89,7 @@ EXPORTS = [
     "fq3_flac_create", "fq3_flac_reset", "fq3_flac_destroy", "fq3_flac_max_bytes", "fq3_flac_process",
     "fq3_flac_last_error",
     "fq3_join_create", "fq3_join_reset", "fq3_join_destroy", "fq3_join_released", "fq3_join_total", "fq3_join_process",
-    "fq3_join_last_error",
+    "fq3_join_last_error", "fq3_join_create_pauses", "fq3_join_reset_pauses",
 ]
 
 
@@ -232,6 +232,8 @@ def load_library() -> C.CDLL:
     lib.fq3_flac_last_error.restype = C.c_char_p
     lib.fq3_join_create.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_void_p)]
     lib.fq3_join_reset.argtypes = [C.c_void_p, C.c_int32, C.c_int32]
+    lib.fq3_join_create_pauses.argtypes = [C.c_int32, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_void_p)]
+    lib.fq3_join_reset_pauses.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_int32)]
     lib.fq3_join_destroy.argtypes = [C.c_void_p]
     lib.fq3_join_destroy.restype = None
     lib.fq3_join_released.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32),

@@ -5,6 +5,10 @@ window, and the rows finish in any order.  The join (``csrc/fq3_join.cu``; ``tes
 their 24 kHz float32 PCM one stream, in segment order:
 
 * ``seg_0``, ``P`` zeros, ``seg_1``, ..., ``seg_{S-1}`` with ``P = 24 * pause_ms``, ``pause_ms`` an integer in [0, 2000].
+* Or, with a pause per boundary (``pauses``, SSML breaks): ``P_0`` zeros, ``seg_0``, ``P_1`` zeros, ..., ``seg_{S-1}``,
+  ``P_S`` zeros with ``P_k = 24 * pauses[k]``, each an integer in [0, 10000].  The leading zeros are released with
+  segment 0's first push, the trailing ones in the call that completes the stream.  ``pause_ms`` is the plan
+  ``[0, P, ..., P, 0]``, bit for bit.
 * Every inner boundary is faded, also at pause 0: sample n of segment k (length L) becomes ``x * a * b`` in fp32, in that
   order, with ``a = w[n]`` for k > 0 and n < F and ``b = w[L - 1 - n]`` for k < S - 1 and L - 1 - n < F (1 otherwise),
   ``F = 120`` (5 ms) and ``w[i] = float32(0.5 - 0.5 cos(pi (i + 0.5) / F))`` (``fade_table``).
@@ -27,6 +31,7 @@ import torch
 RATE = 24000
 FADE = 120
 PAUSE_MAX_MS = 2000
+BREAK_MAX_MS = 10000            # one boundary of a pause plan (an SSML document's breaks)
 
 
 def check_pause(pause_ms) -> int:
@@ -34,6 +39,17 @@ def check_pause(pause_ms) -> int:
     if isinstance(pause_ms, bool) or not isinstance(pause_ms, (int, np.integer)) or not 0 <= pause_ms <= PAUSE_MAX_MS:
         raise ValueError(f"pause_ms must be an integer in [0, {PAUSE_MAX_MS}], got {pause_ms!r}")
     return int(pause_ms)
+
+
+def check_pauses(pauses, n_segments: int) -> List[int]:
+    """a pause plan (``n_segments + 1`` integers in [0, 10000] ms) as a list; ValueError otherwise"""
+    pauses = list(pauses)
+    if len(pauses) != n_segments + 1:
+        raise ValueError(f"a pause plan has one entry per boundary: {n_segments + 1}, got {len(pauses)}")
+    for p in pauses:
+        if isinstance(p, bool) or not isinstance(p, (int, np.integer)) or not 0 <= p <= BREAK_MAX_MS:
+            raise ValueError(f"every pause must be an integer in [0, {BREAK_MAX_MS}] ms, got {p!r}")
+    return [int(p) for p in pauses]
 
 
 def pause_samples(pause_ms: int) -> int:
@@ -47,25 +63,33 @@ def fade_table() -> np.ndarray:
 
 class Join:
     """Device state of one segmented request (C ABI ``fq3_join_*``): the held tail of the segment being played and the
-    samples of later segments.  ``close`` hands the handle back to a per-device pool."""
+    samples of later segments.  ``pauses``: a pause per boundary (module docstring) instead of ``pause_ms``.  ``close``
+    hands the handle back to a per-device pool."""
 
     _pool = {}   # device index -> released handles
 
-    def __init__(self, n_segments: int, pause_ms: int = 0, device=None):
+    def __init__(self, n_segments: int, pause_ms: int = 0, device=None, pauses=None):
         if int(n_segments) < 1:
             raise ValueError("a join needs at least one segment")
         self.n_segments, self.pause_ms = int(n_segments), check_pause(pause_ms)
+        self.pauses = None if pauses is None else check_pauses(pauses, self.n_segments)
         from .engine import load_library
         self._lib = load_library()
         dev = torch.device(device if device is not None else "cuda")
         self.device = torch.device("cuda", dev.index if dev.index is not None else torch.cuda.current_device())
+        plan = None if self.pauses is None else (C.c_int32 * len(self.pauses))(*self.pauses)
         pool = Join._pool.get(self.device.index)
         if pool:
             self._h = pool.pop()
-            self._lib.fq3_join_reset(self._h, self.n_segments, self.pause_ms)
+            if plan is None:
+                self._lib.fq3_join_reset(self._h, self.n_segments, self.pause_ms)
+            else:
+                self._lib.fq3_join_reset_pauses(self._h, self.n_segments, plan)
         else:
             h = C.c_void_p()
-            if self._lib.fq3_join_create(self.device.index, self.n_segments, self.pause_ms, C.byref(h)):
+            rc = (self._lib.fq3_join_create(self.device.index, self.n_segments, self.pause_ms, C.byref(h)) if plan is None
+                  else self._lib.fq3_join_create_pauses(self.device.index, self.n_segments, plan, C.byref(h)))
+            if rc:
                 raise RuntimeError(self._lib.fq3_join_last_error().decode())
             self._h = h
         self.ended = [False] * self.n_segments
@@ -145,9 +169,9 @@ def process(joins: Sequence[Join], pushes: Sequence[Tuple[Join, int, torch.Tenso
     return list(torch.split(out, counts))
 
 
-def join(pcms: Sequence[torch.Tensor], pause_ms: int = 0) -> torch.Tensor:
+def join(pcms: Sequence[torch.Tensor], pause_ms: int = 0, pauses=None) -> torch.Tensor:
     """The whole join of complete segments (1-D float32 on one CUDA device), each pushed once with its end."""
-    j = Join(len(pcms), pause_ms, pcms[0].device)
+    j = Join(len(pcms), pause_ms, pcms[0].device, pauses)
     try:
         return process([j], [(j, k, p, True) for k, p in enumerate(pcms)])[0]
     finally:

@@ -900,8 +900,15 @@ class FasterQwen3TTS:
         """A ``split=True`` request (DESIGN.md "Long inputs"): ``text`` cut by ``segment.split_text``, one row per
         segment with the prompt ``make(segment_text)()`` builds, all decoded side by side through a
         ``serving.ContinuousBatcher`` on this model and joined on the device; yields (audio, sample_rate, timing)."""
-        from .serving import batcher_for_model, segment_requests
-        segs = segment_requests(make, text, max_segment_chars)
+        from .serving import segment_requests
+        yield from self._segments_stream(segment_requests(make, text, max_segment_chars), pause_ms, seed, chunk_size,
+                                         gen, speed, sample_rate, pitch, gain_db)
+
+    def _segments_stream(self, segs, pause_ms, seed, chunk_size, gen, speed=1.0, sample_rate=None, pitch=0.0,
+                         gain_db=0.0):
+        """``serving.Segments`` spoken side by side through a ``serving.ContinuousBatcher`` on this model and joined on
+        the device; yields (audio, sample_rate, timing)."""
+        from .serving import batcher_for_model
         b = batcher_for_model(self, chunk_size=chunk_size)
         try:
             ticket = b.submit(segs, split=True, pause_ms=pause_ms, seed=seed, **_post_kw(speed, sample_rate, pitch, gain_db),
@@ -926,10 +933,54 @@ class FasterQwen3TTS:
         return make
 
     def _split_one_shot(self, *args, **kw):
-        sr, parts = _rate_of(self.sample_rate, kw.get("sample_rate")), []
-        for audio, sr, _ in self._split_stream(*args, **kw):
+        return self._collect(self._split_stream(*args, **kw), kw.get("sample_rate"))
+
+    def _collect(self, chunks, sample_rate):
+        sr, parts = None, []
+        for audio, sr, _ in chunks:
             parts.append(audio)
+        if sr is None:
+            sr = _rate_of(self.sample_rate, sample_rate)
         return [np.concatenate(parts) if parts else np.zeros(1, dtype=np.float32)], sr
+
+    # ------------------------------------------------------------------ SSML
+    _SAMPLING = dict(max_new_tokens=2048, min_new_tokens=2, temperature=0.9, top_k=50, top_p=1.0, do_sample=True,
+                     repetition_penalty=1.05)
+
+    @torch.inference_mode()
+    def speak_ssml(self, ssml: str, voices: Dict[str, dict], voice: Optional[str] = None, language: str = "Auto",
+                      max_segment_chars: int = 400, pause_ms: int = 0, seed: Optional[int] = None, speed: float = 1.0,
+                      pitch: float = 0.0, gain_db: float = 0.0, sample_rate: Optional[int] = None,
+                      **sampling) -> Tuple[list, int]:
+        """An SSML document (``ssml.py``; DESIGN.md "SSML") spoken as segment rows and joined on the device.  ``voices``:
+        name -> voice spec (``ssml.voice_request``); ``voice``: the name spoken outside every ``<voice>``;
+        ``pause_ms``: the pause at an inner boundary without a ``<break>``; ``speed`` / ``pitch`` / ``gain_db`` /
+        ``sample_rate`` apply once to the joined stream, on top of the document's prosody; ``sampling``: the keywords
+        of ``generate_custom_voice`` from ``max_new_tokens`` to ``repetition_penalty`` (``max_new_tokens`` is per
+        segment).  Returns ([audio], sample_rate).  (Not a ``generate_*`` method: those share one argument layout, with
+        ``text`` first and ``pitch`` / ``gain_db`` right after ``sample_rate``.)"""
+        return self._collect(self.speak_ssml_streaming(
+            ssml, voices, voice, language, max_segment_chars, pause_ms, seed, speed, pitch, gain_db, sample_rate,
+            **sampling), sample_rate)
+
+    @torch.inference_mode()
+    def speak_ssml_streaming(self, ssml: str, voices: Dict[str, dict], voice: Optional[str] = None,
+                                language: str = "Auto", max_segment_chars: int = 400, pause_ms: int = 0,
+                                seed: Optional[int] = None, speed: float = 1.0, pitch: float = 0.0, gain_db: float = 0.0,
+                                sample_rate: Optional[int] = None, chunk_size: int = 12, **sampling
+                                ) -> Generator[Tuple[np.ndarray, int, dict], None, None]:
+        """``speak_ssml`` as a stream of (audio, sample_rate, timing); the timing carries ``segment`` and
+        ``n_segments``."""
+        from .serving import ssml_request
+        _check_speed(speed, pitch, gain_db)
+        _check_rate(sample_rate)
+        self._check_split(True, max_segment_chars, pause_ms, seed)
+        unknown = set(sampling) - set(self._SAMPLING)
+        if unknown:
+            raise TypeError(f"speak_ssml got unexpected keyword arguments {sorted(unknown)}")
+        segs = ssml_request(self, ssml, voices, voice, language, max_segment_chars)
+        yield from self._segments_stream(segs, pause_ms, seed, chunk_size, dict(self._SAMPLING, **sampling),
+                                         **_post_kw(speed, sample_rate, pitch, gain_db))
 
     @staticmethod
     def _check_split(split, max_segment_chars, pause_ms, seed=None):

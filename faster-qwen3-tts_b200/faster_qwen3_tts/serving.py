@@ -104,14 +104,21 @@ class Ticket:
 
 class Segments(list):
     """The per-segment ``prepare`` callables of a segmented request, in order (what the ``*_request`` helpers return
-    with ``split=True``), with the texts they speak; on the worker also the request's state: the next segment to admit,
-    the frames each row has made, which rows have ended, and the join."""
+    with ``split=True``, or ``ssml_request``), with the texts they speak; ``prosody``: each segment's (speed, pitch,
+    gain_db), applied to its row before the join (None: all (1, 0, 0)); ``breaks``: the S + 1 boundaries' pauses in ms,
+    None where the request's ``pause_ms`` applies (``ssml.parse``).  On the worker also the request's state: the pause
+    plan, the next segment to admit, the frames each row has made, which rows have ended, and the join."""
 
-    def __init__(self, prepares, texts):
+    def __init__(self, prepares, texts, prosody=None, breaks=None):
         super().__init__(prepares)
         if not self:
             raise ValueError("the text has no segment to speak")
         self.texts = list(texts)
+        self.prosody = [(1.0, 0.0, 0.0)] * len(self) if prosody is None else [tuple(map(float, p)) for p in prosody]
+        self.breaks = [None] * (len(self) + 1) if breaks is None else list(breaks)
+        if len(self.texts) != len(self) or len(self.prosody) != len(self) or len(self.breaks) != len(self) + 1:
+            raise ValueError("Segments needs one text and one prosody per segment and one break per boundary")
+        self.pauses = None                  # the filled pause plan (``plan``), set by ``submit``
         self.next = 0                       # rows [0, next) have been admitted
         self.frames = [0] * len(self)
         self.ended = [False] * len(self)
@@ -123,6 +130,11 @@ class Segments(list):
     def current(self) -> int:
         """the segment being played: the first that has not ended"""
         return next((k for k, e in enumerate(self.ended) if not e), len(self) - 1)
+
+    def plan(self, pause_ms: int) -> List[int]:
+        """the pause of every boundary in ms: the document's breaks, else ``pause_ms`` inside and 0 at the two ends"""
+        S = len(self)
+        return [b if b is not None else (pause_ms if 0 < k < S else 0) for k, b in enumerate(self.breaks)]
 
 
 def segment_requests(make, text: str, max_segment_chars: int):
@@ -273,7 +285,12 @@ class ContinuousBatcher:
         if seed is None:
             import random
             seed = random.getrandbits(62)
+        from .join import check_pauses
         prepare.seed, prepare.pause_ms = int(seed), pause_ms
+        prepare.pauses = check_pauses(prepare.plan(pause_ms), len(prepare))
+        for speed, pitch, gain_db in set(prepare.prosody):
+            self._speed(speed, pitch, gain_db)
+            self._output(None, "f32", pitch, gain_db)   # warms a pitched 24 kHz table on the caller's thread
         return prepare
 
     @staticmethod
@@ -368,10 +385,11 @@ class ContinuousBatcher:
             uniforms = getattr(self.joiner, "uniforms", None)
             if uniforms is not None:
                 gen["uniforms"] = uniforms(segment_seed(segs.seed, k), int(gen.get("max_new_tokens", 2048)))
+            speed, pitch, gain_db = segs.prosody[k]
             with self._lock:
                 self._rid += 1
                 row = Ticket(self._rid, segs[k], gen, submitted_at=t.submitted_at, cancelled=t.cancelled, parent=t,
-                             seg=k)
+                             seg=k, speed=speed, pitch=pitch, gain_db=gain_db)
             segs.rows[k] = row
         return row
 
@@ -393,13 +411,14 @@ class ContinuousBatcher:
             lead = self._made_s(t) - t.pace * (now - t.first_chunk_at)
         before = 0.0
         for j in range(cur, k):
-            made = segs.frames[j] * self.frame_s / t.speed
-            est = len(segs.texts[j]) / CHARS_PER_S / t.speed
+            speed = t.speed * segs.prosody[j][0]   # the row's own rate, then the request's
+            made = segs.frames[j] * self.frame_s / speed
+            est = len(segs.texts[j]) / CHARS_PER_S / speed
             if j == cur:
                 before += 0.0 if segs.ended[j] else max(0.0, est - made)
             else:
                 before += made if segs.ended[j] else max(made, est)
-            before += segs.pause_ms / 1000.0 / t.speed
+            before += segs.pauses[j + 1] / 1000.0 / t.speed
         return lead + before
 
     def _candidate_rows(self) -> List[Ticket]:
@@ -448,12 +467,19 @@ class ContinuousBatcher:
         """the request's codec window, built for the request's own chunk size where it has one (the window policy's
         calibration point depends on it); a short first chunk is for windows whose audio does not depend on the chunking"""
         own = t.gen_kwargs.get("chunk_size")
-        kw = {"segment": True} if t.parent is not None else self._out_kw(t)
+        kw = self._row_kw(t) if t.parent is not None else self._out_kw(t)
         win = self.window_factory(ref_codes, **kw) if own is None else self.window_factory(ref_codes, own, **kw)
         if t.gen_kwargs.get("first_chunk") and not getattr(win, "any_chunking", False):
             raise ValueError("first_chunk needs a codec window whose audio does not depend on the chunking (the stateful "
                              "codec stream); under the window policy the audio of a request is defined by one chunk_size")
         return win
+
+    @staticmethod
+    def _row_kw(t: Ticket) -> dict:
+        """a row's window keywords: codec only, or with its segment's prosody where that is not the identity"""
+        if t.flushes:
+            return {"segment": True, "speed": t.speed, "pitch": t.pitch, "gain_db": t.gain_db}
+        return {"segment": True}
 
     @staticmethod
     def _out_kw(t: Ticket) -> dict:
@@ -600,11 +626,17 @@ class ContinuousBatcher:
                 t, win = self.live[rq.tag]
                 n = int(codes.shape[0])
                 if t.parent is not None:
-                    pcm = pcm_of[rq.tag][0] if rq.tag in pcm_of else (win.push(codes)[0] if n else None)
+                    if rq.tag in pcm_of:
+                        pcm = pcm_of[rq.tag][0]
+                    elif t.flushes and (n or rq.finished):
+                        pcm = win.push(codes, final=bool(rq.finished))[0]
+                    else:
+                        pcm = win.push(codes)[0] if n else None
                     pushes.append((t, n, pcm, bool(rq.finished)))
                     if rq.finished:
                         del self.live[rq.tag]
                         self.requests.pop(rq.tag, None)
+                        self._drop_stages(win)
                     continue
                 if n or rq.tag in pcm_of:
                     if rq.tag in pcm_of:
@@ -683,10 +715,10 @@ def batcher_for_model(model, chunk_size: int = 8, to_host: bool = True, **kw) ->
             return codes.cpu().numpy(), model.sample_rate
 
     def window(ref_codes, chunk=chunk_size, speed=1.0, segment=False, **out):
-        if segment:   # a row of a segmented request: codec only, its PCM stays on the device for the join
+        if segment:   # a row of a segmented request: its PCM stays on the device for the join, at 24 kHz f32
             if st is None:
                 raise ValueError("split=True needs the codec (PCM)")
-            return model._make_window(st, ref_codes, chunk, False)
+            return model._make_window(st, ref_codes, chunk, False, **({} if speed == 1.0 else {"speed": speed}), **out)
         if st is None:
             if speed != 1.0:
                 raise ValueError("a speaking rate other than 1 needs the codec (PCM)")
@@ -725,8 +757,9 @@ class _Joiner:
     def open(self, t, out_kw):
         from .join import Join
         from .model import _Chain
-        return Join(len(t.segments), t.segments.pause_ms, self.device), _Chain(self.model, self.st, self.to_host,
-                                                                               **out_kw)
+        segs = t.segments
+        return (Join(len(segs), segs.pause_ms, self.device, segs.pauses),
+                _Chain(self.model, self.st, self.to_host, **out_kw))
 
     def run(self, states, pushes):
         import torch
@@ -791,3 +824,14 @@ def custom_voice_request(model, text: str, speaker: Optional[str], language: str
             return tie, tam, tth, tpe, None
         return prepare
     return segment_requests(make, text, max_segment_chars) if split else make(text)
+
+
+def ssml_request(model, ssml: str, voices, voice: Optional[str] = None, language: str = "Auto",
+                 max_segment_chars: int = 400) -> Segments:
+    """``Segments`` of an SSML document (``ssml.py``) for ``ContinuousBatcher.submit(..., split=True)``: each segment's
+    prompt in its voice (``voices``: name -> voice spec, ``ssml.voice_request``; ``voice``: the name spoken outside every
+    ``<voice>``) and language, its prosody and the document's breaks.  Every refusal is a ValueError."""
+    from .ssml import parse, voice_request
+    doc = parse(ssml, voices, voice, language, max_segment_chars)
+    return Segments([voice_request(model, voices[s.voice], s.text, s.language) for s in doc.spans],
+                    [s.text for s in doc.spans], [(s.speed, s.pitch, s.gain_db) for s in doc.spans], doc.breaks)

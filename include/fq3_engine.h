@@ -513,10 +513,19 @@ const char* fq3_flac_last_error(void);
 #define FQ3_JOIN_RATE 24000
 #define FQ3_JOIN_FADE 120
 #define FQ3_JOIN_PAUSE_MAX_MS 2000
+#define FQ3_JOIN_BREAK_MAX_MS 10000
 typedef struct fq3_join fq3_join;
 int fq3_join_create(int32_t device, int32_t n_segments, int32_t pause_ms, fq3_join** out);
 /* a new request of n_segments at pause_ms; frees the samples still held (host-side, nothing is launched) */
 int fq3_join_reset(fq3_join* j, int32_t n_segments, int32_t pause_ms);
+/* A pause per boundary (SSML breaks, faster_qwen3_tts/ssml.py): pauses_ms (host, n_segments + 1 entries, each in
+ * [0, FQ3_JOIN_BREAK_MAX_MS]) is the plan P_0 zeros, seg_0, P_1 zeros, seg_1, ..., seg_{S-1}, P_S zeros, P_k = pauses_ms[k]
+ * * FQ3_JOIN_RATE / 1000.  pauses_ms[0] is leading silence, released with segment 0's first push; pauses_ms[S] is
+ * trailing silence, released in the call that completes the stream (the one that ends the last segment, or with it the
+ * last of the earlier ones).  Fades, hold and release are the rule above: the outer edges are not faded.
+ * fq3_join_create / fq3_join_reset are the plan [0, P, ..., P, 0] and give the same bits. */
+int fq3_join_create_pauses(int32_t device, int32_t n_segments, const int32_t* pauses_ms, fq3_join** out);
+int fq3_join_reset_pauses(fq3_join* j, int32_t n_segments, const int32_t* pauses_ms);
 void fq3_join_destroy(fq3_join* j);
 /* A call's pushes: push i gives lens[i] new samples of segment seg[i] of join join_of[i] (index into joins), ends[i] != 0
  * ends that segment; all host arrays, one push per (join, segment) and call.  released[j] (host, n_joins) receives the
